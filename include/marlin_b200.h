@@ -167,6 +167,35 @@ int32_t mb_block_inverse(mb_ctx* ctx, const mb_block* A, mb_block* out);
  * this also covers X T = B.  Used for `l \ b` and `b * inv(u)` of the block algorithms. */
 int32_t mb_block_trsm(mb_ctx* ctx, const mb_block* T, int32_t lower, int32_t unit_diagonal, mb_block* B);
 
+/* ---- f5: DenseVecMatrix.computeSVD (matrix/DenseVecMatrix.scala:1531-1652): the Gramian A^T A, its symmetric
+ *      eigendecomposition and the two decisions of the reference's driver code.  U = A (V_k S_k^-1) is then
+ *      mb_block_div on column views of V and mb_matmul_rowsharded. ---- */
+#define MB_ERR_NO_CONVERGENCE -8   /* the eigensolver hit its sweep cap -> IllegalStateException (:1798-1807)      */
+/* DenseVecMatrix.computeGramianMatrix (:1464-1486, dspr + triuToFull): G (n x n) = A^T A for any fp64 view A (m x n),
+ * e.g. the transposed view of a row shard.  Exactly symmetric; bitwise reproducible from run to run (fixed-order split-K
+ * sum).  More than 65535 columns is MB_ERR_INVALID_ARG, as in the reference. */
+int32_t mb_block_gramian(mb_ctx* ctx, const mb_block* A, mb_block* G);
+/* Bytes of temporary device memory mb_block_gramian takes for an m x n operand on num_sms SMs (TMA-addressable operand;
+ * other views take none): the split-K partials, 0 unless the lower triangle has fewer than two waves of 128 x 128 tiles,
+ * never more than 256 MiB.  Stream-ordered (cudaMallocAsync), returned when the call's work completes.  Pure logic. */
+int64_t mb_gramian_workspace_bytes(int64_t n, int64_t m, int32_t num_sms);
+/* brzSvd(G) / EigenValueDecomposition.symmetricEigs (:1596-1606, :1725-1834) for a symmetric G (lower triangle read):
+ * all n eigenvalues into the HOST array w_out, ordered by |w| descending (ties: lower index first) — what dgesdd returns
+ * as singular values of a symmetric G — and the matching orthonormal eigenvectors as the columns of V (n x n).
+ * sweeps_out (may be NULL) receives the number of Jacobi sweeps.  Blocking.  Takes 32 * N^2 bytes of temporary device
+ * memory (N = n rounded up to even) for the duration of the call. */
+int32_t mb_block_syev(mb_ctx* ctx, const mb_block* G, mb_block* V, double* w_out, int32_t* sweeps_out);
+/* The mode chooser and every `require` of computeSVD (:1565-1604) plus the column cap of computeGramianMatrix
+ * (:1466-1468), with the reference's messages.  mode: "auto", "local-svd", "local-eigs" or "dist-eigs"; *compute_mode
+ * receives MB_SVD_LOCAL_LAPACK / MB_SVD_LOCAL_ARPACK / MB_SVD_DIST_ARPACK.  Pure integer logic, no GPU needed. */
+#define MB_SVD_LOCAL_LAPACK 0
+#define MB_SVD_LOCAL_ARPACK 1
+#define MB_SVD_DIST_ARPACK  2
+int32_t mb_svd_mode(int64_t n, int32_t k, const char* mode, int32_t* compute_mode);
+/* The effective rank sk of :1607-1621: the number of leading sigmas >= rcond * sigmas[0], at most min(k, count).
+ * Returns sk (>= 0) or a negative error code. */
+int32_t mb_svd_rank(const double* sigmas, int32_t count, int32_t k, double rcond);
+
 /* ---- a11: MTUtils.randomDenVecMatrix / randomBlockMatrix input generation
  *      (utils/MTUtils.scala:34-73, rdd/RandomRDD.scala:28-101, utils/RandomDataGenerator.scala:53-65,113-131).
  * Fills `count` consecutive values of partition stream `partition_seed` (one XORShift stream per

@@ -184,6 +184,16 @@ public:
     }
     SubMatrix cholesky() const { SubMatrix r = copy(); check(mb_block_cholesky(Context::get(), r.h_.get())); return r; }
     SubMatrix inverse() const { SubMatrix r = empty(rows(), cols()); check(mb_block_inverse(Context::get(), h_.get(), r.h_.get())); return r; }
+    // the local steps of DenseVecMatrix.computeSVD: computeGramianMatrix (DenseVecMatrix.scala:1464-1486) and the eigen step
+    // (:1589-1606); eigenvalues ordered by |w| descending, eigenvectors as the columns of the returned block
+    SubMatrix gramian() const { SubMatrix r = empty(cols(), cols()); check(mb_block_gramian(Context::get(), h_.get(), r.h_.get())); return r; }
+    std::pair<std::vector<double>, SubMatrix> symmetricEigen() const {
+        SubMatrix v = empty(rows(), rows());
+        std::vector<double> w((size_t)std::max(1, rows()));
+        check(mb_block_syev(Context::get(), h_.get(), v.h_.get(), w.data(), nullptr));
+        w.resize((size_t)rows());
+        return {w, v};
+    }
     SubMatrix solveTriangular(const SubMatrix& rhs, bool lower, bool unit = false) const {      // this \ rhs
         SubMatrix x = rhs.copy();
         check(mb_block_trsm(Context::get(), h_.get(), lower ? 1 : 0, unit ? 1 : 0, x.h_.get()));
@@ -680,6 +690,41 @@ public:
         if (numRows() != numCols()) throw std::invalid_argument("Inversion only support square matrix: " + std::to_string(numRows()) + " v.s " + std::to_string(numCols()));
         if (modeIsDist(mode, numRows())) throw std::invalid_argument("the C++ mirror runs the local (breeze) mode; use the Python host for mode dist");
         return BlockMatrix({{BlockID(0, 0), asOneBlock().inverse()}}, numRows(), numCols(), 1, 1);
+    }
+
+    // ---- computeSVD(k, computeU, rCond) :1531-1541 and the mode overload :1557-1652 (one process: every row is local).
+    //      Every mode forms one Gramian on the device and decomposes it fully (see marlin_b200/matrix/dense_vec_matrix.py). ----
+    struct SVD {
+        std::shared_ptr<DenseVecMatrix> U;                                           // null unless computeU
+        std::vector<double> s;
+        DenseMatrix V;                                                                // n x sk
+    };
+    SVD computeSVD(int k, bool computeU = false, double rCond = 1e-9) { return computeSVD(k, computeU, rCond, "auto"); }
+    SVD computeSVD(int k, bool computeU, double rCond, const std::string& mode) {
+        const long n = numCols();
+        int32_t cm = 0;
+        check(mb_svd_mode(n, k, mode.c_str(), &cm));
+        SubMatrix g = data_.gramian();
+        auto eig = g.symmetricEigen();
+        std::vector<double> sigmas(eig.first.size());
+        for (size_t i = 0; i < sigmas.size(); ++i) sigmas[i] = std::sqrt(std::fabs(eig.first[i]));
+        const int32_t sk = mb_svd_rank(sigmas.data(), (int32_t)sigmas.size(), k, rCond);
+        if (sk < 0) check(sk);
+        SVD out;
+        out.s.assign(sigmas.begin(), sigmas.begin() + sk);
+        out.V = DenseMatrix((int)n, sk);
+        if (sk == 0) return out;
+        out.V = eig.second.slice(0, (int)n, 0, sk).copy().denseBlock();
+        if (computeU) {
+            // N = V_k S_k^-1 (:1635-1646) column by column on the device, then U = this.multiply(N) (:1647)
+            SubMatrix nm = SubMatrix::empty((int)n, sk);
+            for (int j = 0; j < sk; ++j) {
+                SubMatrix dst = nm.slice(0, (int)n, j, j + 1);
+                check(mb_block_div(Context::get(), eig.second.slice(0, (int)n, j, j + 1).handle(), sigmas[(size_t)j], 0, dst.handle()));
+            }
+            out.U = std::make_shared<DenseVecMatrix>(multiply(nm.denseBlock()));
+        }
+        return out;
     }
 
 private:

@@ -21,6 +21,7 @@
 #  include "jni_compile_check.h"
 #endif
 #include <stdlib.h>
+#include <string.h>
 #include "marlin_b200.h"
 
 #define NATIVE(ret, name) JNIEXPORT ret JNICALL Java_edu_nju_pasalab_marlin_matrix_Native_00024_##name
@@ -145,6 +146,39 @@ NATIVE(void, lu)(JNIEnv* e, jobject o, jlong ctx, jlong a, jintArray permOut) {
 }
 NATIVE(void, cholesky)(JNIEnv* e, jobject o, jlong ctx, jlong a) { raise(e, mb_block_cholesky(CTX(ctx), BLK(a))); }
 NATIVE(void, inverse)(JNIEnv* e, jobject o, jlong ctx, jlong a, jlong out) { raise(e, mb_block_inverse(CTX(ctx), BLK(a), BLK(out))); }
+/* ---- f5: the local steps of computeSVD (matrix/DenseVecMatrix.scala:1464-1486, 1565-1621) ---- */
+NATIVE(void, gramian)(JNIEnv* e, jobject o, jlong ctx, jlong a, jlong g) { raise(e, mb_block_gramian(CTX(ctx), BLK(a), BLK(g))); }
+NATIVE(jint, syev)(JNIEnv* e, jobject o, jlong ctx, jlong g, jlong v, jdoubleArray wOut) {
+    /* wOut (n entries): eigenvalues by |w| descending; returns the number of Jacobi sweeps */
+    const jsize n = (*e)->GetArrayLength(e, wOut);
+    double* w = (double*)malloc(sizeof(double) * (size_t)(n > 0 ? n : 1));
+    int32_t sweeps = 0;
+    const int32_t rc = mb_block_syev(CTX(ctx), BLK(g), BLK(v), w, &sweeps);
+    if (rc == MB_OK && n > 0) {
+        double* dst = (double*)(*e)->GetPrimitiveArrayCritical(e, wOut, NULL);
+        memcpy(dst, w, sizeof(double) * (size_t)n);
+        (*e)->ReleasePrimitiveArrayCritical(e, wOut, dst, 0);
+    }
+    free(w);
+    raise(e, rc);
+    return sweeps;
+}
+NATIVE(jint, svdMode)(JNIEnv* e, jobject o, jlong n, jint k, jstring mode) {
+    const char* m = (*e)->GetStringUTFChars(e, mode, NULL);
+    int32_t cm = 0;
+    const int32_t rc = mb_svd_mode(n, k, m, &cm);
+    (*e)->ReleaseStringUTFChars(e, mode, m);
+    raise(e, rc);
+    return cm;
+}
+NATIVE(jint, svdRank)(JNIEnv* e, jobject o, jdoubleArray sigmas, jint k, jdouble rCond) {
+    const jsize n = (*e)->GetArrayLength(e, sigmas);
+    double* s = (double*)(*e)->GetPrimitiveArrayCritical(e, sigmas, NULL);
+    const int32_t sk = mb_svd_rank(s, n, k, rCond);
+    (*e)->ReleasePrimitiveArrayCritical(e, sigmas, s, JNI_ABORT);
+    if (sk < 0) raise(e, sk);
+    return sk;
+}
 NATIVE(void, trsm)(JNIEnv* e, jobject o, jlong ctx, jlong t, jboolean lower, jboolean unitDiagonal, jlong b) {
     raise(e, mb_block_trsm(CTX(ctx), BLK(t), lower ? 1 : 0, unitDiagonal ? 1 : 0, BLK(b)));
 }

@@ -18,8 +18,10 @@ MB_ERR_CUDA = -4
 MB_ERR_OOM = -5
 MB_ERR_EMPTY = -6
 MB_ERR_TIMEOUT = -7
+MB_ERR_NO_CONVERGENCE = -8
 
 MB_F64, MB_BF16, MB_F32 = 0, 1, 2
+MB_SVD_LOCAL_LAPACK, MB_SVD_LOCAL_ARPACK, MB_SVD_DIST_ARPACK = 0, 1, 2
 
 _LIB_PATH = Path(__file__).resolve().parent / "lib" / "libmarlin_b200.so"
 
@@ -76,6 +78,11 @@ SIGNATURES = {
     "mb_block_cholesky": (c_i32, [c_ctx, c_blk]),
     "mb_block_inverse": (c_i32, [c_ctx, c_blk, c_blk]),
     "mb_block_trsm": (c_i32, [c_ctx, c_blk, c_i32, c_i32, c_blk]),
+    "mb_block_gramian": (c_i32, [c_ctx, c_blk, c_blk]),
+    "mb_gramian_workspace_bytes": (c_i64, [c_i64, c_i64, c_i32]),
+    "mb_block_syev": (c_i32, [c_ctx, c_blk, c_blk, c_dp, C.POINTER(c_i32)]),
+    "mb_svd_mode": (c_i32, [c_i64, c_i32, C.c_char_p, C.POINTER(c_i32)]),
+    "mb_svd_rank": (c_i32, [c_dp, c_i32, c_i32, c_f64]),
     "mb_fill_uniform": (c_i32, [c_ctx, c_blk, c_i64, c_i64, c_f64, c_f64, c_i32]),
     "mb_hash_seed": (c_i64, [c_i64]),
     "mb_partition_seeds": (c_i32, [c_i64, c_i32, C.POINTER(c_i64)]),

@@ -8,6 +8,7 @@
 #include "gemm_ozaki.h"
 #include "blas12.h"
 #include "factor.h"
+#include "eigen.h"
 
 #include <cuda_runtime.h>
 #include <algorithm>
@@ -1194,6 +1195,65 @@ int32_t mb_block_trsm(mb_ctx* ctx, const mb_block* T, int32_t lower, int32_t uni
     int launches = 0;
     MB_CUDA(mb::trsm_left(fview(T), lower != 0, unit_diagonal != 0, fview(B), ctx->num_sms, ctx->stream, &launches));
     ctx->launches += launches;
+    return MB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------- SVD (SURVEY 8 f5)
+// DenseVecMatrix.computeGramianMatrix (matrix/DenseVecMatrix.scala:1464-1486): dspr per row into a packed upper triangle,
+// `+=` over partitions, triuToFull.  Here: the lower-triangle tiles on the DMMA mainloop, split over the rows, one
+// fixed-order sum of the partials that writes both triangles.
+int32_t mb_block_gramian(mb_ctx* ctx, const mb_block* A, mb_block* G) {
+    MB_CTX(ctx);
+    MB_LOCK(ctx);
+    if (!A || !G) return fail(MB_ERR_INVALID_ARG, "mb_block_gramian: null block");
+    if (A->dtype != MB_F64 || G->dtype != MB_F64) return fail(MB_ERR_UNSUPPORTED, "mb_block_gramian: fp64 blocks only");
+    const int m = A->rows, n = A->cols;
+    if (n > 65535) return fail(MB_ERR_INVALID_ARG, "Argument with more than 65535 cols: %d", n);
+    if (G->rows != n || G->cols != n)
+        return fail(MB_ERR_DIM_MISMATCH, "mb_block_gramian: result block is %dx%d, expected %dx%d", G->rows, G->cols, n, n);
+    if (n == 0) return MB_OK;
+    // a transposed view (a DenseVecMatrix row shard) is the column-major n x m array X underneath: G = X X^T;
+    // a column-major view: G = A^T A.  G is symmetric, so a transposed G is written through the same array.
+    const bool trans = !A->is_transpose;
+    // split-K partials only when the triangle is too small for the SMs (at most 256 MiB), stream-ordered and returned
+    // after the call; with one split the product is written into G directly
+    const size_t need = mb::gemm_f64_tma_eligible(f64_ptr(A), A->ld, f64_ptr(A), A->ld) ? mb::gram_workspace_doubles(n, m, ctx->num_sms) : 0;
+    double* ws = nullptr;
+    if (need) MB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&ws), need * sizeof(double), ctx->stream));
+    int launches = 0;
+    const cudaError_t e = mb::gram_f64(trans, n, m, f64_ptr(A), A->ld, f64_ptr(G), G->ld, ws, ctx->num_sms, ctx->stream, &launches);
+    if (ws) cudaFreeAsync(ws, ctx->stream);
+    ctx->launches += launches;
+    if (e != cudaSuccess) return cuda_fail(e, "mb_block_gramian");
+    return MB_OK;
+}
+
+int64_t mb_gramian_workspace_bytes(int64_t n, int64_t m, int32_t num_sms) {
+    if (n <= 0 || n > 65535 || m < 0 || num_sms <= 0) return 0;
+    return (int64_t)(mb::gram_workspace_doubles((int)n, m, num_sms) * sizeof(double));
+}
+
+// The eigen step of computeSVD (:1589-1606): brzSvd(G) (dgesdd) in local-svd mode, ARPACK's symmetricEigs (:1725-1834) in
+// the eigs modes.  One full decomposition by parallel cyclic Jacobi; MB_ERR_NO_CONVERGENCE plays the part of ARPACK's
+// IllegalStateException (:1798-1807).
+int32_t mb_block_syev(mb_ctx* ctx, const mb_block* G, mb_block* V, double* w_out, int32_t* sweeps_out) {
+    MB_CTX(ctx);
+    MB_LOCK(ctx);
+    if (!G || !V || !w_out) return fail(MB_ERR_INVALID_ARG, "mb_block_syev: null argument");
+    if (G->dtype != MB_F64 || V->dtype != MB_F64) return fail(MB_ERR_UNSUPPORTED, "mb_block_syev: fp64 blocks only");
+    if (G->rows != G->cols) return fail(MB_ERR_DIM_MISMATCH, "mb_block_syev: the matrix is %dx%d, not square", G->rows, G->cols);
+    if (V->rows != G->rows || V->cols != G->cols)
+        return fail(MB_ERR_DIM_MISMATCH, "mb_block_syev: eigenvector block is %dx%d, expected %dx%d", V->rows, V->cols, G->rows, G->rows);
+    constexpr int MAX_SWEEPS = 30;
+    int sweeps = 0;
+    long long launches = 0;
+    const cudaError_t e = mb::syev_jacobi(G->rows, f64_ptr(G), rs(G), cs(G), f64_ptr(V), rs(V), cs(V), w_out, &sweeps, MAX_SWEEPS,
+                                          ctx->stream, &launches);
+    ctx->launches += launches;
+    if (sweeps_out) *sweeps_out = sweeps;
+    if (e == cudaErrorNotReady)
+        return fail(MB_ERR_NO_CONVERGENCE, "Jacobi eigensolver: no convergence after %d sweeps (n = %d)", MAX_SWEEPS, G->rows);
+    if (e != cudaSuccess) return cuda_fail(e, "mb_block_syev");
     return MB_OK;
 }
 

@@ -56,10 +56,27 @@ __device__ __forceinline__ void tile_coords(int t, int tiles_m, int tiles_n, int
     tm = band * BAND + (r - tn * rows_in_band);
 }
 
-template <bool TA, bool TB>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_f64_dmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
-                     const Params p) {
+// Split-K schedule of the Gramian (syrk_f64_dmma_kernel): work item w = split * tri_tiles + t covers lower-triangle tile t
+// (tm >= tn, row-major over the triangle) for k in [split * kchunk, min(K, (split + 1) * kchunk)) and stores its partial
+// tile at C + split * split_stride.
+struct SyrkSched {
+    int splits, tri_tiles, kchunk;
+    long long split_stride;
+};
+
+__device__ __forceinline__ void tri_coords(int t, int& tm, int& tn) {
+    int r = (int)((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
+    while ((r + 1) * (r + 2) / 2 <= t) ++r;
+    while (r * (r + 1) / 2 > t) --r;
+    tm = r;
+    tn = t - r * (r + 1) / 2;
+}
+
+// The persistent TMA + DMMA mainloop shared by the GEMM (SYRK = false: every tile of C, the whole K range, C = alpha*acc +
+// beta*C) and the Gramian (SYRK = true: lower-triangle tiles only, split-K partials stored to a workspace).
+template <bool TA, bool TB, bool SYRK>
+__device__ __forceinline__ void dmma_persistent(const CUtensorMap& mapA, const CUtensorMap& mapB, const Params& p,
+                                                const SyrkSched& sk) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     const uint32_t bar_full = smem_base + NUM_STAGES * STAGE_BYTES;
@@ -67,7 +84,7 @@ gemm_f64_dmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const int num_tiles = p.tiles_m * p.tiles_n;
+    const int num_tiles = SYRK ? sk.tri_tiles * sk.splits : p.tiles_m * p.tiles_n;
     const int num_kb = (p.K + BK - 1) / BK;
 
     if (threadIdx.x == 0) {
@@ -88,10 +105,17 @@ gemm_f64_dmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
             int stage = 0;
             uint32_t phase = 0;
             for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-                int tm, tn;
-                tile_coords(t, p.tiles_m, p.tiles_n, tm, tn);
+                int tm, tn, kb_begin = 0, kb_end = num_kb;
+                if constexpr (SYRK) {
+                    const int split = t / sk.tri_tiles;
+                    tri_coords(t - split * sk.tri_tiles, tm, tn);
+                    kb_begin = split * (sk.kchunk / BK);
+                    kb_end = min(num_kb, kb_begin + sk.kchunk / BK);
+                } else {
+                    tile_coords(t, p.tiles_m, p.tiles_n, tm, tn);
+                }
                 const int m0 = tm * BM, n0 = tn * BN;
-                for (int kb = 0; kb < num_kb; ++kb) {
+                for (int kb = kb_begin; kb < kb_end; ++kb) {
                     mbar_wait(bar_empty + 8 * stage, phase ^ 1);
                     const uint32_t full = bar_full + 8 * stage;
                     const uint32_t sA = smem_base + stage * STAGE_BYTES;
@@ -149,8 +173,17 @@ gemm_f64_dmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
     const bool vec_ok = ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0) && ((p.ldc & 1) == 0);
 
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        int tm_, tn_;
-        tile_coords(t, p.tiles_m, p.tiles_n, tm_, tn_);
+        int tm_, tn_, k_begin = 0, k_end = p.K;
+        double* Cout = p.C;
+        if constexpr (SYRK) {
+            const int split = t / sk.tri_tiles;
+            tri_coords(t - split * sk.tri_tiles, tm_, tn_);
+            k_begin = split * sk.kchunk;
+            k_end = min(p.K, k_begin + sk.kchunk);
+            Cout = p.C + split * sk.split_stride;
+        } else {
+            tile_coords(t, p.tiles_m, p.tiles_n, tm_, tn_);
+        }
         const int m0 = tm_ * BM, n0 = tn_ * BN;
 
         double acc[8][4][2];
@@ -161,7 +194,7 @@ gemm_f64_dmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
 
         // bounded by p.K (a kernel parameter) rather than num_kb: one register fewer, which the <N,T> instance needs
         // to fit sm_90a's 168-register budget without a spill
-        for (int k0 = 0; k0 < p.K; k0 += BK) {
+        for (int k0 = k_begin; k0 < k_end; k0 += BK) {
             mbar_wait(bar_full + 8 * stage, phase);
             const uint32_t sA = smem_base + stage * STAGE_BYTES;
             const uint32_t sB = sA + OPERAND_BYTES;
@@ -215,7 +248,7 @@ gemm_f64_dmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
                 const int cj = 2 * q + jj;
                 const int n = n0 + warp_n * 32 + (!TB ? (8 * j + perm8(cj)) : (16 * (j >> 1) + 2 * cj + (j & 1)));
                 if (n >= p.N) continue;
-                double* ccol = p.C + (long long)n * p.ldc;
+                double* ccol = Cout + (long long)n * p.ldc;
                 if (!TA) {
 #pragma unroll
                     for (int tp = 0; tp < 4; ++tp) {
@@ -253,6 +286,21 @@ gemm_f64_dmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
             }
         }
     }
+}
+
+template <bool TA, bool TB>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+gemm_f64_dmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
+                     const Params p) {
+    dmma_persistent<TA, TB, false>(mapA, mapB, p, SyrkSched{});
+}
+
+// Gramian partials: only the lower-triangle tiles of C = op(A) op(B) with op(B) = op(A)^T, split over K (see SyrkSched).
+template <bool TA, bool TB>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+syrk_f64_dmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
+                     const Params p, const SyrkSched sk) {
+    dmma_persistent<TA, TB, true>(mapA, mapB, p, sk);
 }
 
 // -------------------------------------------------------------------------------------------
@@ -701,6 +749,149 @@ cudaError_t gemm_f64(bool transA, bool transB, int M, int N, int K, double alpha
     return cudaGetLastError();
 }
 
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Gramian G = op(A) op(A)^T (DenseVecMatrix.computeGramianMatrix, matrix/DenseVecMatrix.scala:1464-1486).
+// ---------------------------------------------------------------------------------------------------------------------
+namespace {
+
+// Sum the split-K partials of lower 32x32 tile (bi, bj), bi >= bj, in split order and store it to G(bi, bj) and, through a
+// shared-memory transpose, to G(bj, bi): G is exactly symmetric and does not depend on the launch order of the partials.
+// With one split the "partial" may be G itself (ws == G, ldw == ldg): a CTA reads only its own lower tile (and, on the
+// diagonal, its own whole tile) before its barrier and no other CTA reads what it writes, so the pass runs in place.
+// Accesses are 128-bit where alignment and the leading dimensions allow.
+template <bool VEC_W>
+__global__ void __launch_bounds__(256) gram_reduce_mirror_kernel(const double* ws, long long ldw, long long stride,
+                                                                 int splits, int n, double* G, long long ldg) {
+    __shared__ double tile[32][33];          // [column][row] of the summed lower tile
+    int bi, bj;
+    tri_coords(blockIdx.x, bi, bj);
+    const int r0 = bi * 32, c0 = bj * 32;
+    const int rp = threadIdx.x & 15, cy = threadIdx.x >> 4;
+    const bool vec_g = ((reinterpret_cast<uintptr_t>(G) & 15) == 0) && ((ldg & 1) == 0);
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+        const int c = cy + 16 * i, r = 2 * rp;
+        double2 acc = make_double2(0.0, 0.0);
+        if (c0 + c < n && r0 + r < n) {
+            const double* src = ws + (r0 + r) + (long long)(c0 + c) * ldw;
+            const bool second = r0 + r + 1 < n;
+            for (int s = 0; s < splits; ++s) {
+                if (VEC_W) {
+                    const double2 v = *reinterpret_cast<const double2*>(src + s * stride);
+                    acc.x += v.x;
+                    acc.y += v.y;
+                } else {
+                    acc.x += src[s * stride];
+                    if (second) acc.y += src[s * stride + 1];
+                }
+            }
+        }
+        tile[c][r] = acc.x;
+        tile[c][r + 1] = acc.y;
+    }
+    __syncthreads();
+    auto store2 = [&](int row, int col, double v0, double v1, bool w0, bool w1) {
+        double* dst = G + row + (long long)col * ldg;
+        if (w0 && w1 && vec_g) {
+            *reinterpret_cast<double2*>(dst) = make_double2(v0, v1);
+        } else {
+            if (w0) dst[0] = v0;
+            if (w1) dst[1] = v1;
+        }
+    };
+    const bool diag = bi == bj;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+        const int y = cy + 16 * i, x = 2 * rp;
+        // direct: G(r0 + x + e, c0 + y), the lower part (row >= col) of a diagonal tile
+        if (c0 + y < n) {
+            const bool w0 = r0 + x < n && (!diag || x >= y), w1 = r0 + x + 1 < n && (!diag || x + 1 >= y);
+            store2(r0 + x, c0 + y, tile[y][x], tile[y][x + 1], w0, w1);
+        }
+        // mirrored: G(c0 + x + e, r0 + y) = S(r0 + y, c0 + x + e), the strict upper part of a diagonal tile
+        if (r0 + y < n) {
+            const bool w0 = c0 + x < n && (!diag || x < y), w1 = c0 + x + 1 < n && (!diag || x + 1 < y);
+            store2(c0 + x, r0 + y, tile[x][y], tile[x + 1][y], w0, w1);
+        }
+    }
+}
+
+}  // namespace
+
+// Split K only when the lower triangle has too few tiles to keep the SMs busy (fewer than two waves), and only as far as
+// the partials fit in GRAM_WS_CAP_DOUBLES: the smallest split that fills the last wave best, a larger one only for at
+// least 1 % more fill, and >= 512 rows per split.  Above 22 tile rows (n > 2816 on 132 SMs) this is always 1 split and
+// the Gramian needs no workspace at all.
+int gram_splits(int n, long long K, int num_sms) {
+    if (n <= 0 || num_sms <= 0) return 1;
+    const long long t = (n + BM - 1) / BM;
+    const long long tri = t * (t + 1) / 2;
+    if (tri >= 2LL * num_sms) return 1;
+    const long long ldw = (n + 1) & ~1;
+    const long long kb = (K + BK - 1) / BK;
+    const long long cap = std::min<long long>(32, GRAM_WS_CAP_DOUBLES / (ldw * n));
+    int best = 1;
+    double best_eff = (double)tri / (double)(((tri + num_sms - 1) / num_sms) * num_sms);
+    for (int s = 2; s <= cap; ++s) {
+        if (kb / s < 32) break;                               // keep >= 512 rows per split
+        const long long items = tri * s;
+        const long long waves = (items + num_sms - 1) / num_sms;
+        const double eff = (double)items / (double)(waves * num_sms);
+        if (eff >= best_eff + 0.01) { best_eff = eff; best = s; }
+    }
+    return best;
+}
+
+size_t gram_workspace_doubles(int n, long long K, int num_sms) {
+    const int s = gram_splits(n, K, num_sms);
+    return s > 1 ? (size_t)s * (size_t)((n + 1) & ~1) * (size_t)n : 0;
+}
+
+cudaError_t gram_f64(bool trans, int n, int K, const double* A, long long lda, double* G, long long ldg, double* ws,
+                     int num_sms, cudaStream_t stream, int* launches) {
+    if (n <= 0) return cudaSuccess;
+    CUtensorMap mA, mB;
+    const bool tma = K > 0 && gemm_f64_tma_eligible(A, lda, A, lda) &&
+                     (!trans ? (make_map_f64(&mA, A, n, K, lda, 16, 16) && make_map_f64(&mB, A, n, K, lda, 16, 16))
+                             : (make_map_f64(&mA, A, K, n, lda, 16, 128) && make_map_f64(&mB, A, K, n, lda, 16, 128)));
+    const int splits = tma ? gram_splits(n, K, num_sms) : 1;
+    if (splits > 1 && ws == nullptr) return cudaErrorInvalidValue;
+    // one split: the product goes straight into G and the mirror pass runs in place
+    double* P = splits > 1 ? ws : G;
+    const long long ldp = splits > 1 ? ((n + 1) & ~1) : ldg;
+    cudaError_t e;
+    if (tma) {
+        const int t = (n + BM - 1) / BM;
+        const long long kb = (K + BK - 1) / BK;
+        Params p;
+        p.M = n; p.N = n; p.K = K; p.alpha = 1.0; p.beta = 0.0; p.C = P; p.ldc = ldp;
+        p.tiles_m = t; p.tiles_n = t;
+        SyrkSched sk;
+        sk.splits = splits;
+        sk.tri_tiles = t * (t + 1) / 2;
+        sk.kchunk = (int)((kb + splits - 1) / splits) * BK;
+        sk.split_stride = ldp * n;
+        auto kern = !trans ? syrk_f64_dmma_kernel<false, true> : syrk_f64_dmma_kernel<true, false>;
+        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
+        if (e != cudaSuccess) return e;
+        kern<<<min(sk.tri_tiles * splits, num_sms), NUM_THREADS, SMEM_BYTES, stream>>>(mA, mB, p, sk);
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+        if (launches) ++*launches;
+    } else {
+        // the whole product on the CUDA cores (views TMA cannot address), or zeros for K = 0
+        e = gemm_f64(trans, !trans, n, n, K, 1.0, A, lda, A, lda, 0.0, P, ldp, num_sms, stream, true, launches);
+        if (e != cudaSuccess) return e;
+    }
+    const int nb = (n + 31) / 32;
+    const unsigned grid = nb * (nb + 1) / 2;
+    if (((reinterpret_cast<uintptr_t>(P) & 15) == 0) && ((ldp & 1) == 0))
+        gram_reduce_mirror_kernel<true><<<grid, 256, 0, stream>>>(P, ldp, ldp * n, splits, n, G, ldg);
+    else
+        gram_reduce_mirror_kernel<false><<<grid, 256, 0, stream>>>(P, ldp, ldp * n, splits, n, G, ldg);
+    if (launches) ++*launches;
+    return cudaGetLastError();
+}
 
 cudaError_t gemm_f64_grouped2(const G2Launch& L, int num_sms, cudaStream_t stream, int* launches) {
     if (L.ne <= 0) return cudaSuccess;

@@ -58,6 +58,18 @@ struct G2Launch {
 };
 cudaError_t gemm_f64_grouped2(const G2Launch& L, int num_sms, cudaStream_t stream, int* launches);
 
+// Gramian: G (n x n, col-major, ldg) = op(A) op(A)^T with op(A) n x K (A stored n x K if !trans, K x n if trans), exactly
+// symmetric.  TMA-addressable operands run the DMMA mainloop over the lower-triangle tiles only; when the triangle has
+// too few tiles for the SMs, K is split into gram_splits() partials held in `ws`.  The rest run the CUDA-core GEMM.  One
+// fixed-order pass then sums the partials and mirrors them (in place in G when there is one split).
+// ws: gram_workspace_doubles(n, K, num_sms) doubles, 16-byte aligned; 0 (ws may be null) unless K is split, and never
+// more than GRAM_WS_CAP_DOUBLES.
+constexpr long long GRAM_WS_CAP_DOUBLES = 32LL << 20;    // 256 MiB
+int gram_splits(int n, long long K, int num_sms);
+size_t gram_workspace_doubles(int n, long long K, int num_sms);
+cudaError_t gram_f64(bool trans, int n, int K, const double* A, long long lda, double* G, long long ldg, double* ws,
+                     int num_sms, cudaStream_t stream, int* launches);
+
 bool gemm_f64_tma_eligible(const double* A, long long lda, const double* B, long long ldb);
 
 }  // namespace mb

@@ -1,6 +1,7 @@
 // Pure integer host logic of the multiply path, exported through the C ABI.
 // Each function cites the reference code it mirrors (src/main/scala/edu/nju/pasalab/marlin/...).
 #include "../../include/marlin_b200.h"
+#include <algorithm>
 #include <cmath>
 #include <cstdint>
 #include <cstring>
@@ -58,6 +59,8 @@ uint32_t mm3_bytes_hash(const uint8_t* data, int len, uint32_t seed) {
 }
 
 }  // namespace
+
+int32_t mb_fail(int32_t code, const char* fmt, ...);   // capi.cu: sets mb_last_error()
 
 extern "C" {
 
@@ -146,6 +149,45 @@ int32_t mb_partition_seeds(int64_t seed, int32_t num_partitions, int64_t* seeds_
         seeds_out[i] = int64_t((uint64_t(hi) << 32) + uint64_t(lo));   // ((long)next(32) << 32) + next(32)
     }
     return MB_OK;
+}
+
+// matrix/DenseVecMatrix.scala:1565-1604 (computeSVD) and :1466-1468 (computeGramianMatrix).  The reference checks the
+// column cap only where it forms the Gramian; every mode forms it here, so every mode checks it, after the mode's own
+// requires.
+int32_t mb_svd_mode(int64_t n, int32_t k, const char* mode, int32_t* compute_mode) {
+    if (!mode || !compute_mode) return mb_fail(MB_ERR_INVALID_ARG, "mb_svd_mode: null argument");
+    if (!(k > 0 && k <= n))
+        return mb_fail(MB_ERR_INVALID_ARG, "Request up to n singular values but got k=%d and n=%lld.", k, (long long)n);
+    int cm;
+    if (std::strcmp(mode, "auto") == 0) {
+        // `k > n / 2` and `k < n / 3` are Int divisions in the reference
+        if (n < 100 || k > n / 2) cm = k < n / 3 ? MB_SVD_LOCAL_ARPACK : MB_SVD_LOCAL_LAPACK;
+        else cm = MB_SVD_DIST_ARPACK;
+    } else if (std::strcmp(mode, "local-svd") == 0) {
+        cm = MB_SVD_LOCAL_LAPACK;
+    } else if (std::strcmp(mode, "local-eigs") == 0) {
+        cm = MB_SVD_LOCAL_ARPACK;
+    } else if (std::strcmp(mode, "dist-eigs") == 0) {
+        cm = MB_SVD_DIST_ARPACK;
+    } else {
+        return mb_fail(MB_ERR_INVALID_ARG, "Do not support mode %s.", mode);
+    }
+    if (cm != MB_SVD_LOCAL_LAPACK && !(k < n))
+        return mb_fail(MB_ERR_INVALID_ARG, "k must be smaller than n in %s mode but got k=%d and n=%lld.",
+                       cm == MB_SVD_LOCAL_ARPACK ? "local-eigs" : "dist-eigs", k, (long long)n);
+    if (n > 65535) return mb_fail(MB_ERR_INVALID_ARG, "Argument with more than 65535 cols: %lld", (long long)n);
+    *compute_mode = cm;
+    return MB_OK;
+}
+
+// matrix/DenseVecMatrix.scala:1607-1621
+int32_t mb_svd_rank(const double* sigmas, int32_t count, int32_t k, double rcond) {
+    if (count <= 0) return 0;
+    if (!sigmas) return mb_fail(MB_ERR_INVALID_ARG, "mb_svd_rank: null sigmas");
+    const double threshold = rcond * sigmas[0];
+    int32_t i = 0;
+    while (i < std::min(k, count) && sigmas[i] >= threshold) ++i;
+    return i;
 }
 
 }  // extern "C"

@@ -181,6 +181,11 @@ class SubMatrix:
         nat.check(rt.lib.mb_block_div(rt.ctx, self.handle(), float(b), 0, out.handle()))               # :79-85
         return out
 
+    def _divide_into(self, b: Number, out: "SubMatrix") -> None:
+        """out := this / b (IEEE division) into an existing view."""
+        rt = Runtime.get(); rt.sync_stream()
+        nat.check(rt.lib.mb_block_div(rt.ctx, self.handle(), float(b), 0, out.handle()))
+
     def subtractBy(self, b: Number) -> "SubMatrix":
         """b - x (matrix/BlockMatrix.scala:414-424; returns a new block instead of mutating in place)."""
         rt = Runtime.get(); rt.sync_stream()
@@ -265,6 +270,29 @@ class SubMatrix:
         x = rhs.copy()
         nat.check(rt.lib.mb_block_trsm(rt.ctx, self.handle(), int(lower), int(unit), x.handle()))
         return x
+
+    # ---- the local steps of DenseVecMatrix.computeSVD (matrix/DenseVecMatrix.scala:1464-1486, 1589-1606) ----
+    def gramian(self) -> "SubMatrix":
+        """This^T * this (n x n, exactly symmetric): the Gramian of computeGramianMatrix for the rows this block holds.
+        A transposed view (a DenseVecMatrix row shard) is read in place."""
+        rt = Runtime.get(); rt.sync_stream()
+        out = SubMatrix.empty(self._cols, self._cols, nat.MB_F64, self.buf.device)
+        nat.check(rt.lib.mb_block_gramian(rt.ctx, self.handle(), out.handle()))
+        return out
+
+    def symmetricEigen(self):
+        """(w, V) of this symmetric block (lower triangle read): all eigenvalues as an ndarray ordered by |w| descending,
+        the eigenvectors as the columns of an n x n block (parallel cyclic Jacobi on the device).  Raises MarlinError with
+        code MB_ERR_NO_CONVERGENCE if the sweep cap is reached, where the reference's ARPACK path throws
+        IllegalStateException."""
+        rt = Runtime.get(); rt.sync_stream()
+        n = self._rows
+        V = SubMatrix.empty(n, n, nat.MB_F64, self.buf.device)
+        w = (C.c_double * max(1, n))()
+        sweeps = C.c_int32()
+        nat.check(rt.lib.mb_block_syev(rt.ctx, self.handle(), V.handle(), w, C.byref(sweeps)))
+        self.last_sweeps = int(sweeps.value)
+        return np.array(w[:n], dtype=np.float64), V
 
     def add_(self, other: "SubMatrix") -> "SubMatrix":
         """In-place accumulate (the reduceByKey combine of BlockMatrix.scala:177 without a new allocation)."""

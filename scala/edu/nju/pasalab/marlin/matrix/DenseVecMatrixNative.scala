@@ -59,6 +59,23 @@ private[marlin] object DenseVecMatrixNative {
     out
   }
 
+  /** computeGramianMatrix (:1464-1486) of the rows in `mat` (a row shard is a transposed view): mat.t * mat, exactly
+   *  symmetric.  Partitions still combine with `+=`. */
+  def gramian(mat: SubMatrix): SubMatrix = {
+    val out = new SubMatrix(Native.alloc(Ctx.get, mat.cols, mat.cols, Native.F64), mat.cols, mat.cols)
+    Native.gramian(Ctx.get, mat.handle, out.handle)
+    out
+  }
+
+  /** The eigen step of computeSVD (:1589-1606) on a symmetric block: all eigenvalues ordered by |w| descending and the
+   *  eigenvectors as columns (parallel Jacobi on the device; every mode uses it). */
+  def symmetricEigen(g: SubMatrix): (Array[Double], SubMatrix) = {
+    val v = new SubMatrix(Native.alloc(Ctx.get, g.rows, g.rows, Native.F64), g.rows, g.rows)
+    val w = new Array[Double](g.rows)
+    Native.syev(Ctx.get, g.handle, v.handle, w)
+    (w, v)
+  }
+
   /** `t \ b` for a triangular t (lower / upper, unit or explicit diagonal): solves in a copy of b. */
   def solveTriangular(t: SubMatrix, lower: Boolean, unitDiagonal: Boolean, b: SubMatrix): SubMatrix = {
     val x = b.copy()

@@ -50,6 +50,11 @@ object Native {
   @native def lu(ctx: Long, a: Long, permOut: Array[Int]): Unit
   @native def cholesky(ctx: Long, a: Long): Unit
   @native def inverse(ctx: Long, a: Long, out: Long): Unit
+  // the local steps of computeSVD: Gramian, symmetric eigendecomposition (returns the sweep count), mode chooser, rank
+  @native def gramian(ctx: Long, a: Long, g: Long): Unit
+  @native def syev(ctx: Long, g: Long, v: Long, wOut: Array[Double]): Int
+  @native def svdMode(n: Long, k: Int, mode: String): Int // 0 local-svd, 1 local-eigs, 2 dist-eigs
+  @native def svdRank(sigmas: Array[Double], k: Int, rCond: Double): Int
   @native def trsm(ctx: Long, t: Long, lower: Boolean, unitDiagonal: Boolean, b: Long): Unit
 
   // whole multiplies on one GPU

@@ -1,8 +1,11 @@
 """Secondary kernel benchmarks (1 GPU): HBM-bound block kernels vs the measured copy bandwidth, and the bf16 wgmma
-GEMM vs cuBLAS.  Prints one JSON document; bench.py stays the headline (fp64 multiply)."""
+GEMM vs cuBLAS, layout conversion, factorizations and the SVD.  Prints one JSON document; bench.py stays the headline
+(fp64 multiply).  `svd` as an argument runs the f5_svd section only."""
 import ctypes as C
 import json
+import subprocess
 import sys
+import time
 from pathlib import Path
 
 import torch
@@ -36,8 +39,9 @@ def timeit(fn, iters=10, warm=3):
     return e0.elapsed_time(e1) / iters
 
 
+ONLY_SVD = "svd" in sys.argv[1:]
 hbm = {}
-for n in (8192, 16384):
+for n in (() if ONLY_SVD else (8192, 16384)):
     A = mb.MTUtils.randomBlockMatrix(None, n, n, 1, 1, seed=1).blocks[0][1]
     B = mb.MTUtils.randomBlockMatrix(None, n, n, 1, 1, seed=2).blocks[0][1]
     O = mb.SubMatrix.empty(n, n)
@@ -86,7 +90,7 @@ for n in (8192, 16384):
 out["hbm_kernels"] = hbm
 
 gemm = {}
-for n in (() if "hbm" in sys.argv[1:] else (4096, 8192, 16384)):
+for n in (() if ONLY_SVD or "hbm" in sys.argv[1:] else (4096, 8192, 16384)):
     A = mb.MTUtils.randomBlockMatrix(None, n, n, 1, 1, seed=3, dtype=nat.MB_BF16).blocks[0][1]
     B = mb.MTUtils.randomBlockMatrix(None, n, n, 1, 1, seed=4, dtype=nat.MB_BF16).blocks[0][1]
     Cm = mb.SubMatrix.empty(n, n, nat.MB_F32)
@@ -107,7 +111,7 @@ out["bf16_gemm"] = gemm
 
 # ---- f1: layout conversion on the device (rows -> blocks -> rows), 2 * 8 * M * N bytes per direction ----
 f1 = {}
-for (M_, N_, gr, gc) in (() if "hbm" in sys.argv[1:] else ((16384, 16384, 2, 2), (1048576, 1024, 8, 1))):
+for (M_, N_, gr, gc) in (() if ONLY_SVD or "hbm" in sys.argv[1:] else ((16384, 16384, 2, 2), (1048576, 1024, 8, 1))):
     D = mb.MTUtils.randomDenVecMatrix(None, M_, N_, numPartitions=1, seed=5)
     torch.cuda.synchronize()
     Bm = D.toBlockMatrix(gr, gc)
@@ -125,7 +129,7 @@ out["f1_layout_conversion"] = f1
 
 # ---- f4: factorizations of one block (recursive; the flops run in the DMMA GEMM) ----
 fac = {}
-for n in (() if "hbm" in sys.argv[1:] else (4096, 8192)):
+for n in (() if ONLY_SVD or "hbm" in sys.argv[1:] else (4096, 8192)):
     A = mb.MTUtils.randomBlockMatrix(None, n, n, 1, 1, seed=6).blocks[0][1]
     S = A.multiply(A.t)
     S.add_(mb.SubMatrix(torch.eye(n, dtype=torch.float64).mul_(float(n)).numpy(), device=rt.device))
@@ -137,6 +141,81 @@ for n in (() if "hbm" in sys.argv[1:] else (4096, 8192)):
                      "note": "times include the working copy of the block and, for LU, the D2H of the pivots"}
     del A, S
 out["f4_factorizations"] = fac
+
+# ---- f5: DenseVecMatrix.computeSVD — split-K DMMA Gramian, Jacobi eigensolver, end to end ----
+f5 = {}
+if "hbm" not in sys.argv[1:]:
+    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i",
+                          str(rt.device_index)], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
+    f5["device"] = {"torch_name": torch.cuda.get_device_name(rt.device_index), "nvidia_smi": smi.stdout.strip()}
+    gram = {}
+    for (M_, N_) in ((1048576, 1024), (131072, 4096)):
+        D = mb.MTUtils.randomDenVecMatrix(None, M_, N_, numPartitions=1, seed=8)
+        X = D.data                                   # the row shard: a transposed view, read in place
+        full = mb.SubMatrix.empty(N_, N_)
+        ms_g = timeit(lambda: X.gramian(), 5, 2)
+        ms_f = timeit(lambda: X.t.multiply(X, out=full), 5, 2)
+        fl_g, fl_f = float(M_) * N_ * (N_ + 1), 2.0 * M_ * N_ * N_
+        gram[f"{M_}x{N_}"] = {"gramian_ms": ms_g, "gramian_tflops_mn(n+1)": fl_g / ms_g / 1e9,
+                              "full_gemm_AtA_ms": ms_f, "full_gemm_tflops_2mn^2": fl_f / ms_f / 1e9}
+        del D, X, full
+        torch.cuda.empty_cache()
+    f5["gramian"] = gram
+    eig = {}
+    for n in (256, 1024, 4096):
+        rng_rows = mb.MTUtils.randomDenVecMatrix(None, 2 * n, n, numPartitions=1, seed=9)
+        G = rng_rows.data.gramian()
+        G.symmetricEigen()                           # warm-up (module load)
+        torch.cuda.synchronize()
+        reps = 3 if n <= 1024 else 1
+        t0 = time.perf_counter()
+        for _ in range(reps):
+            w, V = G.symmetricEigen()
+        ms = (time.perf_counter() - t0) * 1e3 / reps
+        eig[f"n={n}"] = {"ms": ms, "sweeps": G.last_sweeps, "ms_per_sweep": ms / max(1, G.last_sweeps),
+                         "note": "host clock around the blocking call: copies, N-1 rounds per sweep, ordering, gather"}
+        del rng_rows, G, V
+        torch.cuda.empty_cache()
+    f5["eigensolver"] = eig
+    # where a sweep's time goes: the round kernels' device time vs the gaps between consecutive rounds of a graph replay
+    # (the launch overhead a persistent grid-barrier kernel could replace with a barrier), and the per-call set-up
+    # (working copies, graph capture and instantiation, ordering, gather) as wall time minus the device span
+    from torch.profiler import ProfilerActivity, profile
+    prof_out = {}
+    for n in (256, 1024):
+        rows_ = mb.MTUtils.randomDenVecMatrix(None, 2 * n, n, numPartitions=1, seed=9)
+        G = rows_.data.gramian()
+        G.symmetricEigen()
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            t0 = time.perf_counter()
+            G.symmetricEigen()
+            wall = (time.perf_counter() - t0) * 1e3
+        evs = sorted([e for e in prof.events() if "jacobi_" in e.name and e.device_type.name == "CUDA"],
+                     key=lambda e: e.time_range.start)
+        rounds = [e for e in evs if "jacobi_round_kernel" in e.name]
+        if len(rounds) < 2:
+            prof_out[f"n={n}"] = {"wall_ms": wall, "note": "round kernels not captured by the profiler"}
+            continue
+        dur = sorted(e.time_range.elapsed_us() for e in rounds)
+        gaps = sorted(b.time_range.start - a.time_range.end for a, b in zip(rounds, rounds[1:]))
+        span_ms = (evs[-1].time_range.end - evs[0].time_range.start) / 1e3
+        prof_out[f"n={n}"] = {"rounds": len(rounds), "sweeps": G.last_sweeps, "round_kernel_us_median": dur[len(dur) // 2],
+                              "gap_between_rounds_us_median": gaps[len(gaps) // 2],
+                              "round_kernels_ms_total": sum(dur) / 1e3, "device_span_ms": span_ms, "wall_ms": wall,
+                              "setup_and_host_ms": wall - span_ms}
+        del rows_, G
+    f5["eigensolver_breakdown"] = prof_out
+    D = mb.MTUtils.randomDenVecMatrix(None, 1048576, 1024, numPartitions=1, seed=10)
+    D.computeSVD(10, computeU=True)
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    U, s_, V_ = D.computeSVD(10, computeU=True)
+    torch.cuda.synchronize()
+    f5["computeSVD_k10_U_1048576x1024_ms"] = (time.perf_counter() - t0) * 1e3
+    del D, U
+    torch.cuda.empty_cache()
+out["f5_svd"] = f5
 Path("gpurun_out").mkdir(exist_ok=True)
 Path("gpurun_out/kernels.json").write_text(json.dumps(out, indent=1))
 print(json.dumps(out, indent=1))
