@@ -44,6 +44,7 @@ typedef enum { MB_F64 = 0, MB_BF16 = 1, MB_F32 = 2 } mb_dtype;
 
 typedef struct mb_ctx   mb_ctx;
 typedef struct mb_block mb_block;
+typedef struct mb_sparse mb_sparse;
 
 /* ---- lifetime (SparkContext lifetime in the reference) --------------------------------- */
 int32_t     mb_init(int32_t device, mb_ctx** out);
@@ -209,6 +210,60 @@ int32_t mb_fill_uniform(mb_ctx* ctx, mb_block* blk, int64_t partition_seed, int6
  * = successive java.util.Random(seed).nextLong() (rdd/RandomRDD.scala:28-45). */
 int64_t mb_hash_seed(int64_t seed);
 int32_t mb_partition_seeds(int64_t seed, int32_t num_partitions, int64_t* seeds_out);
+
+/* ---- f6: sparse blocks (matrix/Matrices.scala:57-173, matrix/LibMatrixMult.scala, matrix/SubMatrix.scala:87-119).
+ * A sparse block is CSC on the device: colptr int32[cols+1], rowidx int32[nnz], values f64[nnz], nnz < 2^31, row indices
+ * strictly increasing within each column.  The reference's SparseMatrix (one SparseVector per column) accepts unsorted or
+ * repeated indices unchecked; here they are MB_ERR_INVALID_ARG.  Products write a dense fp64 block or view; every output
+ * element is summed by one thread in the reference loop's order with separate multiplies and adds, so results are bitwise
+ * reproducible.  accumulate != 0: C := C + P, the complete product P added once (reduceByKey(add), BlockMatrix.scala:177). */
+/* The structure checks of mb_sparse_upload on host arrays: colptr from 0 to nnz without decreasing, rows in [0, rows)
+ * and strictly increasing within each column.  Pure logic; MB_ERR_INVALID_ARG with the first violation. */
+int32_t mb_sparse_check(int32_t rows, int32_t cols, const int32_t* colptr, const int32_t* rowidx);
+/* A handle over caller-owned device arrays (like mb_block_wrap: torch owns the memory, NCCL can move it).  The contents
+ * are not read here; the caller guarantees the structure (e.g. a block that passed mb_sparse_check, or one that
+ * mb_fill_sparse_uniform is about to write). */
+int32_t mb_sparse_wrap(mb_ctx* ctx, int32_t rows, int32_t cols, int64_t nnz, void* colptr, void* rowidx, void* values,
+                       mb_sparse** out);
+/* Host CSC -> a library-owned device block, after mb_sparse_check.  nnz = colptr[cols].  Blocking. */
+int32_t mb_sparse_upload(mb_ctx* ctx, int32_t rows, int32_t cols, const int32_t* colptr, const int32_t* rowidx,
+                         const double* values, mb_sparse** out);
+/* Device -> host arrays of cols+1, nnz and nnz elements.  Blocking. */
+int32_t mb_sparse_download(mb_ctx* ctx, const mb_sparse* S, int32_t* colptr, int32_t* rowidx, double* values);
+int32_t mb_sparse_info(const mb_sparse* S, int32_t* rows, int32_t* cols, int64_t* nnz);
+/* A library-owned block with room for nnz entries (contents undefined until mb_fill_sparse_uniform or a copy writes them),
+ * for callers that own no device memory of their own (the C++ mirror, the JVM). */
+int32_t mb_sparse_alloc(mb_ctx* ctx, int32_t rows, int32_t cols, int64_t nnz, mb_sparse** out);
+int32_t mb_sparse_free(mb_ctx* ctx, mb_sparse* S);
+/* The scalar ops of a sparse SubMatrix (SubMatrix.scala:52-58, 71-85, 121-129): a new library-owned block with S's
+ * structure whose stored values are v + b, v - b, v * b or v / b (op = MB_SPARSE_ADD / _SUB / _MUL / _DIV), computed by the
+ * dense element-wise kernels; only the stored values change, as in the reference. */
+#define MB_SPARSE_ADD 0
+#define MB_SPARSE_SUB 1
+#define MB_SPARSE_MUL 2
+#define MB_SPARSE_DIV 3
+int32_t mb_sparse_values_op(mb_ctx* ctx, const mb_sparse* S, int32_t op, double b, mb_sparse** out);
+/* SparseMatrix.toDense (Matrices.scala:106-119) into a dense fp64 block or view of the same shape. */
+int32_t mb_sparse_to_dense(mb_ctx* ctx, const mb_sparse* S, mb_block* out);
+/* LibMatrixMult.multDenseSparse (LibMatrixMult.scala:15-41): C [+]= A * B for a dense view A.  C(:, j) sums B's column j
+ * in stored order; a column holding exactly one value equal to 1.0 copies the A column (:28-29). */
+int32_t mb_spmm_dense_sparse(mb_ctx* ctx, const mb_block* A, const mb_sparse* B, mb_block* C, int32_t accumulate);
+/* LibMatrixMult.multSparseDense (:43-77): C [+]= A * B for a dense view B, C(r, i) summed over k ascending.  The reference
+ * reads B(bi + k, i) where it means B(bk + k, i) (:60) and is right only for K <= 32 and N <= 32; this is the true product,
+ * bit-identical to the corrected loop.  The first call builds a CSR copy of A on the device and keeps it with the handle
+ * (about 12 * nnz + 4 * rows bytes, freed by mb_sparse_free). */
+int32_t mb_spmm_sparse_dense(mb_ctx* ctx, mb_sparse* A, const mb_block* B, mb_block* C, int32_t accumulate);
+/* SparseMatrix.multiply (Matrices.scala:129-152): C [+]= A * B, both sparse, the result dense. */
+int32_t mb_spgemm_dense_out(mb_ctx* ctx, const mb_sparse* A, const mb_sparse* B, mb_block* C, int32_t accumulate);
+/* The column count and the checks of a sparse randomBlockMatrix (SparseMatrix.rand, Matrices.scala:157-173):
+ * s = (int)(cols * density) with the JVM's double product and truncation.  density <= 0 (or NaN) and s > rows (where the
+ * reference's sampling loop never ends) are MB_ERR_INVALID_ARG.  Pure logic. */
+int32_t mb_sparse_column_count(int32_t rows, int32_t cols, double density, int32_t* s_out);
+/* The deterministic sparse generator of block `partition_seed` (the dense generator's per-block seed) into a block wrapped
+ * over preallocated arrays with nnz = s * cols: values = positions [0, s*cols) of the block's XORShift stream (U[0,1),
+ * column j taking [j*s, (j+1)*s)); column j's rows by selection sampling over positions [s*cols + j*rows, +rows):
+ * exactly s sorted rows, every s-subset equally likely.  rows * cols draws per block whatever the density. */
+int32_t mb_fill_sparse_uniform(mb_ctx* ctx, mb_sparse* S, int64_t partition_seed);
 
 /* ---- a7/a8: strategy + partitioning (pure integer logic) --------------------------------- */
 /* MTUtils.splitMethod(m,k,n,cores) (utils/MTUtils.scala:150-175, dimToSplit :204-213) */

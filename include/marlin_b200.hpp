@@ -101,8 +101,43 @@ struct BlockID {
     int hashCode() const { return row * 31 + column + seq; }
 };
 
+// ---------------------------------------------------------------------------------------------- sparse host types
+// matrix/Vectors.scala:217-229: a sorted index array and its values.
+struct SparseVector {
+    int size = 0;
+    std::vector<int32_t> indices;
+    std::vector<double> values;
+    SparseVector() = default;
+    SparseVector(int n, std::vector<int32_t> idx, std::vector<double> vals) : size(n), indices(std::move(idx)), values(std::move(vals)) {
+        if (indices.size() != values.size()) throw std::invalid_argument("SparseVector: indices and values differ in length");
+    }
+};
+
+// matrix/Matrices.scala:57-173: one SparseVector per column.  toDense and multiply run on the GPU (defined below SubMatrix).
+struct SparseMatrix {
+    int numRows = 0, numCols = 0;
+    std::vector<SparseVector> values;
+    SparseMatrix(int r, int c, std::vector<SparseVector> v) : numRows(r), numCols(c), values(std::move(v)) {
+        if ((int)values.size() != numCols) throw std::invalid_argument("SparseMatrix: one SparseVector per column expected");
+    }
+    // toBreeze's CSC flattening (:70-104); mb_sparse_upload checks it
+    void toCSC(std::vector<int32_t>& colptr, std::vector<int32_t>& rowidx, std::vector<double>& vals) const {
+        colptr.assign((size_t)numCols + 1, 0);
+        rowidx.clear(); vals.clear();
+        for (int j = 0; j < numCols; ++j) {
+            rowidx.insert(rowidx.end(), values[j].indices.begin(), values[j].indices.end());
+            vals.insert(vals.end(), values[j].values.begin(), values[j].values.end());
+            colptr[j + 1] = (int32_t)rowidx.size();
+        }
+    }
+    DenseMatrix toDense() const;
+    DenseMatrix multiply(const SparseMatrix& other) const;
+};
+
 // ---------------------------------------------------------------------------------------------- SubMatrix
-// matrix/SubMatrix.scala — the per-block value type, device resident (dense branch; sparse is out of scope).
+// matrix/SubMatrix.scala — the per-block value type, device resident: a dense block (mb_block) or a sparse one (mb_sparse,
+// CSC).  multiply dispatches the four sparsity pairs (:87-119); the scalar ops of a sparse block change only its stored
+// values (:52-58, 71-85, 121-129).
 class SubMatrix {
 public:
     SubMatrix() = default;
@@ -110,6 +145,21 @@ public:
         mb_block* b = nullptr;
         check(mb_block_upload(Context::get(), m.data.data(), 0, m.rows, m.cols, std::max(1, m.rows), 0, MB_F64, &b));
         own(b);
+    }
+    explicit SubMatrix(const SparseMatrix& m) {                                       // new SubMatrix(spMatrix = ...)
+        std::vector<int32_t> cp, ri;
+        std::vector<double> va;
+        m.toCSC(cp, ri, va);
+        mb_sparse* s = nullptr;
+        check(mb_sparse_upload(Context::get(), m.numRows, m.numCols, cp.data(), ri.data(), va.data(), &s));
+        ownSparse(s);
+    }
+    static SubMatrix emptySparse(int rows, int cols, long nnz) {
+        mb_sparse* s = nullptr;
+        check(mb_sparse_alloc(Context::get(), rows, cols, nnz, &s));
+        SubMatrix r;
+        r.ownSparse(s);
+        return r;
     }
     static SubMatrix empty(int rows, int cols) {
         mb_block* b = nullptr;
@@ -126,10 +176,38 @@ public:
         s.own(b);
         return s;
     }
-    int rows() const { int r = 0; mb_block_info(h_.get(), &r, nullptr, nullptr, nullptr, nullptr, nullptr); return r; }
-    int cols() const { int c = 0; mb_block_info(h_.get(), nullptr, &c, nullptr, nullptr, nullptr, nullptr); return c; }
-    bool isSparse() const { return false; }
+    int rows() const {
+        int r = 0;
+        if (sp_) mb_sparse_info(sp_.get(), &r, nullptr, nullptr); else mb_block_info(h_.get(), &r, nullptr, nullptr, nullptr, nullptr, nullptr);
+        return r;
+    }
+    int cols() const {
+        int c = 0;
+        if (sp_) mb_sparse_info(sp_.get(), nullptr, &c, nullptr); else mb_block_info(h_.get(), nullptr, &c, nullptr, nullptr, nullptr, nullptr);
+        return c;
+    }
+    bool isSparse() const { return (bool)sp_; }
     mb_block* handle() const { return h_.get(); }
+    mb_sparse* sparseHandle() const { return sp_.get(); }
+    long nnz() const { int64_t n = 0; if (sp_) mb_sparse_info(sp_.get(), nullptr, nullptr, &n); return (long)n; }
+    SparseMatrix sparseBlock() const {                                                // download the CSC as SparseVectors
+        if (!sp_) throw std::invalid_argument("sparseBlock of a dense block");
+        const int r = rows(), c = cols();
+        std::vector<int32_t> cp((size_t)c + 1), ri((size_t)std::max(1L, nnz()));
+        std::vector<double> va((size_t)std::max(1L, nnz()));
+        check(mb_sparse_download(Context::get(), sp_.get(), cp.data(), ri.data(), va.data()));
+        std::vector<SparseVector> cols_;
+        for (int j = 0; j < c; ++j)
+            cols_.emplace_back(r, std::vector<int32_t>(ri.begin() + cp[j], ri.begin() + cp[j + 1]),
+                               std::vector<double>(va.begin() + cp[j], va.begin() + cp[j + 1]));
+        return SparseMatrix(r, c, cols_);
+    }
+    SubMatrix toDenseBlock() const {                                                  // SparseMatrix.toDense on the device
+        if (!sp_) return *this;
+        SubMatrix r = empty(rows(), cols());
+        check(mb_sparse_to_dense(Context::get(), sp_.get(), r.h_.get()));
+        return r;
+    }
 
     SubMatrix t() const {                                                             // Breeze `.t`: a view
         mb_block* v = nullptr;
@@ -141,21 +219,28 @@ public:
         check(mb_block_slice(Context::get(), h_.get(), r0, r1, c0, c1, &v));
         return view(v);
     }
-    SubMatrix add(const SubMatrix& o) const { SubMatrix r = empty(rows(), cols()); check(mb_block_add(Context::get(), h_.get(), o.h_.get(), r.h_.get())); return r; }        // :41-45
-    SubMatrix add(double b) const { SubMatrix r = empty(rows(), cols()); check(mb_block_axpb(Context::get(), h_.get(), 1.0, b, r.h_.get())); return r; }                    // :52-58
-    SubMatrix subtract(const SubMatrix& o) const { SubMatrix r = empty(rows(), cols()); check(mb_block_sub(Context::get(), h_.get(), o.h_.get(), r.h_.get())); return r; }   // :60-64
-    SubMatrix subtract(double b) const { SubMatrix r = empty(rows(), cols()); check(mb_block_axpb(Context::get(), h_.get(), 1.0, -b, r.h_.get())); return r; }              // :71-77
-    SubMatrix divide(double b) const { SubMatrix r = empty(rows(), cols()); check(mb_block_div(Context::get(), h_.get(), b, 0, r.h_.get())); return r; }                     // :79-85
-    SubMatrix multiply(double b) const { SubMatrix r = empty(rows(), cols()); check(mb_block_axpb(Context::get(), h_.get(), b, 0.0, r.h_.get())); return r; }               // :123-131
+    SubMatrix add(const SubMatrix& o) const { bothDense(o, "add"); SubMatrix r = empty(rows(), cols()); check(mb_block_add(Context::get(), h_.get(), o.h_.get(), r.h_.get())); return r; }        // :41-50
+    SubMatrix add(double b) const { if (sp_) return valuesOp(MB_SPARSE_ADD, b); SubMatrix r = empty(rows(), cols()); check(mb_block_axpb(Context::get(), h_.get(), 1.0, b, r.h_.get())); return r; }                    // :52-58
+    SubMatrix subtract(const SubMatrix& o) const { bothDense(o, "subtract"); SubMatrix r = empty(rows(), cols()); check(mb_block_sub(Context::get(), h_.get(), o.h_.get(), r.h_.get())); return r; }   // :60-69
+    SubMatrix subtract(double b) const { if (sp_) return valuesOp(MB_SPARSE_SUB, b); SubMatrix r = empty(rows(), cols()); check(mb_block_axpb(Context::get(), h_.get(), 1.0, -b, r.h_.get())); return r; }              // :71-77
+    SubMatrix divide(double b) const { if (sp_) return valuesOp(MB_SPARSE_DIV, b); SubMatrix r = empty(rows(), cols()); check(mb_block_div(Context::get(), h_.get(), b, 0, r.h_.get())); return r; }                     // :79-85
+    SubMatrix multiply(double b) const { if (sp_) return valuesOp(MB_SPARSE_MUL, b); SubMatrix r = empty(rows(), cols()); check(mb_block_axpb(Context::get(), h_.get(), b, 0.0, r.h_.get())); return r; }               // :121-129
     SubMatrix elementMultiply(const SubMatrix& o) const { SubMatrix r = empty(rows(), cols()); check(mb_block_hadamard(Context::get(), h_.get(), o.h_.get(), r.h_.get())); return r; }
-    SubMatrix multiply(const SubMatrix& o) const {                                    // :87-91 -> dgemm
+    SubMatrix multiply(const SubMatrix& o) const {                                    // :87-105 -> dgemm / LibMatrixMult / SparseMatrix.multiply
         if (cols() != o.rows())
             throw std::invalid_argument("Dimension mismatch during matrix-matrix multiplication: " + std::to_string(cols()) + " vs " + std::to_string(o.rows()));
         SubMatrix r = empty(rows(), o.cols());
-        check(mb_block_gemm(Context::get(), h_.get(), o.h_.get(), r.h_.get(), 0));
+        multiplyInto(o, r, false);
         return r;
     }
-    void multiplyInto(const SubMatrix& o, SubMatrix& out, bool accumulate) const { check(mb_block_gemm(Context::get(), h_.get(), o.h_.get(), out.h_.get(), accumulate ? 1 : 0)); }
+    void multiplyInto(const SubMatrix& o, SubMatrix& out, bool accumulate) const {
+        mb_ctx* c = Context::get();
+        const int32_t acc = accumulate ? 1 : 0;
+        if (sp_ && o.sp_) check(mb_spgemm_dense_out(c, sp_.get(), o.sp_.get(), out.h_.get(), acc));
+        else if (sp_) check(mb_spmm_sparse_dense(c, sp_.get(), o.h_.get(), out.h_.get(), acc));
+        else if (o.sp_) check(mb_spmm_dense_sparse(c, h_.get(), o.sp_.get(), out.h_.get(), acc));
+        else check(mb_block_gemm(c, h_.get(), o.h_.get(), out.h_.get(), acc));
+    }
     SubMatrix transpose() const {                                                     // denseBlock.t.copy (BlockMatrix.scala:517)
         SubMatrix r = empty(cols(), rows());
         check(mb_block_transpose(Context::get(), h_.get(), r.h_.get()));
@@ -202,12 +287,27 @@ public:
     void assign(const SubMatrix& src) { check(mb_block_copy(Context::get(), src.h_.get(), h_.get())); }   // this(range) := src
     double sum() const { double s = 0; check(mb_block_sum(Context::get(), h_.get(), &s)); return s; }
     DenseMatrix denseBlock() const {                                                  // collect to the host (toBreeze)
+        if (sp_) return toDenseBlock().denseBlock();
         DenseMatrix m(rows(), cols());
         check(mb_block_download(Context::get(), h_.get(), m.data.data(), std::max(1, m.rows)));
         return m;
     }
 private:
     void own(mb_block* b) { h_ = std::shared_ptr<mb_block>(b, [](mb_block* p) { mb_block_free(Context::get(), p); }); }
+    void ownSparse(mb_sparse* s) { sp_ = std::shared_ptr<mb_sparse>(s, [](mb_sparse* p) { mb_sparse_free(Context::get(), p); }); }
+    void bothDense(const SubMatrix& o, const char* op) const {
+        if (sp_ || o.sp_)
+            throw std::invalid_argument(std::string("Not supported ") + op + "-operator between matrices of sparsity with " +
+                                        (sp_ ? "true" : "false") + " and " + (o.sp_ ? "true" : "false"));
+    }
+    SubMatrix valuesOp(int32_t op, double b) const {
+        mb_sparse* out = nullptr;
+        check(mb_sparse_values_op(Context::get(), sp_.get(), op, b, &out));
+        SubMatrix r;
+        r.ownSparse(out);
+        return r;
+    }
+    std::shared_ptr<mb_sparse> sp_;
     SubMatrix view(mb_block* v) const {
         SubMatrix s;
         auto parent = h_;       // a view keeps its parent's storage alive
@@ -215,6 +315,24 @@ private:
         return s;
     }
     std::shared_ptr<mb_block> h_;
+};
+
+inline DenseMatrix SparseMatrix::toDense() const { return SubMatrix(*this).denseBlock(); }                    // Matrices.scala:106-119
+inline DenseMatrix SparseMatrix::multiply(const SparseMatrix& o) const {                                          // :129-152
+    return SubMatrix(*this).multiply(SubMatrix(o)).denseBlock();
+}
+
+// matrix/LibMatrixMult.scala on the device.  multSparseDense is the true product (the reference reads `bi` for `bk` at :60
+// and is right only for K, N <= 32); both are bit-identical to the reference loops (corrected at :60).
+struct LibMatrixMult {
+    static DenseMatrix multDenseSparse(const DenseMatrix& d, const SparseMatrix& s) {                             // :15-41
+        if (d.cols != s.numRows) throw std::invalid_argument("matrix dimension mismatch: " + std::to_string(d.cols) + " v.s " + std::to_string(s.numRows));
+        return SubMatrix(d).multiply(SubMatrix(s)).denseBlock();
+    }
+    static DenseMatrix multSparseDense(const SparseMatrix& s, const DenseMatrix& d) {                             // :43-77
+        if (s.numCols != d.rows) throw std::invalid_argument("matrix dimension mismatch: " + std::to_string(s.numCols) + " v.s " + std::to_string(d.rows));
+        return SubMatrix(s).multiply(SubMatrix(d)).denseBlock();
+    }
 };
 
 class DenseVecMatrix;
@@ -250,6 +368,13 @@ public:
     int numBlksByRow() { if (blksByRow_ <= 0) { int n = 0; for (auto& kv : blocks) n += kv.first.column == 0; blksByRow_ = n; } return blksByRow_; }   // :52-57
     int numBlksByCol() { if (blksByCol_ <= 0) { int n = 0; for (auto& kv : blocks) n += kv.first.row == 0; blksByCol_ = n; } return blksByCol_; }     // :60-65
     const Blocks& getBlocks() const { return blocks; }
+    bool hasSparse() const { for (auto& kv : blocks) if (kv.second.isSparse()) return true; return false; }
+    // toDenseBlocks (:596-603): sparse blocks become dense; dense blocks are kept (the reference throws on them)
+    BlockMatrix toDenseBlocks() const {
+        Blocks res;
+        for (auto& kv : blocks) res.emplace_back(kv.first, kv.second.toDenseBlock());
+        return BlockMatrix(res, nRows_, nCols_, blksByRow_, blksByCol_);
+    }
     long elementsCount() const { return (long)blocks.size(); }                        // :477-479
 
     DenseMatrix toBreeze() {                                                          // :70-85
@@ -276,6 +401,19 @@ public:
             for (auto& kv : blocks) { ta[{kv.first.row, kv.first.column}] = kv.second; A[(size_t)kv.first.row * k + kv.first.column] = kv.second.handle(); }
             for (auto& kv : other.blocks) { tb[{kv.first.row, kv.first.column}] = kv.second; B[(size_t)kv.first.row * n + kv.first.column] = kv.second.handle(); }
             Blocks res;
+            if (hasSparse() || other.hasSparse()) {
+                // a sparse side: one product per partition, the kk partials added in kk order (the grouped launch is dense-only)
+                for (int i = 0; i < m; ++i)
+                    for (int j = 0; j < n; ++j) {
+                        bool complete = true;
+                        for (int kk = 0; kk < k; ++kk) complete = complete && ta.count({i, kk}) && tb.count({kk, j});
+                        if (!complete) continue;
+                        SubMatrix c = ta[{i, 0}].multiply(tb[{0, j}]);
+                        for (int kk = 1; kk < k; ++kk) ta[{i, kk}].multiplyInto(tb[{kk, j}], c, true);
+                        res.emplace_back(BlockID(i, j), c);
+                    }
+                return BlockMatrix(res, numRows(), other.numCols(), m, n);
+            }
             std::vector<int32_t> ids;
             for (int i = 0; i < m; ++i)
                 for (int j = 0; j < n; ++j) {
@@ -982,6 +1120,32 @@ struct MTUtils {
             if ((idx + 1) % byCol == 0 && (long)bcs * byCol > nCols) cols = (int)(nCols - (long)bcs * (byCol - 1));
             SubMatrix blk = SubMatrix::empty(rows, cols);
             check(mb_fill_uniform(Context::get(), blk.handle(), seeds[idx], 0, lo, hi, 0));
+            blocks.emplace_back(BlockID(idx / byCol, idx % byCol), blk);
+        }
+        return BlockMatrix(blocks, nRows, nCols, byRow, byCol);
+    }
+    // randomBlockMatrix(..., sparseInfo = (true, density)) (:34-50, RandomRDD.scala:83-101, Matrices.scala:157-173): seeded
+    // sparse blocks, s = (int)(block cols * density) per column (mb_fill_sparse_uniform); every block shape is checked first
+    static BlockMatrix randomBlockMatrix(long nRows, long nCols, int numByRow, int numByCol, std::pair<bool, double> sparseInfo, long seed) {
+        if (!sparseInfo.first) return randomBlockMatrix(nRows, nCols, numByRow, numByCol, seed);
+        const int brs = ceilLen(nRows, numByRow), bcs = ceilLen(nCols, numByCol);
+        const int byRow = (int)std::ceil((double)nRows / brs), byCol = (int)std::ceil((double)nCols / bcs);
+        std::vector<int64_t> seeds((size_t)byRow * byCol);
+        check(mb_partition_seeds(seed, byRow * byCol, seeds.data()));
+        auto shape = [&](int idx) {
+            int rows = brs, cols = bcs;
+            if (idx >= (byRow - 1) * byCol && (long)brs * byRow > nRows) rows = (int)(nRows - (long)brs * (byRow - 1));
+            if ((idx + 1) % byCol == 0 && (long)bcs * byCol > nCols) cols = (int)(nCols - (long)bcs * (byCol - 1));
+            return std::make_pair(rows, cols);
+        };
+        std::vector<int32_t> s((size_t)byRow * byCol);
+        for (int idx = 0; idx < byRow * byCol; ++idx)
+            check(mb_sparse_column_count(shape(idx).first, shape(idx).second, sparseInfo.second, &s[idx]));
+        BlockMatrix::Blocks blocks;
+        for (int idx = 0; idx < byRow * byCol; ++idx) {
+            const auto rc = shape(idx);
+            SubMatrix blk = SubMatrix::emptySparse(rc.first, rc.second, (long)s[idx] * rc.second);
+            check(mb_fill_sparse_uniform(Context::get(), blk.sparseHandle(), seeds[idx]));
             blocks.emplace_back(BlockID(idx / byCol, idx % byCol), blk);
         }
         return BlockMatrix(blocks, nRows, nCols, byRow, byCol);

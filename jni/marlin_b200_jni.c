@@ -28,6 +28,7 @@
 #define CTX(h) ((mb_ctx*)(intptr_t)(h))
 #define BLK(h) ((mb_block*)(intptr_t)(h))
 #define COMM(h) ((mb_comm*)(intptr_t)(h))
+#define SP(h) ((mb_sparse*)(intptr_t)(h))
 
 /* status -> exception (SURVEY 8b error convention) */
 static void raise(JNIEnv* env, int32_t rc) {
@@ -296,4 +297,65 @@ NATIVE(jlongArray, partitionSeeds)(JNIEnv* e, jobject o, jlong seed, jint numPar
     free(buf);
     raise(e, rc);
     return out;
+}
+
+/* ---- sparse blocks (matrix/SubMatrix.scala:22-25, 87-129; Matrices.scala:57-173; LibMatrixMult.scala) ---- */
+NATIVE(jlong, sparseUpload)(JNIEnv* e, jobject o, jlong ctx, jint rows, jint cols, jintArray colptr, jintArray rowidx,
+                            jdoubleArray values) {
+    mb_sparse* sp = NULL;
+    jint* cp = (jint*)(*e)->GetPrimitiveArrayCritical(e, colptr, NULL);
+    jint* ri = (jint*)(*e)->GetPrimitiveArrayCritical(e, rowidx, NULL);
+    jdouble* va = (jdouble*)(*e)->GetPrimitiveArrayCritical(e, values, NULL);
+    const int32_t rc = mb_sparse_upload(CTX(ctx), rows, cols, (const int32_t*)cp, (const int32_t*)ri, va, &sp);
+    (*e)->ReleasePrimitiveArrayCritical(e, values, va, JNI_ABORT);
+    (*e)->ReleasePrimitiveArrayCritical(e, rowidx, ri, JNI_ABORT);
+    (*e)->ReleasePrimitiveArrayCritical(e, colptr, cp, JNI_ABORT);
+    raise(e, rc);
+    return (jlong)(intptr_t)sp;
+}
+NATIVE(void, sparseDownload)(JNIEnv* e, jobject o, jlong ctx, jlong sp, jintArray colptr, jintArray rowidx, jdoubleArray values) {
+    jint* cp = (jint*)(*e)->GetPrimitiveArrayCritical(e, colptr, NULL);
+    jint* ri = (jint*)(*e)->GetPrimitiveArrayCritical(e, rowidx, NULL);
+    jdouble* va = (jdouble*)(*e)->GetPrimitiveArrayCritical(e, values, NULL);
+    const int32_t rc = mb_sparse_download(CTX(ctx), SP(sp), (int32_t*)cp, (int32_t*)ri, va);
+    (*e)->ReleasePrimitiveArrayCritical(e, values, va, 0);
+    (*e)->ReleasePrimitiveArrayCritical(e, rowidx, ri, 0);
+    (*e)->ReleasePrimitiveArrayCritical(e, colptr, cp, 0);
+    raise(e, rc);
+}
+NATIVE(jlong, sparseNnz)(JNIEnv* e, jobject o, jlong sp) {
+    int64_t nnz = 0;
+    raise(e, mb_sparse_info(SP(sp), NULL, NULL, &nnz));
+    return (jlong)nnz;
+}
+NATIVE(jlong, sparseAlloc)(JNIEnv* e, jobject o, jlong ctx, jint rows, jint cols, jlong nnz) {
+    mb_sparse* sp = NULL;
+    raise(e, mb_sparse_alloc(CTX(ctx), rows, cols, nnz, &sp));
+    return (jlong)(intptr_t)sp;
+}
+NATIVE(void, sparseFree)(JNIEnv* e, jobject o, jlong ctx, jlong sp) { raise(e, mb_sparse_free(CTX(ctx), SP(sp))); }
+NATIVE(jlong, sparseValuesOp)(JNIEnv* e, jobject o, jlong ctx, jlong sp, jint op, jdouble b) {
+    mb_sparse* out = NULL;
+    raise(e, mb_sparse_values_op(CTX(ctx), SP(sp), op, b, &out));
+    return (jlong)(intptr_t)out;
+}
+NATIVE(void, sparseToDense)(JNIEnv* e, jobject o, jlong ctx, jlong sp, jlong out) {
+    raise(e, mb_sparse_to_dense(CTX(ctx), SP(sp), BLK(out)));
+}
+NATIVE(void, spmmDenseSparse)(JNIEnv* e, jobject o, jlong ctx, jlong a, jlong b, jlong c, jboolean accumulate) {
+    raise(e, mb_spmm_dense_sparse(CTX(ctx), BLK(a), SP(b), BLK(c), accumulate ? 1 : 0));
+}
+NATIVE(void, spmmSparseDense)(JNIEnv* e, jobject o, jlong ctx, jlong a, jlong b, jlong c, jboolean accumulate) {
+    raise(e, mb_spmm_sparse_dense(CTX(ctx), SP(a), BLK(b), BLK(c), accumulate ? 1 : 0));
+}
+NATIVE(void, spgemm)(JNIEnv* e, jobject o, jlong ctx, jlong a, jlong b, jlong c, jboolean accumulate) {
+    raise(e, mb_spgemm_dense_out(CTX(ctx), SP(a), SP(b), BLK(c), accumulate ? 1 : 0));
+}
+NATIVE(jint, sparseColumnCount)(JNIEnv* e, jobject o, jint rows, jint cols, jdouble density) {
+    int32_t s = 0;
+    raise(e, mb_sparse_column_count(rows, cols, density, &s));
+    return s;
+}
+NATIVE(void, fillSparseUniform)(JNIEnv* e, jobject o, jlong ctx, jlong sp, jlong partitionSeed) {
+    raise(e, mb_fill_sparse_uniform(CTX(ctx), SP(sp), partitionSeed));
 }

@@ -12,10 +12,11 @@ import os as _os
 _os.environ.setdefault("CUDA_DEVICE_MAX_CONNECTIONS", "32")
 
 from ._native import MarlinArgumentError, MarlinError
-from .matrix import BlockID, BlockMatrix, DenseVecMatrix, DistributedMatrix, DistributedVector, SubMatrix
+from .matrix import (BlockID, BlockMatrix, DenseVecMatrix, DistributedMatrix, DistributedVector, SparseMatrix, SparseVector,
+                     SubMatrix)
 from .rdd import MatrixElemOpPartitioner, MatrixMultPartitioner
 from .runtime import Runtime
 from .utils import MTUtils
 
-__all__ = ["BlockID", "BlockMatrix", "DenseVecMatrix", "DistributedMatrix", "DistributedVector", "SubMatrix", "MTUtils",
-           "MatrixElemOpPartitioner", "MatrixMultPartitioner", "Runtime", "MarlinError", "MarlinArgumentError"]
+__all__ = ["BlockID", "BlockMatrix", "DenseVecMatrix", "DistributedMatrix", "DistributedVector", "SparseMatrix", "SparseVector",
+           "SubMatrix", "MTUtils", "MatrixElemOpPartitioner", "MatrixMultPartitioner", "Runtime", "MarlinError", "MarlinArgumentError"]

@@ -27,6 +27,7 @@ _LIB_PATH = Path(__file__).resolve().parent / "lib" / "libmarlin_b200.so"
 
 c_ctx = C.c_void_p
 c_blk = C.c_void_p
+c_sp = C.c_void_p
 c_i32 = C.c_int32
 c_i64 = C.c_int64
 c_f64 = C.c_double
@@ -84,6 +85,20 @@ SIGNATURES = {
     "mb_svd_mode": (c_i32, [c_i64, c_i32, C.c_char_p, C.POINTER(c_i32)]),
     "mb_svd_rank": (c_i32, [c_dp, c_i32, c_i32, c_f64]),
     "mb_fill_uniform": (c_i32, [c_ctx, c_blk, c_i64, c_i64, c_f64, c_f64, c_i32]),
+    "mb_sparse_check": (c_i32, [c_i32, c_i32, C.c_void_p, C.c_void_p]),
+    "mb_sparse_wrap": (c_i32, [c_ctx, c_i32, c_i32, c_i64, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(c_sp)]),
+    "mb_sparse_upload": (c_i32, [c_ctx, c_i32, c_i32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(c_sp)]),
+    "mb_sparse_download": (c_i32, [c_ctx, c_sp, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "mb_sparse_info": (c_i32, [c_sp, C.POINTER(c_i32), C.POINTER(c_i32), C.POINTER(c_i64)]),
+    "mb_sparse_alloc": (c_i32, [c_ctx, c_i32, c_i32, c_i64, C.POINTER(c_sp)]),
+    "mb_sparse_free": (c_i32, [c_ctx, c_sp]),
+    "mb_sparse_values_op": (c_i32, [c_ctx, c_sp, c_i32, c_f64, C.POINTER(c_sp)]),
+    "mb_sparse_to_dense": (c_i32, [c_ctx, c_sp, c_blk]),
+    "mb_spmm_dense_sparse": (c_i32, [c_ctx, c_blk, c_sp, c_blk, c_i32]),
+    "mb_spmm_sparse_dense": (c_i32, [c_ctx, c_sp, c_blk, c_blk, c_i32]),
+    "mb_spgemm_dense_out": (c_i32, [c_ctx, c_sp, c_sp, c_blk, c_i32]),
+    "mb_sparse_column_count": (c_i32, [c_i32, c_i32, c_f64, C.POINTER(c_i32)]),
+    "mb_fill_sparse_uniform": (c_i32, [c_ctx, c_sp, c_i64]),
     "mb_hash_seed": (c_i64, [c_i64]),
     "mb_partition_seeds": (c_i32, [c_i64, c_i32, C.POINTER(c_i64)]),
     "mb_choose_split": (c_i32, [c_i64, c_i64, c_i64, c_i32, C.POINTER(c_i32)]),

@@ -9,6 +9,7 @@
 #include "blas12.h"
 #include "factor.h"
 #include "eigen.h"
+#include "sparse.h"
 
 #include <cuda_runtime.h>
 #include <algorithm>
@@ -1268,6 +1269,223 @@ int32_t mb_fill_uniform(mb_ctx* ctx, mb_block* blk, int64_t partition_seed, int6
     MB_CUDA(mb::fill_uniform_f64(f64_ptr(blk), rs(blk), cs(blk), blk->rows, blk->cols, row_major ? 1 : 0, state0, first, lo,
                                  hi, ctx->stream, &launches));
     ctx->launches += launches;
+    return MB_OK;
+}
+
+// ------------------------------------------------------------------------------------------- sparse blocks (SURVEY 8 f6)
+static mb::CscView csc(const mb_sparse* S) { return mb::CscView{S->rows, S->cols, S->colptr, S->rowidx, S->values}; }
+static mb::DView dview(const mb_block* b) { return mb::DView{f64_ptr(b), rs(b), cs(b)}; }
+
+static void sparse_release(mb_sparse* S) {
+    if (S->owns) {
+        cudaFree(S->colptr);
+        cudaFree(S->rowidx);
+        cudaFree(S->values);
+    }
+    cudaFree(S->csr_rowptr);
+    cudaFree(S->csr_colidx);
+    cudaFree(S->csr_values);
+    delete S;
+}
+
+int32_t mb_sparse_wrap(mb_ctx* ctx, int32_t rows, int32_t cols, int64_t nnz, void* colptr, void* rowidx, void* values,
+                       mb_sparse** out) {
+    if (!ctx) return fail(MB_ERR_INVALID_ARG, "null context");
+    if (!out || rows < 0 || cols < 0 || nnz < 0 || !colptr || (nnz > 0 && (!rowidx || !values)))
+        return fail(MB_ERR_INVALID_ARG, "mb_sparse_wrap: bad argument");
+    if (nnz > 0x7fffffffLL) return fail(MB_ERR_INVALID_ARG, "sparse block with %lld non-zeros: at most 2^31 - 1", (long long)nnz);
+    mb_sparse* S = new (std::nothrow) mb_sparse();
+    if (!S) return fail(MB_ERR_OOM, "host allocation failed");
+    S->rows = rows; S->cols = cols; S->nnz = nnz; S->device = ctx->device;
+    S->colptr = static_cast<int*>(colptr); S->rowidx = static_cast<int*>(rowidx); S->values = static_cast<double*>(values);
+    *out = S;
+    return MB_OK;
+}
+
+int32_t mb_sparse_upload(mb_ctx* ctx, int32_t rows, int32_t cols, const int32_t* colptr, const int32_t* rowidx,
+                         const double* values, mb_sparse** out) {
+    MB_CTX(ctx);
+    if (!out || !colptr) return fail(MB_ERR_INVALID_ARG, "mb_sparse_upload: null argument");
+    int32_t r = mb_sparse_check(rows, cols, colptr, rowidx);
+    if (r) return r;
+    const long long nnz = colptr[cols];
+    if (nnz > 0 && !values) return fail(MB_ERR_INVALID_ARG, "mb_sparse_upload: null values");
+    mb_sparse* S = new (std::nothrow) mb_sparse();
+    if (!S) return fail(MB_ERR_OOM, "host allocation failed");
+    S->rows = rows; S->cols = cols; S->nnz = nnz; S->owns = 1; S->device = ctx->device;
+    cudaError_t e = cudaMalloc(&S->colptr, sizeof(int) * ((size_t)cols + 1));
+    if (e == cudaSuccess && nnz) e = cudaMalloc(&S->rowidx, sizeof(int) * (size_t)nnz);
+    if (e == cudaSuccess && nnz) e = cudaMalloc(&S->values, sizeof(double) * (size_t)nnz);
+    if (e == cudaSuccess) e = cudaMemcpy(S->colptr, colptr, sizeof(int) * ((size_t)cols + 1), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && nnz) e = cudaMemcpy(S->rowidx, rowidx, sizeof(int) * (size_t)nnz, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && nnz) e = cudaMemcpy(S->values, values, sizeof(double) * (size_t)nnz, cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) { sparse_release(S); return cuda_fail(e, "mb_sparse_upload"); }
+    *out = S;
+    return MB_OK;
+}
+
+int32_t mb_sparse_download(mb_ctx* ctx, const mb_sparse* S, int32_t* colptr, int32_t* rowidx, double* values) {
+    MB_CTX(ctx);
+    if (!S || !colptr || (S->nnz > 0 && (!rowidx || !values))) return fail(MB_ERR_INVALID_ARG, "mb_sparse_download: null argument");
+    MB_CUDA(cudaStreamSynchronize(ctx->stream));
+    MB_CUDA(cudaMemcpy(colptr, S->colptr, sizeof(int) * ((size_t)S->cols + 1), cudaMemcpyDeviceToHost));
+    if (S->nnz) {
+        MB_CUDA(cudaMemcpy(rowidx, S->rowidx, sizeof(int) * (size_t)S->nnz, cudaMemcpyDeviceToHost));
+        MB_CUDA(cudaMemcpy(values, S->values, sizeof(double) * (size_t)S->nnz, cudaMemcpyDeviceToHost));
+    }
+    return MB_OK;
+}
+
+int32_t mb_sparse_info(const mb_sparse* S, int32_t* rows, int32_t* cols, int64_t* nnz) {
+    if (!S) return fail(MB_ERR_INVALID_ARG, "null sparse block");
+    if (rows) *rows = S->rows;
+    if (cols) *cols = S->cols;
+    if (nnz) *nnz = S->nnz;
+    return MB_OK;
+}
+
+int32_t mb_sparse_alloc(mb_ctx* ctx, int32_t rows, int32_t cols, int64_t nnz, mb_sparse** out) {
+    MB_CTX(ctx);
+    if (!out || rows < 0 || cols < 0 || nnz < 0) return fail(MB_ERR_INVALID_ARG, "mb_sparse_alloc: bad argument");
+    if (nnz > 0x7fffffffLL) return fail(MB_ERR_INVALID_ARG, "sparse block with %lld non-zeros: at most 2^31 - 1", (long long)nnz);
+    mb_sparse* S = new (std::nothrow) mb_sparse();
+    if (!S) return fail(MB_ERR_OOM, "host allocation failed");
+    S->rows = rows; S->cols = cols; S->nnz = nnz; S->owns = 1; S->device = ctx->device;
+    cudaError_t e = cudaMalloc(&S->colptr, sizeof(int) * ((size_t)cols + 1));
+    if (e == cudaSuccess && nnz) e = cudaMalloc(&S->rowidx, sizeof(int) * (size_t)nnz);
+    if (e == cudaSuccess && nnz) e = cudaMalloc(&S->values, sizeof(double) * (size_t)nnz);
+    if (e != cudaSuccess) { sparse_release(S); return cuda_fail(e, "mb_sparse_alloc"); }
+    *out = S;
+    return MB_OK;
+}
+
+int32_t mb_sparse_values_op(mb_ctx* ctx, const mb_sparse* S, int32_t op, double b, mb_sparse** out) {
+    MB_CTX(ctx);
+    if (!S || !out || op < MB_SPARSE_ADD || op > MB_SPARSE_DIV) return fail(MB_ERR_INVALID_ARG, "mb_sparse_values_op: bad argument");
+    mb_sparse* R = nullptr;
+    int32_t r = mb_sparse_alloc(ctx, S->rows, S->cols, S->nnz, &R);
+    if (r) return r;
+    cudaError_t e = cudaMemcpyAsync(R->colptr, S->colptr, sizeof(int) * ((size_t)S->cols + 1), cudaMemcpyDeviceToDevice, ctx->stream);
+    if (e == cudaSuccess && S->nnz)
+        e = cudaMemcpyAsync(R->rowidx, S->rowidx, sizeof(int) * (size_t)S->nnz, cudaMemcpyDeviceToDevice, ctx->stream);
+    if (e == cudaSuccess && S->nnz) {
+        // the values as an nnz x 1 block through the dense kernels: the same arithmetic as SubMatrix.add(b) etc. on a dense block
+        const int n = (int)S->nnz;
+        if (op == MB_SPARSE_DIV) e = mb::ew_unary(mb::EW_DIV, n, 1, S->values, 1, n, R->values, 1, n, b, 0.0, ctx->stream);
+        else {
+            const double alpha = op == MB_SPARSE_MUL ? b : 1.0;
+            const double beta = op == MB_SPARSE_ADD ? b : (op == MB_SPARSE_SUB ? -b : 0.0);
+            e = mb::ew_unary(mb::EW_AXPB, n, 1, S->values, 1, n, R->values, 1, n, alpha, beta, ctx->stream);
+        }
+        ctx->launches++;
+    }
+    if (e != cudaSuccess) { mb_sparse_free(ctx, R); return cuda_fail(e, "mb_sparse_values_op"); }
+    *out = R;
+    return MB_OK;
+}
+
+int32_t mb_sparse_free(mb_ctx* ctx, mb_sparse* S) {
+    if (!S) return MB_OK;
+    if (ctx) {
+        cudaSetDevice(ctx->device);
+        cudaStreamSynchronize(ctx->stream);      // a product may still read the CSR copy
+    }
+    sparse_release(S);
+    return MB_OK;
+}
+
+static int32_t dense_f64_out(const mb_block* C, int rows, int cols, const char* what) {
+    if (C->dtype != MB_F64) return fail(MB_ERR_UNSUPPORTED, "%s: fp64 blocks only", what);
+    if (C->rows != rows || C->cols != cols)
+        return fail(MB_ERR_DIM_MISMATCH, "%s: result block is %dx%d, expected %dx%d", what, C->rows, C->cols, rows, cols);
+    return MB_OK;
+}
+
+int32_t mb_sparse_to_dense(mb_ctx* ctx, const mb_sparse* S, mb_block* out) {
+    MB_CTX(ctx);
+    if (!S || !out) return fail(MB_ERR_INVALID_ARG, "mb_sparse_to_dense: null argument");
+    int32_t r = dense_f64_out(out, S->rows, S->cols, "toDense");
+    if (r) return r;
+    MB_CUDA(mb::csc_to_dense(csc(S), dview(out), ctx->stream));
+    ctx->launches++;
+    return MB_OK;
+}
+
+int32_t mb_spmm_dense_sparse(mb_ctx* ctx, const mb_block* A, const mb_sparse* B, mb_block* C, int32_t accumulate) {
+    MB_CTX(ctx);
+    if (!A || !B || !C) return fail(MB_ERR_INVALID_ARG, "mb_spmm_dense_sparse: null argument");
+    if (A->dtype != MB_F64) return fail(MB_ERR_UNSUPPORTED, "multDenseSparse: fp64 blocks only");
+    if (A->cols != B->rows) return fail(MB_ERR_DIM_MISMATCH, "matrix dimension mismatch: %d v.s %d", A->cols, B->rows);
+    int32_t r = dense_f64_out(C, A->rows, B->cols, "multDenseSparse");
+    if (r) return r;
+    MB_CUDA(mb::spmm_dense_sparse(A->rows, dview(A), csc(B), dview(C), accumulate != 0, ctx->stream));
+    ctx->launches++;
+    return MB_OK;
+}
+
+int32_t mb_spmm_sparse_dense(mb_ctx* ctx, mb_sparse* A, const mb_block* B, mb_block* C, int32_t accumulate) {
+    MB_CTX(ctx);
+    MB_LOCK(ctx);
+    if (!A || !B || !C) return fail(MB_ERR_INVALID_ARG, "mb_spmm_sparse_dense: null argument");
+    if (B->dtype != MB_F64) return fail(MB_ERR_UNSUPPORTED, "multSparseDense: fp64 blocks only");
+    if (A->cols != B->rows) return fail(MB_ERR_DIM_MISMATCH, "matrix dimension mismatch: %d v.s %d", A->cols, B->rows);
+    int32_t r = dense_f64_out(C, A->rows, B->cols, "multSparseDense");
+    if (r) return r;
+    if (!A->csr_rowptr) {
+        int *rowptr = nullptr, *colidx = nullptr;
+        double* vals = nullptr;
+        cudaError_t e = cudaMalloc(&rowptr, sizeof(int) * ((size_t)A->rows + 1));
+        if (e == cudaSuccess) e = cudaMalloc(&colidx, sizeof(int) * std::max<size_t>(1, (size_t)A->nnz));
+        if (e == cudaSuccess) e = cudaMalloc(&vals, sizeof(double) * std::max<size_t>(1, (size_t)A->nnz));
+        int launches = 0;
+        if (e == cudaSuccess) e = mb::csc_to_csr(csc(A), A->nnz, rowptr, colidx, vals, ctx->stream, &launches);
+        if (e != cudaSuccess) {
+            cudaFree(rowptr); cudaFree(colidx); cudaFree(vals);
+            return cuda_fail(e, "multSparseDense: CSR copy");
+        }
+        ctx->launches += launches;
+        A->csr_rowptr = rowptr; A->csr_colidx = colidx; A->csr_values = vals;
+    }
+    const mb::CsrView csr{A->rows, A->cols, A->csr_rowptr, A->csr_colidx, A->csr_values};
+    MB_CUDA(mb::spmm_sparse_dense(csr, B->cols, dview(B), dview(C), accumulate != 0, ctx->stream));
+    ctx->launches++;
+    return MB_OK;
+}
+
+int32_t mb_spgemm_dense_out(mb_ctx* ctx, const mb_sparse* A, const mb_sparse* B, mb_block* C, int32_t accumulate) {
+    MB_CTX(ctx);
+    if (!A || !B || !C) return fail(MB_ERR_INVALID_ARG, "mb_spgemm_dense_out: null argument");
+    if (A->cols != B->rows) return fail(MB_ERR_DIM_MISMATCH, "matrix dimension mismatch: %d v.s %d", A->cols, B->rows);
+    int32_t r = dense_f64_out(C, A->rows, B->cols, "SparseMatrix.multiply");
+    if (r) return r;
+    MB_CUDA(mb::spgemm_dense_out(csc(A), csc(B), dview(C), accumulate != 0, ctx->stream));
+    ctx->launches++;
+    return MB_OK;
+}
+
+int32_t mb_fill_sparse_uniform(mb_ctx* ctx, mb_sparse* S, int64_t partition_seed) {
+    MB_CTX(ctx);
+    if (!S) return fail(MB_ERR_INVALID_ARG, "mb_fill_sparse_uniform: null block");
+    if (S->cols == 0) {
+        if (S->nnz != 0) return fail(MB_ERR_INVALID_ARG, "mb_fill_sparse_uniform: %lld non-zeros in 0 columns", (long long)S->nnz);
+        MB_CUDA(cudaMemsetAsync(S->colptr, 0, sizeof(int), ctx->stream));      // colptr = {0}
+        return MB_OK;
+    }
+    if (S->nnz % S->cols != 0)
+        return fail(MB_ERR_INVALID_ARG, "mb_fill_sparse_uniform: nnz %lld is not a multiple of cols %d", (long long)S->nnz, S->cols);
+    const int s = (int)(S->nnz / S->cols);
+    if (s > S->rows) return fail(MB_ERR_INVALID_ARG, "mb_fill_sparse_uniform: %d rows per column of %d", s, S->rows);
+    // the row sampling's last stream position must stay within the 2^39 positions the jump tables reach
+    if ((long long)S->rows * S->cols + S->nnz >= (1LL << 39))
+        return fail(MB_ERR_UNSUPPORTED, "mb_fill_sparse_uniform: a %dx%d block exceeds the generator's 2^39 stream positions",
+                    S->rows, S->cols);
+    const unsigned long long state0 = (unsigned long long)mb_hash_seed(partition_seed);
+    int launches = 0;
+    if (S->nnz) {
+        MB_CUDA(mb::fill_uniform_f64(S->values, 1, S->nnz, (int)S->nnz, 1, 0, state0, 0, 0.0, 1.0, ctx->stream, &launches));
+    }
+    MB_CUDA(mb::sparse_sample_rows(S->rows, S->cols, s, state0, S->colptr, S->rowidx, ctx->stream));
+    ctx->launches += launches + 1;
     return MB_OK;
 }
 

@@ -760,6 +760,15 @@ cudaError_t fill_uniform_init_tables() {
     return e;
 }
 
+cudaError_t fill_jump_tables(const unsigned long long** tables) {
+    cudaError_t e = fill_uniform_init_tables();
+    if (e != cudaSuccess) return e;
+    void* p = nullptr;
+    e = cudaGetSymbolAddress(&p, g_jump);
+    *tables = static_cast<const unsigned long long*>(p);
+    return e;
+}
+
 // The fast kernel must reproduce the general kernel (the one pinned against the JVM stream) bit for bit.  That is checked
 // ONCE per device and process, on the device itself: two CTAs of each kernel at a far, odd stream offset, unit and affine
 // range, compared on the host (about a millisecond).  A mismatch — a compiler or driver that breaks one of the kernel's

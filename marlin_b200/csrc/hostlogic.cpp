@@ -180,6 +180,42 @@ int32_t mb_svd_mode(int64_t n, int32_t k, const char* mode, int32_t* compute_mod
     return MB_OK;
 }
 
+int32_t mb_sparse_check(int32_t rows, int32_t cols, const int32_t* colptr, const int32_t* rowidx) {
+    if (rows < 0 || cols < 0 || !colptr) return mb_fail(MB_ERR_INVALID_ARG, "mb_sparse_check: bad argument");
+    if (colptr[0] != 0) return mb_fail(MB_ERR_INVALID_ARG, "sparse block: colptr[0] is %d, not 0", colptr[0]);
+    // colptr first, so that no row index past colptr[cols] (= nnz, the length of rowidx) is read
+    for (int32_t j = 0; j < cols; ++j)
+        if (colptr[j + 1] < colptr[j])
+            return mb_fail(MB_ERR_INVALID_ARG, "sparse block: colptr decreases at column %d (%d -> %d)", j, colptr[j], colptr[j + 1]);
+    if (colptr[cols] > 0 && !rowidx) return mb_fail(MB_ERR_INVALID_ARG, "mb_sparse_check: null rowidx");
+    for (int32_t j = 0; j < cols; ++j) {
+        const int32_t p0 = colptr[j], p1 = colptr[j + 1];
+        for (int32_t p = p0; p < p1; ++p) {
+            if (rowidx[p] < 0 || rowidx[p] >= rows)
+                return mb_fail(MB_ERR_INVALID_ARG, "sparse block: row index %d of column %d is outside [0, %d)", rowidx[p], j, rows);
+            if (p > p0 && rowidx[p] <= rowidx[p - 1])
+                return mb_fail(MB_ERR_INVALID_ARG, "sparse block: row indices of column %d are not strictly increasing (%d after %d)",
+                               j, rowidx[p], rowidx[p - 1]);
+        }
+    }
+    return MB_OK;
+}
+
+// matrix/Matrices.scala:161 `(numCols * sparsity).toInt`, plus the two requires the reference lacks
+int32_t mb_sparse_column_count(int32_t rows, int32_t cols, double density, int32_t* s_out) {
+    if (!s_out || rows < 0 || cols < 0) return mb_fail(MB_ERR_INVALID_ARG, "mb_sparse_column_count: bad argument");
+    if (!(density > 0.0))
+        return mb_fail(MB_ERR_INVALID_ARG, "requirement failed: the density of sparse blocks must be positive, but got %g", density);
+    const double x = (double)cols * density;
+    // JVM d2i: truncate toward zero, saturate at Int.MaxValue (x > 0 here)
+    const int32_t s = x >= 2147483647.0 ? INT32_MAX : (int32_t)x;
+    if (s > rows)
+        return mb_fail(MB_ERR_INVALID_ARG, "requirement failed: %d non-zeros per column asked of a block with %d rows "
+                       "(cols * density = %d * %g)", s, rows, cols, density);
+    *s_out = s;
+    return MB_OK;
+}
+
 // matrix/DenseVecMatrix.scala:1607-1621
 int32_t mb_svd_rank(const double* sigmas, int32_t count, int32_t k, double rcond) {
     if (count <= 0) return 0;

@@ -54,6 +54,21 @@ struct mb_block {
     void* ready_event = nullptr;   // optional cudaEvent_t: the block's contents are final once it has completed
 };
 
+// A CSC block (column j: rowidx/values[colptr[j] .. colptr[j+1]), rows strictly increasing).  The CSR copy that the
+// sparse x dense product reads is built on first use and kept with the handle: blocks are immutable values.
+struct mb_sparse {
+    int rows = 0, cols = 0;
+    long long nnz = 0;
+    int* colptr = nullptr;
+    int* rowidx = nullptr;
+    double* values = nullptr;
+    int owns = 0;
+    int device = 0;
+    int* csr_rowptr = nullptr;      // owned by the handle
+    int* csr_colidx = nullptr;
+    double* csr_values = nullptr;
+};
+
 namespace mb {
 cudaError_t ipc_export(const void* dptr, unsigned char handle[64], long long* offset, long long* alloc_bytes);
 cudaError_t ipc_open(const unsigned char handle[64], void** base_out);

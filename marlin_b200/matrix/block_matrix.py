@@ -22,6 +22,7 @@ from .. import profiling
 from ..runtime import Runtime, world
 from .block import BlockID
 from .distributed_matrix import DistributedMatrix
+from .sparse_matrix import SparseBlock
 from .sub_matrix import SubMatrix
 
 
@@ -31,7 +32,9 @@ def _ceil_len(total: int, parts: int) -> int:
 
 class BlockMatrix(DistributedMatrix):
     def __init__(self, blocks: Iterable[Tuple[BlockID, SubMatrix]], nRows: int = 0, nCols: int = 0, blksByRow: int = 0,
-                 blksByCol: int = 0, placement: Optional[Callable[[int, int], int]] = None):
+                 blksByCol: int = 0, placement: Optional[Callable[[int, int], int]] = None, sparse: Optional[bool] = None):
+        """`sparse` says whether any block, on any rank, is sparse; when None it is gathered from all ranks on first use."""
+        self._sparse_flag = sparse
         self.blocks: List[Tuple[BlockID, SubMatrix]] = [(b if isinstance(b, BlockID) else BlockID(*b), s) for b, s in blocks]
         self._nRows, self._nCols, self._blksByRow, self._blksByCol = int(nRows), int(nCols), int(blksByRow), int(blksByCol)
         self._placement = placement
@@ -89,6 +92,24 @@ class BlockMatrix(DistributedMatrix):
     def elementsCount(self) -> int:
         """:477-479 (blocks.count())"""
         return len(self._all_gather_meta([1 for _ in self.blocks]))
+
+    # ------------------------------------------------------------------ sparse blocks
+    def _has_sparse(self) -> bool:
+        """Whether any block of this matrix, on any rank, is sparse (every rank gets the same answer)."""
+        if self._sparse_flag is None:
+            self._sparse_flag = any(self._all_gather_meta([any(s.isSparse for _, s in self.blocks)]))
+        return self._sparse_flag
+
+    def _dense_only(self, what: str) -> None:
+        if self._has_sparse():
+            raise nat.MarlinArgumentError(nat.MB_ERR_UNSUPPORTED, f"{what} is not supported on sparse blocks: call "
+                                          "toDenseBlocks first")
+
+    def toDenseBlocks(self) -> "BlockMatrix":
+        """:596-603 — every sparse block as a dense one (SparseMatrix.toDense).  Dense blocks are kept as they are (the
+        reference throws a NullPointerException on them)."""
+        res = [(b, s.toDense()) for b, s in self.blocks]
+        return BlockMatrix(res, self._nRows, self._nCols, self._blksByRow, self._blksByCol, self._placement, sparse=False)
 
     # ------------------------------------------------------------------ collect (:70-85)
     def toBreeze(self) -> np.ndarray:
@@ -169,6 +190,8 @@ class BlockMatrix(DistributedMatrix):
                                           f"{self.numCols()} vs {other.numRows()}")
         if self.numBlksByCol() == other.numBlksByRow():
             return self._multiply_same_grid(other)
+        self._dense_only("multiply with a different block grid")
+        other._dense_only("multiply with a different block grid")
         if self.numBlksByCol() % other.numBlksByRow() == 0:                    # :187-201
             self._check_even_cols()
             ratio = self.numBlksByCol() // other.numBlksByRow()
@@ -177,7 +200,7 @@ class BlockMatrix(DistributedMatrix):
                 for i in range(ratio):
                     blks.append((BlockID(b.row * ratio + i, b.column),
                                  mat.slice(i * mat.rows // ratio, (i + 1) * mat.rows // ratio, 0, mat.cols)))
-            split = BlockMatrix(blks, placement=lambda r, c, o=other, q=ratio: o.owner(r // q, c))
+            split = BlockMatrix(blks, placement=lambda r, c, o=other, q=ratio: o.owner(r // q, c), sparse=False)
             return self._multiply_block(split)
         if other.numBlksByRow() % self.numBlksByCol() == 0:                    # :202-216 (row slices of `this`, as written)
             self._check_even_cols()
@@ -187,7 +210,7 @@ class BlockMatrix(DistributedMatrix):
                 for i in range(ratio):
                     blks.append((BlockID(b.row * ratio + i, b.column),
                                  mat.slice(i * mat.rows // ratio, (i + 1) * mat.rows // ratio, 0, mat.cols)))
-            split = BlockMatrix(blks, placement=lambda r, c, o=self, q=ratio: o.owner(r // q, c))
+            split = BlockMatrix(blks, placement=lambda r, c, o=self, q=ratio: o.owner(r // q, c), sparse=False)
             return split._multiply_block(other)
         raise nat.MarlinArgumentError(nat.MB_ERR_UNSUPPORTED, "currently not supported for the two dimension of matrices")
 
@@ -207,7 +230,9 @@ class BlockMatrix(DistributedMatrix):
         a_tiles: Dict[Tuple[int, int], SubMatrix] = dict(a_local)
         b_tiles: Dict[Tuple[int, int], SubMatrix] = dict(b_local)
         M, N = self.numRows(), other.numCols()
-        if ws > 1 and Runtime.available():
+        # the NVLink engine and the grouped launch are dense-only; every rank takes the same branch
+        sparse = self._has_sparse() or other._has_sparse()
+        if ws > 1 and Runtime.available() and not sparse:
             mesh = peer.PeerMesh.get()
             if mesh is not None:
                 res = self._multiply_p2p(other, mesh, plan, a_local, b_local)
@@ -220,10 +245,17 @@ class BlockMatrix(DistributedMatrix):
             dims_a = lambda i, kk: (min(bm, M - i * bm), min(bk, K - kk * bk))
             dims_b = lambda kk, j: (min(bk, K - kk * bk), min(bn, N - j * bn))
             sends = [(s, d, ("A",) + key) for s, d, key in plan.a_sends] + [(s, d, ("B",) + key) for s, d, key in plan.b_sends]
+            # a sparse tile travels as one packed buffer; its nnz is agreed before any rank allocates
+            nnz = dict(self._all_gather_meta([(("A",) + k_, s.sparseBlock.nnz) for k_, s in a_local.items() if s.isSparse] +
+                                             [(("B",) + k_, s.sparseBlock.nnz) for k_, s in b_local.items() if s.isSparse])) \
+                if sparse else {}
             send_bufs, keep = {}, []
             for s, d, key in sends:
                 if s == rank and key not in send_bufs:
                     src = (a_local if key[0] == "A" else b_local)[key[1:]]
+                    if src.isSparse:
+                        send_bufs[key] = src.sparseBlock.pack()
+                        continue
                     if not src.is_packed():
                         src = src.copy(); keep.append(src)
                     send_bufs[key] = src.buf[: src.rows * src.cols]
@@ -232,13 +264,17 @@ class BlockMatrix(DistributedMatrix):
 
             def alloc(key):
                 r, c = dims_a(*key[1:]) if key[0] == "A" else dims_b(*key[1:])
+                if key in nnz:
+                    return torch.empty(SparseBlock.packed_bytes(c, nnz[key]), dtype=torch.uint8, device=dev)
                 return torch.empty(r * c, dtype=dtype_a, device=dev)
 
             with profiling.phase("exchange"):
                 got = comm.exchange(sends, send_bufs, alloc, rank)
             for key, buf in got.items():
                 r, c = dims_a(*key[1:]) if key[0] == "A" else dims_b(*key[1:])
-                (a_tiles if key[0] == "A" else b_tiles)[key[1:]] = SubMatrix(buf=buf, rows=r, cols=c, ld=max(1, r))
+                tile = SubMatrix(sparse=SparseBlock.unpack(buf, r, c, nnz[key])) if key in nnz else \
+                    SubMatrix(buf=buf, rows=r, cols=c, ld=max(1, r))
+                (a_tiles if key[0] == "A" else b_tiles)[key[1:]] = tile
         # the join + one dgemm per partition (:173-176), kk-partials of a C tile accumulated in place (:177)
         partial: Dict[Tuple[int, int], SubMatrix] = {}
         mine = plan.products.get(rank, [])
@@ -246,7 +282,7 @@ class BlockMatrix(DistributedMatrix):
         for (i, j, kk) in mine:
             by_c.setdefault((i, j), []).append(kk)
         whole = bool(by_c) and all(sorted(v) == list(range(k)) for v in by_c.values())
-        if whole and len(by_c) <= 16 and k <= 16:
+        if whole and len(by_c) <= 16 and k <= 16 and not sparse:
             # this rank holds every kk of its C tiles: ONE grouped persistent launch (K loop concatenated over kk)
             import ctypes as C
             rt = Runtime.get(); rt.sync_stream()
@@ -292,7 +328,7 @@ class BlockMatrix(DistributedMatrix):
                     partial.pop(key, None)
         result = [(BlockID(i, j), blk) for (i, j), blk in sorted(partial.items())]
         owners = dict(plan.c_owner)
-        return BlockMatrix(result, M, N, m, n, placement=(lambda r, c, o=owners: o[(r, c)]) if ws > 1 else None)
+        return BlockMatrix(result, M, N, m, n, placement=(lambda r, c, o=owners: o[(r, c)]) if ws > 1 else None, sparse=False)
 
     # ------------------------------------------------------------------ NVLink peer-memory path
     def _multiply_p2p(self, other: "BlockMatrix", mesh, plan, a_local: dict, b_local: dict) -> Optional["BlockMatrix"]:
@@ -334,7 +370,7 @@ class BlockMatrix(DistributedMatrix):
             nat.check(rt.lib.mb_matmul_blocked_dist(mesh.comm, a_arr, a_own, b_arr, b_own, m, k, n, row_len, k_len, col_len, dt, c_arr))
         result = [(BlockID(i, j), blk.mark_ready()) for (i, j), blk in sorted(partial.items())]
         owners = {(i, j): c_owner[i * n + j] for i in range(m) for j in range(n)}
-        return BlockMatrix(result, M, N, m, n, placement=lambda r, c, o=owners: o[(r, c)])
+        return BlockMatrix(result, M, N, m, n, placement=lambda r, c, o=owners: o[(r, c)], sparse=False)
 
     def inverse(self) -> "BlockMatrix":
         """inverse() :527-531 — toDenseVecMatrix().inverse()"""
@@ -342,13 +378,13 @@ class BlockMatrix(DistributedMatrix):
 
     def _local_dtype(self):
         for _, s in self.blocks:
-            return s.buf.dtype
+            return torch.float64 if s.isSparse else s.buf.dtype
         return torch.float64
 
     def _global_dtype(self):
         """Element type of the tiles, agreed by all ranks (a rank may hold no tile of this matrix)."""
         if getattr(self, "_gdtype", None) is None:
-            names = self._all_gather_meta([str(s.buf.dtype) for _, s in self.blocks[:1]])
+            names = self._all_gather_meta(["torch.float64" if s.isSparse else str(s.buf.dtype) for _, s in self.blocks[:1]])
             self._gdtype = {"torch.float64": torch.float64, "torch.bfloat16": torch.bfloat16,
                             "torch.float32": torch.float32}[names[0]] if names else torch.float64
         return self._gdtype
@@ -365,7 +401,8 @@ class BlockMatrix(DistributedMatrix):
             Bd = SubMatrix(B)
         if self.numBlksByCol() == 1:
             res = [(b, blk.multiply(Bd)) for b, blk in self.blocks]
-            return BlockMatrix(res, self.numRows(), b_cols, self.numBlksByRow(), self.numBlksByCol(), self._placement)
+            return BlockMatrix(res, self.numRows(), b_cols, self.numBlksByRow(), self.numBlksByCol(), self._placement,
+                               sparse=False)
         col_blk = _ceil_len(self.numCols(), self.numBlksByCol())
         acc: Dict[int, SubMatrix] = {}
         for b, blk in sorted(self.blocks, key=lambda t: (t[0].row, t[0].column)):
@@ -382,7 +419,7 @@ class BlockMatrix(DistributedMatrix):
         res = [(BlockID(r, 0), blk) for r, blk in sorted(acc.items())]
         # the reference reports numBlksByCol() although every key has column 0 (:301); kept
         return BlockMatrix(res, self.numRows(), b_cols, self.numBlksByRow(), self.numBlksByCol(),
-                           placement=(lambda r, c, s=self: s.owner(r, 0)) if ws > 1 else None)
+                           placement=(lambda r, c, s=self: s.owner(r, 0)) if ws > 1 else None, sparse=False)
 
     def _multiply_dist_vector(self, v):
         """multiply(v: DistributedVector) :240-259 — piece `id` of v meets every block of block column `id`
@@ -395,6 +432,7 @@ class BlockMatrix(DistributedMatrix):
                                           f"{self.numCols()} v.s {v.length}")
         if self.numBlksByCol() != v.splitNum:
             raise nat.MarlinArgumentError(nat.MB_ERR_UNSUPPORTED, "not supported matrix or vector")
+        self._no_sparse_vector()
         pieces = v._replicated()
         acc: Dict[int, SubMatrix] = {}
         for b, blk in sorted(self.blocks, key=lambda t: (t[0].row, t[0].column)):
@@ -417,9 +455,16 @@ class BlockMatrix(DistributedMatrix):
                                           f"matrix columns size {self.numCols()} not support vector length {v.shape[0]}")
         if self.numBlksByCol() != 1:
             raise nat.MarlinArgumentError(nat.MB_ERR_UNSUPPORTED, "should not split the matrix by column")
+        self._no_sparse_vector()
         x = SubMatrix(v.reshape(-1, 1))
         res = [(b.row, blk.multiply(x)) for b, blk in sorted(self.blocks, key=lambda t: t[0].row)]
         return DistributedVector(res, self.numRows(), self.numBlksByRow(), placement=lambda i, s=self: s.owner(i, 0))
+
+    def _no_sparse_vector(self) -> None:
+        """SubMatrix.multiply(v: Vector) (matrix/SubMatrix.scala:131-139) with a sparse block."""
+        if self._has_sparse():
+            raise nat.MarlinArgumentError(nat.MB_ERR_UNSUPPORTED, "Not supported multiply-operator between matrices sparsity "
+                                          "with true and vector: class edu.nju.pasalab.marlin.matrix.DenseVector")
 
     def multiplyBy(self, B) -> "BlockMatrix":
         """multiplyBy(B: BDM[Double]) :309-335 — a small local matrix times this block matrix (B replicated on every
@@ -439,7 +484,8 @@ class BlockMatrix(DistributedMatrix):
         if self.numBlksByRow() == 1:
             res = [(b, Bd.multiply(blk)) for b, blk in self.blocks]                       # :315-319
             # the reference labels the result numRows() x B.cols (:319); the data is B.rows x numCols()
-            return BlockMatrix(res, Bd.rows, self.numCols(), self.numBlksByRow(), self.numBlksByCol(), self._placement)
+            return BlockMatrix(res, Bd.rows, self.numCols(), self.numBlksByRow(), self.numBlksByCol(), self._placement,
+                               sparse=False)
         row_blk = _ceil_len(self.numRows(), self.numBlksByRow())
         res = []
         for b, blk in self.blocks:
@@ -449,7 +495,8 @@ class BlockMatrix(DistributedMatrix):
                 raise nat.MarlinArgumentError(nat.MB_ERR_INVALID_ARG, f"multiplyBy: column range {start} until {end} of the local "
                                               f"matrix is out of bounds ({Bd.cols} columns)")
             res.append((b, Bd.slice(0, Bd.rows, start, end).multiply(blk)))                               # :330-331
-        return BlockMatrix(res, Bd.rows, self.numCols(), self.numBlksByRow(), self.numBlksByCol(), self._placement)
+        return BlockMatrix(res, Bd.rows, self.numCols(), self.numBlksByRow(), self.numBlksByCol(), self._placement,
+                           sparse=False)
 
     def _reduce_row_partials(self, acc: Dict[int, SubMatrix]) -> Dict[int, SubMatrix]:
         """reduceByKey over column blocks held by different ranks (:300): partials go to owner(row, 0)."""
@@ -482,7 +529,7 @@ class BlockMatrix(DistributedMatrix):
         f = {"add": lambda s: s.add(b), "subtract": lambda s: s.subtract(b), "multiply": lambda s: s.multiply(b),
              "divide": lambda s: s.divide(b), "subtractBy": lambda s: s.subtractBy(b), "divideBy": lambda s: s.divideBy(b)}[op]
         return BlockMatrix([(k, f(v)) for k, v in self.blocks], self.numRows(), self.numCols(), self.numBlksByRow(),
-                           self.numBlksByCol(), self._placement)
+                           self.numBlksByCol(), self._placement, sparse=self._sparse_flag)
 
     def _binary(self, other, op: str):
         from .dense_vec_matrix import DenseVecMatrix
@@ -490,6 +537,9 @@ class BlockMatrix(DistributedMatrix):
             return self._scalar(op, float(other))
         if self.numRows() != other.numRows() or self.numCols() != other.numCols():
             raise nat.MarlinArgumentError(nat.MB_ERR_DIM_MISMATCH, "matrix dimension mismatch")
+        self._dense_only(op)
+        if isinstance(other, BlockMatrix):
+            other._dense_only(op)
         if isinstance(other, DenseVecMatrix):                                  # :346-349
             return getattr(self.toDenseVecMatrix(), op)(other)
         if self.numBlksByRow() != other.numBlksByRow() or self.numBlksByCol() != other.numBlksByCol():
@@ -520,7 +570,8 @@ class BlockMatrix(DistributedMatrix):
                 theirs[key] = SubMatrix(buf=buf, rows=p.rows, cols=p.cols, ld=max(1, p.rows))
         fn = {"add": SubMatrix.add, "subtract": SubMatrix.subtract, "dotProduct": SubMatrix.elementMultiply}[op]
         res = [(b, fn(s, theirs[(b.row, b.column)])) for b, s in self.blocks if (b.row, b.column) in theirs]
-        return BlockMatrix(res, self.numRows(), self.numCols(), self.numBlksByRow(), self.numBlksByCol(), self._placement)
+        return BlockMatrix(res, self.numRows(), self.numCols(), self.numBlksByRow(), self.numBlksByCol(), self._placement,
+                           sparse=False)
 
     def add(self, other):
         """add(other: DistributedMatrix) :344-360, add(b: Double) :368-371"""
@@ -546,6 +597,7 @@ class BlockMatrix(DistributedMatrix):
 
     def sum(self) -> float:
         """:467-472"""
+        self._dense_only("sum")
         parts = self._all_gather_meta([s.sum() for _, s in self.blocks])
         if not parts:
             raise nat.MarlinError(nat.MB_ERR_EMPTY, "empty collection")
@@ -556,20 +608,23 @@ class BlockMatrix(DistributedMatrix):
 
     def transpose(self) -> "BlockMatrix":
         """:514-523 — per-block materialised transpose, key (r, c) -> (c, r); no data leaves its GPU."""
+        self._dense_only("transpose")
         res = [(BlockID(b.column, b.row), s.transpose()) for b, s in self.blocks]
         return BlockMatrix(res, self.numCols(), self.numRows(), self.numBlksByCol(), self.numBlksByRow(),
-                           placement=lambda r, c, s=self: s.owner(c, r))
+                           placement=lambda r, c, s=self: s.owner(c, r), sparse=False)
 
     # ------------------------------------------------------------------ conversions
     def toDenseVecMatrix(self):
         """:575-594 — blocks -> rows.  Rows of block-row r are assembled on owner(r, 0)."""
         from .dense_vec_matrix import DenseVecMatrix
+        self._dense_only("toDenseVecMatrix")
         return DenseVecMatrix._from_block_matrix(self)
 
     def toBlockMatrix(self, newNumByRow: int, newNumByCol: int) -> "BlockMatrix":
         """:610-665 — re-grid.  Pieces are cut as views, shipped once, and pasted into the new blocks."""
         if self._blksByRow == newNumByRow and self._blksByCol == newNumByCol:
             return self
+        self._dense_only("toBlockMatrix (re-grid)")
         nr, nc = self.numRows(), self.numCols()
         rl, cl = _ceil_len(nr, self.numBlksByRow()), _ceil_len(nc, self.numBlksByCol())
         nrl, ncl = _ceil_len(nr, newNumByRow), _ceil_len(nc, newNumByCol)
@@ -622,12 +677,13 @@ class BlockMatrix(DistributedMatrix):
                 piece = SubMatrix(buf=got[key], rows=r, cols=c, ld=max(1, r))
             new_blocks[(nrow, ncol)].slice(r0, r1, c0, c1).assign(piece)
         res = [(BlockID(r, c), blk) for (r, c), blk in sorted(new_blocks.items())]
-        return BlockMatrix(res, nr, nc, new_br, new_bc)
+        return BlockMatrix(res, nr, nc, new_br, new_bc, sparse=False)
 
     # ------------------------------------------------------------------ I/O (next-row (f)-3)
     def saveToFileSystem(self, path: str, format: str = " ") -> None:
         """:550-559 — "blockmatrix": `row-col-rows-cols:v,v,...` column-major; else DenseVecMatrix format."""
         from ..utils.mt_utils import _jdouble
+        self._dense_only("saveToFileSystem")
         if format.lower() == "blockmatrix":
             lines = []
             for b, s in self.blocks:

@@ -231,7 +231,7 @@ class DenseVecMatrix(DistributedMatrix):
         from .block_matrix import BlockMatrix
         rank, ws = world()
         owner = lambda r, c: comm.elem_owner(r, c, nb, ws)
-        return BlockMatrix(fz.block_pairs(blocks, owner, rank), n, n, nb, nb)
+        return BlockMatrix(fz.block_pairs(blocks, owner, rank), n, n, nb, nb, sparse=False)
 
     def luDecompose(self, mode: str = "auto", baseSize: Optional[int] = None, keepUnfactoredDiagonal: bool = False):
         """luDecompose(mode) :283-466 -> (BlockMatrix holding L (unit lower) and U packed, permutation array: row i of
@@ -472,7 +472,7 @@ class DenseVecMatrix(DistributedMatrix):
                 piece = SubMatrix(buf=got[key], rows=take, cols=width, ld=max(1, take))
             blocks[(br, bc)].slice(r0, r0 + take, 0, width).assign(piece)
         res = [(BlockID(r, c), blk) for (r, c), blk in sorted(blocks.items())]
-        return BlockMatrix(res, mRows, mCols, by_row, by_col)
+        return BlockMatrix(res, mRows, mCols, by_row, by_col, sparse=False)
 
     def toBlocks(self, m: int, k: int, n: int, mode: str):
         """:1084-1223 — the blocks of toBlockMatrix plus the seq replication keys; on GPUs the replicas are the

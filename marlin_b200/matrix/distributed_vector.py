@@ -170,7 +170,7 @@ class DistributedVector:
                     rt.sync_stream()
                     nat.check(rt.lib.mb_block_ger(rt.ctx, x.handle(), y.handle(), blk.handle()))
                     blocks.append((BlockID(i, j), blk))
-            return BlockMatrix(blocks, self.length, self.length, s, s)
+            return BlockMatrix(blocks, self.length, self.length, s, s, sparse=False)
         if not self.columnMajor and other.columnMajor:
             m = mode.lower()
             if m == "dist":

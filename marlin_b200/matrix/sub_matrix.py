@@ -3,7 +3,9 @@
 The reference's SubMatrix wraps a Breeze DenseMatrix[Double] on the JVM heap; here the same
 (data, offset, rows, cols, majorStride, isTranspose) record points into HBM.  The buffer is a torch
 tensor only so that torch.distributed (NCCL) can move it; every arithmetic method calls the C ABI
-of libmarlin_b200.so (the kernel seam named in SURVEY.md §2 #3).  Sparse blocks are out of scope.
+of libmarlin_b200.so (the kernel seam named in SURVEY.md §2 #3).  A sparse block (`SubMatrix(spMatrix=...)`) holds a
+device CSC block instead (sparse_matrix.SparseBlock); multiply dispatches the four sparsity pairs as the reference does
+(:87-119) and the scalar ops change only the stored values (:52-58, 71-85, 121-129).
 """
 from __future__ import annotations
 
@@ -15,6 +17,7 @@ import torch
 
 from .. import _native as nat
 from ..runtime import Runtime
+from .sparse_matrix import SparseBlock, SparseMatrix
 
 _TORCH_DTYPE = {nat.MB_F64: torch.float64, nat.MB_BF16: torch.bfloat16, nat.MB_F32: torch.float32}
 _MB_DTYPE = {v: k for k, v in _TORCH_DTYPE.items()}
@@ -26,9 +29,19 @@ class SubMatrix:
     """A dense block.  Element (r, c) = buf.flatten()[offset + r + c*ld] (or [offset + c + r*ld] if
     is_transpose), exactly Breeze's DenseMatrix indexing."""
 
-    def __init__(self, denseMatrix=None, *, buf: Optional[torch.Tensor] = None, rows: int = 0, cols: int = 0,
+    def __init__(self, denseMatrix=None, *, spMatrix: Optional[SparseMatrix] = None, sparse: Optional[SparseBlock] = None,
+                 buf: Optional[torch.Tensor] = None, rows: int = 0, cols: int = 0,
                  ld: Optional[int] = None, offset: int = 0, is_transpose: bool = False, device=None):
         self._handle = None
+        self._sparse: Optional[SparseBlock] = None
+        if spMatrix is not None:
+            sparse = SparseBlock.from_host(spMatrix.numRows, spMatrix.numCols, *spMatrix.to_csc(), device=device)
+        if sparse is not None:
+            self._sparse = sparse
+            self.buf = None
+            self._rows, self._cols = sparse.rows, sparse.cols
+            self.ld, self.offset, self.is_transpose = max(1, sparse.rows), 0, False
+            return
         if denseMatrix is not None:
             if isinstance(denseMatrix, SubMatrix):
                 src = denseMatrix
@@ -79,24 +92,47 @@ class SubMatrix:
 
     @property
     def isSparse(self) -> bool:
-        return False
+        return self._sparse is not None
+
+    @property
+    def sparseBlock(self) -> SparseBlock:
+        if self._sparse is None:
+            raise nat.MarlinArgumentError(nat.MB_ERR_UNSUPPORTED, "sparseBlock of a dense block")
+        return self._sparse
 
     @property
     def denseBlock(self) -> "SubMatrix":
+        self._dense_only("denseBlock")
         return self
+
+    def _dense_only(self, what: str) -> None:
+        if self._sparse is not None:
+            raise nat.MarlinArgumentError(nat.MB_ERR_UNSUPPORTED, f"{what} is not supported on sparse blocks: call "
+                                          "toDenseBlocks first")
+
+    def toDense(self) -> "SubMatrix":
+        """SparseMatrix.toDense (Matrices.scala:106-119) as a packed column-major block; a dense block is returned as is."""
+        if self._sparse is None:
+            return self
+        rt = Runtime.get(); rt.sync_stream()
+        out = SubMatrix.empty(self._rows, self._cols, nat.MB_F64, self._sparse.values.device)
+        nat.check(rt.lib.mb_sparse_to_dense(rt.ctx, self._sparse.handle(), out.handle()))
+        return out
 
     @property
     def dtype(self) -> int:
-        return _MB_DTYPE[self.buf.dtype]
+        return nat.MB_F64 if self._sparse is not None else _MB_DTYPE[self.buf.dtype]
 
     @property
     def t(self) -> "SubMatrix":
         """Breeze `.t`: a transposed view, no copy."""
+        self._dense_only("transpose")
         return SubMatrix(buf=self.buf, rows=self._cols, cols=self._rows, ld=self.ld, offset=self.offset,
                          is_transpose=not self.is_transpose)
 
     def slice(self, r0: int, r1: int, c0: int, c1: int) -> "SubMatrix":
         """Breeze `m(r0 until r1, c0 until c1)`: a view with the parent's majorStride (BlockMatrix.scala:198,299)."""
+        self._dense_only("slice")
         if not (0 <= r0 <= r1 <= self._rows and 0 <= c0 <= c1 <= self._cols):
             raise ValueError("slice out of range")
         rs, cs = (self.ld, 1) if self.is_transpose else (1, self.ld)
@@ -104,10 +140,12 @@ class SubMatrix:
                          is_transpose=self.is_transpose)
 
     def is_packed(self) -> bool:
-        return (not self.is_transpose) and self.offset == 0 and self.ld == max(1, self._rows)
+        return self._sparse is None and (not self.is_transpose) and self.offset == 0 and self.ld == max(1, self._rows)
 
     # ---- native handle ----
     def handle(self):
+        """The dense block handle; every dense-only operation goes through here."""
+        self._dense_only("this operation")
         if self._handle is None:
             if not self.buf.is_cuda:
                 raise nat.MarlinError(nat.MB_ERR_CUDA, "block lives in host memory: marlin_b200 computes on H100 only "
@@ -126,7 +164,7 @@ class SubMatrix:
         """Record that everything queued so far on the current stream produces this block's FINAL contents (blocks are
         immutable values, like the blocks of a cached RDD): the multi-GPU multiply then offers the block to other ranks as
         soon as this event completes instead of after all later work on the stream (see mb_block_set_ready_event)."""
-        if self.buf.is_cuda:
+        if self.buf is not None and self.buf.is_cuda:
             ev = torch.cuda.Event()
             ev.record(torch.cuda.current_stream(self.buf.device))
             self._ready_event = ev
@@ -157,7 +195,28 @@ class SubMatrix:
         return SubMatrix.empty(rows, cols, dtype, self.buf.device)
 
     # ---- arithmetic (matrix/SubMatrix.scala:41-139) ----
+    def _values_block(self) -> "SubMatrix":
+        """The stored values of a sparse block as an nnz x 1 dense block."""
+        v = self._sparse.values
+        return SubMatrix(buf=v, rows=v.numel(), cols=1, ld=max(1, v.numel()))
+
+    def _sparse_values_op(self, op) -> "SubMatrix":
+        """A scalar op on a sparse block: the reference maps only the stored values (:52-58, 71-85, 121-129), so the
+        result keeps the pattern (a sparse block plus 1 is not A + 1).  Runs the dense element-wise kernel on them."""
+        vals = self._values_block()
+        res = op(vals) if vals.rows else vals
+        return SubMatrix(sparse=self._sparse.with_values(res.buf if vals.rows else self._sparse.values.clone()))
+
+    def _check_both_dense(self, other: "SubMatrix", opname: str) -> None:
+        if self.isSparse or other.isSparse:
+            raise nat.MarlinArgumentError(nat.MB_ERR_UNSUPPORTED, f"Not supported {opname}-operator between matrices of "
+                                          f"sparsity with {str(self.isSparse).lower()} and {str(other.isSparse).lower()}")
+
     def add(self, other: Union["SubMatrix", Number]) -> "SubMatrix":
+        if isinstance(other, SubMatrix):
+            self._check_both_dense(other, "add")
+        elif self.isSparse:
+            return self._sparse_values_op(lambda v: v.add(other))
         rt = Runtime.get(); rt.sync_stream()
         out = self._new_like()
         if isinstance(other, SubMatrix):
@@ -167,6 +226,10 @@ class SubMatrix:
         return out
 
     def subtract(self, other: Union["SubMatrix", Number]) -> "SubMatrix":
+        if isinstance(other, SubMatrix):
+            self._check_both_dense(other, "subtract")
+        elif self.isSparse:
+            return self._sparse_values_op(lambda v: v.subtract(other))
         rt = Runtime.get(); rt.sync_stream()
         out = self._new_like()
         if isinstance(other, SubMatrix):
@@ -176,6 +239,8 @@ class SubMatrix:
         return out
 
     def divide(self, b: Number) -> "SubMatrix":
+        if self.isSparse:
+            return self._sparse_values_op(lambda v: v.divide(b))
         rt = Runtime.get(); rt.sync_stream()
         out = self._new_like()
         nat.check(rt.lib.mb_block_div(rt.ctx, self.handle(), float(b), 0, out.handle()))               # :79-85
@@ -208,14 +273,33 @@ class SubMatrix:
 
     def multiply(self, other, out: Optional["SubMatrix"] = None, accumulate: bool = False,
                  out_dtype: Optional[int] = None) -> "SubMatrix":
-        """:87-111 (block x block, block x local matrix) and :123-131 (scalar)."""
+        """:87-111 (block x block, block x local matrix) and :123-131 (scalar).  With a sparse side the product is dense:
+        multDenseSparse, multSparseDense (the true product; the reference's loop is right only for K, N <= 32) or
+        SparseMatrix.multiply, each summed in the reference's order (see include/marlin_b200.h)."""
         rt = Runtime.get(); rt.sync_stream()
         if isinstance(other, (int, float)):
+            if self.isSparse:
+                return self._sparse_values_op(lambda v: v.multiply(float(other)))
             res = self._new_like()
             nat.check(rt.lib.mb_block_axpb(rt.ctx, self.handle(), float(other), 0.0, res.handle()))
             return res
         if not isinstance(other, SubMatrix):
-            other = SubMatrix(other, device=self.buf.device)
+            other = SubMatrix(other, device=self.device)
+        if self.isSparse or other.isSparse:
+            if out is None:
+                if accumulate:
+                    raise ValueError("accumulate needs an output block")
+                out = SubMatrix.empty(self._rows, other._cols, nat.MB_F64, self.device)
+            if self.isSparse and other.isSparse:
+                nat.check(rt.lib.mb_spgemm_dense_out(rt.ctx, self._sparse.handle(), other._sparse.handle(), out.handle(),
+                                                     int(accumulate)))
+            elif self.isSparse:
+                nat.check(rt.lib.mb_spmm_sparse_dense(rt.ctx, self._sparse.handle(), other.handle(), out.handle(),
+                                                      int(accumulate)))
+            else:
+                nat.check(rt.lib.mb_spmm_dense_sparse(rt.ctx, self.handle(), other._sparse.handle(), out.handle(),
+                                                      int(accumulate)))
+            return out
         if out is None:
             if accumulate:
                 raise ValueError("accumulate needs an output block")
@@ -327,10 +411,16 @@ class SubMatrix:
         return float(out.value)
 
     # ---- host transfer (toBreeze / collect) ----
+    @property
+    def device(self):
+        return self._sparse.values.device if self._sparse is not None else self.buf.device
+
     def toBreeze(self) -> np.ndarray:
-        """Download as a (rows x cols) Fortran-ordered float64 ndarray."""
+        """Download as a (rows x cols) Fortran-ordered float64 ndarray (a sparse block through toDense)."""
         if self._rows == 0 or self._cols == 0:
             return np.zeros((self._rows, self._cols), order="F")
+        if self._sparse is not None:
+            return self.toDense().toBreeze()
         if self.buf.is_cuda:
             blk = self if (self.is_packed() and self.dtype == nat.MB_F64) else self.copy(nat.MB_F64)
             flat = blk.buf[: self._rows * self._cols].cpu().numpy()
@@ -345,6 +435,8 @@ class SubMatrix:
     to_numpy = toBreeze
 
     def __repr__(self):
+        if self._sparse is not None:
+            return f"SubMatrix({self._rows}x{self._cols}, sparse, nnz={self._sparse.nnz}, {self.device})"
         return f"SubMatrix({self._rows}x{self._cols}, ld={self.ld}, t={self.is_transpose}, {self.buf.dtype}, {self.buf.device})"
 
 

@@ -21,6 +21,7 @@ from .. import comm
 from ..matrix.block import BlockID
 from ..matrix.block_matrix import BlockMatrix
 from ..matrix.dense_vec_matrix import DenseVecMatrix
+from ..matrix.sparse_matrix import SparseBlock, column_count
 from ..matrix.sub_matrix import SubMatrix
 from ..runtime import Runtime, world
 
@@ -85,6 +86,14 @@ class MTUtils:
         rt = Runtime.get(); rt.sync_stream()
         nat.check(rt.lib.mb_fill_uniform(rt.ctx, blk.handle(), partition_seed, first, dist.start, dist.end, int(row_major)))
 
+    @staticmethod
+    def _sparse_block(rows: int, cols: int, density: float, partition_seed: int) -> SubMatrix:
+        s = column_count(rows, cols, density)
+        blk = SparseBlock.empty(rows, cols, s * cols)
+        rt = Runtime.get(); rt.sync_stream()
+        nat.check(rt.lib.mb_fill_sparse_uniform(rt.ctx, blk.handle(), partition_seed))
+        return SubMatrix(sparse=blk)
+
     # ------------------------------------------------------------------ generators
     @staticmethod
     def randomDenVecMatrix(sc, nRows: int, nColumns: int, numPartitions: int = 0,
@@ -125,9 +134,20 @@ class MTUtils:
                           distribution: Optional[UniformGenerator] = None, seed: Optional[int] = None,
                           dtype: int = nat.MB_F64) -> BlockMatrix:
         """utils/MTUtils.scala:34-50 -> RandomBlockRDD (rdd/RandomRDD.scala:184-223): one partition per block in
-        row-major BlockID order, `BDM.create(rows, cols, Array.fill(rows*cols)(nextValue()))` (column-major)."""
-        if sparseInfo[0]:
-            raise nat.MarlinArgumentError(nat.MB_ERR_UNSUPPORTED, "sparse blocks are out of scope")
+        row-major BlockID order, `BDM.create(rows, cols, Array.fill(rows*cols)(nextValue()))` (column-major).
+
+        sparseInfo = (True, density): sparse blocks (SparseMatrix.rand, Matrices.scala:157-173) with
+        s = (int)(block cols * density) U[0,1) values in every column.  The reference draws them from unseeded generators,
+        so its blocks change on every run; here block b is a function of (seed, b) alone: its values are positions
+        [0, s*cols) of the same XORShift stream the dense generator gives that block, and its rows come from selection
+        sampling over the next rows*cols positions (mb_fill_sparse_uniform).  density <= 0 and s > block rows are
+        rejected; so is a `distribution`, which the reference ignores for sparse blocks."""
+        sparse, density = bool(sparseInfo[0]), float(sparseInfo[1])
+        if sparse and distribution is not None:
+            raise nat.MarlinArgumentError(nat.MB_ERR_INVALID_ARG, "sparse blocks always draw U[0,1) values: the "
+                                          "`distribution` argument is not supported with sparseInfo")
+        if sparse and dtype != nat.MB_F64:
+            raise nat.MarlinArgumentError(nat.MB_ERR_UNSUPPORTED, "sparse blocks are fp64 only")
         dist_ = distribution or UniformGenerator(0.0, 1.0)
         brs = int(math.ceil(float(nRows) / float(numByRow)))
         bcs = int(math.ceil(float(nColumns) / float(numByCol)))
@@ -136,23 +156,35 @@ class MTUtils:
             seed = time.time_ns()
         seeds = MTUtils._partition_seeds(seed, by_row * by_col)
         rank, ws = world()
-        blocks = []
-        for idx in range(by_row * by_col):
-            i, j = divmod(idx, by_col)
-            if comm.elem_owner(i, j, by_col, ws) != rank:
-                continue
+
+        def shape(idx: int) -> Tuple[int, int]:
             rows = brs
             if idx >= (by_row - 1) * by_col and brs * by_row > nRows:
                 rows = nRows - brs * (by_row - 1)
             cols = bcs
             if (idx + 1) % by_col == 0 and bcs * by_col > nColumns:
                 cols = nColumns - bcs * (by_col - 1)
+            return rows, cols
+
+        if sparse:
+            # every rank checks every block shape (pure host logic) before any generates, so all raise together
+            for rows, cols in sorted({shape(idx) for idx in range(by_row * by_col)}):
+                column_count(rows, cols, density)
+        blocks = []
+        for idx in range(by_row * by_col):
+            i, j = divmod(idx, by_col)
+            if comm.elem_owner(i, j, by_col, ws) != rank:
+                continue
+            rows, cols = shape(idx)
+            if sparse:
+                blocks.append((BlockID(i, j), MTUtils._sparse_block(rows, cols, density, seeds[idx])))
+                continue
             blk = SubMatrix.empty(rows, cols, nat.MB_F64)
             MTUtils._fill(blk, seeds[idx], 0, dist_, row_major=False)
             if dtype != nat.MB_F64:
                 blk = blk.copy(dtype)
             blocks.append((BlockID(i, j), blk.mark_ready()))
-        return BlockMatrix(blocks, nRows, nColumns, by_row, by_col)
+        return BlockMatrix(blocks, nRows, nColumns, by_row, by_col, sparse=sparse)
 
     @staticmethod
     def randomDistVector(sc, length: int, numSplits: int, distribution: Optional[UniformGenerator] = None,
@@ -270,4 +302,4 @@ class MTUtils:
             dist.all_gather_object(keys, [(b.row, b.column) for b, _ in blocks])
             table = {k: r for r, ks in enumerate(keys) for k in ks}
             placement = lambda r, c, t=table: t[(r, c)]
-        return BlockMatrix(blocks, placement=placement)
+        return BlockMatrix(blocks, placement=placement, sparse=False)

@@ -57,6 +57,21 @@ object Native {
   @native def svdRank(sigmas: Array[Double], k: Int, rCond: Double): Int
   @native def trsm(ctx: Long, t: Long, lower: Boolean, unitDiagonal: Boolean, b: Long): Unit
 
+  // sparse blocks: a CSC block in HBM (SparseMatrix / LibMatrixMult / SparseMatrix.rand on the device)
+  @native def sparseUpload(ctx: Long, rows: Int, cols: Int, colptr: Array[Int], rowidx: Array[Int],
+                           values: Array[Double]): Long
+  @native def sparseDownload(ctx: Long, sp: Long, colptr: Array[Int], rowidx: Array[Int], values: Array[Double]): Unit
+  @native def sparseNnz(sp: Long): Long
+  @native def sparseAlloc(ctx: Long, rows: Int, cols: Int, nnz: Long): Long
+  @native def sparseFree(ctx: Long, sp: Long): Unit
+  @native def sparseValuesOp(ctx: Long, sp: Long, op: Int, b: Double): Long // 0 add, 1 subtract, 2 multiply, 3 divide
+  @native def sparseToDense(ctx: Long, sp: Long, out: Long): Unit
+  @native def spmmDenseSparse(ctx: Long, a: Long, b: Long, c: Long, accumulate: Boolean): Unit
+  @native def spmmSparseDense(ctx: Long, a: Long, b: Long, c: Long, accumulate: Boolean): Unit
+  @native def spgemm(ctx: Long, a: Long, b: Long, c: Long, accumulate: Boolean): Unit
+  @native def sparseColumnCount(rows: Int, cols: Int, density: Double): Int
+  @native def fillSparseUniform(ctx: Long, sp: Long, partitionSeed: Long): Unit
+
   // whole multiplies on one GPU
   @native def matmulBlocked(ctx: Long, aTiles: Array[Long], bTiles: Array[Long], m: Int, k: Int, n: Int,
                             cTiles: Array[Long]): Unit

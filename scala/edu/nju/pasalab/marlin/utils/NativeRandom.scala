@@ -29,6 +29,17 @@ private[marlin] object NativeRandom {
     new SubMatrix(blk, vectorSize, size).t                             // seen as size x vectorSize, no copy
   }
 
+  /** A sparse block of `MTUtils.randomBlockMatrix(..., sparseInfo = (true, density))` (RandomRDD.scala:97-99,
+   *  SparseMatrix.rand, Matrices.scala:157-173), seeded: s = (blockCols * density).toInt rows per column (density <= 0
+   *  and s > blockRows are IllegalArgumentException), values from the block's partition stream, rows by selection
+   *  sampling (mb_fill_sparse_uniform). */
+  def sparseBlock(partitionSeed: Long, blockRows: Int, blockCols: Int, density: Double): SubMatrix = {
+    val s = Native.sparseColumnCount(blockRows, blockCols, density)
+    val sp = Native.sparseAlloc(Ctx.get, blockRows, blockCols, s.toLong * blockCols)
+    Native.fillSparseUniform(Ctx.get, sp, partitionSeed)
+    new SubMatrix(0L, blockRows, blockCols, sp)
+  }
+
   /** Seeds of the `numPartitions` partitions of a RandomRDD built with `seed` (rdd/RandomRDD.scala:28-45). */
   def partitionSeeds(seed: Long, numPartitions: Int): Array[Long] = Native.partitionSeeds(seed, numPartitions)
 

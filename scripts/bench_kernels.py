@@ -1,6 +1,6 @@
 """Secondary kernel benchmarks (1 GPU): HBM-bound block kernels vs the measured copy bandwidth, and the bf16 wgmma
 GEMM vs cuBLAS, layout conversion, factorizations and the SVD.  Prints one JSON document; bench.py stays the headline
-(fp64 multiply).  `svd` as an argument runs the f5_svd section only."""
+(fp64 multiply).  `svd` as an argument runs the f5_svd section only, `sparse` the f6_sparse section only."""
 import ctypes as C
 import json
 import subprocess
@@ -39,9 +39,11 @@ def timeit(fn, iters=10, warm=3):
     return e0.elapsed_time(e1) / iters
 
 
+ONLY_SPARSE = "sparse" in sys.argv[1:]
 ONLY_SVD = "svd" in sys.argv[1:]
+SKIP_DENSE = ONLY_SVD or ONLY_SPARSE
 hbm = {}
-for n in (() if ONLY_SVD else (8192, 16384)):
+for n in (() if SKIP_DENSE else (8192, 16384)):
     A = mb.MTUtils.randomBlockMatrix(None, n, n, 1, 1, seed=1).blocks[0][1]
     B = mb.MTUtils.randomBlockMatrix(None, n, n, 1, 1, seed=2).blocks[0][1]
     O = mb.SubMatrix.empty(n, n)
@@ -90,7 +92,7 @@ for n in (() if ONLY_SVD else (8192, 16384)):
 out["hbm_kernels"] = hbm
 
 gemm = {}
-for n in (() if ONLY_SVD or "hbm" in sys.argv[1:] else (4096, 8192, 16384)):
+for n in (() if SKIP_DENSE or "hbm" in sys.argv[1:] else (4096, 8192, 16384)):
     A = mb.MTUtils.randomBlockMatrix(None, n, n, 1, 1, seed=3, dtype=nat.MB_BF16).blocks[0][1]
     B = mb.MTUtils.randomBlockMatrix(None, n, n, 1, 1, seed=4, dtype=nat.MB_BF16).blocks[0][1]
     Cm = mb.SubMatrix.empty(n, n, nat.MB_F32)
@@ -111,7 +113,7 @@ out["bf16_gemm"] = gemm
 
 # ---- f1: layout conversion on the device (rows -> blocks -> rows), 2 * 8 * M * N bytes per direction ----
 f1 = {}
-for (M_, N_, gr, gc) in (() if ONLY_SVD or "hbm" in sys.argv[1:] else ((16384, 16384, 2, 2), (1048576, 1024, 8, 1))):
+for (M_, N_, gr, gc) in (() if SKIP_DENSE or "hbm" in sys.argv[1:] else ((16384, 16384, 2, 2), (1048576, 1024, 8, 1))):
     D = mb.MTUtils.randomDenVecMatrix(None, M_, N_, numPartitions=1, seed=5)
     torch.cuda.synchronize()
     Bm = D.toBlockMatrix(gr, gc)
@@ -129,7 +131,7 @@ out["f1_layout_conversion"] = f1
 
 # ---- f4: factorizations of one block (recursive; the flops run in the DMMA GEMM) ----
 fac = {}
-for n in (() if ONLY_SVD or "hbm" in sys.argv[1:] else (4096, 8192)):
+for n in (() if SKIP_DENSE or "hbm" in sys.argv[1:] else (4096, 8192)):
     A = mb.MTUtils.randomBlockMatrix(None, n, n, 1, 1, seed=6).blocks[0][1]
     S = A.multiply(A.t)
     S.add_(mb.SubMatrix(torch.eye(n, dtype=torch.float64).mul_(float(n)).numpy(), device=rt.device))
@@ -144,7 +146,7 @@ out["f4_factorizations"] = fac
 
 # ---- f5: DenseVecMatrix.computeSVD — split-K DMMA Gramian, Jacobi eigensolver, end to end ----
 f5 = {}
-if "hbm" not in sys.argv[1:]:
+if "hbm" not in sys.argv[1:] and not ONLY_SPARSE:
     smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i",
                           str(rt.device_index)], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     f5["device"] = {"torch_name": torch.cuda.get_device_name(rt.device_index), "nvidia_smi": smi.stdout.strip()}
@@ -216,6 +218,92 @@ if "hbm" not in sys.argv[1:]:
     del D, U
     torch.cuda.empty_cache()
 out["f5_svd"] = f5
+
+
+# ---- f6: sparse blocks — the three sparse products against DMMA on the same block made dense, the generator, and
+#      BlockMatrix.multiply in the reference's SparseMultiply modes.  The sparse kernels sum in the reference's order with
+#      separate multiplies and adds, so they are bound by memory traffic, not by the tensor cores. ----
+def timed(fn, budget_ms=1500.0):
+    """Mean ms per call: one warm-up call, then as many calls as fit in about budget_ms (at least one, at most 10)."""
+    fn()
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    fn()
+    torch.cuda.synchronize()
+    first = (time.perf_counter() - t0) * 1e3
+    iters = int(max(1, min(10, budget_ms / max(first, 1e-3))))
+    return timeit(fn, iters, 0) if iters > 1 else first
+
+
+f6 = {}
+if ONLY_SPARSE or not (ONLY_SVD or "hbm" in sys.argv[1:]):
+    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i",
+                          str(rt.device_index)], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
+    f6["device"] = {"torch_name": torch.cuda.get_device_name(rt.device_index), "nvidia_smi": smi.stdout.strip()}
+    densities = (1e-4, 1e-3, 1e-2, 5e-2, 0.1)
+    kernels = {}
+    for n in (4096, 16384):
+        D = mb.MTUtils.randomBlockMatrix(None, n, n, 1, 1, seed=21).blocks[0][1]
+        O = mb.SubMatrix.empty(n, n)
+        ms_dmma = timed(lambda: D.multiply(D, out=O))
+        per_n = {"dmma_dense_product_ms": ms_dmma, "by_density": {}}
+        for d in densities:
+            S = mb.MTUtils.randomBlockMatrix(None, n, n, 1, 1, (True, d), seed=22).blocks[0][1]
+            nnz = S.sparseBlock.nnz
+            s = nnz // n
+            sp_bytes = 12.0 * nnz
+            dense_io = 16.0 * n * n                                  # read the dense operand once, write C once
+            row = {"nnz": nnz}
+            for name, fn, flops, by in (
+                    ("dense_x_sparse", lambda: D.multiply(S, out=O), 2.0 * n * nnz, dense_io + sp_bytes),
+                    ("sparse_x_dense", lambda: S.multiply(D, out=O), 2.0 * n * nnz, dense_io + sp_bytes),
+                    ("sparse_x_sparse", lambda: S.multiply(S, out=O), 2.0 * nnz * s, 8.0 * n * n + 2 * sp_bytes)):
+                # the first call on a fresh block: for sparse x dense it includes building the cached CSR copy
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
+                fn()
+                torch.cuda.synchronize()
+                first_ms = (time.perf_counter() - t0) * 1e3
+                ms = timed(fn)
+                row[name] = {"ms": ms, "gflops": flops / ms / 1e6, "min_bytes": by, "GB/s_of_min_bytes": by / ms / 1e6,
+                             "speedup_vs_dmma": ms_dmma / ms, "first_call_ms": first_ms}
+            per_n["by_density"][str(d)] = row
+            del S
+            torch.cuda.empty_cache()
+        # crossover: the densities bracketing the point where the sparse kernel stops beating DMMA on the dense block
+        cross = {}
+        for name in ("dense_x_sparse", "sparse_x_dense", "sparse_x_sparse"):
+            for key, label in (("ms", ""), ("first_call_ms", "_first_call")):
+                wins = [d for d in densities if per_n["by_density"][str(d)][name][key] < ms_dmma]
+                loses = [d for d in densities if per_n["by_density"][str(d)][name][key] >= ms_dmma]
+                cross[name + label] = {"sparse_wins_up_to": max(wins) if wins else None,
+                                       "dmma_wins_from": min(loses) if loses else None}
+        per_n["crossover_density"] = cross
+        kernels[f"{n}^2"] = per_n
+        del D, O
+        torch.cuda.empty_cache()
+    f6["kernels"] = kernels
+    n = 16384
+    ms_gen = timed(lambda: mb.MTUtils.randomBlockMatrix(None, n, n, 1, 1, (True, 1e-3), seed=23))
+    ms_fill = timed(lambda: mb.MTUtils.randomBlockMatrix(None, n, n, 1, 1, seed=23))
+    f6["generator_16384^2"] = {"sparse_density_1e-3_ms": ms_gen, "dense_fill_ms": ms_fill,
+                               "note": "the sparse generator draws rows*cols stream positions whatever the density"}
+    modes = {}
+    d = 1e-3
+    Ad = mb.MTUtils.randomBlockMatrix(None, n, n, 2, 2, seed=24)
+    As = mb.MTUtils.randomBlockMatrix(None, n, n, 2, 2, (True, d), seed=25)
+    Bs = mb.MTUtils.randomBlockMatrix(None, n, n, 2, 2, (True, d), seed=26)
+    Asd, Bsd = As.toDenseBlocks(), Bs.toDenseBlocks()           # converted before the clock starts, as in the reference
+    for mode, fn in (("3_sparse_x_sparse", lambda: As.multiply(Bs)),
+                     ("4_dense_blocks_x_dense_blocks", lambda: Asd.multiply(Bsd)),
+                     ("5_dense_x_sparse", lambda: Ad.multiply(Bs)),
+                     ("6_dense_x_sparse_as_dense_blocks", lambda: Ad.multiply(Bsd))):
+        modes[mode] = {"ms": timed(lambda: (fn(), torch.cuda.synchronize()))}
+        torch.cuda.empty_cache()
+    f6[f"SparseMultiply_16384^2_2x2_density_{d}"] = modes
+    del Ad, As, Bs, Asd, Bsd
+    torch.cuda.empty_cache()
+out["f6_sparse"] = f6
 Path("gpurun_out").mkdir(exist_ok=True)
 Path("gpurun_out/kernels.json").write_text(json.dumps(out, indent=1))
 print(json.dumps(out, indent=1))
