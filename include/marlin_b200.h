@@ -110,7 +110,8 @@ int32_t mb_dgemm_host(mb_ctx* ctx, char transa, char transb, int32_t m, int32_t 
  * 7-bit digit planes per operand (Ozaki split; 2..8, 7 recommended): error <= ~K * 2^(-7*slices+2) relative to
  * rowmax(A) * colmax(B), i.e. well inside 1e-10 for well-scaled data but NOT an element-wise fp64 guarantee, hence
  * opt-in.  Products the split does not cover (transposed views, small blocks, K too large for exact int32
- * accumulation) silently use the native kernel. */
+ * accumulation) silently use the native kernel.  Rows of A / columns of B holding a NaN or Inf are left out of the split
+ * and their entries of C recomputed in plain fp64, so NaN / Inf propagate as with the native kernel. */
 #define MB_FP64_NATIVE      0
 #define MB_FP64_INT8_SPLIT  1   /* 7-bit digits (|d| <= 64):  P = 7*slices - 1 fractional bits, K*slices < 2^19  */
 #define MB_FP64_INT8_SPLIT8 2   /* 8-bit digits (|d| <= 128): P = 8*slices - 2 fractional bits, K*slices < 2^17;
@@ -184,7 +185,9 @@ int64_t mb_gramian_workspace_bytes(int64_t n, int64_t m, int32_t num_sms);
  * all n eigenvalues into the HOST array w_out, ordered by |w| descending (ties: lower index first) — what dgesdd returns
  * as singular values of a symmetric G — and the matching orthonormal eigenvectors as the columns of V (n x n).
  * sweeps_out (may be NULL) receives the number of Jacobi sweeps.  Blocking.  Takes 32 * N^2 bytes of temporary device
- * memory (N = n rounded up to even) for the duration of the call. */
+ * memory (N = n rounded up to even) for the duration of the call.  G is first scaled by the power of two that brings
+ * max|g| into [1, 2), so 2^k G gives V and the sweep count of G bit for bit and w * 2^k (while w * 2^k stays normal).
+ * A NaN or +-Inf in the lower triangle of G is MB_ERR_INVALID_ARG before any sweep runs (w_out and V unset). */
 int32_t mb_block_syev(mb_ctx* ctx, const mb_block* G, mb_block* V, double* w_out, int32_t* sweeps_out);
 /* The mode chooser and every `require` of computeSVD (:1565-1604) plus the column cap of computeGramianMatrix
  * (:1466-1468), with the reference's messages.  mode: "auto", "local-svd", "local-eigs" or "dist-eigs"; *compute_mode

@@ -44,6 +44,7 @@ __global__ void __launch_bounds__(GEMV_THREADS) gemv_n_kernel(const double* a, l
 #pragma unroll
             for (int u = 0; u < 8; ++u) {
                 const double t = xs[c + u];
+                if (t == 0.0) continue;            // dgemv 'N' skips x(j) = 0: an Inf / NaN in that column is not read
                 y0 = __dadd_rn(y0, __dmul_rn(t, v[u].x));
                 y1 = __dadd_rn(y1, __dmul_rn(t, v[u].y));
             }
@@ -51,6 +52,7 @@ __global__ void __launch_bounds__(GEMV_THREADS) gemv_n_kernel(const double* a, l
         for (; c < nc; ++c) {
             const double2 v = *reinterpret_cast<const double2*>(col + (long long)c * lda);
             const double t = xs[c];
+            if (t == 0.0) continue;
             y0 = __dadd_rn(y0, __dmul_rn(t, v.x));
             y1 = __dadd_rn(y1, __dmul_rn(t, v.y));
         }
@@ -66,9 +68,11 @@ __global__ void __launch_bounds__(GEMV_THREADS) gemv_n_kernel(const double* a, l
 #pragma unroll
                 for (int u = 0; u < 4; ++u) v[u] = col[(long long)(c + u) * lda + q];
 #pragma unroll
-                for (int u = 0; u < 4; ++u) y = __dadd_rn(y, __dmul_rn(xs[c + u], v[u]));
+                for (int u = 0; u < 4; ++u)
+                    if (xs[c + u] != 0.0) y = __dadd_rn(y, __dmul_rn(xs[c + u], v[u]));
             }
-            for (; c < nc; ++c) y = __dadd_rn(y, __dmul_rn(xs[c], col[(long long)c * lda + q]));
+            for (; c < nc; ++c)
+                if (xs[c] != 0.0) y = __dadd_rn(y, __dmul_rn(xs[c], col[(long long)c * lda + q]));
             out[q] = y;
         }
     }

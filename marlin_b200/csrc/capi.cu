@@ -1248,10 +1248,13 @@ int32_t mb_block_syev(mb_ctx* ctx, const mb_block* G, mb_block* V, double* w_out
     constexpr int MAX_SWEEPS = 30;
     int sweeps = 0;
     long long launches = 0;
+    bool non_finite = false;
     const cudaError_t e = mb::syev_jacobi(G->rows, f64_ptr(G), rs(G), cs(G), f64_ptr(V), rs(V), cs(V), w_out, &sweeps, MAX_SWEEPS,
-                                          ctx->stream, &launches);
+                                          ctx->stream, &launches, &non_finite);
     ctx->launches += launches;
     if (sweeps_out) *sweeps_out = sweeps;
+    if (e == cudaSuccess && non_finite)
+        return fail(MB_ERR_INVALID_ARG, "mb_block_syev: the matrix holds NaN or Inf (n = %d)", G->rows);
     if (e == cudaErrorNotReady)
         return fail(MB_ERR_NO_CONVERGENCE, "Jacobi eigensolver: no convergence after %d sweeps (n = %d)", MAX_SWEEPS, G->rows);
     if (e != cudaSuccess) return cuda_fail(e, "mb_block_syev");

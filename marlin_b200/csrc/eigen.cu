@@ -2,11 +2,14 @@
 // reference hands to LAPACK (brzSvd = dgesdd of the Gramian) or ARPACK (symmetricEigs, :1725-1834).
 //
 // Parallel cyclic two-sided Jacobi on a working copy of G (n padded to even N with a zero row / column):
+//   * the copy is G times the power of two that brings max|g| into [1, 2) (an order-independent max reduction finds it;
+//     a NaN or Inf in G is reported before any sweep), and the eigenvalues are scaled back exactly at the end: 2^k G runs
+//     exactly the sweeps of G, and no product of two entries overflows or flushes the threshold below to zero;
 //   * round-robin ordering: position 2a and 2a+1 form pair a.  A round rotates all N/2 pairs at once; between rounds the
 //     positions move by the circle method (position 0 fixed, the others on one cycle of length N-1), so a sweep of N-1
 //     rounds meets every index pair once and ends with every index back at its own position;
 //   * one kernel per round (jacobi_round_kernel): every CTA computes the rotations (Rutishauser's stable formulas, skipped
-//     when |g_pq| <= eps * sqrt(|g_pp g_qq|)) of the pairs it touches from the round's input, then updates its 2x2 blocks
+//     when |g_pq| <= eps * sqrt|g_pp| * sqrt|g_qq|) of the pairs it touches from the round's input, then updates its 2x2 blocks
 //     G_ab <- R_a^T G_ab R_b and the column pairs V_b <- V_b R_b, storing them to their next-round positions in the other
 //     buffer of a ping-pong pair;
 //   * every element of G_ab is a four-term sum taken in an order that is the same for G_ba, with rounding fixed
@@ -19,6 +22,7 @@
 #include <algorithm>
 #include <cfloat>
 #include <cmath>
+#include <cstring>
 #include <numeric>
 #include <vector>
 
@@ -38,13 +42,30 @@ __device__ __forceinline__ int next_pos(int p, int m) {
     return a == 0 ? 2 : 2 * (a - 1) + 1;       // bot[0] -> top[1], bot[a] -> bot[a-1]
 }
 
+// *maxbits = max over the lower triangle of the bit pattern of |g|.  Non-negative doubles order like their bit patterns and
+// NaN (any payload, sign cleared) lies above +Inf, so the result is max|g|, or +Inf / NaN when G holds one; an integer
+// max is the same whatever order the atomics land in.
+__global__ void __launch_bounds__(256) jacobi_maxabs_kernel(const double* __restrict__ G, long long rs, long long cs, int n,
+                                                            unsigned long long* __restrict__ maxbits) {
+    const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    unsigned long long b = 0;
+    if (e < (long long)n * n) {
+        const int i = (int)(e % n), j = (int)(e / n);
+        if (i >= j) b = (unsigned long long)__double_as_longlong(fabs(G[i * rs + j * cs]));
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) b = max(b, __shfl_xor_sync(0xffffffffu, b, o));
+    if ((threadIdx.x & 31) == 0 && b) atomicMax(maxbits, b);
+}
+
+// W = 2^shift G (exact: shift brings max|g| into [1, 2), so nothing that matters underflows), V = I
 __global__ void __launch_bounds__(256) jacobi_init_kernel(const double* __restrict__ G, long long rs, long long cs, int n, int N,
-                                                          double* __restrict__ W, double* __restrict__ V) {
+                                                          int shift, double* __restrict__ W, double* __restrict__ V) {
     const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
     if (e >= (long long)N * N) return;
     const int i = (int)(e % N), j = (int)(e / N);
     double g = 0.0;
-    if (i < n && j < n) g = i >= j ? G[i * rs + j * cs] : G[j * rs + i * cs];     // lower triangle, mirrored
+    if (i < n && j < n) g = ldexp(i >= j ? G[i * rs + j * cs] : G[j * rs + i * cs], shift);     // lower triangle, mirrored
     W[e] = g;
     V[e] = i == j ? 1.0 : 0.0;
 }
@@ -69,7 +90,9 @@ __global__ void __launch_bounds__(256) jacobi_round_kernel(const double* __restr
         if (a < m) {
             const double gpp = Gin[2 * a + 2 * a * ld], gqq = Gin[2 * a + 1 + (2 * a + 1) * ld];
             const double gpq = Gin[2 * a + 1 + 2 * a * ld];
-            if (!(fabs(gpq) <= DBL_EPSILON * sqrt(fabs(gpp * gqq)))) {
+            // eps sqrt|gpp| sqrt|gqq| rather than eps sqrt|gpp gqq|: the product under- or overflows long before the
+            // threshold does
+            if (!(fabs(gpq) <= DBL_EPSILON * sqrt(fabs(gpp)) * sqrt(fabs(gqq)))) {
                 const double th = (gqq - gpp) / (2.0 * gpq);
                 t = fabs(th) > 1e150 ? 0.5 / th : (th >= 0.0 ? 1.0 : -1.0) / (fabs(th) + sqrt(1.0 + th * th));
                 c = 1.0 / sqrt(1.0 + t * t);
@@ -149,8 +172,10 @@ struct Buffers {
     int* flag = nullptr;
     int* flag_host = nullptr;
     int* order = nullptr;
+    unsigned long long* maxbits = nullptr;
     cudaGraphExec_t exec[2] = {nullptr, nullptr};
     ~Buffers() {
+        if (maxbits) cudaFree(maxbits);
         for (int i = 0; i < 2; ++i) {
             if (W[i]) cudaFree(W[i]);
             if (V[i]) cudaFree(V[i]);
@@ -190,8 +215,10 @@ cudaError_t capture_sweep(Buffers& B, int N, int from, cudaGraphExec_t* exec) {
 }  // namespace
 
 cudaError_t syev_jacobi(int n, const double* G, long long rs, long long cs, double* V, long long vrs, long long vcs,
-                        double* w_host, int* sweeps, int max_sweeps, cudaStream_t stream, long long* launches) {
+                        double* w_host, int* sweeps, int max_sweeps, cudaStream_t stream, long long* launches,
+                        bool* non_finite) {
     if (sweeps) *sweeps = 0;
+    if (non_finite) *non_finite = false;
     if (n <= 0) return cudaSuccess;
     const int N = n + (n & 1);
     const size_t bytes = (size_t)N * N * sizeof(double);
@@ -204,8 +231,27 @@ cudaError_t syev_jacobi(int n, const double* G, long long rs, long long cs, doub
     if ((e = cudaMalloc(&B.flag, sizeof(int))) != cudaSuccess) return e;
     if ((e = cudaMallocHost(&B.flag_host, sizeof(int))) != cudaSuccess) return e;
     if ((e = cudaMalloc(&B.order, sizeof(int) * n)) != cudaSuccess) return e;
+    // Prescale by the power of two that brings max|g| into [1, 2): the rotations then never see products or squares of
+    // huge or tiny entries, and 2^k G runs the very same sweeps as G (the eigenvalues are scaled back exactly below).
+    if ((e = cudaMalloc(&B.maxbits, sizeof(unsigned long long))) != cudaSuccess) return e;
+    unsigned long long* maxbits = B.maxbits;
+    if ((e = cudaMemsetAsync(maxbits, 0, sizeof(unsigned long long), stream)) != cudaSuccess) return e;
+    const long long nn = (long long)n * n;
+    jacobi_maxabs_kernel<<<(unsigned)((nn + 255) / 256), 256, 0, stream>>>(G, rs, cs, n, maxbits);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    if (launches) ++*launches;
+    unsigned long long mb_host = 0;
+    if ((e = cudaMemcpyAsync(&mb_host, maxbits, sizeof(mb_host), cudaMemcpyDeviceToHost, stream)) != cudaSuccess) return e;
+    if ((e = cudaStreamSynchronize(stream)) != cudaSuccess) return e;
+    double gmax;
+    std::memcpy(&gmax, &mb_host, sizeof(gmax));
+    if (!std::isfinite(gmax)) {
+        if (non_finite) *non_finite = true;
+        return cudaSuccess;
+    }
+    const int shift = gmax > 0.0 ? -std::ilogb(gmax) : 0;
     const long long total = (long long)N * N;
-    jacobi_init_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(G, rs, cs, n, N, B.W[0], B.V[0]);
+    jacobi_init_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(G, rs, cs, n, N, shift, B.W[0], B.V[0]);
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     if (launches) ++*launches;
     int cur = 0, done = 0;
@@ -228,9 +274,9 @@ cudaError_t syev_jacobi(int n, const double* G, long long rs, long long cs, doub
     std::vector<int> order(n);
     std::iota(order.begin(), order.end(), 0);
     std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return std::fabs(w[x]) > std::fabs(w[y]); });
-    for (int j = 0; j < n; ++j) w_host[j] = w[order[j]];
+    // undo the prescaling: exact unless an eigenvalue leaves the normal range
+    for (int j = 0; j < n; ++j) w_host[j] = std::ldexp(w[order[j]], -shift);
     if ((e = cudaMemcpyAsync(B.order, order.data(), sizeof(int) * n, cudaMemcpyHostToDevice, stream)) != cudaSuccess) return e;
-    const long long nn = (long long)n * n;
     jacobi_gather_kernel<<<(unsigned)((nn + 255) / 256), 256, 0, stream>>>(B.V[cur], N, B.order, n, V, vrs, vcs);
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     if (launches) ++*launches;

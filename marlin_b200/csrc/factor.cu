@@ -14,6 +14,7 @@
 #include "gemm_f64.h"
 
 #include <algorithm>
+#include <cfloat>
 
 namespace mb {
 
@@ -74,10 +75,12 @@ lu_panel_kernel(double* a, long long rs, long long cs, int rows, int w, int* piv
         __syncthreads();
         const double pv = s_row[c];
         if (pv != 0.0) {
-            // 3. + 4. scale the column by the reciprocal (dgetf2) and update the rest of the panel
+            // 3. + 4. scale the column by the reciprocal (dgetf2) and update the rest of the panel; like dgetf2, divide
+            // instead when |pv| < sfmin = DBL_MIN, whose reciprocal overflows (1 / 2^-1060 = +Inf)
+            const bool recip = fabs(pv) >= DBL_MIN;
             const double rinv = 1.0 / pv;
             for (int r = c + 1 + tid; r < rows; r += 1024) {
-                const double l = a[r * rs + c * cs] * rinv;
+                const double l = recip ? a[r * rs + c * cs] * rinv : a[r * rs + c * cs] / pv;
                 a[r * rs + c * cs] = l;
                 for (int cc = c + 1; cc < w; ++cc) a[r * rs + cc * cs] -= l * s_row[cc];
             }

@@ -200,7 +200,11 @@ gemm_ozaki_i8_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
                         for (int e = 0; e < 2; ++e) {
                             const int n = nc + 8 * (jc + j) + e;
                             if (n < p.N) {
-                                const double term = (double)acc[4 * (jc + j) + 2 * h + e] * pow2_scale(ex_m + __ldg(p.eB + n));
+                                // a zero group adds +0 without forming 2^ex, which overflows to +Inf for the low groups
+                                // of rows / columns near DBL_MAX (0 * Inf = NaN) and is meaningless for the sentinel
+                                // exponent of a non-finite row / column
+                                const int32_t av = acc[4 * (jc + j) + 2 * h + e];
+                                const double term = av != 0 ? (double)av * pow2_scale(ex_m + __ldg(p.eB + n)) : 0.0;
                                 crow[(long long)n * p.ldc] = init ? term : (old[2 * j + e] + term);
                             }
                         }
@@ -211,25 +215,42 @@ gemm_ozaki_i8_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
 }
 
 // ------------------------------------------------------------------------------------------- operand splitting
+// Row / column maxima are taken over the bit patterns of |a|: non-negative doubles order like their bit patterns, and
+// +Inf and every NaN (sign cleared) lie above all finite values, so a non-finite entry always shows in its maximum (fmax
+// would drop a NaN).  Such a row / column gets the exponent NONFINITE_EXP and zero digits, so it adds nothing to the
+// int8 products, and ozaki_fixup_kernel recomputes its entries of C in plain fp64.
+constexpr unsigned long long INF_BITS = 0x7FF0000000000000ull;
+constexpr int NONFINITE_EXP = 1 << 20;
+
+__device__ __forceinline__ unsigned long long abs_bits(double a) {
+    return (unsigned long long)__double_as_longlong(a) & 0x7FFFFFFFFFFFFFFFull;
+}
+
 __global__ void ozaki_rowmax_kernel(const double* __restrict__ A, long long lda, int M, int K, int kchunk,
                                     unsigned long long* __restrict__ rowmax_bits) {
     const int m = blockIdx.x * blockDim.x + threadIdx.x;
     if (m >= M) return;
     const int k0 = blockIdx.y * kchunk, k1 = min(K, k0 + kchunk);
-    double r = 0.0;
-    for (int k = k0; k < k1; ++k) r = fmax(r, fabs(A[m + (long long)k * lda]));
-    // non-negative doubles order like their bit patterns; NaN/Inf propagate as a huge max (caller's data problem)
-    atomicMax(rowmax_bits + m, (unsigned long long)__double_as_longlong(r));
+    unsigned long long r = 0;
+    for (int k = k0; k < k1; ++k) r = max(r, abs_bits(A[m + (long long)k * lda]));
+    atomicMax(rowmax_bits + m, r);
 }
 
-__device__ __forceinline__ int scale_exponent(double r) {
-    // smallest e with r < 2^e (r > 0); 0 for an all-zero row/column
+__device__ __forceinline__ int scale_exponent(unsigned long long rbits) {
+    // smallest e with r < 2^e (r > 0); 0 for an all-zero row/column; NONFINITE_EXP for a row/column holding NaN or Inf
+    if (rbits >= INF_BITS) return NONFINITE_EXP;
+    const double r = __longlong_as_double((long long)rbits);
     if (!(r > 0.0)) return 0;
     return ilogb(r) + 1;
 }
 
-// digits of X = rint(a * 2^(P - e)), most significant first: out[t] for t = 0..s-1, each in [-64, 64]
+// digits of X = rint(a * 2^(P - e)), most significant first: out[t] for t = 0..s-1, each in [-64, 64]; all zero for a
+// non-finite row / column, which the fix-up pass recomputes
 __device__ __forceinline__ void split_digits(double a, int e, int s, int bits, int P, signed char* digs) {
+    if (e == NONFINITE_EXP) {
+        for (int t = 0; t < s; ++t) digs[t] = 0;
+        return;
+    }
     long long X = __double2ll_rn(ldexp(a, P - e));
     const long long half = 1ll << (bits - 1), mask = (1ll << bits) - 1;
     for (int t = s - 1; t >= 1; --t) {
@@ -247,7 +268,7 @@ __global__ void ozaki_split_a_kernel(const double* __restrict__ A, long long lda
                                      long long ld8, long long plane, int* __restrict__ eA) {
     const int m = blockIdx.x * blockDim.x + threadIdx.x;
     if (m >= M) return;
-    const int e = scale_exponent(__longlong_as_double((long long)rowmax_bits[m]));
+    const int e = scale_exponent(rowmax_bits[m]);
     if (blockIdx.y == 0) eA[m] = e;
     const int kchunk = ((K + gridDim.y - 1) / gridDim.y + 7) & ~7;
     const int k0 = blockIdx.y * kchunk, k1 = min(K, k0 + kchunk);
@@ -272,24 +293,46 @@ __global__ void __launch_bounds__(256) ozaki_split_b_kernel(const double* __rest
                                                            int bits, int P,
                                                            signed char* __restrict__ B8, long long ld8, long long plane,
                                                            int* __restrict__ eB) {
-    __shared__ double red[8];
+    __shared__ unsigned long long red[8];
     const int j = blockIdx.x;
     const double* col = B + (long long)j * ldb;
-    double r = 0.0;
-    for (int k = threadIdx.x; k < K; k += 256) r = fmax(r, fabs(col[k]));
+    unsigned long long r = 0;
+    for (int k = threadIdx.x; k < K; k += 256) r = max(r, abs_bits(col[k]));
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) r = fmax(r, __shfl_xor_sync(0xffffffffu, r, o));
+    for (int o = 16; o > 0; o >>= 1) r = max(r, __shfl_xor_sync(0xffffffffu, r, o));
     if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = r;
     __syncthreads();
     r = red[0];
 #pragma unroll
-    for (int w = 1; w < 8; ++w) r = fmax(r, red[w]);
+    for (int w = 1; w < 8; ++w) r = max(r, red[w]);
     const int e = scale_exponent(r);
     if (threadIdx.x == 0) eB[j] = e;
     signed char digs[8];
     for (int k = threadIdx.x; k < K; k += 256) {
         split_digits(col[k], e, s, bits, P, digs);
         for (int t = 0; t < s; ++t) B8[t * plane + (long long)j * ld8 + k] = digs[t];
+    }
+}
+
+// C(i, j) (+)= sum_k A(i, k) B(k, j) in fp64, k ascending, for every i whose row of A or j whose column of B holds a NaN
+// or Inf (eA / eB == NONFINITE_EXP): the IEEE result the DMMA kernel gives, instead of the digits' finite nonsense.
+// Blocks 0..M-1 take row i, blocks M..M+N-1 column j (skipping flagged rows, done by their row block); a block whose
+// row / column is finite exits at once, so the pass costs one tiny launch when nothing is flagged.
+__global__ void __launch_bounds__(128) ozaki_fixup_kernel(const double* __restrict__ A, long long lda, const double* __restrict__ B,
+                                                          long long ldb, double* __restrict__ C, long long ldc, int M, int N,
+                                                          int K, int accumulate, const int* __restrict__ eA,
+                                                          const int* __restrict__ eB) {
+    const bool row = blockIdx.x < (unsigned)M;
+    const int idx = row ? blockIdx.x : blockIdx.x - M;
+    if ((row ? eA[idx] : eB[idx]) != NONFINITE_EXP) return;
+    const int count = row ? N : M;
+    for (int o = threadIdx.x; o < count; o += blockDim.x) {
+        const int i = row ? idx : o, j = row ? o : idx;
+        if (!row && eA[i] == NONFINITE_EXP) continue;
+        double s = 0.0;
+        for (int k = 0; k < K; ++k) s = __dadd_rn(s, __dmul_rn(A[i + (long long)k * lda], B[k + (long long)j * ldb]));
+        double* c = C + i + (long long)j * ldc;
+        *c = accumulate ? __dadd_rn(*c, s) : s;
     }
 }
 
@@ -382,6 +425,10 @@ cudaError_t gemm_f64_ozaki(int M, int N, int K, const double* A, long long lda, 
     }
     const int grid = min(p.tiles_m * p.tiles_n, num_sms);
     gemm_ozaki_i8_kernel<<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(mA, mB, p);
+    if (launches) ++*launches;
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    // stream-ordered after the int8 kernel, which leaves the flagged entries of C as they were (accumulate) or +0
+    ozaki_fixup_kernel<<<M + N, 128, 0, stream>>>(A, lda, B, ldb, C, ldc, M, N, K, p.accumulate, eA, eB);
     if (launches) ++*launches;
     return cudaGetLastError();
 }
