@@ -92,7 +92,9 @@ int32_t mb_block_slice(mb_ctx* ctx, const mb_block* blk, int32_t r0, int32_t r1,
  *      matrix/DenseVecMatrix.scala:122,129,1676) -> Breeze `*` -> netlib dgemm -------------- */
 /* C = A*B (accumulate=0) or C += A*B (accumulate=1; the k-way reduceByKey sum of
  * BlockMatrix.scala:177 fused into the product).  fp64: DMMA tensor-core kernel (TMA staged).
- * bf16 inputs: wgmma kernel with fp32 register accumulation, C may be F32 or BF16. */
+ * bf16 inputs: wgmma kernel with fp32 register accumulation, C may be F32 or BF16; any shape, offset and ld
+ * (operands the TMA cannot address are copied to a packed buffer first), K = 0 gives C = 0, and an F32 C is built
+ * from accumulation chains of at most MARLIN_B200_BF16_KCHAIN (default 8192) k per launch. */
 int32_t mb_block_gemm(mb_ctx* ctx, const mb_block* A, const mb_block* B, mb_block* C, int32_t accumulate);
 /* Same GEMM on raw device pointers (column-major, BLAS trans flags 'N'/'T'). */
 int32_t mb_dgemm_device(mb_ctx* ctx, char transa, char transb, int32_t m, int32_t n, int32_t k,

@@ -473,6 +473,97 @@ int32_t mb_dgemm_host(mb_ctx* ctx, char transa, char transb, int32_t m, int32_t 
     return r;
 }
 
+// One contraction segment of a bf16 product: op(A) is M x k, op(B) is k x N, stored as the kernel reads them
+// (A is M x k if !transA else k x M; B is k x N if !transB else N x k; column-major with leading dimension lda / ldb).
+struct bf16_seg {
+    const char* a;
+    long long lda;
+    const char* b;
+    long long ldb;
+    int k;
+};
+
+// The tensor cores add into the fp32 accumulator with truncation, so one accumulation chain drifts in proportion to its
+// length in K on same-sign data.  fp32 results are therefore built from chains of at most this many k
+// (MARLIN_B200_BF16_KCHAIN, default 8192; 0 = unlimited), read once per process.
+static long long bf16_kchain() {
+    static const long long v = [] { const char* e = getenv("MARLIN_B200_BF16_KCHAIN"); return e ? atoll(e) : 8192ll; }();
+    return v;
+}
+
+// C (M x N, column-major, fp32 or bf16) = sum over segs of op(A_s) op(B_s) (+ C if accumulate), for any shape, offset
+// and leading dimension:
+//   * fp32 C: the segments are cut into chains of at most bf16_kchain() k (and 8 pieces) per launch; the first launch
+//     overwrites C unless the caller accumulates, the later ones add into it.  bf16 C: one launch, so one rounding
+//     (callers pass at most 8 segments);
+//   * a piece whose operand the TMA cannot address (base not 16-byte aligned or ld % 8 != 0: odd block heights,
+//     views, cuts inside a segment) is first copied into a packed stream-ordered buffer with ld rounded up to 8.  A
+//     copy changes no value, so the result is bit-identical to the same call on aligned operands;
+//   * total K = 0 writes zeros into C (nothing under accumulate), as the fp64 path does.
+static int32_t bf16_gemm(mb_ctx* ctx, bool ta, bool tb, int M, int N, int nseg, const bf16_seg* segs, void* C,
+                         long long ldc, bool c_f32, bool accumulate) {
+    if (M <= 0 || N <= 0) return MB_OK;
+    const long long cap = (c_f32 && bf16_kchain() > 0) ? bf16_kchain() : (1ll << 62);
+    std::vector<bf16_seg> pieces;
+    std::vector<size_t> group_end;            // pieces [group_end[g-1], group_end[g]) make launch g
+    long long in_group = 0;
+    for (int s = 0; s < nseg; ++s)
+        for (int k0 = 0; k0 < segs[s].k;) {
+            const int len = (int)std::min<long long>(segs[s].k - k0, cap - in_group);
+            const bf16_seg& sg = segs[s];
+            pieces.push_back({sg.a + 2 * (ta ? (long long)k0 : k0 * sg.lda), sg.lda,     // k0-th row / column of A
+                              sg.b + 2 * (tb ? k0 * sg.ldb : (long long)k0), sg.ldb, len});
+            in_group += len;
+            k0 += len;
+            const size_t first = group_end.empty() ? 0 : group_end.back();
+            if (in_group >= cap || pieces.size() - first == 8) { group_end.push_back(pieces.size()); in_group = 0; }
+        }
+    if (group_end.empty() || group_end.back() != pieces.size()) group_end.push_back(pieces.size());
+    if (pieces.empty()) {
+        if (accumulate) return MB_OK;
+        const size_t esz = c_f32 ? 4 : 2;
+        MB_CUDA(cudaMemset2DAsync(C, (size_t)ldc * esz, 0, (size_t)M * esz, (size_t)N, ctx->stream));
+        return MB_OK;
+    }
+    auto misaligned = [](const char* p, long long ld) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0 || ld % 8 != 0; };
+    std::vector<void*> staged;
+    auto release = [&]() { for (void* p : staged) cudaFreeAsync(p, ctx->stream); staged.clear(); };
+    // the stored (rows x cols) array of an operand -> a packed copy with ld rounded up to 8 (256-byte aligned base)
+    auto stage = [&](const char*& p, long long& ld, int rows, int cols) -> cudaError_t {
+        const long long ld8 = (rows + 7) / 8 * 8;
+        void* dst = nullptr;
+        cudaError_t e = cudaMallocAsync(&dst, (size_t)ld8 * cols * 2, ctx->stream);
+        if (e != cudaSuccess) return e;
+        staged.push_back(dst);
+        if ((e = mb::convert_strided(MB_BF16, MB_BF16, rows, cols, p, 1, ld, dst, 1, ld8, ctx->stream)) != cudaSuccess) return e;
+        ctx->launches++;
+        p = static_cast<const char*>(dst);
+        ld = ld8;
+        return cudaSuccess;
+    };
+    for (size_t g = 0; g < group_end.size(); ++g) {
+        const size_t first = g ? group_end[g - 1] : 0;
+        const int ns = (int)(group_end[g] - first);
+        const void* pa[8]; const void* pb[8]; long long la[8], lb[8]; int ks[8];
+        cudaError_t e = cudaSuccess;
+        for (int s = 0; s < ns && e == cudaSuccess; ++s) {
+            bf16_seg pc = pieces[first + s];
+            if (misaligned(pc.a, pc.lda)) e = stage(pc.a, pc.lda, ta ? pc.k : M, ta ? M : pc.k);
+            if (e == cudaSuccess && misaligned(pc.b, pc.ldb)) e = stage(pc.b, pc.ldb, tb ? N : pc.k, tb ? pc.k : N);
+            pa[s] = pc.a; la[s] = pc.lda; pb[s] = pc.b; lb[s] = pc.ldb; ks[s] = pc.k;
+        }
+        int launches = 0;
+        if (e == cudaSuccess)
+            e = mb::gemm_bf16_segments(ta, tb, M, N, ns, ks, pa, la, pb, lb, C, ldc, c_f32, accumulate || g > 0, ctx->num_sms,
+                                       ctx->stream, &launches);
+        release();
+        if (e == cudaErrorNotSupported) return fail(MB_ERR_UNSUPPORTED, "bf16 GEMM: cuTensorMapEncodeTiled is not available");
+        if (e != cudaSuccess) return cuda_fail(e, "gemm_bf16_segments");
+        ctx->launches += launches;
+    }
+    return MB_OK;
+}
+
 int32_t mb_block_gemm(mb_ctx* ctx, const mb_block* A, const mb_block* B, mb_block* C, int32_t accumulate) {
     MB_CTX(ctx);
     if (!A || !B || !C) return fail(MB_ERR_INVALID_ARG, "mb_block_gemm: null block");
@@ -502,20 +593,16 @@ int32_t mb_block_gemm(mb_ctx* ctx, const mb_block* A, const mb_block* B, mb_bloc
                                  B->ld, f64_ptr(A), A->ld, accumulate ? 1.0 : 0.0, f64_ptr(C), C->ld, false);
     }
     if (A->dtype == MB_BF16 && B->dtype == MB_BF16 && (C->dtype == MB_F32 || C->dtype == MB_BF16)) {
-        int launches = 0;
-        cudaError_t e;
+        // any shape, offset and ld (misaligned operands are staged), fp32 chains capped at bf16_kchain()
         if (!C->is_transpose) {
-            e = mb::gemm_bf16(A->is_transpose, B->is_transpose, M, N, K, elem_ptr(A), A->ld, elem_ptr(B), B->ld,
-                              elem_ptr(C), C->ld, C->dtype == MB_F32, accumulate != 0, ctx->num_sms, ctx->stream, &launches);
-        } else {
-            e = mb::gemm_bf16(!B->is_transpose, !A->is_transpose, N, M, K, elem_ptr(B), B->ld, elem_ptr(A), A->ld,
-                              elem_ptr(C), C->ld, C->dtype == MB_F32, accumulate != 0, ctx->num_sms, ctx->stream, &launches);
+            const bf16_seg seg = {elem_ptr(A), A->ld, elem_ptr(B), B->ld, K};
+            return bf16_gemm(ctx, A->is_transpose, B->is_transpose, M, N, 1, &seg, elem_ptr(C), C->ld, C->dtype == MB_F32,
+                             accumulate != 0);
         }
-        if (e == cudaErrorNotSupported)
-            return fail(MB_ERR_UNSUPPORTED, "mb_block_gemm(bf16): operands must be 16-byte aligned with ld %% 8 == 0");
-        if (e != cudaSuccess) return cuda_fail(e, "gemm_bf16");
-        ctx->launches += launches;
-        return MB_OK;
+        // row-major result: C^T = B^T A^T, as in the fp64 branch
+        const bf16_seg seg = {elem_ptr(B), B->ld, elem_ptr(A), A->ld, K};
+        return bf16_gemm(ctx, !B->is_transpose, !A->is_transpose, N, M, 1, &seg, elem_ptr(C), C->ld, C->dtype == MB_F32,
+                         accumulate != 0);
     }
     return fail(MB_ERR_UNSUPPORTED, "mb_block_gemm: unsupported dtype combination (%d,%d)->%d", A->dtype, B->dtype, C->dtype);
 }
@@ -578,51 +665,19 @@ int32_t mb_matmul_blocked_subset(mb_ctx* ctx, mb_block* const* A_tiles, mb_block
     for (int c = 0; c < num_c; ++c) {
         const int id = c_ids[c], i = id / n, j = id % n;
         mb_block* cb = C_tiles[id];
-        // bf16 tiles: fold the kk-sum into ONE wgmma launch per C block (K segments; accumulator stays in registers)
+        // bf16 tiles: fold the kk-sum into ONE wgmma launch per C block (K segments; accumulator stays in registers) —
+        // per K chain of bf16_kchain() for fp32 C blocks
         bool seg_ok = k <= 8 && !cb->is_transpose && (cb->dtype == MB_F32 || cb->dtype == MB_BF16);
-        const void* Ap[8]; const void* Bp[8]; long long la[8], lb[8]; int Ks[8];
+        bf16_seg segs[8];
         for (int kk = 0; kk < k && seg_ok; ++kk) {
             const mb_block *a = A_tiles[i * k + kk], *b = B_tiles[kk * n + j];
-            seg_ok = a->dtype == MB_BF16 && b->dtype == MB_BF16 && !a->is_transpose && !b->is_transpose && a->cols > 0;
-            Ap[kk] = elem_ptr(a); Bp[kk] = elem_ptr(b); la[kk] = a->ld; lb[kk] = b->ld; Ks[kk] = a->cols;
+            seg_ok = a->dtype == MB_BF16 && b->dtype == MB_BF16 && !a->is_transpose && !b->is_transpose;
+            segs[kk] = {elem_ptr(a), a->ld, elem_ptr(b), b->ld, a->cols};
         }
         if (seg_ok) {
-            // The tensor cores add into the fp32 accumulator with truncation, so one accumulation chain drifts in proportion
-            // to its length in K on same-sign data.  Chains are therefore
-            // capped (MARLIN_B200_BF16_KCHAIN, default 8192; 0 = unlimited): an fp32 C block is produced by several
-            // launches whose epilogues add into C with round-to-nearest.  bf16 C blocks keep the single launch (one rounding).
-            static const long long kchain = [] { const char* e = getenv("MARLIN_B200_BF16_KCHAIN"); return e ? atoll(e) : 8192ll; }();
-            long long total_k = 0;
-            for (int kk = 0; kk < k; ++kk) total_k += Ks[kk];
-            int launches = 0;
-            cudaError_t e = cudaSuccess;
-            if (cb->dtype != MB_F32 || kchain <= 0 || total_k <= kchain) {
-                e = mb::gemm_bf16_segments(false, false, cb->rows, cb->cols, k, Ks, Ap, la, Bp, lb, elem_ptr(cb), cb->ld,
-                                           cb->dtype == MB_F32, false, ctx->num_sms, ctx->stream, &launches);
-            } else {
-                const void* sa[8]; const void* sb[8]; long long sla[8], slb[8]; int sk[8];
-                int ns = 0, group = 0;
-                long long in_group = 0;
-                auto flush = [&]() {
-                    if (ns == 0 || e != cudaSuccess) return;
-                    e = mb::gemm_bf16_segments(false, false, cb->rows, cb->cols, ns, sk, sa, sla, sb, slb, elem_ptr(cb), cb->ld, true,
-                                               group > 0, ctx->num_sms, ctx->stream, &launches);
-                    ++group; ns = 0; in_group = 0;
-                };
-                for (int kk = 0; kk < k && e == cudaSuccess; ++kk)
-                    for (int k0 = 0; k0 < Ks[kk] && e == cudaSuccess;) {
-                        const int len = (int)std::min<long long>(Ks[kk] - k0, kchain - in_group);
-                        sa[ns] = static_cast<const char*>(Ap[kk]) + (size_t)k0 * la[kk] * 2;       // columns k0.. of A(i,kk)
-                        sb[ns] = static_cast<const char*>(Bp[kk]) + (size_t)k0 * 2;                // rows k0.. of B(kk,j)
-                        sla[ns] = la[kk]; slb[ns] = lb[kk]; sk[ns] = len;
-                        ++ns; in_group += len; k0 += len;
-                        if (in_group >= kchain || ns == 8) flush();
-                    }
-                flush();
-            }
-            if (e == cudaSuccess) { ctx->launches += launches; continue; }
-            if (e != cudaErrorNotSupported) return cuda_fail(e, "gemm_bf16_segments");
-            cudaGetLastError();
+            int32_t r = bf16_gemm(ctx, false, false, cb->rows, cb->cols, k, segs, elem_ptr(cb), cb->ld, cb->dtype == MB_F32, false);
+            if (r) return r;
+            continue;
         }
         for (int kk = 0; kk < k; ++kk) {
             int32_t r = mb_block_gemm(ctx, A_tiles[i * k + kk], B_tiles[kk * n + j], C_tiles[id], kk > 0);

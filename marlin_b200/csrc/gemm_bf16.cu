@@ -296,13 +296,4 @@ cudaError_t gemm_bf16_segments(bool transA, bool transB, int M, int N, int nseg,
     return launch<true, true>(maps, p, num_sms, stream);
 }
 
-cudaError_t gemm_bf16(bool transA, bool transB, int M, int N, int K, const void* A, long long lda, const void* B,
-                      long long ldb, void* C, long long ldc, bool c_is_f32, bool accumulate, int num_sms,
-                      cudaStream_t stream, int* launches) {
-    if (M <= 0 || N <= 0) return cudaSuccess;
-    if (K <= 0) return accumulate ? cudaSuccess : cudaErrorNotSupported;
-    return gemm_bf16_segments(transA, transB, M, N, 1, &K, &A, &lda, &B, &ldb, C, ldc, c_is_f32, accumulate, num_sms, stream,
-                              launches);
-}
-
 }  // namespace mb

@@ -48,7 +48,8 @@ def main():
         assert abs(ga.sum() - A.sum()) <= 1e-9 * abs(A).sum()
     # ---- bf16 tiles (config-5 path): C-stationary (4,4,4) and a k-split that reduces fp32 partials across ranks
     from marlin_b200 import _native as nat
-    for (n_, g_, kgrid) in [(512, 4, None), (256, None, (1, 4, 1))]:
+    # 1000 on a 3 x 3 grid: 334- and 332-row blocks packed with ld = rows, so their operands are staged before the TMA
+    for (n_, g_, kgrid) in [(512, 4, None), (256, None, (1, 4, 1)), (1000, 3, None)]:
         if kgrid is None:
             Ab = mb.MTUtils.randomBlockMatrix(None, n_, n_, g_, g_, seed=21, dtype=nat.MB_BF16)
             Bb = mb.MTUtils.randomBlockMatrix(None, n_, n_, g_, g_, seed=22, dtype=nat.MB_BF16)
