@@ -18,7 +18,7 @@
 //   B 'T' (N x K, n contiguous)  -> MN-major B : 4 atoms [64 k-rows][64 n]
 #include "gemm_bf16.h"
 #include "ptx.cuh"
-#include <atomic>
+#include "tma.h"
 #include <cuda_bf16.h>
 
 namespace mb {
@@ -217,56 +217,13 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ SegMaps maps, const Params p) {
     }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn get_encode_fn() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
-        void* ptr = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess &&
-            qres == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<EncodeTiledFn>(ptr);
-    }
-    return fn;
-}
-
-bool make_map_bf16(CUtensorMap* map, const void* base, uint64_t dim0, uint64_t dim1, uint64_t ld, uint32_t box0,
-                   uint32_t box1) {
-    EncodeTiledFn fn = get_encode_fn();
-    if (!fn) return false;
-    cuuint64_t dims[2] = {dim0, dim1};
-    cuuint64_t strides[1] = {ld * 2};
-    cuuint32_t box[2] = {box0, box1};
-    cuuint32_t estr[2] = {1, 1};
-    return fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
-template <bool TA, bool TB>
-cudaError_t launch(const SegMaps& maps, const Params& p, int num_sms, cudaStream_t stream) {
-    auto kern = gemm_bf16_wgmma_kernel<TA, TB>;
-    static std::atomic<bool> attr_done{false};   // idempotent attribute set; atomic so threads sharing a context may race here
-    if (!attr_done.load(std::memory_order_acquire)) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-        if (e != cudaSuccess) return e;
-        attr_done.store(true, std::memory_order_release);
-    }
-    const int grid = min(p.tiles_m * p.tiles_n, num_sms);
-    kern<<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(maps, p);
-    return cudaGetLastError();
-}
-
 }  // namespace
 
 cudaError_t gemm_bf16_segments(bool transA, bool transB, int M, int N, int nseg, const int* Kseg, const void* const* A,
                                const long long* lda, const void* const* B, const long long* ldb, void* C, long long ldc,
                                bool c_is_f32, bool accumulate, int num_sms, cudaStream_t stream, int* launches) {
     if (M <= 0 || N <= 0) return cudaSuccess;
-    if (nseg <= 0 || nseg > MAX_SEG || !get_encode_fn()) return cudaErrorNotSupported;
+    if (nseg <= 0 || nseg > MAX_SEG || !tma_encode_fn()) return cudaErrorNotSupported;
     static thread_local SegMaps maps;
     maps.nseg = nseg;
     int Ktot = 0;
@@ -276,9 +233,11 @@ cudaError_t gemm_bf16_segments(bool transA, bool transB, int M, int N, int nseg,
         const bool aligned = ((reinterpret_cast<uintptr_t>(A[sg]) | reinterpret_cast<uintptr_t>(B[sg])) & 15) == 0 &&
                              (lda[sg] % 8 == 0) && (ldb[sg] % 8 == 0);
         if (!aligned) return cudaErrorNotSupported;
-        bool ok = true;
-        ok = ok && (!transA ? make_map_bf16(&maps.a[sg], A[sg], M, K, lda[sg], 64, 64) : make_map_bf16(&maps.a[sg], A[sg], K, M, lda[sg], 64, 128));
-        ok = ok && (!transB ? make_map_bf16(&maps.b[sg], B[sg], K, N, ldb[sg], 64, 256) : make_map_bf16(&maps.b[sg], B[sg], N, K, ldb[sg], 64, 64));
+        constexpr CUtensorMapDataType BF16 = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+        const bool ok = (!transA ? tma_map(&maps.a[sg], BF16, A[sg], M, K, lda[sg] * 2, 64, 64)
+                                 : tma_map(&maps.a[sg], BF16, A[sg], K, M, lda[sg] * 2, 64, 128)) &&
+                        (!transB ? tma_map(&maps.b[sg], BF16, B[sg], K, N, ldb[sg] * 2, 64, 256)
+                                 : tma_map(&maps.b[sg], BF16, B[sg], N, K, ldb[sg] * 2, 64, 64));
         if (!ok) return cudaErrorNotSupported;
         maps.num_kb[sg] = (K + BK - 1) / BK;
         Ktot += K;
@@ -290,10 +249,11 @@ cudaError_t gemm_bf16_segments(bool transA, bool transB, int M, int N, int nseg,
     p.c_is_f32 = c_is_f32 ? 1 : 0;
     p.accumulate = accumulate ? 1 : 0;
     if (launches) ++*launches;
-    if (!transA && !transB) return launch<false, false>(maps, p, num_sms, stream);
-    if (transA && !transB) return launch<true, false>(maps, p, num_sms, stream);
-    if (!transA && transB) return launch<false, true>(maps, p, num_sms, stream);
-    return launch<true, true>(maps, p, num_sms, stream);
+    const int grid = min(p.tiles_m * p.tiles_n, num_sms);
+    if (!transA && !transB) return launch_with_smem<gemm_bf16_wgmma_kernel<false, false>>(grid, NUM_THREADS, SMEM_BYTES, stream, maps, p);
+    if (transA && !transB) return launch_with_smem<gemm_bf16_wgmma_kernel<true, false>>(grid, NUM_THREADS, SMEM_BYTES, stream, maps, p);
+    if (!transA && transB) return launch_with_smem<gemm_bf16_wgmma_kernel<false, true>>(grid, NUM_THREADS, SMEM_BYTES, stream, maps, p);
+    return launch_with_smem<gemm_bf16_wgmma_kernel<true, true>>(grid, NUM_THREADS, SMEM_BYTES, stream, maps, p);
 }
 
 }  // namespace mb

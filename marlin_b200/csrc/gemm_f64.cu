@@ -16,10 +16,16 @@
 //
 // Both operands may be 'N' or 'T' (Breeze isTranspose views): an operand whose contiguous
 // dimension is M/N ("MN form") is staged as 8 boxes of [16 k-rows][16 mn] and one whose
-// contiguous dimension is K ("K form") as one box of [128 mn-rows][16 k].
+// contiguous dimension is K ("K form") as one box of [128 mn-rows][16 k] (operand_map).
+//
+// Three kernels run this mainloop: gemm_f64_dmma_kernel (every tile of C), syrk_f64_dmma_kernel (the Gramian's
+// lower-triangle tiles, split over K) and gemm_f64_dmma_grouped_kernel (a list of C regions, each over its own K
+// segments).  They share one set of pieces, templated on the operands' forms: ring_setup, load_slab (producer),
+// consumer_lane + mma_slab (consumers) and store_tile (epilogue).  Each kernel keeps only its tile schedule, its K
+// range and what its epilogue waits for or signals.
 #include "gemm_f64.h"
 #include "ptx.cuh"
-#include <atomic>
+#include "tma.h"
 #include <cstdlib>
 
 namespace mb {
@@ -72,31 +78,222 @@ __device__ __forceinline__ void tri_coords(int t, int& tm, int& tn) {
     tn = t - r * (r + 1) / 2;
 }
 
+// ---- the mainloop pieces of the three DMMA kernels.  A is in MN form when !TA, B when TB. ----
+
+// NUM_STAGES stages of [A tile | B tile] from a 1024-byte aligned base (SWIZZLE_128B needs it), then the full and the
+// empty mbarrier of every stage.
+struct Ring {
+    uint32_t base, full, empty;
+};
+
+// Thread 0 initialises the barriers and prefetches the descriptors it is given; every thread returns after the CTA barrier.
+__device__ __forceinline__ Ring ring_setup(const CUtensorMap* prefetchA, const CUtensorMap* prefetchB) {
+    extern __shared__ uint8_t smem_raw[];
+    Ring ring;
+    ring.base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+    ring.full = ring.base + NUM_STAGES * STAGE_BYTES;
+    ring.empty = ring.full + NUM_STAGES * 8;
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < NUM_STAGES; ++s) {
+            mbar_init(ring.full + 8 * s, 1);
+            mbar_init(ring.empty + 8 * s, NUM_CONSUMER_WARPS);
+        }
+        fence_barrier_init();
+        if (prefetchA) tma_prefetch_desc(prefetchA);
+        if (prefetchB) tma_prefetch_desc(prefetchB);
+    }
+    __syncthreads();
+    return ring;
+}
+
+// Producer: wait until `stage` is free (its empty barrier completed the phase of parity empty_parity, the producer's
+// own phase ^ 1), then load k16 slab kb of the A tile at row m0 and of the B tile at column n0 into it.
+template <bool TA, bool TB>
+__device__ __forceinline__ void load_slab(const Ring& ring, int stage, uint32_t empty_parity, const CUtensorMap* mapA,
+                                          const CUtensorMap* mapB, int m0, int n0, int kb) {
+    mbar_wait(ring.empty + 8 * stage, empty_parity);
+    const uint32_t full = ring.full + 8 * stage;
+    const uint32_t sA = ring.base + stage * STAGE_BYTES;
+    const uint32_t sB = sA + OPERAND_BYTES;
+    mbar_arrive_expect_tx(full, STAGE_BYTES);
+    const int k0 = kb * BK;
+    if (!TA) {
+#pragma unroll
+        for (int b = 0; b < 8; ++b) tma_load_2d(sA + b * 2048, mapA, full, m0 + 16 * b, k0);
+    } else {
+        tma_load_2d(sA, mapA, full, k0, m0);
+    }
+    if (!TB) {
+        tma_load_2d(sB, mapB, full, k0, n0);
+    } else {
+#pragma unroll
+        for (int b = 0; b < 8; ++b) tma_load_2d(sB + b * 2048, mapB, full, n0 + 16 * b, k0);
+    }
+}
+
+// A consumer thread: its 64x32 warp tile (warp_m: 64-row slab, warp_n: 32-column slab), its MMA row (A) / column (B) r
+// and k slot q, and the byte offsets of its fragment loads inside one operand tile, [h][p] for an MN-form operand and
+// [h][0] for a K-form one:
+//  MN form: box t' (16 mn x 16 k, 2 KiB), k-row = 8h + 2q + p, 16B chunk = r ^ ((2q+p)&7)
+//           -> doubles (mn = 16t' + 2r, 16t' + 2r + 1)  = MMA tiles 2t', 2t'+1, row r.
+//  K  form: row mn = base + 8u + perm8(r), 16B chunk = (4h + q) ^ perm8(r)
+//           -> doubles (k = 8h + 2q, 8h + 2q + 1)       = phases p = 0, 1.
+struct Consumer {
+    int lane, warp_m, warp_n, r, q;
+    uint32_t offA[2][2], offB[2][2];
+};
+
+template <bool TA, bool TB>
+__device__ __forceinline__ Consumer consumer_lane(int cw, int lane) {
+    Consumer c;
+    c.lane = lane;
+    c.warp_m = cw & 1;
+    c.warp_n = cw >> 1;
+    c.r = lane >> 2;
+    c.q = lane & 3;
+    const int pr = perm8(c.r);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int pp = 0; pp < 2; ++pp) {
+            const int krow = 8 * h + 2 * c.q + pp;
+            const uint32_t mn_off = krow * 128 + ((c.r ^ (krow & 7)) << 4);
+            const uint32_t k_off = pr * 128 + ((((4 * h + c.q) ^ pr) & 7) << 4);
+            c.offA[h][pp] = !TA ? (c.warp_m * 4 * 2048 + mn_off) : (c.warp_m * 64 * 128 + k_off);
+            c.offB[h][pp] = TB ? (c.warp_n * 2 * 2048 + mn_off) : (c.warp_n * 32 * 128 + k_off);
+        }
+    }
+    return c;
+}
+
+// Consumer: wait for the slab in `stage`, read the fragments (24 LDS.128 per warp), hand the stage back to the producer
+// and issue the slab's 128 DMMA into acc.
+template <bool TA, bool TB>
+__device__ __forceinline__ void mma_slab(double (&acc)[8][4][2], const Ring& ring, int stage, uint32_t phase,
+                                         const Consumer c) {
+    mbar_wait(ring.full + 8 * stage, phase);
+    const uint32_t sA = ring.base + stage * STAGE_BYTES;
+    const uint32_t sB = sA + OPERAND_BYTES;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        double a[8][2];   // [m-tile][phase]
+        double b[4][2];   // [n-tile][phase]
+        if (!TA) {
+#pragma unroll
+            for (int tp = 0; tp < 4; ++tp)
+#pragma unroll
+                for (int pp = 0; pp < 2; ++pp) lds128(a[2 * tp][pp], a[2 * tp + 1][pp], sA + c.offA[h][pp] + tp * 2048);
+        } else {
+#pragma unroll
+            for (int u = 0; u < 8; ++u) lds128(a[u][0], a[u][1], sA + c.offA[h][0] + u * 8 * 128);
+        }
+        if (!TB) {
+#pragma unroll
+            for (int u = 0; u < 4; ++u) lds128(b[u][0], b[u][1], sB + c.offB[h][0] + u * 8 * 128);
+        } else {
+#pragma unroll
+            for (int tp = 0; tp < 2; ++tp)
+#pragma unroll
+                for (int pp = 0; pp < 2; ++pp) lds128(b[2 * tp][pp], b[2 * tp + 1][pp], sB + c.offB[h][pp] + tp * 2048);
+        }
+        if (h == 1) {
+            // all reads of this stage are issued; hand the slot back to the producer
+            __syncwarp();
+            if (c.lane == 0) mbar_arrive(ring.empty + 8 * stage);
+        }
+#pragma unroll
+        for (int pp = 0; pp < 2; ++pp)
+#pragma unroll
+            for (int i = 0; i < 8; ++i)
+#pragma unroll
+                for (int j = 0; j < 4; ++j) dmma_m8n8k4(acc[i][j][0], acc[i][j][1], a[i][pp], b[j][pp]);
+    }
+}
+
+// Row (A: slot x = r) or column (B: slot x = 2q + jj) inside the warp tile that MMA tile t of the accumulators holds,
+// for an operand in MN form or in K form: the slot permutation of the fragment loads, undone.
+template <bool MN>
+__device__ __forceinline__ int tile_index(int t, int x) {
+    return MN ? 16 * (t >> 1) + 2 * x + (t & 1) : 8 * t + perm8(x);
+}
+
+// Epilogue: stores this thread's accumulators of the tile at (m0, n0) into the M x N column-major D, combined with
+// what D held or with an addend by op: D(m, n) = v after v = op.scale(acc) and op.add(v, col, m), where col =
+// op.column(n) is the column the old values are read from (op.add2 combines rows m, m + 1 with one 16-byte read).
+// vec allows 16-byte accesses: D and col 16-byte aligned with even leading dimensions.
+template <bool TA, bool TB, class Op>
+__device__ __forceinline__ void store_tile(const double (&acc)[8][4][2], const Consumer c, int m0, int n0, int M, int N,
+                                           double* D, long long ldd, bool vec, const Op op) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+#pragma unroll
+        for (int jj = 0; jj < 2; ++jj) {
+            const int n = n0 + c.warp_n * 32 + tile_index<TB>(j, 2 * c.q + jj);
+            if (n >= N) continue;
+            double* dcol = D + (long long)n * ldd;
+            const double* col = op.column(n);
+            if (!TA) {
+#pragma unroll
+                for (int tp = 0; tp < 4; ++tp) {
+                    const int m = m0 + c.warp_m * 64 + tile_index<true>(2 * tp, c.r);
+                    if (m >= M) continue;
+                    double v0 = op.scale(acc[2 * tp][j][jj]), v1 = op.scale(acc[2 * tp + 1][j][jj]);
+                    if (vec && m + 1 < M) {
+                        op.add2(v0, v1, col, m);
+                        *reinterpret_cast<double2*>(dcol + m) = make_double2(v0, v1);
+                    } else {
+                        op.add(v0, col, m);
+                        dcol[m] = v0;
+                        if (m + 1 < M) {
+                            op.add(v1, col, m + 1);
+                            dcol[m + 1] = v1;
+                        }
+                    }
+                }
+            } else {
+#pragma unroll
+                for (int i = 0; i < 8; ++i) {
+                    const int m = m0 + c.warp_m * 64 + tile_index<false>(i, c.r);
+                    if (m >= M) continue;
+                    double v = op.scale(acc[i][j][jj]);
+                    op.add(v, col, m);
+                    dcol[m] = v;
+                }
+            }
+        }
+    }
+}
+
+// C = alpha * acc + beta * C; C is not read when beta == 0.
+struct ScaleAddC {
+    const double* C;
+    long long ldc;
+    double alpha, beta;
+    bool use_beta;
+    __device__ __forceinline__ double scale(double a) const { return alpha * a; }
+    __device__ __forceinline__ const double* column(int n) const { return C + (long long)n * ldc; }
+    __device__ __forceinline__ void add(double& v, const double* col, int m) const {
+        if (use_beta) v += beta * col[m];
+    }
+    __device__ __forceinline__ void add2(double& v0, double& v1, const double* col, int m) const {
+        if (use_beta) {
+            const double2 old = *reinterpret_cast<const double2*>(col + m);
+            v0 += beta * old.x;
+            v1 += beta * old.y;
+        }
+    }
+};
+
 // The persistent TMA + DMMA mainloop shared by the GEMM (SYRK = false: every tile of C, the whole K range, C = alpha*acc +
 // beta*C) and the Gramian (SYRK = true: lower-triangle tiles only, split-K partials stored to a workspace).
 template <bool TA, bool TB, bool SYRK>
 __device__ __forceinline__ void dmma_persistent(const CUtensorMap& mapA, const CUtensorMap& mapB, const Params& p,
                                                 const SyrkSched& sk) {
-    extern __shared__ uint8_t smem_raw[];
-    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const uint32_t bar_full = smem_base + NUM_STAGES * STAGE_BYTES;
-    const uint32_t bar_empty = bar_full + NUM_STAGES * 8;
-
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     const int num_tiles = SYRK ? sk.tri_tiles * sk.splits : p.tiles_m * p.tiles_n;
     const int num_kb = (p.K + BK - 1) / BK;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < NUM_STAGES; ++s) {
-            mbar_init(bar_full + 8 * s, 1);
-            mbar_init(bar_empty + 8 * s, NUM_CONSUMER_WARPS);
-        }
-        fence_barrier_init();
-        tma_prefetch_desc(&mapA);
-        tma_prefetch_desc(&mapB);
-    }
-    __syncthreads();
+    const Ring ring = ring_setup(&mapA, &mapB);
 
     if (warp < 4) {
         // ===================== producer warpgroup =====================
@@ -116,24 +313,7 @@ __device__ __forceinline__ void dmma_persistent(const CUtensorMap& mapA, const C
                 }
                 const int m0 = tm * BM, n0 = tn * BN;
                 for (int kb = kb_begin; kb < kb_end; ++kb) {
-                    mbar_wait(bar_empty + 8 * stage, phase ^ 1);
-                    const uint32_t full = bar_full + 8 * stage;
-                    const uint32_t sA = smem_base + stage * STAGE_BYTES;
-                    const uint32_t sB = sA + OPERAND_BYTES;
-                    mbar_arrive_expect_tx(full, STAGE_BYTES);
-                    const int k0 = kb * BK;
-                    if (!TA) {
-#pragma unroll
-                        for (int b = 0; b < 8; ++b) tma_load_2d(sA + b * 2048, &mapA, full, m0 + 16 * b, k0);
-                    } else {
-                        tma_load_2d(sA, &mapA, full, k0, m0);
-                    }
-                    if (!TB) {
-                        tma_load_2d(sB, &mapB, full, k0, n0);
-                    } else {
-#pragma unroll
-                        for (int b = 0; b < 8; ++b) tma_load_2d(sB + b * 2048, &mapB, full, n0 + 16 * b, k0);
-                    }
+                    load_slab<TA, TB>(ring, stage, phase ^ 1, &mapA, &mapB, m0, n0, kb);
                     if (++stage == NUM_STAGES) { stage = 0; phase ^= 1; }
                 }
             }
@@ -143,31 +323,7 @@ __device__ __forceinline__ void dmma_persistent(const CUtensorMap& mapA, const C
 
     // ========================= consumer warpgroups =========================
     setmaxnreg_inc<232>();
-    const int cw = warp - 4;          // 0..7
-    const int warp_m = cw & 1;        // 64-row slab
-    const int warp_n = cw >> 1;       // 32-col slab
-    const int r = lane >> 2;          // MMA row (A) / col (B) index of this lane
-    const int q = lane & 3;           // MMA k slot of this lane
-    const int pr = perm8(r);
-
-    // Per-lane byte offsets of the fragment loads inside one operand tile (see header comment).
-    //  MN form: box t' (16 mn x 16 k, 2 KiB), k-row = 8h + 2q + p, 16B chunk = r ^ ((2q+p)&7)
-    //           -> doubles (mn = 16t' + 2r, 16t' + 2r + 1)  = MMA tiles 2t', 2t'+1, row r.
-    //  K  form: row mn = base + 8u + perm8(r), 16B chunk = (4h + q) ^ perm8(r)
-    //           -> doubles (k = 8h + 2q, 8h + 2q + 1)       = phases p = 0, 1.
-    uint32_t offA[2][2], offB[2][2];   // [h][p] for MN form, [h][0] used for K form
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-#pragma unroll
-        for (int pp = 0; pp < 2; ++pp) {
-            const int krow = 8 * h + 2 * q + pp;
-            const uint32_t mn_off = krow * 128 + ((r ^ (krow & 7)) << 4);
-            const uint32_t k_off = pr * 128 + ((((4 * h + q) ^ pr) & 7) << 4);
-            offA[h][pp] = !TA ? (warp_m * 4 * 2048 + mn_off) : (warp_m * 64 * 128 + k_off);
-            offB[h][pp] = TB ? (warp_n * 2 * 2048 + mn_off) : (warp_n * 32 * 128 + k_off);
-        }
-    }
-
+    const Consumer c = consumer_lane<TA, TB>(warp - 4, lane);
     int stage = 0;
     uint32_t phase = 0;
     const bool vec_ok = ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0) && ((p.ldc & 1) == 0);
@@ -184,7 +340,6 @@ __device__ __forceinline__ void dmma_persistent(const CUtensorMap& mapA, const C
         } else {
             tile_coords(t, p.tiles_m, p.tiles_n, tm_, tn_);
         }
-        const int m0 = tm_ * BM, n0 = tn_ * BN;
 
         double acc[8][4][2];
 #pragma unroll
@@ -195,96 +350,12 @@ __device__ __forceinline__ void dmma_persistent(const CUtensorMap& mapA, const C
         // bounded by p.K (a kernel parameter) rather than num_kb: one register fewer, which the <N,T> instance needs
         // to fit sm_90a's 168-register budget without a spill
         for (int k0 = k_begin; k0 < k_end; k0 += BK) {
-            mbar_wait(bar_full + 8 * stage, phase);
-            const uint32_t sA = smem_base + stage * STAGE_BYTES;
-            const uint32_t sB = sA + OPERAND_BYTES;
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                double a[8][2];   // [m-tile][phase]
-                double b[4][2];   // [n-tile][phase]
-                if (!TA) {
-#pragma unroll
-                    for (int tp = 0; tp < 4; ++tp)
-#pragma unroll
-                        for (int pp = 0; pp < 2; ++pp)
-                            lds128(a[2 * tp][pp], a[2 * tp + 1][pp], sA + offA[h][pp] + tp * 2048);
-                } else {
-#pragma unroll
-                    for (int u = 0; u < 8; ++u) lds128(a[u][0], a[u][1], sA + offA[h][0] + u * 8 * 128);
-                }
-                if (!TB) {
-#pragma unroll
-                    for (int u = 0; u < 4; ++u) lds128(b[u][0], b[u][1], sB + offB[h][0] + u * 8 * 128);
-                } else {
-#pragma unroll
-                    for (int tp = 0; tp < 2; ++tp)
-#pragma unroll
-                        for (int pp = 0; pp < 2; ++pp)
-                            lds128(b[2 * tp][pp], b[2 * tp + 1][pp], sB + offB[h][pp] + tp * 2048);
-                }
-                if (h == 1) {
-                    // all reads of this stage are issued; hand the slot back to the producer
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(bar_empty + 8 * stage);
-                }
-#pragma unroll
-                for (int pp = 0; pp < 2; ++pp)
-#pragma unroll
-                    for (int i = 0; i < 8; ++i)
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) dmma_m8n8k4(acc[i][j][0], acc[i][j][1], a[i][pp], b[j][pp]);
-            }
+            mma_slab<TA, TB>(acc, ring, stage, phase, c);
             if (++stage == NUM_STAGES) { stage = 0; phase ^= 1; }
         }
 
-        // ---------------- epilogue: C = alpha*acc + beta*C ----------------
-        // lane holds C[mrow(i-tile, r)][ncol(j-tile, 2q + jj)]
-        const double alpha = p.alpha, beta = p.beta;
-        const bool use_beta = (beta != 0.0);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-#pragma unroll
-            for (int jj = 0; jj < 2; ++jj) {
-                const int cj = 2 * q + jj;
-                const int n = n0 + warp_n * 32 + (!TB ? (8 * j + perm8(cj)) : (16 * (j >> 1) + 2 * cj + (j & 1)));
-                if (n >= p.N) continue;
-                double* ccol = Cout + (long long)n * p.ldc;
-                if (!TA) {
-#pragma unroll
-                    for (int tp = 0; tp < 4; ++tp) {
-                        const int m = m0 + warp_m * 64 + 16 * tp + 2 * r;
-                        if (m >= p.M) continue;
-                        double v0 = alpha * acc[2 * tp][j][jj];
-                        double v1 = alpha * acc[2 * tp + 1][j][jj];
-                        if (vec_ok && m + 1 < p.M) {
-                            double2* ptr = reinterpret_cast<double2*>(ccol + m);
-                            if (use_beta) {
-                                const double2 old = *ptr;
-                                v0 += beta * old.x;
-                                v1 += beta * old.y;
-                            }
-                            *ptr = make_double2(v0, v1);
-                        } else {
-                            if (use_beta) v0 += beta * ccol[m];
-                            ccol[m] = v0;
-                            if (m + 1 < p.M) {
-                                if (use_beta) v1 += beta * ccol[m + 1];
-                                ccol[m + 1] = v1;
-                            }
-                        }
-                    }
-                } else {
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) {
-                        const int m = m0 + warp_m * 64 + 8 * i + pr;
-                        if (m >= p.M) continue;
-                        double v = alpha * acc[i][j][jj];
-                        if (use_beta) v += beta * ccol[m];
-                        ccol[m] = v;
-                    }
-                }
-            }
-        }
+        store_tile<TA, TB>(acc, c, tm_ * BM, tn_ * BN, p.M, p.N, Cout, p.ldc, vec_ok,
+                           ScaleAddC{Cout, p.ldc, p.alpha, p.beta, p.beta != 0.0});
     }
 }
 
@@ -385,24 +456,30 @@ __device__ __forceinline__ void wait_flag_ge(const unsigned long long* flag, uns
     }
 }
 
+// D = acc + Cin, or D = acc without an addend.  Cin is read with __ldcg: another GPU wrote it during this launch.
+struct AddCin {
+    const double* Cin;
+    long long ldcin;
+    __device__ __forceinline__ double scale(double a) const { return a; }
+    __device__ __forceinline__ const double* column(int n) const { return Cin ? Cin + (long long)n * ldcin : nullptr; }
+    __device__ __forceinline__ void add(double& v, const double* col, int m) const {
+        if (col) v += __ldcg(col + m);
+    }
+    __device__ __forceinline__ void add2(double& v0, double& v1, const double* col, int m) const {
+        if (col) {
+            const double2 old = __ldcg(reinterpret_cast<const double2*>(col + m));
+            v0 += old.x;
+            v1 += old.y;
+        }
+    }
+};
+
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_f64_dmma_grouped_kernel(const __grid_constant__ G2Params g) {
-    extern __shared__ uint8_t smem_raw[];
-    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const uint32_t bar_full = smem_base + NUM_STAGES * STAGE_BYTES;
-    const uint32_t bar_empty = bar_full + NUM_STAGES * 8;
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     const int num_tiles = g.num_tiles;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < NUM_STAGES; ++s) {
-            mbar_init(bar_full + 8 * s, 1);
-            mbar_init(bar_empty + 8 * s, NUM_CONSUMER_WARPS);
-        }
-        fence_barrier_init();
-    }
-    __syncthreads();
+    const Ring ring = ring_setup(nullptr, nullptr);
 
     auto locate = [&](int t, int& c, int& tm, int& tn) {
         c = 0;
@@ -429,19 +506,9 @@ gemm_f64_dmma_grouped_kernel(const __grid_constant__ G2Params g) {
                     if (g.b_ready[ib] >= 0)
                         wait_flag_ge<false>(g.ready + g.b_ready[ib] + n0 / g.b_band[ib], g.ready_val, g.timeout_ns, g.status,
                                             (1ull << 56) | (2ull << 48) | (unsigned long long)(g.b_ready[ib] + n0 / g.b_band[ib]));
-                    const CUtensorMap* mA = &g.mapA[ia];
-                    const CUtensorMap* mB = &g.mapB[ib];
                     const int nkb = en.nkb[sg];
                     for (int kb = 0; kb < nkb; ++kb) {
-                        mbar_wait(bar_empty + 8 * stage, phase ^ 1);
-                        const uint32_t full = bar_full + 8 * stage;
-                        const uint32_t sA = smem_base + stage * STAGE_BYTES;
-                        const uint32_t sB = sA + OPERAND_BYTES;
-                        mbar_arrive_expect_tx(full, STAGE_BYTES);
-                        const int k0 = kb * BK;
-#pragma unroll
-                        for (int b = 0; b < 8; ++b) tma_load_2d(sA + b * 2048, mA, full, m0 + 16 * b, k0);
-                        tma_load_2d(sB, mB, full, k0, n0);
+                        load_slab<false, false>(ring, stage, phase ^ 1, &g.mapA[ia], &g.mapB[ib], m0, n0, kb);
                         if (++stage == NUM_STAGES) { stage = 0; phase ^= 1; }
                     }
                 }
@@ -452,22 +519,7 @@ gemm_f64_dmma_grouped_kernel(const __grid_constant__ G2Params g) {
 
     setmaxnreg_inc<232>();
     const int cw = warp - 4;
-    const int warp_m = cw & 1;
-    const int warp_n = cw >> 1;
-    const int r = lane >> 2;
-    const int q = lane & 3;
-    const int pr = perm8(r);
-    uint32_t offA[2][2], offB[2];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-#pragma unroll
-        for (int pp = 0; pp < 2; ++pp) {
-            const int krow = 8 * h + 2 * q + pp;
-            offA[h][pp] = warp_m * 4 * 2048 + krow * 128 + ((r ^ (krow & 7)) << 4);
-        }
-        offB[h] = warp_n * 32 * 128 + pr * 128 + ((((4 * h + q) ^ pr) & 7) << 4);
-    }
-
+    const Consumer cons = consumer_lane<false, false>(cw, lane);
     int stage = 0;
     uint32_t phase = 0;
     const unsigned long long* cin_seen = nullptr;      // last addend flag this thread has already observed
@@ -475,7 +527,6 @@ gemm_f64_dmma_grouped_kernel(const __grid_constant__ G2Params g) {
         int c, tm_, tn_;
         locate(t, c, tm_, tn_);
         const G2Ent& en = g.e[c];
-        const int m0 = tm_ * BM, n0 = tn_ * BN;       // relative to the entry's region
         int total_kb = 0;
         for (int sg = 0; sg < en.nseg; ++sg) total_kb += en.nkb[sg];
         double acc[8][4][2];
@@ -485,77 +536,26 @@ gemm_f64_dmma_grouped_kernel(const __grid_constant__ G2Params g) {
             for (int j = 0; j < 4; ++j) acc[i][j][0] = acc[i][j][1] = 0.0;
 
         for (int kb = 0; kb < total_kb; ++kb) {
-            mbar_wait(bar_full + 8 * stage, phase);
-            const uint32_t sA = smem_base + stage * STAGE_BYTES;
-            const uint32_t sB = sA + OPERAND_BYTES;
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                double a[8][2], b[4][2];
-#pragma unroll
-                for (int tp = 0; tp < 4; ++tp)
-#pragma unroll
-                    for (int pp = 0; pp < 2; ++pp) lds128(a[2 * tp][pp], a[2 * tp + 1][pp], sA + offA[h][pp] + tp * 2048);
-#pragma unroll
-                for (int u = 0; u < 4; ++u) lds128(b[u][0], b[u][1], sB + offB[h] + u * 8 * 128);
-                if (h == 1) {
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(bar_empty + 8 * stage);
-                }
-#pragma unroll
-                for (int pp = 0; pp < 2; ++pp)
-#pragma unroll
-                    for (int i = 0; i < 8; ++i)
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) dmma_m8n8k4(acc[i][j][0], acc[i][j][1], a[i][pp], b[j][pp]);
-            }
+            mma_slab<false, false>(acc, ring, stage, phase, cons);
             if (++stage == NUM_STAGES) { stage = 0; phase ^= 1; }
         }
 
         // ---------------- epilogue: D = acc (+ Cin) ----------------
-        double* Db = en.D;
-        const double* Ci = en.Cin;
-        const long long ldd = en.ldd, ldci = en.ldcin;
+        double* D = en.D;
+        const AddCin add{en.Cin, en.ldcin};
+        const long long ldd = en.ldd;
         const int Mc = en.M, Nc = en.N;
-        if (Ci != nullptr && en.cin_flag != nullptr && en.cin_flag != cin_seen) {
+        if (add.Cin != nullptr && en.cin_flag != nullptr && en.cin_flag != cin_seen) {
             // the other holder's partial must have landed in this GPU's staging buffer (every lane acquires)
             if (g.poll_mode == 0 || lane == 0)
                 wait_flag_ge<true>(en.cin_flag, en.cin_val, g.timeout_ns, g.status, (1ull << 56) | (3ull << 48) | (unsigned long long)c);
             if (g.poll_mode != 0) __syncwarp();
             cin_seen = en.cin_flag;
         }
-        const bool vec_ok = ((reinterpret_cast<uintptr_t>(Db) & 15) == 0) && ((ldd & 1) == 0) &&
-                            (Ci == nullptr || (((reinterpret_cast<uintptr_t>(Ci) & 15) == 0) && ((ldci & 1) == 0)));
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-#pragma unroll
-            for (int jj = 0; jj < 2; ++jj) {
-                const int n = n0 + warp_n * 32 + 8 * j + perm8(2 * q + jj);
-                if (n >= Nc) continue;
-                double* dcol = Db + (long long)n * ldd;
-                const double* ccol = Ci ? Ci + (long long)n * ldci : nullptr;
-#pragma unroll
-                for (int tp = 0; tp < 4; ++tp) {
-                    const int m = m0 + warp_m * 64 + 16 * tp + 2 * r;
-                    if (m >= Mc) continue;
-                    double v0 = acc[2 * tp][j][jj], v1 = acc[2 * tp + 1][j][jj];
-                    if (vec_ok && m + 1 < Mc) {
-                        if (ccol) {
-                            const double2 old = __ldcg(reinterpret_cast<const double2*>(ccol + m));
-                            v0 += old.x;
-                            v1 += old.y;
-                        }
-                        *reinterpret_cast<double2*>(dcol + m) = make_double2(v0, v1);
-                    } else {
-                        if (ccol) v0 += __ldcg(ccol + m);
-                        dcol[m] = v0;
-                        if (m + 1 < Mc) {
-                            if (ccol) v1 += __ldcg(ccol + m + 1);
-                            dcol[m + 1] = v1;
-                        }
-                    }
-                }
-            }
-        }
+        const bool vec_ok = ((reinterpret_cast<uintptr_t>(D) & 15) == 0) && ((ldd & 1) == 0) &&
+                            (add.Cin == nullptr || (((reinterpret_cast<uintptr_t>(add.Cin) & 15) == 0) && ((add.ldcin & 1) == 0)));
+        // tile coordinates relative to the entry's region
+        store_tile<false, false>(acc, cons, tm_ * BM, tn_ * BN, Mc, Nc, D, ldd, vec_ok, add);
         if (en.done_ctr != nullptr) {
             // every consumer thread's stores of this tile, then ONE thread counts the tile and, if it was the entry's last,
             // publishes the completion flags with system scope (peer GPUs and the copy streams poll them).
@@ -653,58 +653,22 @@ __global__ void scale_matrix_kernel(int M, int N, double beta, double* C, long l
     }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+// How the DMMA kernels stage an fp64 operand that is mn x k in the product (mn = M for A, N for B).
+enum class Form {
+    MN,   // stored mn x k, mn contiguous: 8 boxes of [16 k][16 mn] per slab (A 'N', B 'T')
+    K,    // stored k x mn, k contiguous: one box of [128 mn][16 k] per slab (A 'T', B 'N')
+};
 
-EncodeTiledFn get_encode_fn() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
-        void* ptr = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess &&
-            qres == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<EncodeTiledFn>(ptr);
-    }
-    return fn;
-}
-
-// 2-D fp64 tensor map over a column-major array: dim0 (contiguous) x dim1 (stride ld), 128B swizzle.
-bool make_map_f64(CUtensorMap* map, const double* base, uint64_t dim0, uint64_t dim1, uint64_t ld,
-                  uint32_t box0, uint32_t box1) {
-    EncodeTiledFn fn = get_encode_fn();
-    if (!fn) return false;
-    cuuint64_t dims[2] = {dim0, dim1};
-    cuuint64_t strides[1] = {ld * 8};
-    cuuint32_t box[2] = {box0, box1};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT64, 2, const_cast<double*>(base), dims, strides, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    return r == CUDA_SUCCESS;
-}
-
-template <bool TA, bool TB>
-cudaError_t launch_dmma(const CUtensorMap& mA, const CUtensorMap& mB, const Params& p, int num_sms,
-                        cudaStream_t stream) {
-    auto kern = gemm_f64_dmma_kernel<TA, TB>;
-    // per template instantiation; idempotent, so concurrent first calls may both set it (no unsynchronised flag)
-    static std::atomic<bool> attr_done{false};
-    if (!attr_done.load(std::memory_order_acquire)) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-        if (e != cudaSuccess) return e;
-        attr_done.store(true, std::memory_order_release);
-    }
-    const int grid = min(p.tiles_m * p.tiles_n, num_sms);
-    kern<<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(mA, mB, p);
-    return cudaGetLastError();
+bool operand_map(CUtensorMap* map, const double* base, int mn, int k, long long ld, Form form) {
+    return form == Form::MN ? tma_map(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT64, base, mn, k, ld * 8, 16, 16)
+                            : tma_map(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT64, base, k, mn, ld * 8, 16, 128);
 }
 
 }  // namespace
 
 bool gemm_f64_tma_eligible(const double* A, long long lda, const double* B, long long ldb) {
     return ((reinterpret_cast<uintptr_t>(A) & 15) == 0) && ((reinterpret_cast<uintptr_t>(B) & 15) == 0) &&
-           (lda % 2 == 0) && (ldb % 2 == 0) && get_encode_fn() != nullptr;
+           (lda % 2 == 0) && (ldb % 2 == 0) && tma_encode_fn() != nullptr;
 }
 
 cudaError_t gemm_f64(bool transA, bool transB, int M, int N, int K, double alpha, const double* A, long long lda,
@@ -719,21 +683,18 @@ cudaError_t gemm_f64(bool transA, bool transB, int M, int N, int K, double alpha
     }
     if (!force_generic && gemm_f64_tma_eligible(A, lda, B, ldb)) {
         CUtensorMap mA, mB;
-        bool ok = true;
-        // A: 'N' -> stored M x K (m contiguous), MN form boxes [16 m][16 k]; 'T' -> stored K x M, K form box [16 k][128 m]
-        ok = ok && (!transA ? make_map_f64(&mA, A, M, K, lda, 16, 16) : make_map_f64(&mA, A, K, M, lda, 16, 128));
-        // B: 'N' -> stored K x N (k contiguous), K form box [16 k][128 n]; 'T' -> stored N x K, MN form boxes [16 n][16 k]
-        ok = ok && (!transB ? make_map_f64(&mB, B, K, N, ldb, 16, 128) : make_map_f64(&mB, B, N, K, ldb, 16, 16));
-        if (ok) {
+        if (operand_map(&mA, A, M, K, lda, transA ? Form::K : Form::MN) &&
+            operand_map(&mB, B, N, K, ldb, transB ? Form::MN : Form::K)) {
             Params p;
             p.M = M; p.N = N; p.K = K; p.alpha = alpha; p.beta = beta; p.C = C; p.ldc = ldc;
             p.tiles_m = (M + BM - 1) / BM;
             p.tiles_n = (N + BN - 1) / BN;
             if (launches) ++*launches;
-            if (!transA && !transB) return launch_dmma<false, false>(mA, mB, p, num_sms, stream);
-            if (transA && !transB) return launch_dmma<true, false>(mA, mB, p, num_sms, stream);
-            if (!transA && transB) return launch_dmma<false, true>(mA, mB, p, num_sms, stream);
-            return launch_dmma<true, true>(mA, mB, p, num_sms, stream);
+            const int grid = min(p.tiles_m * p.tiles_n, num_sms);
+            if (!transA && !transB) return launch_with_smem<gemm_f64_dmma_kernel<false, false>>(grid, NUM_THREADS, SMEM_BYTES, stream, mA, mB, p);
+            if (transA && !transB) return launch_with_smem<gemm_f64_dmma_kernel<true, false>>(grid, NUM_THREADS, SMEM_BYTES, stream, mA, mB, p);
+            if (!transA && transB) return launch_with_smem<gemm_f64_dmma_kernel<false, true>>(grid, NUM_THREADS, SMEM_BYTES, stream, mA, mB, p);
+            return launch_with_smem<gemm_f64_dmma_kernel<true, true>>(grid, NUM_THREADS, SMEM_BYTES, stream, mA, mB, p);
         }
     }
     dim3 grid((M + 63) / 64, (N + 63) / 64);
@@ -851,10 +812,9 @@ size_t gram_workspace_doubles(int n, long long K, int num_sms) {
 cudaError_t gram_f64(bool trans, int n, int K, const double* A, long long lda, double* G, long long ldg, double* ws,
                      int num_sms, cudaStream_t stream, int* launches) {
     if (n <= 0) return cudaSuccess;
-    CUtensorMap mA, mB;
-    const bool tma = K > 0 && gemm_f64_tma_eligible(A, lda, A, lda) &&
-                     (!trans ? (make_map_f64(&mA, A, n, K, lda, 16, 16) && make_map_f64(&mB, A, n, K, lda, 16, 16))
-                             : (make_map_f64(&mA, A, K, n, lda, 16, 128) && make_map_f64(&mB, A, K, n, lda, 16, 128)));
+    // op(A) and op(A)^T are read from the same storage in the same form, so A and B share one map
+    CUtensorMap mA;
+    const bool tma = K > 0 && gemm_f64_tma_eligible(A, lda, A, lda) && operand_map(&mA, A, n, K, lda, trans ? Form::K : Form::MN);
     const int splits = tma ? gram_splits(n, K, num_sms) : 1;
     if (splits > 1 && ws == nullptr) return cudaErrorInvalidValue;
     // one split: the product goes straight into G and the mirror pass runs in place
@@ -872,11 +832,10 @@ cudaError_t gram_f64(bool trans, int n, int K, const double* A, long long lda, d
         sk.tri_tiles = t * (t + 1) / 2;
         sk.kchunk = (int)((kb + splits - 1) / splits) * BK;
         sk.split_stride = ldp * n;
-        auto kern = !trans ? syrk_f64_dmma_kernel<false, true> : syrk_f64_dmma_kernel<true, false>;
-        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
+        const int grid = min(sk.tri_tiles * splits, num_sms);
+        e = !trans ? launch_with_smem<syrk_f64_dmma_kernel<false, true>>(grid, NUM_THREADS, SMEM_BYTES, stream, mA, mA, p, sk)
+                   : launch_with_smem<syrk_f64_dmma_kernel<true, false>>(grid, NUM_THREADS, SMEM_BYTES, stream, mA, mA, p, sk);
         if (e != cudaSuccess) return e;
-        kern<<<min(sk.tri_tiles * splits, num_sms), NUM_THREADS, SMEM_BYTES, stream>>>(mA, mB, p, sk);
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
         if (launches) ++*launches;
     } else {
         // the whole product on the CUDA cores (views TMA cannot address), or zeros for K = 0
@@ -895,12 +854,12 @@ cudaError_t gram_f64(bool trans, int n, int K, const double* A, long long lda, d
 
 cudaError_t gemm_f64_grouped2(const G2Launch& L, int num_sms, cudaStream_t stream, int* launches) {
     if (L.ne <= 0) return cudaSuccess;
-    if (L.ne > G2_MAX_ENTRIES || L.na > G2_MAX_OPS || L.nb > G2_MAX_OPS || !get_encode_fn()) return cudaErrorNotSupported;
+    if (L.ne > G2_MAX_ENTRIES || L.na > G2_MAX_OPS || L.nb > G2_MAX_OPS || !tma_encode_fn()) return cudaErrorNotSupported;
     static thread_local G2Params g;          // ~20 KB parameter block: kept off the stack, one per calling thread
     for (int i = 0; i < L.na; ++i) {
         const G2Operand& o = L.A[i];
         if (o.rows <= 0 || o.cols <= 0 || !gemm_f64_tma_eligible(o.ptr, o.ld, o.ptr, 2)) return cudaErrorNotSupported;
-        if (!make_map_f64(&g.mapA[i], o.ptr, o.rows, o.cols, o.ld, 16, 16)) return cudaErrorNotSupported;
+        if (!operand_map(&g.mapA[i], o.ptr, o.rows, o.cols, o.ld, Form::MN)) return cudaErrorNotSupported;
         if (o.ready_base >= 0 && (o.band <= 0 || o.band % BM != 0)) return cudaErrorInvalidValue;
         g.a_band[i] = o.band > 0 ? o.band : (1 << 30);
         g.a_ready[i] = (short)o.ready_base;
@@ -908,7 +867,7 @@ cudaError_t gemm_f64_grouped2(const G2Launch& L, int num_sms, cudaStream_t strea
     for (int i = 0; i < L.nb; ++i) {
         const G2Operand& o = L.B[i];
         if (o.rows <= 0 || o.cols <= 0 || !gemm_f64_tma_eligible(o.ptr, o.ld, o.ptr, 2)) return cudaErrorNotSupported;
-        if (!make_map_f64(&g.mapB[i], o.ptr, o.rows, o.cols, o.ld, 16, 128)) return cudaErrorNotSupported;
+        if (!operand_map(&g.mapB[i], o.ptr, o.cols, o.rows, o.ld, Form::K)) return cudaErrorNotSupported;
         if (o.ready_base >= 0 && (o.band <= 0 || o.band % BN != 0)) return cudaErrorInvalidValue;
         g.b_band[i] = o.band > 0 ? o.band : (1 << 30);
         g.b_ready[i] = (short)o.ready_base;
@@ -945,16 +904,9 @@ cudaError_t gemm_f64_grouped2(const G2Launch& L, int num_sms, cudaStream_t strea
     g.fence_all = fence_all;
     static const int poll_mode = [] { const char* e = getenv("MARLIN_B200_CIN_POLL"); return (e && e[0] == '1') ? 1 : 0; }();
     g.poll_mode = poll_mode;
-    static std::atomic<bool> attr_done{false};
-    if (!attr_done.load(std::memory_order_acquire)) {
-        cudaError_t e = cudaFuncSetAttribute(gemm_f64_dmma_grouped_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-        if (e != cudaSuccess) return e;
-        attr_done.store(true, std::memory_order_release);
-    }
-    const int grid = min(tiles, num_sms);
-    gemm_f64_dmma_grouped_kernel<<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(g);
-    if (launches) ++*launches;
-    return cudaGetLastError();
+    const cudaError_t e = launch_with_smem<gemm_f64_dmma_grouped_kernel>(min(tiles, num_sms), NUM_THREADS, SMEM_BYTES, stream, g);
+    if (launches && e == cudaSuccess) ++*launches;
+    return e;
 }
 
 cudaError_t gemm_f64_grouped(int m, int k, int n, const int* my_c, int num_c, const double* const* A, const long long* lda,

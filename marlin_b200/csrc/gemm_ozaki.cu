@@ -18,7 +18,7 @@
 // bracket of a group the consumers fold the accumulator into C with an fp64 read-modify-write.
 #include "gemm_ozaki.h"
 #include "ptx.cuh"
-#include <atomic>
+#include "tma.h"
 
 namespace mb {
 
@@ -336,34 +336,6 @@ __global__ void __launch_bounds__(128) ozaki_fixup_kernel(const double* __restri
     }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn get_encode_fn() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
-        void* ptr = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess &&
-            qres == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<EncodeTiledFn>(ptr);
-    }
-    return fn;
-}
-
-bool make_map_i8_3d(CUtensorMap* map, const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t stride1,
-                    uint64_t stride2, uint32_t b0, uint32_t b1) {
-    EncodeTiledFn fn = get_encode_fn();
-    if (!fn) return false;
-    cuuint64_t dims[3] = {d0, d1, d2};
-    cuuint64_t strides[2] = {stride1, stride2};
-    cuuint32_t box[3] = {b0, b1, 1};
-    cuuint32_t estr[3] = {1, 1, 1};
-    return fn(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<void*>(base), dims, strides, box, estr,
-              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
 inline size_t round_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
 }  // namespace
@@ -377,7 +349,7 @@ size_t ozaki_workspace_bytes(int M, int N, int K, int s) {
 bool ozaki_supported(int M, int N, int K, int s, int bits) {
     // int32 accumulation of up to s pairs of K products of magnitude <= 2^(2*(bits-1)) must stay below 2^31
     return s >= 2 && s <= 8 && (bits == 7 || bits == 8) && M > 0 && N > 0 && K > 0 &&
-           (long long)K * s * (1ll << (2 * (bits - 1))) < (1ll << 31) && get_encode_fn() != nullptr;
+           (long long)K * s * (1ll << (2 * (bits - 1))) < (1ll << 31) && tma_encode_fn() != nullptr;
 }
 
 cudaError_t gemm_f64_ozaki(int M, int N, int K, const double* A, long long lda, const double* B, long long ldb, double* C,
@@ -410,23 +382,16 @@ cudaError_t gemm_f64_ozaki(int M, int N, int K, const double* A, long long lda, 
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
 
     CUtensorMap mA, mB;
-    if (!make_map_i8_3d(&mA, A8, K, M, s, ldA, planeA, 128, 128)) return cudaErrorNotSupported;
-    if (!make_map_i8_3d(&mB, B8, K, N, s, ldB, planeB, 128, 256)) return cudaErrorNotSupported;
+    if (!tma_map_3d(&mA, CU_TENSOR_MAP_DATA_TYPE_UINT8, A8, K, M, s, ldA, planeA, 128, 128)) return cudaErrorNotSupported;
+    if (!tma_map_3d(&mB, CU_TENSOR_MAP_DATA_TYPE_UINT8, B8, K, N, s, ldB, planeB, 128, 256)) return cudaErrorNotSupported;
     Params p;
     p.M = M; p.N = N; p.K = K; p.s = s; p.bits = bits; p.P = P; p.C = C; p.ldc = ldc; p.eA = eA; p.eB = eB;
     p.tiles_m = (M + BM - 1) / BM;
     p.tiles_n = (N + BN - 1) / BN;
     p.accumulate = accumulate ? 1 : 0;
-    static std::atomic<bool> attr_done{false};   // idempotent attribute set; atomic so threads sharing a context may race here
-    if (!attr_done.load(std::memory_order_acquire)) {
-        e = cudaFuncSetAttribute(gemm_ozaki_i8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-        if (e != cudaSuccess) return e;
-        attr_done.store(true, std::memory_order_release);
-    }
-    const int grid = min(p.tiles_m * p.tiles_n, num_sms);
-    gemm_ozaki_i8_kernel<<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(mA, mB, p);
+    e = launch_with_smem<gemm_ozaki_i8_kernel>(min(p.tiles_m * p.tiles_n, num_sms), NUM_THREADS, SMEM_BYTES, stream, mA, mB, p);
+    if (e != cudaSuccess) return e;
     if (launches) ++*launches;
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
     // stream-ordered after the int8 kernel, which leaves the flagged entries of C as they were (accumulate) or +0
     ozaki_fixup_kernel<<<M + N, 128, 0, stream>>>(A, lda, B, ldb, C, ldc, M, N, K, p.accumulate, eA, eB);
     if (launches) ++*launches;
