@@ -125,6 +125,14 @@ int32_t mb_dgemm_device_generic(mb_ctx* ctx, char transa, char transb, int32_t m
                                 double alpha, const double* A, int32_t lda, const double* B, int32_t ldb,
                                 double beta, double* C, int32_t ldc);
 
+/* Test and measurement hook, not a user option (off by default).  on != 0: every fp64 DMMA kernel that later calls on ctx
+ * launch (block and device GEMMs, the grouped blocked multiply, the distributed multiply, the row-sharded multiply, the
+ * factorizations' updates and the Gramian) runs its m8n8k4 instance (SASS DMMA.8x8x4) instead of the m16n8k4 one
+ * (DMMA.16x8x4, twice the issue rate on H100).  The two share all source but the instruction shape and give the same
+ * results bit for bit: the m8n8k4 instances are the reference the m16n8k4 kernels are tested against and the A/B switch
+ * for measuring them. */
+int32_t mb_set_dmma_reference(mb_ctx* ctx, int32_t on);
+
 /* ---- a2/a10: SubMatrix.add/subtract/scalar ops (matrix/SubMatrix.scala:41-85,123-131),
  *      BlockMatrix.subtractBy/divideBy (matrix/BlockMatrix.scala:414-452) ------------------- */
 int32_t mb_block_add(mb_ctx* ctx, const mb_block* A, const mb_block* B, mb_block* out);      /* A + B */

@@ -423,6 +423,12 @@ int32_t mb_set_fp64_mode(mb_ctx* ctx, int32_t mode, int32_t slices) {
     return MB_OK;
 }
 
+int32_t mb_set_dmma_reference(mb_ctx* ctx, int32_t on) {
+    if (!ctx) return fail(MB_ERR_INVALID_ARG, "null context");
+    ctx->dmma_reference = on != 0;
+    return MB_OK;
+}
+
 int32_t mb_dgemm_device(mb_ctx* ctx, char transa, char transb, int32_t m, int32_t n, int32_t k, double alpha,
                         const double* A, int32_t lda, const double* B, int32_t ldb, double beta, double* C, int32_t ldc) {
     return dgemm_device_impl(ctx, transa, transb, m, n, k, alpha, A, lda, B, ldb, beta, C, ldc, false);

@@ -1,8 +1,8 @@
 // fp64 block GEMM for sm_90a — replaces SubMatrix.multiply -> Breeze `*` -> netlib dgemm
 // (reference: matrix/SubMatrix.scala:87-91; inline twins matrix/DenseVecMatrix.scala:122,129,1676).
 //
-// wgmma has no fp64 type, so the fp64 tensor-core path on H100 is
-// DMMA (mma.sync.m8n8k4.f64 -> SASS DMMA.8x8x4).  Design:
+// wgmma has no fp64 type, so the fp64 tensor-core path on H100 is DMMA: mma.sync.m16n8k4.f64 (SASS DMMA.16x8x4), which
+// issues at twice the rate of the Ampere shape m8n8k4 (SASS DMMA.8x8x4).  Design:
 //   * persistent CTAs (one per SM), 128x128 C tile per CTA, accumulators in registers
 //     (8 consumer warps x 64x32 warp tile = 64 doubles / thread);
 //   * a dedicated producer warp streams A/B k-slabs (BK = 16) through a 6-stage shared-memory
@@ -18,11 +18,17 @@
 // dimension is M/N ("MN form") is staged as 8 boxes of [16 k-rows][16 mn] and one whose
 // contiguous dimension is K ("K form") as one box of [128 mn-rows][16 k] (operand_map).
 //
-// Three kernels run this mainloop: gemm_f64_dmma_kernel (every tile of C), syrk_f64_dmma_kernel (the Gramian's
-// lower-triangle tiles, split over K) and gemm_f64_dmma_grouped_kernel (a list of C regions, each over its own K
+// Three kernels run this mainloop: gemm_f64_dmma16x8_kernel (every tile of C), syrk_f64_dmma16x8_kernel (the Gramian's
+// lower-triangle tiles, split over K) and gemm_f64_dmma16x8_grouped_kernel (a list of C regions, each over its own K
 // segments).  They share one set of pieces, templated on the operands' forms: ring_setup, load_slab (producer),
 // consumer_lane + mma_slab (consumers) and store_tile (epilogue).  Each kernel keeps only its tile schedule, its K
 // range and what its epilogue waits for or signals.
+//
+// Each of the three also exists as an m8n8k4 instance under its older name (gemm_f64_dmma_kernel, syrk_f64_dmma_kernel,
+// gemm_f64_dmma_grouped_kernel): the same source with only the instruction shape changed (mma_slab).  m16n8k4 is two
+// m8n8k4 stacked in M that share the B fragment, so both shapes give every element of C the same 4-term steps over the
+// same k in the same order, and the results are identical bit for bit.  The m8n8k4 instances are the in-library
+// reference of the production kernels and run only when a context asks for them (mb_set_dmma_reference).
 #include "gemm_f64.h"
 #include "ptx.cuh"
 #include "tma.h"
@@ -40,6 +46,12 @@ constexpr int NUM_CONSUMER_WARPS = 8;
 constexpr int NUM_THREADS = 128 + NUM_CONSUMER_WARPS * 32;   // producer warpgroup + 2 consumer warpgroups
 constexpr int SMEM_BYTES = NUM_STAGES * STAGE_BYTES + 2 * NUM_STAGES * 8 + 1024;
 constexpr int BAND = 16;                            // tile-rows per rasterisation band (L2 reuse)
+
+// The DMMA instruction shape of the mainloop: m16n8k4 in production, m8n8k4 for the reference instances.
+enum class Dmma { m8n8k4, m16n8k4 };
+
+// Set by every C-ABI entry from its context (mb_set_dmma_reference) before it launches anything.
+thread_local bool g_dmma_reference = false;
 
 struct Params {
     int M, N, K;
@@ -167,8 +179,9 @@ __device__ __forceinline__ Consumer consumer_lane(int cw, int lane) {
 }
 
 // Consumer: wait for the slab in `stage`, read the fragments (24 LDS.128 per warp), hand the stage back to the producer
-// and issue the slab's 128 DMMA into acc.
-template <bool TA, bool TB>
+// and issue the slab into acc: 128 m8n8k4, or 64 m16n8k4 that each take m-tiles 2i' and 2i'+1 together (for an MN-form
+// A the two a values come from one LDS.128 and are adjacent registers already).
+template <Dmma S, bool TA, bool TB>
 __device__ __forceinline__ void mma_slab(double (&acc)[8][4][2], const Ring& ring, int stage, uint32_t phase,
                                          const Consumer c) {
     mbar_wait(ring.full + 8 * stage, phase);
@@ -201,12 +214,23 @@ __device__ __forceinline__ void mma_slab(double (&acc)[8][4][2], const Ring& rin
             __syncwarp();
             if (c.lane == 0) mbar_arrive(ring.empty + 8 * stage);
         }
+        if constexpr (S == Dmma::m8n8k4) {
 #pragma unroll
-        for (int pp = 0; pp < 2; ++pp)
+            for (int pp = 0; pp < 2; ++pp)
 #pragma unroll
-            for (int i = 0; i < 8; ++i)
+                for (int i = 0; i < 8; ++i)
 #pragma unroll
-                for (int j = 0; j < 4; ++j) dmma_m8n8k4(acc[i][j][0], acc[i][j][1], a[i][pp], b[j][pp]);
+                    for (int j = 0; j < 4; ++j) dmma_m8n8k4(acc[i][j][0], acc[i][j][1], a[i][pp], b[j][pp]);
+        } else {
+#pragma unroll
+            for (int pp = 0; pp < 2; ++pp)
+#pragma unroll
+                for (int i = 0; i < 8; i += 2)
+#pragma unroll
+                    for (int j = 0; j < 4; ++j)
+                        dmma_m16n8k4(acc[i][j][0], acc[i][j][1], acc[i + 1][j][0], acc[i + 1][j][1], a[i][pp], a[i + 1][pp],
+                                     b[j][pp]);
+        }
     }
 }
 
@@ -286,7 +310,7 @@ struct ScaleAddC {
 
 // The persistent TMA + DMMA mainloop shared by the GEMM (SYRK = false: every tile of C, the whole K range, C = alpha*acc +
 // beta*C) and the Gramian (SYRK = true: lower-triangle tiles only, split-K partials stored to a workspace).
-template <bool TA, bool TB, bool SYRK>
+template <Dmma S, bool TA, bool TB, bool SYRK>
 __device__ __forceinline__ void dmma_persistent(const CUtensorMap& mapA, const CUtensorMap& mapB, const Params& p,
                                                 const SyrkSched& sk) {
     const int warp = threadIdx.x >> 5;
@@ -350,7 +374,7 @@ __device__ __forceinline__ void dmma_persistent(const CUtensorMap& mapA, const C
         // bounded by p.K (a kernel parameter) rather than num_kb: one register fewer, which the <N,T> instance needs
         // to fit sm_90a's 168-register budget without a spill
         for (int k0 = k_begin; k0 < k_end; k0 += BK) {
-            mma_slab<TA, TB>(acc, ring, stage, phase, c);
+            mma_slab<S, TA, TB>(acc, ring, stage, phase, c);
             if (++stage == NUM_STAGES) { stage = 0; phase ^= 1; }
         }
 
@@ -361,17 +385,32 @@ __device__ __forceinline__ void dmma_persistent(const CUtensorMap& mapA, const C
 
 template <bool TA, bool TB>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_f64_dmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
-                     const Params p) {
-    dmma_persistent<TA, TB, false>(mapA, mapB, p, SyrkSched{});
+gemm_f64_dmma16x8_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
+                         const Params p) {
+    dmma_persistent<Dmma::m16n8k4, TA, TB, false>(mapA, mapB, p, SyrkSched{});
 }
 
 // Gramian partials: only the lower-triangle tiles of C = op(A) op(B) with op(B) = op(A)^T, split over K (see SyrkSched).
 template <bool TA, bool TB>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
+syrk_f64_dmma16x8_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
+                         const Params p, const SyrkSched sk) {
+    dmma_persistent<Dmma::m16n8k4, TA, TB, true>(mapA, mapB, p, sk);
+}
+
+// The m8n8k4 reference instances of the two (see the top of the file).
+template <bool TA, bool TB>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+gemm_f64_dmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
+                     const Params p) {
+    dmma_persistent<Dmma::m8n8k4, TA, TB, false>(mapA, mapB, p, SyrkSched{});
+}
+
+template <bool TA, bool TB>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
 syrk_f64_dmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
                      const Params p, const SyrkSched sk) {
-    dmma_persistent<TA, TB, true>(mapA, mapB, p, sk);
+    dmma_persistent<Dmma::m8n8k4, TA, TB, true>(mapA, mapB, p, sk);
 }
 
 // -------------------------------------------------------------------------------------------
@@ -474,8 +513,8 @@ struct AddCin {
     }
 };
 
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_f64_dmma_grouped_kernel(const __grid_constant__ G2Params g) {
+template <Dmma S>
+__device__ __forceinline__ void dmma_grouped(const G2Params& g) {
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     const int num_tiles = g.num_tiles;
@@ -536,7 +575,7 @@ gemm_f64_dmma_grouped_kernel(const __grid_constant__ G2Params g) {
             for (int j = 0; j < 4; ++j) acc[i][j][0] = acc[i][j][1] = 0.0;
 
         for (int kb = 0; kb < total_kb; ++kb) {
-            mma_slab<false, false>(acc, ring, stage, phase, cons);
+            mma_slab<S, false, false>(acc, ring, stage, phase, cons);
             if (++stage == NUM_STAGES) { stage = 0; phase ^= 1; }
         }
 
@@ -578,6 +617,17 @@ gemm_f64_dmma_grouped_kernel(const __grid_constant__ G2Params g) {
             }
         }
     }
+}
+
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+gemm_f64_dmma16x8_grouped_kernel(const __grid_constant__ G2Params g) {
+    dmma_grouped<Dmma::m16n8k4>(g);
+}
+
+// The m8n8k4 reference instance (see the top of the file).
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+gemm_f64_dmma_grouped_kernel(const __grid_constant__ G2Params g) {
+    dmma_grouped<Dmma::m8n8k4>(g);
 }
 
 // -------------------------------------------------------------------------------------------
@@ -664,7 +714,23 @@ bool operand_map(CUtensorMap* map, const double* base, int mn, int k, long long 
                             : tma_map(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT64, base, k, mn, ld * 8, 16, 128);
 }
 
+template <bool TA, bool TB>
+cudaError_t launch_gemm(int grid, cudaStream_t stream, const CUtensorMap& mA, const CUtensorMap& mB, const Params& p) {
+    return g_dmma_reference
+               ? launch_with_smem<gemm_f64_dmma_kernel<TA, TB>>(grid, NUM_THREADS, SMEM_BYTES, stream, mA, mB, p)
+               : launch_with_smem<gemm_f64_dmma16x8_kernel<TA, TB>>(grid, NUM_THREADS, SMEM_BYTES, stream, mA, mB, p);
+}
+
+template <bool TA, bool TB>
+cudaError_t launch_syrk(int grid, cudaStream_t stream, const CUtensorMap& mA, const Params& p, const SyrkSched& sk) {
+    return g_dmma_reference
+               ? launch_with_smem<syrk_f64_dmma_kernel<TA, TB>>(grid, NUM_THREADS, SMEM_BYTES, stream, mA, mA, p, sk)
+               : launch_with_smem<syrk_f64_dmma16x8_kernel<TA, TB>>(grid, NUM_THREADS, SMEM_BYTES, stream, mA, mA, p, sk);
+}
+
 }  // namespace
+
+void set_dmma_reference(bool on) { g_dmma_reference = on; }
 
 bool gemm_f64_tma_eligible(const double* A, long long lda, const double* B, long long ldb) {
     return ((reinterpret_cast<uintptr_t>(A) & 15) == 0) && ((reinterpret_cast<uintptr_t>(B) & 15) == 0) &&
@@ -691,10 +757,10 @@ cudaError_t gemm_f64(bool transA, bool transB, int M, int N, int K, double alpha
             p.tiles_n = (N + BN - 1) / BN;
             if (launches) ++*launches;
             const int grid = min(p.tiles_m * p.tiles_n, num_sms);
-            if (!transA && !transB) return launch_with_smem<gemm_f64_dmma_kernel<false, false>>(grid, NUM_THREADS, SMEM_BYTES, stream, mA, mB, p);
-            if (transA && !transB) return launch_with_smem<gemm_f64_dmma_kernel<true, false>>(grid, NUM_THREADS, SMEM_BYTES, stream, mA, mB, p);
-            if (!transA && transB) return launch_with_smem<gemm_f64_dmma_kernel<false, true>>(grid, NUM_THREADS, SMEM_BYTES, stream, mA, mB, p);
-            return launch_with_smem<gemm_f64_dmma_kernel<true, true>>(grid, NUM_THREADS, SMEM_BYTES, stream, mA, mB, p);
+            if (!transA && !transB) return launch_gemm<false, false>(grid, stream, mA, mB, p);
+            if (transA && !transB) return launch_gemm<true, false>(grid, stream, mA, mB, p);
+            if (!transA && transB) return launch_gemm<false, true>(grid, stream, mA, mB, p);
+            return launch_gemm<true, true>(grid, stream, mA, mB, p);
         }
     }
     dim3 grid((M + 63) / 64, (N + 63) / 64);
@@ -833,8 +899,7 @@ cudaError_t gram_f64(bool trans, int n, int K, const double* A, long long lda, d
         sk.kchunk = (int)((kb + splits - 1) / splits) * BK;
         sk.split_stride = ldp * n;
         const int grid = min(sk.tri_tiles * splits, num_sms);
-        e = !trans ? launch_with_smem<syrk_f64_dmma_kernel<false, true>>(grid, NUM_THREADS, SMEM_BYTES, stream, mA, mA, p, sk)
-                   : launch_with_smem<syrk_f64_dmma_kernel<true, false>>(grid, NUM_THREADS, SMEM_BYTES, stream, mA, mA, p, sk);
+        e = !trans ? launch_syrk<false, true>(grid, stream, mA, p, sk) : launch_syrk<true, false>(grid, stream, mA, p, sk);
         if (e != cudaSuccess) return e;
         if (launches) ++*launches;
     } else {
@@ -904,7 +969,9 @@ cudaError_t gemm_f64_grouped2(const G2Launch& L, int num_sms, cudaStream_t strea
     g.fence_all = fence_all;
     static const int poll_mode = [] { const char* e = getenv("MARLIN_B200_CIN_POLL"); return (e && e[0] == '1') ? 1 : 0; }();
     g.poll_mode = poll_mode;
-    const cudaError_t e = launch_with_smem<gemm_f64_dmma_grouped_kernel>(min(tiles, num_sms), NUM_THREADS, SMEM_BYTES, stream, g);
+    const cudaError_t e =
+        g_dmma_reference ? launch_with_smem<gemm_f64_dmma_grouped_kernel>(min(tiles, num_sms), NUM_THREADS, SMEM_BYTES, stream, g)
+                         : launch_with_smem<gemm_f64_dmma16x8_grouped_kernel>(min(tiles, num_sms), NUM_THREADS, SMEM_BYTES, stream, g);
     if (launches && e == cudaSuccess) ++*launches;
     return e;
 }

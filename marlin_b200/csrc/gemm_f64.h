@@ -72,4 +72,8 @@ cudaError_t gram_f64(bool trans, int n, int K, const double* A, long long lda, d
 
 bool gemm_f64_tma_eligible(const double* A, long long lda, const double* B, long long ldb);
 
+// Run the m8n8k4 reference instances of the DMMA kernels instead of the m16n8k4 ones for the launches this thread makes
+// from now on (a test and measurement switch: mb_set_dmma_reference).  Every C-ABI entry sets it from its context.
+void set_dmma_reference(bool on);
+
 }  // namespace mb

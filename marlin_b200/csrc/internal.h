@@ -2,6 +2,7 @@
 // records, error plumbing and small helpers.  Not installed; include/marlin_b200.h is the public surface.
 #pragma once
 #include "../../include/marlin_b200.h"
+#include "gemm_f64.h"
 
 #include <cuda_runtime.h>
 #include <atomic>
@@ -26,6 +27,7 @@ struct mb_ctx {
     int fp64_mode = MB_FP64_NATIVE;
     int fp64_slices = 7;
     int fp64_bits = 7;
+    bool dmma_reference = false;        // mb_set_dmma_reference: the m8n8k4 instances of the fp64 DMMA kernels
     void* ozaki_ws = nullptr;
     size_t ozaki_ws_bytes = 0;
     // partial vectors of the matrix x vector kernels (grow-only)
@@ -108,6 +110,7 @@ inline int32_t check_ctx(mb_ctx* ctx) {
     if (!ctx) return fail(MB_ERR_INVALID_ARG, "null context");
     cudaError_t e = cudaSetDevice(ctx->device);
     if (e != cudaSuccess) return cuda_fail(e, "cudaSetDevice");
+    mb::set_dmma_reference(ctx->dmma_reference);    // the DMMA kernels this call launches follow its context
     return MB_OK;
 }
 #define MB_CTX(ctx)                        \

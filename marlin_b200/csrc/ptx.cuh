@@ -186,6 +186,16 @@ __device__ __forceinline__ void dmma_m8n8k4(double& c0, double& c1, double a, do
                  : "d"(a), "d"(b));
 }
 
+// ---- fp64 tensor core: DMMA m16n8k4 (SASS DMMA.16x8x4, sm_90) --------------------------------------
+// Two m8n8k4 stacked in M that share the B fragment: a0 is A[lane/4][lane%4] and a1 is A[lane/4 + 8][lane%4]; b as in
+// m8n8k4; c0, c1 hold C[lane/4][2*(lane%4) + {0,1}] and c2, c3 hold C[lane/4 + 8][2*(lane%4) + {0,1}].  On H100 it issues
+// at twice the fp64 rate of m8n8k4.
+__device__ __forceinline__ void dmma_m16n8k4(double& c0, double& c1, double& c2, double& c3, double a0, double a1, double b) {
+    asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
+                 : "+d"(c0), "+d"(c1), "+d"(c2), "+d"(c3)
+                 : "d"(a0), "d"(a1), "d"(b));
+}
+
 __device__ __forceinline__ void lds128(double& x, double& y, uint32_t addr) {
     asm volatile("ld.shared.v2.f64 {%0,%1}, [%2];" : "=d"(x), "=d"(y) : "r"(addr));
 }

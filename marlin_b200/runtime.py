@@ -51,6 +51,11 @@ class Runtime:
         code = {"native": 0, "int8x7": 1, "int8x8": 2}[mode]
         nat.check(self.lib.mb_set_fp64_mode(self.ctx, code, slices))
 
+    def set_dmma_reference(self, on: bool) -> None:
+        """Test and measurement hook, off by default: run the m8n8k4 reference instances of the fp64 DMMA kernels instead
+        of the m16n8k4 ones.  See include/marlin_b200.h: mb_set_dmma_reference."""
+        nat.check(self.lib.mb_set_dmma_reference(self.ctx, 1 if on else 0))
+
     def launch_count(self) -> int:
         return int(self.lib.mb_launch_count(self.ctx))
 

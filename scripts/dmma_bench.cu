@@ -1,5 +1,6 @@
-// Microbenchmark: peak DMMA rate per SM on the attached GPU for the f64 mma.sync shapes m8n8k4 (the shape the GEMM
-// kernels issue) and m16n8k4 / m16n8k16 (sm_90), and the plain DFMA rate.  Not part of the product.
+// Microbenchmark: peak DMMA rate per SM on the attached GPU for the f64 mma.sync shapes m8n8k4 (the reference instances
+// of the GEMM kernels) and m16n8k4 (the shape the GEMM kernels issue) / m16n8k16 (sm_90), and the plain DFMA rate.
+// Not part of the product.
 #include <cstdio>
 #include <cuda_runtime.h>
 
@@ -123,5 +124,13 @@ int main() {
     cudaEventElapsedTime(&ms, e0, e1);
     double fma = 40.0 * sms * 8 * iters * 4 * 16 * 256.0;
     printf("DMMA sustained (%.0f ms): %.2f TFLOP/s\n", ms, 2 * fma / ms / 1e9);
+    // the same for m16n8k4, the shape the GEMM kernels issue (~3 s at 66 TFLOP/s): the ceiling on a power-capped card
+    cudaEventRecord(e0);
+    for (int i = 0; i < 60; ++i) dmma16_kernel<8, 4><<<sms, 8 * 32>>>(out, iters * 16, 1.0, 2.0);
+    cudaEventRecord(e1);
+    cudaEventSynchronize(e1);
+    cudaEventElapsedTime(&ms, e0, e1);
+    fma = 60.0 * sms * 8 * iters * 16 * 8 * 512.0;
+    printf("DMMA m16n8k4 sustained (%.0f ms): %.2f TFLOP/s\n", ms, 2 * fma / ms / 1e9);
     return 0;
 }
