@@ -210,6 +210,22 @@ int32_t mb_svd_mode(int64_t n, int32_t k, const char* mode, int32_t* compute_mod
  * Returns sk (>= 0) or a negative error code. */
 int32_t mb_svd_rank(const double* sigmas, int32_t count, int32_t k, double rcond);
 
+/* ---- DenseVecMatrix.lr (matrix/DenseVecMatrix.scala:1005-1035): logistic regression by gradient steps over the rows.
+ *      `rows` is an fp64 view with one training row per matrix row (a row shard's transposed view is read in place, any
+ *      other view is first copied into a row-major buffer).  Column 0 is the label; the features are the row with
+ *      column 0 replaced by the intercept 1.  The input is never written.  Per row: margin = -1.0 * (features . w),
+ *      sequential in column order with separate multiplies and adds (BLAS ddot as F2J runs it), gradientMul =
+ *      1 / (1 + exp(margin)) - label, gradient = features * gradientMul.  The rows' gradients are summed in a fixed
+ *      order (bitwise reproducible).  A block with no rows is MB_ERR_EMPTY, a non-fp64 block MB_ERR_UNSUPPORTED. ---- */
+/* The sum of the per-row gradients for the weights w: w and grad are HOST arrays of rows->cols doubles.  This is the
+ * body of one partition of one iteration.  Blocking. */
+int32_t mb_lr_gradient(mb_ctx* ctx, const mb_block* rows, const double* w, double* grad);
+/* The whole loop on one device: w = 0, then for i = 1..iters: w = w - delta_i * (step / data_size / sqrt(i)) with
+ * delta_i the gradient sum at the current w.  Every iteration is enqueued without a host synchronisation; the final w
+ * (rows->cols doubles) goes to the HOST array w_out.  iters <= 0 gives zeros.  data_size is the reference's numRows()
+ * (max row id + 1) and must be positive.  Blocking. */
+int32_t mb_lr_train(mb_ctx* ctx, const mb_block* rows, int64_t data_size, double step, int32_t iters, double* w_out);
+
 /* ---- a11: MTUtils.randomDenVecMatrix / randomBlockMatrix input generation
  *      (utils/MTUtils.scala:34-73, rdd/RandomRDD.scala:28-101, utils/RandomDataGenerator.scala:53-65,113-131).
  * Fills `count` consecutive values of partition stream `partition_seed` (one XORShift stream per

@@ -865,6 +865,21 @@ public:
         return out;
     }
 
+    // ---- lr(stepSize, iters) :1005-1035 (one process: every row is local, the whole loop runs on the device).  Column 0
+    //      of a row is its label; w starts at zeros; dataSize = numRows() (max row id + 1).  fp64 rows only. ----
+    std::vector<double> lr(double stepSize, int iters) {
+        const long n = numCols();
+        const long dataSize = numRows();
+        std::vector<double> w((size_t)n, 0.0);
+        if (iters <= 0) return w;
+        if (ids_.empty()) throw std::runtime_error("empty collection");                // gradientRDD.reduce on no rows
+        if (data_.cols() != n)        // features.dot(weights) on rows of another length than the numCols() weights
+            throw std::invalid_argument("requirement failed: Vectors must have the same length: rows of " +
+                                        std::to_string(data_.cols()) + " vs " + std::to_string(n) + " weights");
+        check(mb_lr_train(Context::get(), data_.handle(), dataSize, stepSize, iters, w.data()));
+        return w;
+    }
+
 private:
     template <class F> DenseVecMatrix unary(F f) {
         if (ids_.empty()) return *this;

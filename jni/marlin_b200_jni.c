@@ -164,6 +164,42 @@ NATIVE(jint, syev)(JNIEnv* e, jobject o, jlong ctx, jlong g, jlong v, jdoubleArr
     raise(e, rc);
     return sweeps;
 }
+/* ---- DenseVecMatrix.lr (matrix/DenseVecMatrix.scala:1005-1035): the gradient sum of one partition's rows ---- */
+NATIVE(void, lrGradient)(JNIEnv* e, jobject o, jlong ctx, jdoubleArray rows, jint numRows, jdoubleArray w, jdoubleArray gradOut) {
+    /* rows: numRows rows of w.length doubles back to back (row-major); w and gradOut: one entry per column.  The rows are
+     * uploaded, used and freed inside this call; the weights are copied out before the (blocking) device call. */
+    const jsize n = (*e)->GetArrayLength(e, w);
+    if (numRows < 0 || (*e)->GetArrayLength(e, gradOut) != n || (jlong)(*e)->GetArrayLength(e, rows) < (jlong)numRows * n) {
+        (*e)->ThrowNew(e, (*e)->FindClass(e, "java/lang/IllegalArgumentException"),
+                       "Dimension mismatch: lrGradient needs numRows rows of w.length doubles and one gradient entry per column");
+        return;
+    }
+    double* buf = (double*)malloc(sizeof(double) * 2 * (size_t)(n > 0 ? n : 1));
+    if (!buf) {
+        (*e)->ThrowNew(e, (*e)->FindClass(e, "java/lang/RuntimeException"), "lrGradient: host allocation failed");
+        return;
+    }
+    double* src = (double*)(*e)->GetPrimitiveArrayCritical(e, w, NULL);
+    memcpy(buf, src, sizeof(double) * (size_t)n);
+    (*e)->ReleasePrimitiveArrayCritical(e, w, src, JNI_ABORT);
+    /* the packed rows are the column-major n x numRows array underneath a row shard: upload it as that, read it through
+     * its transposed view */
+    mb_block *blk = NULL, *view = NULL;
+    jdouble* p = (jdouble*)(*e)->GetPrimitiveArrayCritical(e, rows, NULL);
+    int32_t rc = mb_block_upload(CTX(ctx), p, 0, n, numRows, n > 0 ? n : 1, 0, MB_F64, &blk);
+    (*e)->ReleasePrimitiveArrayCritical(e, rows, p, JNI_ABORT);
+    if (rc == MB_OK) rc = mb_block_view_t(CTX(ctx), blk, &view);
+    if (rc == MB_OK) rc = mb_lr_gradient(CTX(ctx), view, buf, buf + n);
+    if (view) mb_block_free(CTX(ctx), view);
+    if (blk) mb_block_free(CTX(ctx), blk);
+    if (rc == MB_OK && n > 0) {
+        double* dst = (double*)(*e)->GetPrimitiveArrayCritical(e, gradOut, NULL);
+        memcpy(dst, buf + n, sizeof(double) * (size_t)n);
+        (*e)->ReleasePrimitiveArrayCritical(e, gradOut, dst, 0);
+    }
+    free(buf);
+    raise(e, rc);
+}
 NATIVE(jint, svdMode)(JNIEnv* e, jobject o, jlong n, jint k, jstring mode) {
     const char* m = (*e)->GetStringUTFChars(e, mode, NULL);
     int32_t cm = 0;

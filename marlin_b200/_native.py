@@ -85,6 +85,8 @@ SIGNATURES = {
     "mb_block_syev": (c_i32, [c_ctx, c_blk, c_blk, c_dp, C.POINTER(c_i32)]),
     "mb_svd_mode": (c_i32, [c_i64, c_i32, C.c_char_p, C.POINTER(c_i32)]),
     "mb_svd_rank": (c_i32, [c_dp, c_i32, c_i32, c_f64]),
+    "mb_lr_gradient": (c_i32, [c_ctx, c_blk, c_dp, c_dp]),
+    "mb_lr_train": (c_i32, [c_ctx, c_blk, c_i64, c_f64, c_i32, c_dp]),
     "mb_fill_uniform": (c_i32, [c_ctx, c_blk, c_i64, c_i64, c_f64, c_f64, c_i32]),
     "mb_sparse_check": (c_i32, [c_i32, c_i32, C.c_void_p, C.c_void_p]),
     "mb_sparse_wrap": (c_i32, [c_ctx, c_i32, c_i32, c_i64, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(c_sp)]),

@@ -10,9 +10,11 @@
 #include "factor.h"
 #include "eigen.h"
 #include "sparse.h"
+#include "logistic.h"
 
 #include <cuda_runtime.h>
 #include <algorithm>
+#include <cmath>
 #include <cstdarg>
 #include <cstdlib>
 #include <cstdio>
@@ -1319,6 +1321,85 @@ int32_t mb_block_syev(mb_ctx* ctx, const mb_block* G, mb_block* V, double* w_out
     if (e == cudaErrorNotReady)
         return fail(MB_ERR_NO_CONVERGENCE, "Jacobi eigensolver: no convergence after %d sweeps (n = %d)", MAX_SWEEPS, G->rows);
     if (e != cudaSuccess) return cuda_fail(e, "mb_block_syev");
+    return MB_OK;
+}
+
+// ------------------------------------------------------------------------------------ logistic regression (DenseVecMatrix.lr)
+// Device buffers of one lr call: the rows as the kernel reads them (row-major, in place or staged), w, the gradient and the
+// per-CTA partials.  Stream-ordered; freed when the call's work completes.
+struct LrBuffers {
+    const double* x = nullptr;
+    long long ld = 0;
+    double* staged = nullptr;
+    double* w = nullptr;          // n weights, then n gradient values, then the partials
+    int m = 0, n = 0;
+    cudaStream_t st = nullptr;
+    ~LrBuffers() {
+        if (staged) cudaFreeAsync(staged, st);
+        if (w) cudaFreeAsync(w, st);
+    }
+};
+
+static int32_t lr_setup(mb_ctx* ctx, const mb_block* A, const char* name, LrBuffers* b) {
+    if (!A) return fail(MB_ERR_INVALID_ARG, "%s: null block", name);
+    if (A->dtype != MB_F64) return fail(MB_ERR_UNSUPPORTED, "%s: fp64 rows only", name);
+    if (A->rows == 0) return fail(MB_ERR_EMPTY, "empty collection");       // numRows() / numCols() on an empty RDD
+    if (A->cols == 0) return fail(MB_ERR_INVALID_ARG, "%s: a row needs at least its label (0 columns)", name);
+    b->m = A->rows;
+    b->n = A->cols;
+    b->st = ctx->stream;
+    if (A->is_transpose || A->cols == 1) {          // row r at data + r * ld (an m x 1 column: ld 1)
+        b->x = f64_ptr(A);
+        b->ld = A->is_transpose ? A->ld : 1;
+    } else {
+        MB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&b->staged), (size_t)b->m * b->n * sizeof(double), ctx->stream));
+        mb_block tmp;
+        tmp.data = b->staged; tmp.rows = b->m; tmp.cols = b->n; tmp.ld = b->n; tmp.is_transpose = 1; tmp.dtype = MB_F64;
+        tmp.device = ctx->device;
+        const int32_t r = copy_convert(ctx, A, &tmp);
+        if (r) return r;
+        b->x = b->staged;
+        b->ld = b->n;
+    }
+    const size_t ws = (size_t)2 * b->n + (size_t)mb::lr_parts(b->m, ctx->num_sms) * b->n;
+    MB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&b->w), ws * sizeof(double), ctx->stream));
+    return MB_OK;
+}
+
+int32_t mb_lr_gradient(mb_ctx* ctx, const mb_block* rows, const double* w, double* grad) {
+    MB_CTX(ctx);
+    MB_LOCK(ctx);
+    if (!w || !grad) return fail(MB_ERR_INVALID_ARG, "mb_lr_gradient: null weights or gradient");
+    LrBuffers b;
+    int32_t r = lr_setup(ctx, rows, "mb_lr_gradient", &b);
+    if (r) return r;
+    double* g = b.w + b.n;
+    MB_CUDA(cudaMemcpyAsync(b.w, w, sizeof(double) * b.n, cudaMemcpyHostToDevice, ctx->stream));
+    MB_CUDA(mb::lr_gradient_f64(b.x, b.ld, b.m, b.n, b.w, g + b.n, g, false, 0.0, ctx->num_sms, ctx->stream));
+    ctx->launches += 2;
+    MB_CUDA(cudaMemcpyAsync(grad, g, sizeof(double) * b.n, cudaMemcpyDeviceToHost, ctx->stream));
+    MB_CUDA(cudaStreamSynchronize(ctx->stream));
+    return MB_OK;
+}
+
+int32_t mb_lr_train(mb_ctx* ctx, const mb_block* rows, int64_t data_size, double step, int32_t iters, double* w_out) {
+    MB_CTX(ctx);
+    MB_LOCK(ctx);
+    if (!w_out) return fail(MB_ERR_INVALID_ARG, "mb_lr_train: null output");
+    if (rows && rows->rows > 0 && data_size <= 0)
+        return fail(MB_ERR_INVALID_ARG, "mb_lr_train: data size %lld must be positive", (long long)data_size);
+    LrBuffers b;
+    int32_t r = lr_setup(ctx, rows, "mb_lr_train", &b);
+    if (r) return r;
+    MB_CUDA(cudaMemsetAsync(b.w, 0, sizeof(double) * b.n, ctx->stream));          // BDV(Array.fill(featureSize)(0.0))
+    for (int i = 1; i <= iters; ++i) {
+        // weights - delta * (stepSize / dataSize / math.sqrt(i)), the scalar evaluated in that order
+        const double scale = step / (double)data_size / std::sqrt((double)i);
+        MB_CUDA(mb::lr_gradient_f64(b.x, b.ld, b.m, b.n, b.w, b.w + 2 * b.n, nullptr, true, scale, ctx->num_sms, ctx->stream));
+        ctx->launches += 2;
+    }
+    MB_CUDA(cudaMemcpyAsync(w_out, b.w, sizeof(double) * b.n, cudaMemcpyDeviceToHost, ctx->stream));
+    MB_CUDA(cudaStreamSynchronize(ctx->stream));
     return MB_OK;
 }
 

@@ -53,6 +53,13 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst_smem, const CUtensorMap
         ::"r"(dst_smem), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1)
         : "memory");
 }
+// Plain bulk copy (no tensor map): `bytes` contiguous bytes from global src to shared dst; both 16-byte aligned and bytes a
+// multiple of 16.  Completes on bar like a TMA load (SASS UBLKCP).
+__device__ __forceinline__ void bulk_load(uint32_t dst_smem, const void* src, uint32_t bytes, uint32_t bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(dst_smem), "l"(src), "r"(bytes), "r"(bar)
+                 : "memory");
+}
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src_smem, int32_t c0, int32_t c1) {
     asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
                  ::"l"(reinterpret_cast<uint64_t>(map)), "r"(src_smem), "r"(c0), "r"(c1)

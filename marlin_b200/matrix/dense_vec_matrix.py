@@ -327,6 +327,63 @@ class DenseVecMatrix(DistributedMatrix):
             vblk.slice(0, n, j, j + 1)._divide_into(float(sigmas[j]), nmat.slice(0, n, j, j + 1))
         return self._multiply_local(nmat), s, V
 
+    # ------------------------------------------------------------------ logistic regression (:1005-1035)
+    def lr(self, stepSize: float, iters: int) -> np.ndarray:
+        """lr(stepSize, iters) :1005-1035 -> the weights (ndarray of numCols()).  Column 0 of every row is its label, the
+        features are the row with column 0 replaced by the intercept 1; w starts at zeros, and iteration i = 1..iters sets
+        w = w - delta * (stepSize / dataSize / sqrt(i)), delta the sum over all rows of features * gradientMul with
+        gradientMul = 1 / (1 + exp(-1.0 * features.dot(w))) - label, and dataSize = numRows() (max row id + 1).
+
+        On the device: each row's margin is sequential in column order with separate multiplies and adds (Breeze/F2J
+        ddot bit for bit); the sum of the gradients runs in a fixed order, so the result is bitwise reproducible (the
+        reference's reduce order follows task completion).  With one rank the whole loop runs on the GPU without host
+        round trips (mb_lr_train).  With several ranks every rank computes the gradient sum of its rows each iteration
+        (zeros if it holds none); the partials are exchanged and summed in rank order on every rank, so all ranks hold
+        the same w bit for bit.  fp64 rows only."""
+        n = self.numCols()
+        data_size = self.numRows()
+        rank, ws = world()
+        has_rows = self.data is not None and len(self.ids) > 0
+        iters = int(iters)
+        w = np.zeros(n)
+        if iters <= 0:
+            return w
+        # every rank learns of a bad shard before any rank enters the exchange below
+        problems = []
+        if has_rows and self.data.dtype != nat.MB_F64:
+            problems.append((nat.MB_ERR_UNSUPPORTED, "lr: fp64 rows only"))
+        elif has_rows and self.data.cols != n:
+            # features.dot(weights) on rows of another length than the numCols() weights (Breeze's require)
+            problems.append((nat.MB_ERR_DIM_MISMATCH, "requirement failed: Vectors must have the same length: rows of "
+                             f"{self.data.cols} vs {n} weights"))
+        problems = self._gather(problems)
+        if problems:
+            raise nat.MarlinArgumentError(*problems[0])
+        rt = Runtime.get()
+        if ws == 1:
+            if not has_rows:
+                raise nat.MarlinError(nat.MB_ERR_EMPTY, "empty collection")       # gradientRDD.reduce on no rows
+            rt.sync_stream()
+            nat.check(rt.lib.mb_lr_train(rt.ctx, self.data.handle(), data_size, float(stepSize), iters, w.ctypes.data_as(nat.c_dp)))
+            return w
+        import torch.distributed as dist
+        # the partials are n doubles already on the host: NCCL moves them from the device, gloo from host memory
+        dev = (self.data.buf.device if self.data is not None else rt.device) if dist.get_backend() == "nccl" else torch.device("cpu")
+        for i in range(1, iters + 1):
+            g = np.zeros(n)
+            if has_rows:
+                rt.sync_stream()
+                nat.check(rt.lib.mb_lr_gradient(rt.ctx, self.data.handle(), w.ctypes.data_as(nat.c_dp), g.ctypes.data_as(nat.c_dp)))
+            mine = torch.from_numpy(g).to(dev)
+            sends = [(src, dst, ("lr", src)) for src in range(ws) for dst in range(ws) if src != dst]
+            got = comm.exchange(sends, {("lr", rank): mine}, lambda key: torch.empty(n, dtype=torch.float64, device=dev), rank)
+            parts = [g if r == rank else got[("lr", r)].cpu().numpy() for r in range(ws)]
+            delta = parts[0].copy()
+            for p in parts[1:]:
+                delta = delta + p
+            w = w - delta * (float(stepSize) / float(data_size) / math.sqrt(i))
+        return w
+
     # ------------------------------------------------------------------ element-wise (:771-871)
     def _scalar(self, op: str, b: float) -> "DenseVecMatrix":
         if self.data is None:

@@ -277,6 +277,38 @@ class MTUtils:
         return DenseVecMatrix(rows)
 
     @staticmethod
+    def loadSVMDenVecMatrix(sc, path: str, vectorLen: int, minPartitions: int = 4) -> DenseVecMatrix:
+        """utils/MTUtils.scala:253-276 — `rowIndex i:v i:v ...` split on single spaces: the first token is the row index
+        (not a label), each entry sets element i - 1 of a zero vector of vectorLen (a later entry for the same index
+        wins).  numRows() is max row index + 1.  Lines are dealt to ranks in contiguous chunks, as loadMatrixFile does;
+        blank lines are skipped.  An index outside 1..vectorLen is rejected (ArrayIndexOutOfBoundsException on the JVM)."""
+        _check_path(path)
+        vectorLen = int(vectorLen)
+        files = [path] if os.path.isfile(path) else sorted(os.path.join(path, f) for f in os.listdir(path)
+                                                           if not f.startswith((".", "_")))
+        lines = []
+        for f in files:
+            with open(f) as fh:
+                lines.extend(l.rstrip("\r\n") for l in fh if l.strip())
+        rank, ws = world()
+        n = len(lines)
+        lo, hi = (rank * n) // ws, ((rank + 1) * n) // ws
+        rows = []
+        for line in lines[lo:hi]:
+            items = line.split(" ")
+            while items and items[-1] == "":                 # java.lang.String.split drops trailing empty strings
+                items.pop()
+            vec = np.zeros(vectorLen)
+            for item in items[1:]:
+                ind, val = item.split(":")[:2]
+                i = int(ind) - 1
+                if not 0 <= i < vectorLen:
+                    raise nat.MarlinArgumentError(nat.MB_ERR_INVALID_ARG, f"index {i} out of bounds for length {vectorLen}")
+                vec[i] = float(val)
+            rows.append((int(items[0]), vec))
+        return DenseVecMatrix(rows, 0, vectorLen)
+
+    @staticmethod
     def loadBlockMatrixFile(sc, path: str, minPartitions: int = 4) -> BlockMatrix:
         """utils/MTUtils.scala:324-340 — `row-col-rows-cols:colmajor,...` (the reference requires an hdfs://,
         tachyon:// or file:// prefix here; a plain absolute path is accepted as well)."""

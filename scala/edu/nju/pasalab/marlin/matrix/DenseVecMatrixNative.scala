@@ -37,6 +37,28 @@ private[marlin] object DenseVecMatrixNative {
     Iterator.tabulate(rows)(r => (part(r)._1, new BDV[Double](out, r * b.cols, 1, b.cols)))
   }
 
+  /** One partition of one iteration of `lr(stepSize, iters)` (:1005-1035): the sum of the partition's per-row gradients
+   *  at `weights`, as one vector (none for an empty partition).  The driver keeps its loop: `reduce(_ + _)` over the
+   *  partitions, then `weights - delta * (stepSize / dataSize / math.sqrt(i))`.  Column 0 of a row is its label. */
+  def lrGradientPartition(iter: Iterator[(Long, BDV[Double])], weights: BDV[Double]): Iterator[BDV[Double]] = {
+    val part = iter.toArray
+    val rows = part.length
+    if (rows == 0) return Iterator.empty
+    val numCols = weights.length
+    val packed = new Array[Double](rows * numCols)                 // row-major, numCols doubles per row
+    var i = 0
+    while (i < rows) {
+      val v = part(i)._2
+      require(v.length == numCols, s"Dimension mismatch: row of ${v.length} vs $numCols weights")
+      if (v.stride == 1) System.arraycopy(v.data, v.offset, packed, i * numCols, numCols)
+      else { var j = 0; while (j < numCols) { packed(i * numCols + j) = v(j); j += 1 } }
+      i += 1
+    }
+    val grad = new Array[Double](numCols)
+    Native.lrGradient(Ctx.get, packed, rows, weights.toArray, grad)          // uploads, computes and frees in one call
+    Iterator.single(BDV(grad))
+  }
+
   /** brzLU(mat): (packed L\U like dgetrf, the reference's permutation array: row i of L*U is row perm(i) of mat). */
   def lu(mat: SubMatrix): (SubMatrix, Array[Int]) = {
     val work = mat.copy()

@@ -56,6 +56,9 @@ object Native {
   @native def svdMode(n: Long, k: Int, mode: String): Int // 0 local-svd, 1 local-eigs, 2 dist-eigs
   @native def svdRank(sigmas: Array[Double], k: Int, rCond: Double): Int
   @native def trsm(ctx: Long, t: Long, lower: Boolean, unitDiagonal: Boolean, b: Long): Unit
+  // DenseVecMatrix.lr: the sum of the per-row logistic gradients at weights w of numRows rows of w.length doubles, packed
+  // row-major in `rows` (column 0 = label); the rows live on the device only for the duration of the call
+  @native def lrGradient(ctx: Long, rows: Array[Double], numRows: Int, w: Array[Double], gradOut: Array[Double]): Unit
 
   // sparse blocks: a CSC block in HBM (SparseMatrix / LibMatrixMult / SparseMatrix.rand on the device)
   @native def sparseUpload(ctx: Long, rows: Int, cols: Int, colptr: Array[Int], rowidx: Array[Int],
