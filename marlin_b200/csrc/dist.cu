@@ -11,8 +11,9 @@
 //     epilogues: each holder first computes the column half the OTHER one reduces, its epilogue storing straight into
 //     the peer's staging buffer over NVLink, then its own half as acc + staged partial; the partner's reduced half is
 //     stored, again by the epilogue, directly into the owner's C tile.  No add pass, no extra copy.  The two halves are
-//     two launches of the same persistent kernel with the exchange flags between them (see fused_variant below for why
-//     not one);
+//     two launches of the same persistent kernel with the exchange flags between them, written by stream memory
+//     operations at the kernel boundary: completion counted inside a kernel whose epilogue stores to peer memory was
+//     measured faulty;
 //   * anything else (three or more holders, bf16 / transposed tiles) takes the staged path: partials are stored into
 //     a per-source slot of the owner's staging buffer and the owner adds them in rank order (deterministic).
 // Processes are ordered by monotonic epoch flags in exported device memory, written and awaited by stream memory
@@ -803,16 +804,21 @@ int32_t mb_matmul_blocked_dist(mb_comm* c, mb_block* const* A_tiles, const int32
     // ---- 3. my block products ----
     std::vector<char> partial_to(world, 0);                  // staged path: owners I have stored a partial for
     std::vector<char> fused_free_to(world, 0);               // fused path: peers whose staged half I have consumed
-    bool launched_fast = false;
     if (fast) {
-        static thread_local mb::G2Launch L;
-        L = mb::G2Launch();
+        // Two launches of the grouped kernel with the exchange flags between them: L0 computes the halves the peers reduce
+        // (stored into their staging buffers) and the plain regions, L2 the halves reduced here (acc + the peer's staged
+        // partial).  Completion counted inside a kernel whose epilogue stores to peer memory was measured faulty — at 8192^2
+        // about one call in three came back with one 16 x 32 patch off by a single product term — so the kernel boundary is
+        // the completion point and the flags are stream memory operations.  Both launches share one operand table.
+        static thread_local mb::G2Launch L0, L2;
+        L0 = mb::G2Launch();
+        L2 = mb::G2Launch();
         bool ok = true;
         auto op_of = [&](Tile& t, bool is_a) {
             if (t.op >= 0) return t.op;
-            int& cnt = is_a ? L.na : L.nb;
+            int& cnt = is_a ? L0.na : L0.nb;
             if (cnt >= mb::G2_MAX_OPS) { ok = false; return 0; }
-            mb::G2Operand& o = (is_a ? L.A : L.B)[cnt];
+            mb::G2Operand& o = (is_a ? L0.A : L0.B)[cnt];
             o.ptr = f64_ptr(&t.blk); o.ld = t.blk.ld; o.rows = t.blk.rows; o.cols = t.blk.cols;
             o.band = t.remote ? t.band : 0;
             o.ready_base = t.remote ? t.ready_base : -1;
@@ -835,11 +841,14 @@ int32_t mb_matmul_blocked_dist(mb_comm* c, mb_block* const* A_tiles, const int32
         }
         std::stable_sort(regs.begin(), regs.end(), [](const Reg& a, const Reg& b) { return a.phase < b.phase; });
         if ((int)regs.size() > mb::G2_MAX_ENTRIES) ok = false;
+        struct Note { int peer, slot; };
+        std::vector<Note> wrote, need, final_to;              // F_PART2 to signal / F_PART2 to wait for / F_FINAL2 to signal
         for (size_t x = 0; x < regs.size() && ok; ++x) {
             const Reg& rg = regs[x];
             const int i = rg.id / n, j = rg.id % n;
             const MyC* mc = nullptr;
             for (const MyC& q : myc) if (q.id == rg.id) mc = &q;
+            mb::G2Launch& L = rg.phase == 2 ? L2 : L0;
             mb::G2Entry& en = L.E[L.ne++];
             en.nseg = (int)mc->kks.size();
             for (int s = 0; s < en.nseg; ++s) {
@@ -861,93 +870,47 @@ int32_t mb_matmul_blocked_dist(mb_comm* c, mb_block* const* A_tiles, const int32
             }
             const int peer = h[0] == rank ? h[1] : h[0];
             const int slot = pair_slot[rg.id];
-            en.done_ctr = c->flags + F_CTR + (L.ne - 1);
-            en.sig_val = e;
             if (rg.phase == 0) {
                 // the half the PEER reduces: my partial of it goes over NVLink into my slot of the peer's staging buffer
                 en.D = reinterpret_cast<double*>(c->staging_peer[peer] + (size_t)rank * c->slot_bytes + slot_off[rg.id]);
                 en.ldd = ldst;
-                en.sig_remote = c->flags_peer[peer] + F_PART2 + rank * MAX_PAIR + slot;
+                wrote.push_back({peer, slot});
             } else {
                 // the half I reduce: acc + the peer's staged partial; the result belongs in the OWNER's C tile
                 en.Cin = reinterpret_cast<const double*>(c->staging + (size_t)peer * c->slot_bytes + slot_off[rg.id]);
                 en.ldcin = ldst;
-                en.cin_flag = c->flags + F_PART2 + peer * MAX_PAIR + slot;
-                en.cin_val = e;
+                need.push_back({peer, slot});
                 if (h[0] == rank) {
                     en.D = f64_ptr(C_tiles[rg.id]) + (size_t)rg.n_off * C_tiles[rg.id]->ld; en.ldd = C_tiles[rg.id]->ld;
-                    en.done_ctr = nullptr;                   // nobody waits for it: stream order is enough
                 } else {
                     if (!entC[rg.id]) return fail(MB_ERR_INVALID_ARG, "mb_matmul_blocked_dist: owner did not publish C tile %d", rg.id);
                     char* cp = nullptr;
                     if ((rc = open_entry(*entC[rg.id], &cp)) != MB_OK) return rc;
                     en.D = reinterpret_cast<double*>(cp) + (size_t)rg.n_off * entC[rg.id]->ld; en.ldd = entC[rg.id]->ld;
-                    en.sig_remote = c->flags_peer[peer] + F_FINAL2 + rank * MAX_PAIR + slot;
+                    final_to.push_back({peer, slot});
                 }
                 fused_free_to[peer] = 1;
             }
         }
-        // 0: one launch, in-kernel signalling and in-kernel addend wait; 1: two launches, flags are stream memory operations;
-        // 2: two launches, first half signals in-kernel, second half launched behind a stream wait; 3: two launches, stream
-        // signal after the first half, second half waits in-kernel (2 and 3 exist to locate the fault of 0)
-        // Default 1.  Variant 0 (and 2) — completion counted INSIDE a kernel whose epilogue stores to peer memory — is
-        // faulty on this hardware/software stack: at 8192^2, roughly one call in three comes back with one 16 x 32 patch (the
-        // counting warp's first fragment pair, one k index of one tile) off by a single product term; 1 and 3 were exact in
-        // every run.  The cause is not understood; the variants stay for diagnosis.
-        static const int fused_variant = [] { const char* v = getenv("MARLIN_B200_FUSED_SPLIT"); return v ? atoi(v) : 1; }();
-        const bool split_phases = fused_variant != 0;
-        if (ok && !split_phases) {
-            L.ready = c->flags + F_BAND; L.ready_val = e; L.status = c->flags + F_STATUS; L.timeout_ns = timeout_ns(c);
-            MB_CUDA(cudaMemsetAsync(c->flags + F_CTR, 0, sizeof(unsigned long long) * mb::G2_MAX_ENTRIES, S));
-            int launches = 0;
-            cudaError_t ce = mb::gemm_f64_grouped2(L, ctx->num_sms, S, &launches);
-            if (ce == cudaSuccess) { ctx->launches += launches; launched_fast = true; }
-            else if (ce != cudaErrorNotSupported) return cuda_fail(ce, "gemm_f64_grouped2");
-            else cudaGetLastError();
-        } else if (ok) {
-            // Two launches with the exchange flags BETWEEN them (MARLIN_B200_FUSED_SPLIT=1): the halves the peers reduce (and
-            // every plain region) first, then — once the peers' flags say their partials have landed — the halves reduced
-            // here.  Completion is a kernel boundary, the flags are stream memory operations: no in-kernel signalling.
-            static thread_local mb::G2Launch L0, L2;
-            L0 = L; L2 = L;
-            L0.ne = L2.ne = 0;
-            struct Note { int peer, slot; bool remote_final; };
-            std::vector<Note> wrote, need, final_to;
-            for (int x = 0; x < L.ne; ++x) {
-                mb::G2Entry en = L.E[x];
-                const Reg& rg = regs[x];
-                const auto& h = plan.holders[rg.id];
-                const int peer = h.size() == 2 ? (h[0] == rank ? h[1] : h[0]) : -1;
-                if (fused_variant != 2 || rg.phase != 0) { en.done_ctr = nullptr; en.sig_remote = nullptr; en.sig_local = nullptr; }
-                if (fused_variant != 3) en.cin_flag = nullptr;
-                if (fused_variant == 3 && rg.phase == 2) { en.done_ctr = nullptr; en.sig_remote = nullptr; }
-                if (rg.phase == 2) {
-                    L2.E[L2.ne++] = en;
-                    need.push_back({peer, pair_slot[rg.id], false});
-                    if (h[0] != rank) final_to.push_back({peer, pair_slot[rg.id], true});
-                } else {
-                    L0.E[L0.ne++] = en;
-                    if (rg.phase == 0) wrote.push_back({peer, pair_slot[rg.id], false});
-                }
-            }
-            L0.ready = L2.ready = c->flags + F_BAND; L0.ready_val = L2.ready_val = e;
-            L0.status = L2.status = c->flags + F_STATUS; L0.timeout_ns = L2.timeout_ns = timeout_ns(c);
-            int launches = 0;
-            if (fused_variant == 2) MB_CUDA(cudaMemsetAsync(c->flags + F_CTR, 0, sizeof(unsigned long long) * mb::G2_MAX_ENTRIES, S));
-            cudaError_t ce = L0.ne ? mb::gemm_f64_grouped2(L0, ctx->num_sms, S, &launches) : cudaSuccess;
-            if (ce != cudaSuccess) return cuda_fail(ce, "gemm_f64_grouped2 (first half)");
-            if (fused_variant != 2) for (const Note& w : wrote) MB_CUDA(sig(c, c->flags_peer[w.peer] + F_PART2 + rank * MAX_PAIR + w.slot, e, S));
-            if (fused_variant != 3) for (const Note& w : need) MB_CUDA(waitf(c, c->flags + F_PART2 + w.peer * MAX_PAIR + w.slot, e, S));
-            ce = L2.ne ? mb::gemm_f64_grouped2(L2, ctx->num_sms, S, &launches) : cudaSuccess;
-            if (ce != cudaSuccess) return cuda_fail(ce, "gemm_f64_grouped2 (second half)");
-            for (const Note& w : final_to) MB_CUDA(sig(c, c->flags_peer[w.peer] + F_FINAL2 + rank * MAX_PAIR + w.slot, e, S));
-            ctx->launches += launches;
-            launched_fast = true;
-        }
-        if (!launched_fast) {
-            // every rank evaluates the same predicates, except TMA encode failures: make a divergence loud, not silent
+        if (!ok) {
+            // the plan-wide limits above keep every rank's share within the tables; should one not fit, fail on every
+            // rank alike rather than fall back here and leave the partner waiting for flags
             return fail(MB_ERR_UNSUPPORTED, "mb_matmul_blocked_dist: grouped launch not possible for this plan (set MARLIN_B200_DIST_SLOW=1)");
         }
+        L2.na = L0.na; L2.nb = L0.nb;
+        std::copy_n(L0.A, L0.na, L2.A);
+        std::copy_n(L0.B, L0.nb, L2.B);
+        L0.ready = L2.ready = c->flags + F_BAND; L0.ready_val = L2.ready_val = e;
+        L0.status = L2.status = c->flags + F_STATUS; L0.timeout_ns = L2.timeout_ns = timeout_ns(c);
+        int launches = 0;
+        cudaError_t ce = mb::gemm_f64_grouped2(L0, ctx->num_sms, S, &launches);
+        if (ce != cudaSuccess) return cuda_fail(ce, "gemm_f64_grouped2 (first half)");
+        for (const Note& w : wrote) MB_CUDA(sig(c, c->flags_peer[w.peer] + F_PART2 + rank * MAX_PAIR + w.slot, e, S));
+        for (const Note& w : need) MB_CUDA(waitf(c, c->flags + F_PART2 + w.peer * MAX_PAIR + w.slot, e, S));
+        ce = mb::gemm_f64_grouped2(L2, ctx->num_sms, S, &launches);
+        if (ce != cudaSuccess) return cuda_fail(ce, "gemm_f64_grouped2 (second half)");
+        for (const Note& w : final_to) MB_CUDA(sig(c, c->flags_peer[w.peer] + F_FINAL2 + rank * MAX_PAIR + w.slot, e, S));
+        ctx->launches += launches;
     } else {
         // ---- general path: per product (or per C tile when all kk are here), tile-level waits, staged partials ----
         for (const MyC& mc : myc) {
@@ -990,13 +953,13 @@ int32_t mb_matmul_blocked_dist(mb_comm* c, mb_block* const* A_tiles, const int32
     // ---- 4. the reduceByKey across ranks ----
     for (int p = 0; p < world; ++p) {
         if (partial_to[p]) MB_CUDA(sig(c, flag_ch(c, p, CH_PARTIAL, rank), e, S));
-        if (partial_to[p] || (launched_fast && writes_to[p])) c->last_write_epoch[p] = e;
+        if (partial_to[p] || (fast && writes_to[p])) c->last_write_epoch[p] = e;
     }
     // staged path, owner side: add the partials in holder order (deterministic), then free the slots
     std::vector<char> free_to(world, 0);
     for (const MyC& mc : myc) {
         const auto& h = plan.holders[mc.id];
-        if (h.size() < 2 || h[0] != rank || (launched_fast && fused_tile(mc.id))) continue;
+        if (h.size() < 2 || h[0] != rank || fused_tile(mc.id)) continue;
         for (size_t s = 1; s < h.size(); ++s) {
             const int src = h[s];
             MB_CUDA(waitf(c, flag_ch(c, rank, CH_PARTIAL, src), e, S));
@@ -1011,12 +974,11 @@ int32_t mb_matmul_blocked_dist(mb_comm* c, mb_block* const* A_tiles, const int32
     for (int p = 0; p < world; ++p)
         if (free_to[p] || fused_free_to[p]) MB_CUDA(sig(c, flag_ch(c, p, CH_FREE, rank), e, S));
     // fused path, owner side: the partner's reduced half has landed in my C tile
-    if (launched_fast)
-        for (const MyC& mc : myc) {
-            const auto& h = plan.holders[mc.id];
-            if (fused_tile(mc.id) && h[0] == rank && col_len[mc.j] > half_cols(mc.id))
-                MB_CUDA(waitf(c, c->flags + F_FINAL2 + h[1] * MAX_PAIR + pair_slot[mc.id], e, S));
-        }
+    for (const MyC& mc : myc) {
+        const auto& h = plan.holders[mc.id];
+        if (fused_tile(mc.id) && h[0] == rank && col_len[mc.j] > half_cols(mc.id))
+            MB_CUDA(waitf(c, c->flags + F_FINAL2 + h[1] * MAX_PAIR + pair_slot[mc.id], e, S));
+    }
 
     // ---- 5. my tiles may not be overwritten / freed until everyone has finished pulling them ----
     for (int p = 0; p < world; ++p)

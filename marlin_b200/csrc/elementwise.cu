@@ -11,7 +11,6 @@
 #include <cuda_bf16.h>
 #include <atomic>
 #include <cstdio>
-#include <cstdlib>
 #include <cstring>
 #include <mutex>
 #include <vector>
@@ -140,102 +139,61 @@ __global__ void binary_strided_f32_kernel(int op, int rows, int cols, const floa
 // Shared-memory slot of 16B unit (rb, cb, half):  rb*64 + 16*(cb>>3) + 8*half + ((cb&7) ^ (rb&7))
 // which is conflict-free for the column-wise writes and the row-wise reads.
 constexpr int TT = 64;
-// A CTA owns RM x CM adjacent 64x64 sub-tiles (all loads of the CTA are issued before its single barrier, so RM = 2
-// reads 1 KiB runs per input column and CM = 2 writes 1 KiB runs per output column).  ORDER picks the tile -> CTA map:
-// 0 row-tile fastest (reads walk down the input columns), 1 8x8 super-tiles, 2 column-tile fastest (writes walk down
-// the output columns), 3 diagonal (tc rotated by tr: neither side strides by a power of two between neighbours).
-template <int ORDER, int RM, int CM>
+// A CTA owns TT_SUB vertically adjacent 64x64 sub-tiles, so it reads 1 KiB runs per input column (all its loads are
+// issued before its single barrier).  CTAs walk bands of TT_BAND tile columns, column-tile fastest inside a band, so
+// the CTAs in flight write TT_BAND * 512 B runs per output column and read long runs per input column.
+constexpr int TT_SUB = 2, TT_BAND = 8;
+constexpr int TT_SMEM = TT_SUB * 32 * 64 * (int)sizeof(double2);
 __global__ void __launch_bounds__(256) transpose_f64_tile_kernel(const double* __restrict__ in, long long ldi,
                                                                 double* __restrict__ out, long long ldo, int rows,
                                                                 int cols, int tiles_r, int tiles_c) {
     extern __shared__ double2 tile_all[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    int tr, tc;
-    if (ORDER == 1) {
-        const int sup_r = (tiles_r + 7) >> 3;
-        const int b = blockIdx.x;
-        const int sup = b >> 6, inner = b & 63;
-        tr = ((sup % sup_r) << 3) + (inner & 7);
-        tc = ((sup / sup_r) << 3) + (inner >> 3);
-        if (tr >= tiles_r || tc >= tiles_c) return;
-    } else if (ORDER == 2) {
-        tc = blockIdx.x % tiles_c;
-        tr = blockIdx.x / tiles_c;
-    } else if (ORDER == 3) {
-        tr = blockIdx.x % tiles_r;
-        tc = (blockIdx.x / tiles_r + tr) % tiles_c;
-    } else if (ORDER >= 4) {
-        // bands of G tile columns, column-tile fastest inside a band: the CTAs in flight write G*512 B runs per output
-        // column and read long runs per input column
-        constexpr int G = ORDER == 4 ? 16 : (ORDER == 5 ? 32 : 8);
-        const int band = blockIdx.x / (G * tiles_r);
-        const int rem = blockIdx.x - band * (G * tiles_r);
-        const int gw = min(G, tiles_c - band * G);          // last band may be narrower
-        tc = band * G + rem % gw;
-        tr = rem / gw;
-    } else {
-        tr = blockIdx.x % tiles_r;
-        tc = blockIdx.x / tiles_r;
-    }
+    const int band = blockIdx.x / (TT_BAND * tiles_r);
+    const int rem = blockIdx.x - band * (TT_BAND * tiles_r);
+    const int gw = min(TT_BAND, tiles_c - band * TT_BAND);       // last band may be narrower
+    const int tc = band * TT_BAND + rem % gw;
+    const int tr = rem / gw;
+    const int c0 = tc * TT;
     // load phase: lane -> micro-row rb, warp -> micro-cols cb = warp + 8*i
 #pragma unroll
-    for (int sr = 0; sr < RM; ++sr)
+    for (int sr = 0; sr < TT_SUB; ++sr) {
+        double2* tile = tile_all + sr * (32 * 64);
+        const int rb = lane;
+        const int r = (tr * TT_SUB + sr) * TT + 2 * rb;
 #pragma unroll
-        for (int sc = 0; sc < CM; ++sc) {
-            double2* tile = tile_all + (sr * CM + sc) * (32 * 64);
-            const int r0 = (tr * RM + sr) * TT, c0 = (tc * CM + sc) * TT;
-            const int rb = lane;
-            const int r = r0 + 2 * rb;
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int cb = warp + 8 * i;
-                const int c = c0 + 2 * cb;
-                double2 v0 = make_double2(0.0, 0.0), v1 = v0;
-                if (r < rows && c < cols) {   // rows, cols even -> whole micro-block in range
-                    v0 = *reinterpret_cast<const double2*>(in + r + (long long)c * ldi);
-                    v1 = *reinterpret_cast<const double2*>(in + r + (long long)(c + 1) * ldi);
-                }
-                const int base = rb * 64 + 16 * (cb >> 3) + ((cb & 7) ^ (rb & 7));
-                tile[base] = make_double2(v0.x, v1.x);       // out column r   : in(r, c), in(r, c+1)
-                tile[base + 8] = make_double2(v0.y, v1.y);   // out column r+1 : in(r+1, c), in(r+1, c+1)
+        for (int i = 0; i < 4; ++i) {
+            const int cb = warp + 8 * i;
+            const int c = c0 + 2 * cb;
+            double2 v0 = make_double2(0.0, 0.0), v1 = v0;
+            if (r < rows && c < cols) {   // rows, cols even -> whole micro-block in range
+                v0 = *reinterpret_cast<const double2*>(in + r + (long long)c * ldi);
+                v1 = *reinterpret_cast<const double2*>(in + r + (long long)(c + 1) * ldi);
             }
+            const int base = rb * 64 + 16 * (cb >> 3) + ((cb & 7) ^ (rb & 7));
+            tile[base] = make_double2(v0.x, v1.x);       // out column r   : in(r, c), in(r, c+1)
+            tile[base + 8] = make_double2(v0.y, v1.y);   // out column r+1 : in(r+1, c), in(r+1, c+1)
         }
+    }
     __syncthreads();
-    // store phase: the CM sub-tiles of one output column are written back to back (CM * 512 B runs)
+    // store phase
 #pragma unroll
-    for (int sr = 0; sr < RM; ++sr)
+    for (int sr = 0; sr < TT_SUB; ++sr) {
+        const double2* tile = tile_all + sr * (32 * 64);
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
             const int rb = warp + 8 * i;
-            const int r = (tr * RM + sr) * TT + 2 * rb;
+            const int r = (tr * TT_SUB + sr) * TT + 2 * rb;
+            const int cb = lane;
+            const int c = c0 + 2 * cb;
 #pragma unroll
             for (int half = 0; half < 2; ++half)
-#pragma unroll
-                for (int sc = 0; sc < CM; ++sc) {
-                    const double2* tile = tile_all + (sr * CM + sc) * (32 * 64);
-                    const int cb = lane;
-                    const int c = (tc * CM + sc) * TT + 2 * cb;
-                    if (r < rows && c < cols) {
-                        const int base = rb * 64 + 16 * (cb >> 3) + ((cb & 7) ^ (rb & 7));
-                        *reinterpret_cast<double2*>(out + c + (long long)(r + half) * ldo) = tile[base + 8 * half];
-                    }
+                if (r < rows && c < cols) {
+                    const int base = rb * 64 + 16 * (cb >> 3) + ((cb & 7) ^ (rb & 7));
+                    *reinterpret_cast<double2*>(out + c + (long long)(r + half) * ldo) = tile[base + 8 * half];
                 }
         }
-}
-
-template <int ORDER, int RM, int CM>
-static cudaError_t launch_transpose_f64(const double* in, long long ldi, double* out, long long ldo, int rows, int cols,
-                                        cudaStream_t st) {
-    const int tiles_r = (rows + TT * RM - 1) / (TT * RM), tiles_c = (cols + TT * CM - 1) / (TT * CM);
-    const int smem = RM * CM * 32 * 64 * (int)sizeof(double2);
-    auto kern = transpose_f64_tile_kernel<ORDER, RM, CM>;
-    if (smem > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-        if (e != cudaSuccess) return e;
     }
-    const int grid = ORDER == 1 ? ((tiles_r + 7) / 8) * ((tiles_c + 7) / 8) * 64 : tiles_r * tiles_c;
-    kern<<<grid, 256, smem, st>>>(in, ldi, out, ldo, rows, cols, tiles_r, tiles_c);
-    return cudaGetLastError();
 }
 
 // generic transpose (any alignment / odd sizes / any element type): 32x32 tile, scalar accesses
@@ -640,34 +598,11 @@ cudaError_t transpose_f64(const double* in, long long ldi, double* out, long lon
     const bool fast = (rows % 2 == 0) && (cols % 2 == 0) && (ldi % 2 == 0) && (ldo % 2 == 0) &&
                       (((reinterpret_cast<uintptr_t>(in) | reinterpret_cast<uintptr_t>(out)) & 15) == 0);
     if (fast) {
-        static int variant = -1;
-        // chosen with the sweep in scripts/bench_transpose.py (not re-run on H100): what matters is that the CTAs in
-        // flight write long runs per output column (column-tile-fastest maps) and that a CTA reads 1 KiB per input
-        // column (RM = 2)
-        if (variant < 0) { const char* ev = getenv("MARLIN_B200_TRANSPOSE_VARIANT"); variant = ev ? atoi(ev) : 16; }
-        switch (variant) {
-            case 0: return launch_transpose_f64<0, 1, 1>(in, ldi, out, ldo, rows, cols, st);
-            case 1: return launch_transpose_f64<1, 1, 1>(in, ldi, out, ldo, rows, cols, st);
-            case 2: return launch_transpose_f64<2, 1, 1>(in, ldi, out, ldo, rows, cols, st);
-            case 3: return launch_transpose_f64<3, 1, 1>(in, ldi, out, ldo, rows, cols, st);
-            case 4: return launch_transpose_f64<0, 2, 1>(in, ldi, out, ldo, rows, cols, st);
-            case 5: return launch_transpose_f64<0, 1, 2>(in, ldi, out, ldo, rows, cols, st);
-            case 6: return launch_transpose_f64<2, 1, 2>(in, ldi, out, ldo, rows, cols, st);
-            case 7: return launch_transpose_f64<3, 2, 1>(in, ldi, out, ldo, rows, cols, st);
-            case 8: return launch_transpose_f64<3, 1, 2>(in, ldi, out, ldo, rows, cols, st);
-            case 9: return launch_transpose_f64<0, 2, 2>(in, ldi, out, ldo, rows, cols, st);
-            case 10: return launch_transpose_f64<2, 2, 1>(in, ldi, out, ldo, rows, cols, st);
-            case 11: return launch_transpose_f64<4, 1, 1>(in, ldi, out, ldo, rows, cols, st);
-            case 12: return launch_transpose_f64<4, 2, 1>(in, ldi, out, ldo, rows, cols, st);
-            case 13: return launch_transpose_f64<5, 1, 1>(in, ldi, out, ldo, rows, cols, st);
-            case 14: return launch_transpose_f64<5, 2, 1>(in, ldi, out, ldo, rows, cols, st);
-            case 15: return launch_transpose_f64<6, 1, 1>(in, ldi, out, ldo, rows, cols, st);
-            case 16: return launch_transpose_f64<6, 2, 1>(in, ldi, out, ldo, rows, cols, st);
-            case 17: return launch_transpose_f64<6, 1, 2>(in, ldi, out, ldo, rows, cols, st);
-            case 18: return launch_transpose_f64<2, 1, 2>(in, ldi, out, ldo, rows, cols, st);
-            case 19: return launch_transpose_f64<4, 1, 2>(in, ldi, out, ldo, rows, cols, st);
-            default: return launch_transpose_f64<6, 2, 1>(in, ldi, out, ldo, rows, cols, st);
-        }
+        const int tiles_r = (rows + TT * TT_SUB - 1) / (TT * TT_SUB), tiles_c = (cols + TT - 1) / TT;
+        // 64 KiB of dynamic shared memory: above the 48 KiB a launch gets without opting in
+        cudaError_t e = cudaFuncSetAttribute(transpose_f64_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TT_SMEM);
+        if (e != cudaSuccess) return e;
+        transpose_f64_tile_kernel<<<tiles_r * tiles_c, 256, TT_SMEM, st>>>(in, ldi, out, ldo, rows, cols, tiles_r, tiles_c);
     } else {
         dim3 grid((rows + 31) / 32, (cols + 31) / 32);
         transpose_generic_kernel<double><<<grid, 256, 0, st>>>(in, ldi, out, ldo, rows, cols);
@@ -824,8 +759,7 @@ cudaError_t fill_uniform_f64(double* out, long long rs, long long cs, int rows, 
     // destinations the general one
     const bool linear = row_major ? (cs == 1 && rs == cols) : (rs == 1 && cs == rows);
     int full = 0;
-    static const bool no_fast = getenv("MARLIN_B200_FILL_GENERAL") != nullptr;     // test hook: force the general kernel
-    if (linear && !no_fast && ((reinterpret_cast<uintptr_t>(out) & 15) == 0) && total >= per_block && fast_fill_state(st) > 0)
+    if (linear &&((reinterpret_cast<uintptr_t>(out) & 15) == 0) && total >= per_block && fast_fill_state(st) > 0)
         full = (int)(total / per_block);
     if (full > 0) {
         if (lo == 0.0 && hi == 1.0)

@@ -428,9 +428,9 @@ syrk_f64_dmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
 //     load that touches the band, so the tensor cores start on the bands that have landed;
 //   * an entry may add a staged addend: D = acc + Cin, gated by a system-scope flag (the other holder of the C block
 //     has finished writing its partial into this GPU's staging buffer), and D may be a PEER pointer: the epilogue's
-//     st.global.v2.f64 go over NVLink.  Together: GEMM + reduce-scatter of the k partials in one kernel;
-//   * completion: when the last CTA tile of an entry has been stored, one thread publishes a flag (st.release.sys)
-//     locally (the D2H stream waits on it) and/or on the peer (its gated entries may start).
+//     st.global.v2.f64 go over NVLink.  Together: the GEMM epilogues do the reduce-scatter of the k partials;
+//   * completion: when the last CTA tile of an entry whose output is local has been stored, one thread publishes a
+//     local flag (st.release.sys) that the copy-out stream waits on.
 // -------------------------------------------------------------------------------------------
 struct G2Ent {
     double* D;
@@ -438,7 +438,6 @@ struct G2Ent {
     const unsigned long long* cin_flag;
     unsigned long long cin_val;
     unsigned long long* done_ctr;
-    unsigned long long* sig_remote;
     unsigned long long* sig_local;
     unsigned long long sig_val;
     long long ldd, ldcin;
@@ -459,8 +458,6 @@ struct G2Params {
     unsigned long long* status;                           // set to 1 if a wait times out
     long long timeout_ns;
     int ne, num_tiles;
-    int poll_mode;                                        // 0: every thread polls the addend flag, 1: lane 0 + __syncwarp
-    int fence_all;                                        // 1: every thread fences its stores before the tile is counted
 };
 
 __device__ __forceinline__ unsigned long long ld_acquire_gpu(const unsigned long long* p) {
@@ -585,10 +582,14 @@ __device__ __forceinline__ void dmma_grouped(const G2Params& g) {
         const long long ldd = en.ldd;
         const int Mc = en.M, Nc = en.N;
         if (add.Cin != nullptr && en.cin_flag != nullptr && en.cin_flag != cin_seen) {
-            // the other holder's partial must have landed in this GPU's staging buffer (every lane acquires)
-            if (g.poll_mode == 0 || lane == 0)
-                wait_flag_ge<true>(en.cin_flag, en.cin_val, g.timeout_ns, g.status, (1ull << 56) | (3ull << 48) | (unsigned long long)c);
-            if (g.poll_mode != 0) __syncwarp();
+            // the other holder's partial must have landed in this GPU's staging buffer: lane 0 polls, then every other lane
+            // acquires the flag through the same bounded wait (which returns on its first load).  Lane-dependent on purpose:
+            // with one warp-uniform wait here nvcc 12.9 schedules the DMMA mainloop differently, and the 16384^2 grouped
+            // multiply ran 18% slower (32.4 vs 39.3 TFLOP/s on an H100 80GB HBM3 at a 400 W power limit).
+            const unsigned long long tag = (1ull << 56) | (3ull << 48) | (unsigned long long)c;
+            if (lane == 0) wait_flag_ge<true>(en.cin_flag, en.cin_val, g.timeout_ns, g.status, tag);
+            __syncwarp();
+            if (lane != 0) wait_flag_ge<true>(en.cin_flag, en.cin_val, g.timeout_ns, g.status, tag);
             cin_seen = en.cin_flag;
         }
         const bool vec_ok = ((reinterpret_cast<uintptr_t>(D) & 15) == 0) && ((ldd & 1) == 0) &&
@@ -596,22 +597,19 @@ __device__ __forceinline__ void dmma_grouped(const G2Params& g) {
         // tile coordinates relative to the entry's region
         store_tile<false, false>(acc, cons, tm_ * BM, tn_ * BN, Mc, Nc, D, ldd, vec_ok, add);
         if (en.done_ctr != nullptr) {
-            // every consumer thread's stores of this tile, then ONE thread counts the tile and, if it was the entry's last,
-            // publishes the completion flags with system scope (peer GPUs and the copy streams poll them).
-            // EVERY thread fences its own stores first (the conservative order: fence, CTA barrier, count).  NOTE: with the
-            // tile stored to a PEER GPU this sequence was still measured faulty — one 16x32 patch of a tile stale in about a
-            // third of the 8192^2 calls, with or without the per-thread fences — so csrc/dist.cu only arms done_ctr for entries whose output is in
-            // LOCAL memory; peer outputs are announced by a stream memory operation after the launch (two-launch
-            // reduce-scatter) or pushed by the copy engine (host path).  The single-launch form stays behind
-            // MARLIN_B200_FUSED_SPLIT=0 for the investigation.
-            if (g.fence_all) __threadfence_system();
+            // The kernel only counts completion for entries whose output is LOCAL.  Every consumer thread fences its own
+            // stores of this tile, the CTA barrier orders those fences before the count, then ONE thread counts the tile
+            // and, if it was the entry's last, publishes the local flag with system scope (the copy-out stream polls it).
+            // With the tile stored to a PEER GPU this sequence was measured faulty — one 16x32 patch of a tile stale in
+            // about a third of the 8192^2 calls — so csrc/dist.cu announces peer outputs after the launch with a stream
+            // memory operation (two-launch reduce-scatter) or pushes them with the copy engine (host path).
+            __threadfence_system();
             asm volatile("bar.sync 1, %0;" ::"n"(NUM_CONSUMER_WARPS * 32) : "memory");
             if (cw == 0 && lane == 0) {
                 __threadfence_system();
                 const unsigned long long prev = atomicAdd(en.done_ctr, 1ull);
                 if (prev + 1ull == (unsigned long long)(en.tiles_m * en.tiles_n)) {
                     __threadfence_system();
-                    if (en.sig_remote) asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(en.sig_remote), "l"(en.sig_val) : "memory");
                     if (en.sig_local) asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(en.sig_local), "l"(en.sig_val) : "memory");
                 }
             }
@@ -945,7 +943,7 @@ cudaError_t gemm_f64_grouped2(const G2Launch& L, int num_sms, cudaStream_t strea
         if ((s.m_off % BM) != 0 || (s.n_off % BN) != 0) return cudaErrorInvalidValue;
         d.D = s.D; d.ldd = s.ldd; d.Cin = s.Cin; d.ldcin = s.ldcin;
         d.cin_flag = s.cin_flag; d.cin_val = s.cin_val;
-        d.done_ctr = s.done_ctr; d.sig_remote = s.sig_remote; d.sig_local = s.sig_local; d.sig_val = s.sig_val;
+        d.done_ctr = s.done_ctr; d.sig_local = s.sig_local; d.sig_val = s.sig_val;
         d.M = s.M; d.N = s.N; d.m_off = s.m_off; d.n_off = s.n_off;
         d.tiles_m = (s.M + BM - 1) / BM;
         d.tiles_n = (s.N + BN - 1) / BN;
@@ -965,10 +963,6 @@ cudaError_t gemm_f64_grouped2(const G2Launch& L, int num_sms, cudaStream_t strea
     g.ready = L.ready; g.ready_val = L.ready_val; g.status = L.status; g.timeout_ns = L.timeout_ns;
     g.ne = L.ne;
     g.num_tiles = tiles;
-    static const int fence_all = [] { const char* e = getenv("MARLIN_B200_FENCE_ALL"); return (e && e[0] == '0') ? 0 : 1; }();
-    g.fence_all = fence_all;
-    static const int poll_mode = [] { const char* e = getenv("MARLIN_B200_CIN_POLL"); return (e && e[0] == '1') ? 1 : 0; }();
-    g.poll_mode = poll_mode;
     const cudaError_t e =
         g_dmma_reference ? launch_with_smem<gemm_f64_dmma_grouped_kernel>(min(tiles, num_sms), NUM_THREADS, SMEM_BYTES, stream, g)
                          : launch_with_smem<gemm_f64_dmma16x8_grouped_kernel>(min(tiles, num_sms), NUM_THREADS, SMEM_BYTES, stream, g);

@@ -43,8 +43,7 @@ struct G2Entry {
     const unsigned long long* cin_flag = nullptr;       // wait until *cin_flag >= cin_val (system scope) before reading Cin
     unsigned long long cin_val = 0;
     unsigned long long* done_ctr = nullptr;             // zeroed device counter; when it reaches the entry's tile count ...
-    unsigned long long* sig_remote = nullptr;           // ... these flags are set to sig_val (st.release.sys)
-    unsigned long long* sig_local = nullptr;
+    unsigned long long* sig_local = nullptr;            // ... this flag is set to sig_val (st.release.sys); D must be local
     unsigned long long sig_val = 0;
 };
 struct G2Launch {

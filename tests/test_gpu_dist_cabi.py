@@ -35,7 +35,8 @@ def _run(world, ndev, slow, timeout=900, big=0, big_fused=0, extra_env=None):
 
 @pytest.mark.parametrize("slow", [False, True])
 def test_dist_multiply_cabi_two_ranks(slow):
-    """fast = one grouped DMMA launch per rank with band flags + the fused reduce-scatter; slow = staged partials and
+    """fast = the grouped DMMA kernel with band flags, two launches per rank with the fused reduce-scatter's exchange flags
+    between them; slow = staged partials and
     per-tile launches (the path bf16 / transposed tiles take), forced here for fp64 so both are checked bit-for-tolerance."""
     import torch
     ndev = torch.cuda.device_count()
@@ -65,9 +66,9 @@ def test_dist_host_path_bench_size_pinned():
 
 
 def test_fused_reduce_scatter_full_size_back_to_back():
-    """8192^2 with the contraction split over two GPUs, six multiplies queued back to back: the GEMM epilogue stores the
-    peer's half over NVLink, the flag that announces it must not overtake those stores (every thread fences before its tile
-    is counted).  Freivalds on the first and the last result."""
+    """8192^2 with the contraction split over two GPUs, six multiplies queued back to back: the first launch's epilogues
+    store the peer's half over NVLink, and the flag that announces it, a stream memory operation after that launch, must
+    not overtake those stores.  Freivalds on the first and the last result."""
     import torch
     if torch.cuda.device_count() < 2:
         pytest.skip("needs 2 GPUs")
