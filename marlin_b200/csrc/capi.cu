@@ -710,10 +710,7 @@ int32_t mb_matmul_blocked_host(mb_ctx* ctx, const double* const* A_host, const d
     MB_LOCK(ctx);
     if (!A_host || !B_host || !C_host || !row_len || !k_len || !col_len || m <= 0 || k <= 0 || n <= 0)
         return fail(MB_ERR_INVALID_ARG, "mb_matmul_blocked_host: bad argument");
-    if (!ctx->h2d_stream) {
-        MB_CUDA(cudaStreamCreateWithFlags(&ctx->h2d_stream, cudaStreamNonBlocking));
-        MB_CUDA(cudaStreamCreateWithFlags(&ctx->d2h_stream, cudaStreamNonBlocking));
-    }
+    MB_CUDA(ensure_copy_streams(ctx));
     // device layout: every tile gets an even leading dimension and a 256-byte aligned slot (TMA eligibility)
     auto even = [](int x) { return (x + 1) & ~1; };
     auto slot = [](size_t bytes) { return (bytes + 255) & ~size_t(255); };
@@ -904,10 +901,7 @@ int32_t mb_matmul_rowsharded_host(mb_ctx* ctx, const double* A_host, int64_t row
     if (rows < 0 || k < 0 || n < 0 || (rows > 0 && ((k > 0 && !A_host) || (n > 0 && !C_host))) || (k > 0 && n > 0 && !B_host))
         return fail(MB_ERR_INVALID_ARG, "mb_matmul_rowsharded_host: bad argument");
     if (rows == 0 || n == 0) return MB_OK;
-    if (!ctx->h2d_stream) {
-        MB_CUDA(cudaStreamCreateWithFlags(&ctx->h2d_stream, cudaStreamNonBlocking));
-        MB_CUDA(cudaStreamCreateWithFlags(&ctx->d2h_stream, cudaStreamNonBlocking));
-    }
+    MB_CUDA(ensure_copy_streams(ctx));
     constexpr int SLOTS = 3;
     // ~256 MiB of A (or C, whichever is wider) per chunk, a multiple of 128 rows (whole GEMM tiles), at least one tile;
     // MARLIN_B200_ROWSHARD_CHUNK_MIB overrides the size (the tests use it to run many chunks on small inputs)

@@ -134,8 +134,6 @@ constexpr size_t RING_SLOTS = 8192;
 
 namespace {
 
-#define MB_ERR_TIMEOUT_CODE MB_ERR_TIMEOUT
-
 inline unsigned long long* flag_ch(mb_comm* c, int on_rank, int ch, int src) { return c->flags_peer[on_rank] + F_CH + ch * MAXW + src; }
 inline long long timeout_ns(const mb_comm* c) { return (long long)(c->timeout_s * 1e9); }
 
@@ -253,10 +251,22 @@ cudaEvent_t next_event(mb_comm* c) {
 }
 
 // ---------------------------------------------------------------------------------------- plan
+struct MyC { int id, i, j; std::vector<int> kks; };   // a C tile (id = i*n + j) with the kk of one rank's products of it
 struct Plan {
     int m, k, n, world;
     std::vector<int> prod_rank;                 // by seq = i*n*k + j*k + kk  (matrix/BlockMatrix.scala:163,168)
     std::vector<std::vector<int>> holders;      // per C tile (i*n + j): ranks holding a partial, in kk order of first appearance
+    // the C tiles rank r computes partials of, in (i, j) order
+    std::vector<MyC> c_tiles_of(int r) const {
+        std::vector<MyC> out;
+        for (int i = 0; i < m; ++i)
+            for (int j = 0; j < n; ++j) {
+                MyC mc{i * n + j, i, j, {}};
+                for (int kk = 0; kk < k; ++kk) if (prod_rank[i * n * k + j * k + kk] == r) mc.kks.push_back(kk);
+                if (!mc.kks.empty()) out.push_back(mc);
+            }
+        return out;
+    }
 };
 // Products are dealt to ranks in contiguous seq ranges: the kk partials of a C tile stay on one rank whenever ranks get
 // whole C tiles; with G = m*k*n this is the reference's partition -> executor identity (MatrixMultPartitioner).
@@ -276,6 +286,33 @@ Plan make_plan(int m, int k, int n, int world) {
             }
     return p;
 }
+
+// Do the distinct A and B tiles that one rank's products read (its C tiles `cs`) fit the operand tables of a grouped
+// launch?  The grouped launch has fixed-size tables, and whether EVERY rank's share fits is decided from the plan alone,
+// so all ranks take the same path (a rank-local fallback would leave its partner waiting for flags that never come).
+// Both entries run this check for every rank together with their own entry limits; the launch builders rely on it and
+// fill the tables unchecked.
+bool operands_fit(const Plan& p, const std::vector<MyC>& cs) {
+    std::vector<char> ua(p.m * p.k, 0), ub(p.k * p.n, 0);
+    int na = 0, nb = 0;
+    for (const MyC& mc : cs)
+        for (int kk : mc.kks) {
+            if (!ua[mc.i * p.k + kk]) { ua[mc.i * p.k + kk] = 1; ++na; }
+            if (!ub[kk * p.n + mc.j]) { ub[kk * p.n + mc.j] = 1; ++nb; }
+        }
+    return na <= mb::G2_MAX_OPS && nb <= mb::G2_MAX_OPS;
+}
+
+// Readiness bands along an operand tile's extent (A: rows, B: columns): up to `most` of them from an extent of 1024 on,
+// each a multiple of 128 wide.
+inline void bands_of(int extent, int most, int& band, int& nbands) {
+    nbands = extent >= 1024 ? most : 1;
+    band = ((extent + nbands - 1) / nbands + 127) / 128 * 128;
+    nbands = (extent + band - 1) / band;
+}
+
+// Fused reduce-scatter: of a C tile N columns wide the owner reduces [0, half_cols(N)), the partner the rest.
+inline int half_cols(int N) { return std::min(N, ((N / 2 + 127) / 128) * 128); }
 
 // ---------------------------------------------------------------------------------------- staging
 // Per-source slots: src only ever writes [src * slot_bytes, +slot_bytes) of dst's buffer, so two sources can never
@@ -364,16 +401,246 @@ int32_t open_entry(const ShmEntry& en, char** ptr) {
     return MB_OK;
 }
 
-struct Tile {                 // an operand tile as this rank sees it during one call
-    mb_block blk;             // local view (the owner's block itself, or the pulled packed copy)
-    bool remote = false;
-    int src = -1;
-    const ShmEntry* ent = nullptr;
-    cudaEvent_t landed = nullptr;     // whole tile is here (slow path)
-    int band = 0, nbands = 1;         // readiness bands (rows for A, columns for B)
+// Checks every entry runs first: the communicator, its context, the arguments (`args_ok`) and an earlier abort.
+int32_t check_call(mb_comm* c, const char* who, bool args_ok) {
+    if (!c) return fail(MB_ERR_INVALID_ARG, "null communicator");
+    MB_CTX(c->ctx);
+    if (!args_ok) return fail(MB_ERR_INVALID_ARG, "%s: bad argument", who);
+    if (c->aborted) return fail(MB_ERR_TIMEOUT, "mb_comm: the communicator was aborted after a peer stopped answering");
+    return MB_OK;
+}
+
+// Publish the tiles this rank offers in call e, read every rank's directory of that call, and map every peer allocation
+// the directories name.
+int32_t exchange_directory(mb_comm* c, unsigned long long e, const std::vector<ShmEntry>& mine, std::vector<std::vector<ShmEntry>>& dir) {
+    int32_t rc = publish(c, e, mine);
+    if (rc) return rc;
+    if ((rc = read_all(c, e, dir)) != MB_OK) return rc;
+    // Map every peer allocation this call will touch BEFORE any pointer is taken: opening a handle can evict stale
+    // mappings (see ipc_open_ex), which would invalidate pointers handed out earlier in the same call.  A second pass
+    // after an eviction only hits the cache.
+    for (int attempt = 0; attempt < 3; ++attempt) {
+        const unsigned long long gen = mb::ipc_evictions();
+        char* dummy = nullptr;
+        for (int p = 0; p < c->world; ++p)
+            if (p != c->rank)
+                for (const ShmEntry& en : dir[p])
+                    if ((rc = open_entry(en, &dummy)) != MB_OK) return rc;
+        if (mb::ipc_evictions() == gen) break;
+    }
+    return MB_OK;
+}
+// The directory entry of every tile of one kind, as published by the rank `owner` names (by any rank if owner is null);
+// null where there is none.
+std::vector<const ShmEntry*> entries_of(const std::vector<std::vector<ShmEntry>>& dir, int kind, int count, const int32_t* owner) {
+    std::vector<const ShmEntry*> out(count, nullptr);
+    for (size_t p = 0; p < dir.size(); ++p)
+        for (const ShmEntry& en : dir[p])
+            if (en.kind == kind && en.idx >= 0 && en.idx < count && (!owner || owner[en.idx] == (int)p)) out[en.idx] = &en;
+    return out;
+}
+
+struct Tile {                         // an operand tile as this rank sees it during one call
+    mb_block blk;                     // its local copy: the owner's block itself, or a packed copy in the arena
+    int src = -1;                     // the rank it comes from: its owner (device tiles) or its uploader (host tiles)
+    const ShmEntry* ent = nullptr;    // the source's directory entry, for tiles pulled from a peer
+    bool need = false;                // one of this rank's products reads it
+    bool remote = false;              // device tiles: pulled from a peer
+    int up_slot = -1;                 // host tiles: index among the tiles its uploader uploads (F_UPREADY)
+    cudaEvent_t landed = nullptr;     // device tiles: the whole tile is here (general path)
+    int band = 0, nbands = 1;         // readiness bands (rows for A, columns for B); band 0 = resident, never polled
     int ready_base = -1;              // first band flag index relative to flags + F_BAND
     int op = -1;                      // operand index in the grouped launch
 };
+
+// Operand index of tile t in the A or B table of L, added on first use (operands_fit bounds the table).
+int op_of(mb::G2Launch& L, Tile& t, bool is_a) {
+    if (t.op >= 0) return t.op;
+    int& cnt = is_a ? L.na : L.nb;
+    mb::G2Operand& o = (is_a ? L.A : L.B)[cnt];
+    o.ptr = f64_ptr(&t.blk); o.ld = t.blk.ld; o.rows = t.blk.rows; o.cols = t.blk.cols;
+    o.band = t.band; o.ready_base = t.ready_base;
+    return t.op = cnt++;
+}
+
+// Copy band b of tile t into its local copy from `src`, an array of the same shape and orientation with leading
+// dimension `sld`.  Bands cut the logical rows (A) / columns (B); in the physical (minor x major) array that is the minor
+// axis (rows [lo, hi) of every column) or the major one (columns [lo, hi)).
+cudaError_t copy_band(const Tile& t, bool is_a, int b, const char* src, size_t sld, cudaMemcpyKind kind, cudaStream_t st) {
+    const bool trans = t.blk.is_transpose != 0;
+    const size_t es = elem_size(t.blk.dtype), dld = t.blk.ld;
+    const int minor = trans ? t.blk.cols : t.blk.rows, major = trans ? t.blk.rows : t.blk.cols;
+    const int lo = b * t.band, hi = std::min(is_a ? t.blk.rows : t.blk.cols, lo + t.band);
+    char* dst = elem_ptr(&t.blk);
+    if (hi <= lo || minor <= 0 || major <= 0) return cudaSuccess;
+    if (is_a != trans)
+        return cudaMemcpy2DAsync(dst + (size_t)lo * es, dld * es, src + (size_t)lo * es, sld * es, (size_t)(hi - lo) * es, major, kind, st);
+    return cudaMemcpy2DAsync(dst + (size_t)lo * dld * es, dld * es, src + (size_t)lo * sld * es, sld * es, (size_t)minor * es, hi - lo,
+                             kind, st);
+}
+
+// The status word is set by any bounded device-side wait that gave up.  read_status queues its copy into status_host
+// behind the work on st; check_status reports the copy read last.
+cudaError_t read_status(mb_comm* c, cudaStream_t st) {
+    return cudaMemcpyAsync(c->status_host, c->flags + F_STATUS, 8, cudaMemcpyDeviceToHost, st);
+}
+int32_t check_status(const mb_comm* c, const char* who) {
+    if (*c->status_host == 0) return MB_OK;
+    return fail(MB_ERR_TIMEOUT, "%s: a device-side wait for a peer timed out (status %llu): a rank died or fell out of step; results since then "
+                "are invalid", who, *c->status_host);
+}
+// My tiles may not be overwritten or freed until every consumer has finished pulling them.
+int32_t wait_consumers(mb_comm* c, const std::vector<char>& consumer, unsigned long long e, cudaStream_t st) {
+    for (int p = 0; p < c->world; ++p)
+        if (consumer[p]) MB_CUDA(waitf(c, flag_ch(c, c->rank, CH_DONE, p), e, st));
+    return MB_OK;
+}
+
+// The grouped-launch tables are about 20 KB each: one pair per thread serves both entries.
+thread_local mb::G2Launch launch_tables[2];
+
+// mb_matmul_blocked_dist's products on the fast path (plain fp64 tiles, C tiles with two holders fused).
+// Two launches of the grouped kernel with the exchange flags between them: L0 computes the halves the peers reduce
+// (stored into their staging buffers) and the plain regions, L2 the halves reduced here (acc + the peer's staged
+// partial).  Completion counted inside a kernel whose epilogue stores to peer memory was measured faulty — at 8192^2
+// about one call in three came back with one 16 x 32 patch off by a single product term — so the kernel boundary is
+// the completion point and the flags are stream memory operations.  Both launches share one operand table.
+int32_t products_fused(mb_comm* c, unsigned long long e, const Plan& plan, const std::vector<MyC>& myc, std::vector<Tile>& tA,
+                       std::vector<Tile>& tB, const int32_t* row_len, const int32_t* col_len, mb_block* const* C_tiles,
+                       const std::vector<const ShmEntry*>& entC, const std::vector<size_t>& slot_off, const std::vector<int>& pair_slot,
+                       std::vector<char>& partial_to, std::vector<char>& fused_free_to) {
+    mb_ctx* ctx = c->ctx;
+    const int rank = c->rank, k = plan.k, n = plan.n;
+    mb::G2Launch& L0 = launch_tables[0];
+    mb::G2Launch& L2 = launch_tables[1];
+    L0 = mb::G2Launch();
+    L2 = mb::G2Launch();
+    // entries: regions that peers wait for first, plain regions next, regions that wait for a peer last; at most two per
+    // C tile, which the plan-wide check keeps within the table
+    struct Reg { const MyC* mc; int n_off, N; int phase; };   // phase 0 = peer's half (store remote), 1 = plain, 2 = my half (needs the peer's)
+    std::vector<Reg> regs;
+    for (const MyC& mc : myc) {
+        const int N_ = col_len[mc.j];
+        if (plan.holders[mc.id].size() == 2) {
+            const int nh = half_cols(N_);
+            const bool owner = plan.holders[mc.id][0] == rank;
+            // the owner reduces the left half [0, nh), the partner the right half [nh, N)
+            if (owner) { if (N_ > nh) regs.push_back({&mc, nh, N_ - nh, 0}); regs.push_back({&mc, 0, nh, 2}); }
+            else { regs.push_back({&mc, 0, nh, 0}); if (N_ > nh) regs.push_back({&mc, nh, N_ - nh, 2}); }
+        } else {
+            regs.push_back({&mc, 0, N_, 1});
+        }
+    }
+    std::stable_sort(regs.begin(), regs.end(), [](const Reg& a, const Reg& b) { return a.phase < b.phase; });
+    struct Note { int peer, slot; };
+    std::vector<Note> wrote, need, final_to;              // F_PART2 to signal / F_PART2 to wait for / F_FINAL2 to signal
+    for (const Reg& rg : regs) {
+        const MyC& mc = *rg.mc;
+        const int id = mc.id;
+        mb::G2Launch& L = rg.phase == 2 ? L2 : L0;
+        mb::G2Entry& en = L.E[L.ne++];
+        en.nseg = (int)mc.kks.size();
+        for (int s = 0; s < en.nseg; ++s) {
+            en.a_op[s] = op_of(L0, tA[mc.i * k + mc.kks[s]], true);
+            en.b_op[s] = op_of(L0, tB[mc.kks[s] * n + mc.j], false);
+        }
+        en.m_off = 0; en.n_off = rg.n_off; en.M = row_len[mc.i]; en.N = rg.N;
+        const auto& h = plan.holders[id];
+        const int ldst = even(row_len[mc.i]);               // leading dimension of a staged partial
+        if (rg.phase == 1) {
+            if (h[0] == rank) {                          // my own tile (other holders, if any, are added in step 4)
+                en.D = f64_ptr(C_tiles[id]); en.ldd = C_tiles[id]->ld;
+            } else {                                     // staged path: straight into my slot of the owner's staging buffer
+                en.D = reinterpret_cast<double*>(c->staging_peer[h[0]] + (size_t)rank * c->slot_bytes + slot_off[id]);
+                en.ldd = ldst;
+                partial_to[h[0]] = 1;
+            }
+            continue;
+        }
+        const int peer = h[0] == rank ? h[1] : h[0];
+        const int slot = pair_slot[id];
+        if (rg.phase == 0) {
+            // the half the PEER reduces: my partial of it goes over NVLink into my slot of the peer's staging buffer
+            en.D = reinterpret_cast<double*>(c->staging_peer[peer] + (size_t)rank * c->slot_bytes + slot_off[id]);
+            en.ldd = ldst;
+            wrote.push_back({peer, slot});
+        } else {
+            // the half I reduce: acc + the peer's staged partial; the result belongs in the OWNER's C tile
+            en.Cin = reinterpret_cast<const double*>(c->staging + (size_t)peer * c->slot_bytes + slot_off[id]);
+            en.ldcin = ldst;
+            need.push_back({peer, slot});
+            if (h[0] == rank) {
+                en.D = f64_ptr(C_tiles[id]) + (size_t)rg.n_off * C_tiles[id]->ld; en.ldd = C_tiles[id]->ld;
+            } else {
+                if (!entC[id]) return fail(MB_ERR_INVALID_ARG, "mb_matmul_blocked_dist: owner did not publish C tile %d", id);
+                char* cp = nullptr;
+                int32_t rc = open_entry(*entC[id], &cp);
+                if (rc) return rc;
+                en.D = reinterpret_cast<double*>(cp) + (size_t)rg.n_off * entC[id]->ld; en.ldd = entC[id]->ld;
+                final_to.push_back({peer, slot});
+            }
+            fused_free_to[peer] = 1;
+        }
+    }
+    L2.na = L0.na; L2.nb = L0.nb;
+    std::copy_n(L0.A, L0.na, L2.A);
+    std::copy_n(L0.B, L0.nb, L2.B);
+    L0.ready = L2.ready = c->flags + F_BAND; L0.ready_val = L2.ready_val = e;
+    L0.status = L2.status = c->flags + F_STATUS; L0.timeout_ns = L2.timeout_ns = timeout_ns(c);
+    int launches = 0;
+    cudaError_t ce = mb::gemm_f64_grouped2(L0, ctx->num_sms, ctx->stream, &launches);
+    if (ce != cudaSuccess) return cuda_fail(ce, "gemm_f64_grouped2 (first half)");
+    for (const Note& w : wrote) MB_CUDA(sig(c, c->flags_peer[w.peer] + F_PART2 + rank * MAX_PAIR + w.slot, e, ctx->stream));
+    for (const Note& w : need) MB_CUDA(waitf(c, c->flags + F_PART2 + w.peer * MAX_PAIR + w.slot, e, ctx->stream));
+    ce = mb::gemm_f64_grouped2(L2, ctx->num_sms, ctx->stream, &launches);
+    if (ce != cudaSuccess) return cuda_fail(ce, "gemm_f64_grouped2 (second half)");
+    for (const Note& w : final_to) MB_CUDA(sig(c, c->flags_peer[w.peer] + F_FINAL2 + rank * MAX_PAIR + w.slot, e, ctx->stream));
+    ctx->launches += launches;
+    return MB_OK;
+}
+
+// mb_matmul_blocked_dist's products on the general path: per product (or per C tile when all kk are here), tile-level
+// waits, staged partials.
+int32_t products_general(mb_comm* c, const Plan& plan, const std::vector<MyC>& myc, std::vector<Tile>& tA, std::vector<Tile>& tB,
+                         const int32_t* row_len, const int32_t* col_len, int out_dtype, mb_block* const* C_tiles,
+                         const std::vector<size_t>& slot_off, std::vector<char>& partial_to) {
+    mb_ctx* ctx = c->ctx;
+    const int rank = c->rank, m = plan.m, k = plan.k, n = plan.n;
+    cudaStream_t S = ctx->stream;
+    int32_t rc = MB_OK;
+    for (const MyC& mc : myc) {
+        const auto& h = plan.holders[mc.id];
+        mb_block out;
+        if (h[0] == rank) { out = *C_tiles[mc.id]; out.owns = 0; }
+        else {
+            out = mb_block();
+            out.data = c->staging_peer[h[0]] + (size_t)rank * c->slot_bytes + slot_off[mc.id];
+            out.rows = row_len[mc.i]; out.cols = col_len[mc.j]; out.ld = even(row_len[mc.i]); out.dtype = out_dtype; out.device = ctx->device;
+            partial_to[h[0]] = 1;
+        }
+        for (int kk : mc.kks) {
+            Tile& a = tA[mc.i * k + kk];
+            Tile& b = tB[kk * n + mc.j];
+            if (a.landed) MB_CUDA(cudaStreamWaitEvent(S, a.landed, 0));
+            if (b.landed) MB_CUDA(cudaStreamWaitEvent(S, b.landed, 0));
+        }
+        if ((int)mc.kks.size() == k) {
+            // every kk of this C tile is here: one launch per tile (bf16: K segments in one wgmma launch; fp64: grouped DMMA)
+            std::vector<mb_block*> at(m * k, nullptr), bt(k * n, nullptr), ct(m * n, nullptr);
+            for (int kk = 0; kk < k; ++kk) { at[mc.i * k + kk] = &tA[mc.i * k + kk].blk; bt[kk * n + mc.j] = &tB[kk * n + mc.j].blk; }
+            ct[mc.id] = &out;
+            const int32_t id = mc.id;
+            if ((rc = mb_matmul_blocked_subset(ctx, at.data(), bt.data(), m, k, n, ct.data(), &id, 1)) != MB_OK) return rc;
+        } else {
+            bool first = true;
+            for (int kk : mc.kks) {
+                if ((rc = mb_block_gemm(ctx, &tA[mc.i * k + kk].blk, &tB[kk * n + mc.j].blk, &out, first ? 0 : 1)) != MB_OK) return rc;
+                first = false;
+            }
+        }
+    }
+    return MB_OK;
+}
 
 }  // namespace
 
@@ -492,16 +759,11 @@ int32_t mb_comm_abort(mb_comm* c) {
 
 // Has any bounded device-side wait given up since the communicator was created?  (Synchronises the context stream.)
 int32_t mb_comm_check(mb_comm* c) {
-    if (!c) return fail(MB_ERR_INVALID_ARG, "null communicator");
-    MB_CTX(c->ctx);
-    if (c->aborted) return fail(MB_ERR_TIMEOUT, "mb_comm: the communicator was aborted after a peer stopped answering");
-    MB_CUDA(cudaMemcpyAsync(c->status_host, c->flags + F_STATUS, 8, cudaMemcpyDeviceToHost, c->ctx->stream));
-    int32_t rs = sync_bounded(c, c->ctx->stream, "mb_comm_check");
-    if (rs) return rs;
-    if (*c->status_host != 0)
-        return fail(MB_ERR_TIMEOUT, "mb_comm: a device-side wait for a peer timed out (code %llu): a rank died or fell out of step; "
-                    "results since then are invalid", *c->status_host);
-    return MB_OK;
+    int32_t r = check_call(c, "mb_comm_check", true);
+    if (r) return r;
+    MB_CUDA(read_status(c, c->ctx->stream));
+    if ((r = sync_bounded(c, c->ctx->stream, "mb_comm_check")) != MB_OK) return r;
+    return check_status(c, "mb_comm_check");
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -512,17 +774,15 @@ int32_t mb_comm_check(mb_comm* c) {
 int32_t mb_matmul_blocked_dist(mb_comm* c, mb_block* const* A_tiles, const int32_t* a_owner, mb_block* const* B_tiles,
                                const int32_t* b_owner, int32_t m, int32_t k, int32_t n, const int32_t* row_len,
                                const int32_t* k_len, const int32_t* col_len, int32_t dtype, mb_block* const* C_tiles) {
-    if (!c) return fail(MB_ERR_INVALID_ARG, "null communicator");
+    int32_t rc = check_call(c, "mb_matmul_blocked_dist", A_tiles && B_tiles && C_tiles && a_owner && b_owner && row_len && k_len && col_len &&
+                                                         m > 0 && k > 0 && n > 0);
+    if (rc) return rc;
     mb_ctx* ctx = c->ctx;
-    MB_CTX(ctx);
     MB_LOCK(ctx);
-    if (!A_tiles || !B_tiles || !C_tiles || !a_owner || !b_owner || !row_len || !k_len || !col_len || m <= 0 || k <= 0 || n <= 0)
-        return fail(MB_ERR_INVALID_ARG, "mb_matmul_blocked_dist: bad argument");
-    if (c->aborted) return fail(MB_ERR_TIMEOUT, "mb_comm: the communicator was aborted after a peer stopped answering");
     if (dtype != MB_F64 && dtype != MB_BF16) return fail(MB_ERR_UNSUPPORTED, "mb_matmul_blocked_dist: fp64 or bf16 tiles");
     const int rank = c->rank, world = c->world;
     const int out_dtype = dtype == MB_BF16 ? MB_F32 : MB_F64;
-    const size_t esz = elem_size(dtype), osz = elem_size(out_dtype);
+    const size_t osz = elem_size(out_dtype);
     cudaStream_t S = ctx->stream, X = c->X;
     const Plan plan = make_plan(m, k, n, world);
     // ---- local validation (before anything collective) ----
@@ -562,32 +822,12 @@ int32_t mb_matmul_blocked_dist(mb_comm* c, mb_block* const* A_tiles, const int32
         if (plan.holders[t][0] == rank && plan.holders[t].size() > 1) {
             ShmEntry en; int32_t r = export_block(C_tiles[t], 2, t, &en); if (r) return r; mine.push_back(en);
         }
-    int32_t rc = publish(c, e, mine);
-    if (rc) return rc;
     std::vector<std::vector<ShmEntry>> dir;
-    if ((rc = read_all(c, e, dir)) != MB_OK) return rc;
-    std::vector<const ShmEntry*> entA(m * k, nullptr), entB(k * n, nullptr), entC(m * n, nullptr);
-    for (int p = 0; p < world; ++p)
-        for (const ShmEntry& en : dir[p]) {
-            if (en.kind == 0 && en.idx >= 0 && en.idx < m * k && a_owner[en.idx] == p) entA[en.idx] = &en;
-            if (en.kind == 1 && en.idx >= 0 && en.idx < k * n && b_owner[en.idx] == p) entB[en.idx] = &en;
-            if (en.kind == 2 && en.idx >= 0 && en.idx < m * n) entC[en.idx] = &en;
-        }
+    if ((rc = exchange_directory(c, e, mine, dir)) != MB_OK) return rc;
+    const std::vector<const ShmEntry*> entA = entries_of(dir, 0, m * k, a_owner), entB = entries_of(dir, 1, k * n, b_owner),
+                                       entC = entries_of(dir, 2, m * n, nullptr);
     for (int t = 0; t < m * k; ++t) if (!entA[t]) return fail(MB_ERR_INVALID_ARG, "mb_matmul_blocked_dist: rank %d did not publish A tile %d", a_owner[t], t);
     for (int t = 0; t < k * n; ++t) if (!entB[t]) return fail(MB_ERR_INVALID_ARG, "mb_matmul_blocked_dist: rank %d did not publish B tile %d", b_owner[t], t);
-
-    // Map every peer allocation this call will touch BEFORE any pointer is taken: opening a handle can evict stale
-    // mappings (see ipc_open_ex), which would invalidate pointers handed out earlier in the same call.  A second pass
-    // after an eviction only hits the cache.
-    for (int attempt = 0; attempt < 3; ++attempt) {
-        const unsigned long long gen = mb::ipc_evictions();
-        char* dummy = nullptr;
-        for (int p = 0; p < world; ++p)
-            if (p != rank)
-                for (const ShmEntry& en : dir[p])
-                    if ((rc = open_entry(en, &dummy)) != MB_OK) return rc;
-        if (mb::ipc_evictions() == gen) break;
-    }
 
     // ---- the same decision on every rank: can the whole call use the grouped DMMA launch / the fused reduce-scatter? ----
     bool fast = dtype == MB_F64 && k <= mb::G2_MAX_SEG;
@@ -596,31 +836,12 @@ int32_t mb_matmul_blocked_dist(mb_comm* c, mb_block* const* A_tiles, const int32
     for (int t = 0; t < k * n && fast; ++t) fast = plain(entB[t]) && entB[t]->cols > 0;
     for (int t = 0; t < m * n && fast; ++t) if (entC[t]) fast = plain(entC[t]);
     if (const char* env = getenv("MARLIN_B200_DIST_SLOW")) if (env[0] == '1') fast = false;
-
-    // my products, my C regions
-    struct MyC { int id, i, j; std::vector<int> kks; };
-    std::vector<MyC> myc;
-    for (int i = 0; i < m; ++i)
-        for (int j = 0; j < n; ++j) {
-            MyC mc{i * n + j, i, j, {}};
-            for (int kk = 0; kk < k; ++kk) if (plan.prod_rank[i * n * k + j * k + kk] == rank) mc.kks.push_back(kk);
-            if (!mc.kks.empty()) myc.push_back(mc);
-        }
-    // the grouped launch has fixed-size tables; whether EVERY rank's share fits is decided from the plan alone, so all
-    // ranks take the same path (a rank-local fallback would leave its fused partner waiting for flags that never come)
+    // one grouped launch per rank: two entries per C tile at most
     for (int r = 0; r < world && fast; ++r) {
-        std::vector<char> ua(m * k, 0), ub(k * n, 0), uc(m * n, 0);
-        int na = 0, nb = 0, nc = 0;
-        for (int i = 0; i < m; ++i)
-            for (int j = 0; j < n; ++j)
-                for (int kk = 0; kk < k; ++kk)
-                    if (plan.prod_rank[i * n * k + j * k + kk] == r) {
-                        if (!ua[i * k + kk]) { ua[i * k + kk] = 1; ++na; }
-                        if (!ub[kk * n + j]) { ub[kk * n + j] = 1; ++nb; }
-                        if (!uc[i * n + j]) { uc[i * n + j] = 1; ++nc; }
-                    }
-        if (na > mb::G2_MAX_OPS || nb > mb::G2_MAX_OPS || 2 * nc > mb::G2_MAX_ENTRIES) fast = false;
+        const std::vector<MyC> cs = plan.c_tiles_of(r);
+        fast = operands_fit(plan, cs) && 2 * (int)cs.size() <= mb::G2_MAX_ENTRIES;
     }
+    const std::vector<MyC> myc = plan.c_tiles_of(rank);      // my products, my C regions
     // fused pairs: C tiles with exactly two holders.  slot = ordinal among the tiles this pair shares, in (i,j) order.
     auto fused_tile = [&](int id) { return fast && plan.holders[id].size() == 2; };
     std::map<std::pair<int, int>, int> pair_count;          // (lo rank, hi rank) -> tiles so far
@@ -633,7 +854,6 @@ int32_t mb_matmul_blocked_dist(mb_comm* c, mb_block* const* A_tiles, const int32
         }
 
     // ---- staging need per (src -> dst), identical arithmetic on every rank ----
-    auto half_cols = [&](int id) { const int N_ = col_len[id % n]; return std::min(N_, ((N_ / 2 + 127) / 128) * 128); };
     std::vector<size_t> slot_off(m * n, 0);                 // offset of tile id inside the (src -> dst) slot, for the pair that uses it
     size_t need_slot = 0;
     {
@@ -642,9 +862,9 @@ int32_t mb_matmul_blocked_dist(mb_comm* c, mb_block* const* A_tiles, const int32
             const auto& h = plan.holders[id];
             if (h.size() < 2) continue;
             const size_t M_ = row_len[id / n], N_ = col_len[id % n];
-            if (fused_tile(id) && fast) {
+            if (fused_tile(id)) {
                 // owner h[0] receives the partner's partial of the left half; the partner receives the owner's partial of the right half
-                const size_t nh = half_cols(id);
+                const size_t nh = half_cols(col_len[id % n]);
                 size_t& u0 = used[{h[1], h[0]}];
                 size_t& u1 = used[{h[0], h[1]}];
                 slot_off[id] = std::max(u0, u1);            // one offset for both directions keeps the bookkeeping simple
@@ -662,12 +882,12 @@ int32_t mb_matmul_blocked_dist(mb_comm* c, mb_block* const* A_tiles, const int32
 
     // ---- 1. tell my consumers that my tiles are final (stream-ordered behind whatever produced them on S) ----
     std::vector<char> consumer(world, 0), source(world, 0);
-    std::vector<char> needA(m * k, 0), needB(k * n, 0);
+    std::vector<Tile> tA(m * k), tB(k * n);
     for (int i = 0; i < m; ++i)
         for (int j = 0; j < n; ++j)
             for (int kk = 0; kk < k; ++kk) {
                 const int r = plan.prod_rank[i * n * k + j * k + kk];
-                if (r == rank) { needA[i * k + kk] = 1; needB[kk * n + j] = 1; }
+                if (r == rank) { tA[i * k + kk].need = true; tB[kk * n + j].need = true; }
                 else {
                     if (a_owner[i * k + kk] == rank) consumer[r] = 1;
                     if (b_owner[kk * n + j] == rank) consumer[r] = 1;
@@ -699,7 +919,6 @@ int32_t mb_matmul_blocked_dist(mb_comm* c, mb_block* const* A_tiles, const int32
     }
 
     // ---- 2. pull the tiles I need, in first-use order, band by band, on the copy stream ----
-    std::vector<Tile> tA(m * k), tB(k * n);
     size_t arena_need = 0;
     std::vector<std::pair<int, int>> pulls;                  // (0 = A / 1 = B, idx) in first-use order
     for (const MyC& mc : myc)
@@ -719,15 +938,11 @@ int32_t mb_matmul_blocked_dist(mb_comm* c, mb_block* const* A_tiles, const int32
         t.blk.dtype = en->dtype; t.blk.device = ctx->device;
         t.blk.offset = (long long)(arena_need / elem_size(en->dtype));      // patched to a pointer once the arena exists
         arena_need += up256((size_t)t.blk.ld * std::max(1, major) * elem_size(en->dtype));
-        const int extent = is_a ? en->rows : en->cols;                      // A: row bands, B: column bands
-        t.nbands = (fast && extent >= 1024) ? MAX_BANDS : 1;
-        t.band = ((extent + t.nbands - 1) / t.nbands + 127) / 128 * 128;
-        t.nbands = (extent + t.band - 1) / t.band;
+        bands_of(is_a ? en->rows : en->cols, fast ? MAX_BANDS : 1, t.band, t.nbands);
         if (fast) { t.ready_base = flag_slot * MAX_BANDS; ++flag_slot; }
     };
-    for (int t = 0; t < m * k; ++t) if (needA[t]) setup_tile(tA[t], entA[t], A_tiles[t], true, a_owner[t]);
-    for (int t = 0; t < k * n; ++t) if (needB[t]) setup_tile(tB[t], entB[t], B_tiles[t], false, b_owner[t]);
-    if (flag_slot > 2 * mb::G2_MAX_OPS) fast = false;       // cannot happen before the operand limit below trips; kept for safety
+    for (int t = 0; t < m * k; ++t) if (tA[t].need) setup_tile(tA[t], entA[t], A_tiles[t], true, a_owner[t]);
+    for (int t = 0; t < k * n; ++t) if (tB[t].need) setup_tile(tB[t], entB[t], B_tiles[t], false, b_owner[t]);
     // two halves, alternating by epoch: the pulls of this call may land while the previous call's products still read theirs
     const int half = (int)(e & 1);
     const size_t half_need = up256(arena_need);
@@ -760,21 +975,7 @@ int32_t mb_matmul_blocked_dist(mb_comm* c, mb_block* const* A_tiles, const int32
                     if (b >= t.nbands) continue;
                     char* src = nullptr;
                     if ((rc = open_entry(*t.ent, &src)) != MB_OK) return rc;
-                    const ShmEntry* en = t.ent;
-                    const size_t es = elem_size(en->dtype);
-                    const int minor = en->trans ? en->cols : en->rows, major = en->trans ? en->rows : en->cols;
-                    char* dst = static_cast<char*>(t.blk.data);
-                    // bands cut the logical rows (A) / columns (B); in the physical array that is the minor or the major axis
-                    const bool cut_minor = is_a ? !en->trans : (en->trans != 0);
-                    const int lo = b * t.band, hi = std::min((is_a ? en->rows : en->cols), lo + t.band);
-                    if (hi > lo && minor > 0 && major > 0) {
-                        if (cut_minor)
-                            MB_CUDA(cudaMemcpy2DAsync(dst + (size_t)lo * es, (size_t)t.blk.ld * es, src + (size_t)lo * es, (size_t)en->ld * es,
-                                                      (size_t)(hi - lo) * es, major, cudaMemcpyDeviceToDevice, X));
-                        else
-                            MB_CUDA(cudaMemcpy2DAsync(dst + (size_t)lo * t.blk.ld * es, (size_t)t.blk.ld * es, src + (size_t)lo * en->ld * es,
-                                                      (size_t)en->ld * es, (size_t)minor * es, hi - lo, cudaMemcpyDeviceToDevice, X));
-                    }
+                    MB_CUDA(copy_band(t, is_a, b, src, t.ent->ld, cudaMemcpyDeviceToDevice, X));
                     if (t.ready_base >= 0) MB_CUDA(sig(c, c->flags + F_BAND + t.ready_base + b, e, X));
                     if (b == t.nbands - 1) {
                         t.landed = next_event(c);
@@ -795,7 +996,7 @@ int32_t mb_matmul_blocked_dist(mb_comm* c, mb_block* const* A_tiles, const int32
         if (h.size() < 2) continue;
         if (fused_tile(mc.id)) {
             // the owner stores the right half [nh, N) into the partner's slot (if there is one), the partner the left half
-            if (h[0] != rank || col_len[mc.j] > half_cols(mc.id)) writes_to[h[0] == rank ? h[1] : h[0]] = 1;
+            if (h[0] != rank || col_len[mc.j] > half_cols(col_len[mc.j])) writes_to[h[0] == rank ? h[1] : h[0]] = 1;
         } else if (h[0] != rank) writes_to[h[0]] = 1;
     }
     for (int p = 0; p < world; ++p)
@@ -804,147 +1005,9 @@ int32_t mb_matmul_blocked_dist(mb_comm* c, mb_block* const* A_tiles, const int32
     // ---- 3. my block products ----
     std::vector<char> partial_to(world, 0);                  // staged path: owners I have stored a partial for
     std::vector<char> fused_free_to(world, 0);               // fused path: peers whose staged half I have consumed
-    if (fast) {
-        // Two launches of the grouped kernel with the exchange flags between them: L0 computes the halves the peers reduce
-        // (stored into their staging buffers) and the plain regions, L2 the halves reduced here (acc + the peer's staged
-        // partial).  Completion counted inside a kernel whose epilogue stores to peer memory was measured faulty — at 8192^2
-        // about one call in three came back with one 16 x 32 patch off by a single product term — so the kernel boundary is
-        // the completion point and the flags are stream memory operations.  Both launches share one operand table.
-        static thread_local mb::G2Launch L0, L2;
-        L0 = mb::G2Launch();
-        L2 = mb::G2Launch();
-        bool ok = true;
-        auto op_of = [&](Tile& t, bool is_a) {
-            if (t.op >= 0) return t.op;
-            int& cnt = is_a ? L0.na : L0.nb;
-            if (cnt >= mb::G2_MAX_OPS) { ok = false; return 0; }
-            mb::G2Operand& o = (is_a ? L0.A : L0.B)[cnt];
-            o.ptr = f64_ptr(&t.blk); o.ld = t.blk.ld; o.rows = t.blk.rows; o.cols = t.blk.cols;
-            o.band = t.remote ? t.band : 0;
-            o.ready_base = t.remote ? t.ready_base : -1;
-            return t.op = cnt++;
-        };
-        // entries: regions that peers wait for first, plain regions next, regions that wait for a peer last
-        struct Reg { int id, n_off, N; int phase; };          // phase 0 = peer's half (store remote), 1 = plain, 2 = my half (needs the peer's)
-        std::vector<Reg> regs;
-        for (const MyC& mc : myc) {
-            const int N_ = col_len[mc.j];
-            if (fused_tile(mc.id)) {
-                const int nh = half_cols(mc.id);
-                const bool owner = plan.holders[mc.id][0] == rank;
-                // the owner reduces the left half [0, nh), the partner the right half [nh, N)
-                if (owner) { if (N_ > nh) regs.push_back({mc.id, nh, N_ - nh, 0}); regs.push_back({mc.id, 0, nh, 2}); }
-                else { regs.push_back({mc.id, 0, nh, 0}); if (N_ > nh) regs.push_back({mc.id, nh, N_ - nh, 2}); }
-            } else {
-                regs.push_back({mc.id, 0, N_, 1});
-            }
-        }
-        std::stable_sort(regs.begin(), regs.end(), [](const Reg& a, const Reg& b) { return a.phase < b.phase; });
-        if ((int)regs.size() > mb::G2_MAX_ENTRIES) ok = false;
-        struct Note { int peer, slot; };
-        std::vector<Note> wrote, need, final_to;              // F_PART2 to signal / F_PART2 to wait for / F_FINAL2 to signal
-        for (size_t x = 0; x < regs.size() && ok; ++x) {
-            const Reg& rg = regs[x];
-            const int i = rg.id / n, j = rg.id % n;
-            const MyC* mc = nullptr;
-            for (const MyC& q : myc) if (q.id == rg.id) mc = &q;
-            mb::G2Launch& L = rg.phase == 2 ? L2 : L0;
-            mb::G2Entry& en = L.E[L.ne++];
-            en.nseg = (int)mc->kks.size();
-            for (int s = 0; s < en.nseg; ++s) {
-                en.a_op[s] = op_of(tA[i * k + mc->kks[s]], true);
-                en.b_op[s] = op_of(tB[mc->kks[s] * n + j], false);
-            }
-            en.m_off = 0; en.n_off = rg.n_off; en.M = row_len[i]; en.N = rg.N;
-            const auto& h = plan.holders[rg.id];
-            const int ldst = even(row_len[i]);               // leading dimension of a staged partial
-            if (rg.phase == 1) {
-                if (h[0] == rank) {                          // my own tile (other holders, if any, are added in step 4)
-                    en.D = f64_ptr(C_tiles[rg.id]); en.ldd = C_tiles[rg.id]->ld;
-                } else {                                     // staged path: straight into my slot of the owner's staging buffer
-                    en.D = reinterpret_cast<double*>(c->staging_peer[h[0]] + (size_t)rank * c->slot_bytes + slot_off[rg.id]);
-                    en.ldd = ldst;
-                    partial_to[h[0]] = 1;
-                }
-                continue;
-            }
-            const int peer = h[0] == rank ? h[1] : h[0];
-            const int slot = pair_slot[rg.id];
-            if (rg.phase == 0) {
-                // the half the PEER reduces: my partial of it goes over NVLink into my slot of the peer's staging buffer
-                en.D = reinterpret_cast<double*>(c->staging_peer[peer] + (size_t)rank * c->slot_bytes + slot_off[rg.id]);
-                en.ldd = ldst;
-                wrote.push_back({peer, slot});
-            } else {
-                // the half I reduce: acc + the peer's staged partial; the result belongs in the OWNER's C tile
-                en.Cin = reinterpret_cast<const double*>(c->staging + (size_t)peer * c->slot_bytes + slot_off[rg.id]);
-                en.ldcin = ldst;
-                need.push_back({peer, slot});
-                if (h[0] == rank) {
-                    en.D = f64_ptr(C_tiles[rg.id]) + (size_t)rg.n_off * C_tiles[rg.id]->ld; en.ldd = C_tiles[rg.id]->ld;
-                } else {
-                    if (!entC[rg.id]) return fail(MB_ERR_INVALID_ARG, "mb_matmul_blocked_dist: owner did not publish C tile %d", rg.id);
-                    char* cp = nullptr;
-                    if ((rc = open_entry(*entC[rg.id], &cp)) != MB_OK) return rc;
-                    en.D = reinterpret_cast<double*>(cp) + (size_t)rg.n_off * entC[rg.id]->ld; en.ldd = entC[rg.id]->ld;
-                    final_to.push_back({peer, slot});
-                }
-                fused_free_to[peer] = 1;
-            }
-        }
-        if (!ok) {
-            // the plan-wide limits above keep every rank's share within the tables; should one not fit, fail on every
-            // rank alike rather than fall back here and leave the partner waiting for flags
-            return fail(MB_ERR_UNSUPPORTED, "mb_matmul_blocked_dist: grouped launch not possible for this plan (set MARLIN_B200_DIST_SLOW=1)");
-        }
-        L2.na = L0.na; L2.nb = L0.nb;
-        std::copy_n(L0.A, L0.na, L2.A);
-        std::copy_n(L0.B, L0.nb, L2.B);
-        L0.ready = L2.ready = c->flags + F_BAND; L0.ready_val = L2.ready_val = e;
-        L0.status = L2.status = c->flags + F_STATUS; L0.timeout_ns = L2.timeout_ns = timeout_ns(c);
-        int launches = 0;
-        cudaError_t ce = mb::gemm_f64_grouped2(L0, ctx->num_sms, S, &launches);
-        if (ce != cudaSuccess) return cuda_fail(ce, "gemm_f64_grouped2 (first half)");
-        for (const Note& w : wrote) MB_CUDA(sig(c, c->flags_peer[w.peer] + F_PART2 + rank * MAX_PAIR + w.slot, e, S));
-        for (const Note& w : need) MB_CUDA(waitf(c, c->flags + F_PART2 + w.peer * MAX_PAIR + w.slot, e, S));
-        ce = mb::gemm_f64_grouped2(L2, ctx->num_sms, S, &launches);
-        if (ce != cudaSuccess) return cuda_fail(ce, "gemm_f64_grouped2 (second half)");
-        for (const Note& w : final_to) MB_CUDA(sig(c, c->flags_peer[w.peer] + F_FINAL2 + rank * MAX_PAIR + w.slot, e, S));
-        ctx->launches += launches;
-    } else {
-        // ---- general path: per product (or per C tile when all kk are here), tile-level waits, staged partials ----
-        for (const MyC& mc : myc) {
-            const auto& h = plan.holders[mc.id];
-            mb_block out;
-            if (h[0] == rank) { out = *C_tiles[mc.id]; out.owns = 0; }
-            else {
-                out = mb_block();
-                out.data = c->staging_peer[h[0]] + (size_t)rank * c->slot_bytes + slot_off[mc.id];
-                out.rows = row_len[mc.i]; out.cols = col_len[mc.j]; out.ld = even(row_len[mc.i]); out.dtype = out_dtype; out.device = ctx->device;
-                partial_to[h[0]] = 1;
-            }
-            for (int kk : mc.kks) {
-                Tile& a = tA[mc.i * k + kk];
-                Tile& b = tB[kk * n + mc.j];
-                if (a.landed) MB_CUDA(cudaStreamWaitEvent(S, a.landed, 0));
-                if (b.landed) MB_CUDA(cudaStreamWaitEvent(S, b.landed, 0));
-            }
-            if ((int)mc.kks.size() == k) {
-                // every kk of this C tile is here: one launch per tile (bf16: K segments in one wgmma launch; fp64: grouped DMMA)
-                std::vector<mb_block*> at(m * k, nullptr), bt(k * n, nullptr), ct(m * n, nullptr);
-                for (int kk = 0; kk < k; ++kk) { at[mc.i * k + kk] = &tA[mc.i * k + kk].blk; bt[kk * n + mc.j] = &tB[kk * n + mc.j].blk; }
-                ct[mc.id] = &out;
-                const int32_t id = mc.id;
-                if ((rc = mb_matmul_blocked_subset(ctx, at.data(), bt.data(), m, k, n, ct.data(), &id, 1)) != MB_OK) return rc;
-            } else {
-                bool first = true;
-                for (int kk : mc.kks) {
-                    if ((rc = mb_block_gemm(ctx, &tA[mc.i * k + kk].blk, &tB[kk * n + mc.j].blk, &out, first ? 0 : 1)) != MB_OK) return rc;
-                    first = false;
-                }
-            }
-        }
-    }
+    rc = fast ? products_fused(c, e, plan, myc, tA, tB, row_len, col_len, C_tiles, entC, slot_off, pair_slot, partial_to, fused_free_to)
+              : products_general(c, plan, myc, tA, tB, row_len, col_len, out_dtype, C_tiles, slot_off, partial_to);
+    if (rc) return rc;
     MB_CUDA(cudaEventRecord(c->ev_compute, S));
     c->have_compute = true;
     MB_CUDA(cudaEventRecord(c->ev_half[half], S));
@@ -976,18 +1039,15 @@ int32_t mb_matmul_blocked_dist(mb_comm* c, mb_block* const* A_tiles, const int32
     // fused path, owner side: the partner's reduced half has landed in my C tile
     for (const MyC& mc : myc) {
         const auto& h = plan.holders[mc.id];
-        if (fused_tile(mc.id) && h[0] == rank && col_len[mc.j] > half_cols(mc.id))
+        if (fused_tile(mc.id) && h[0] == rank && col_len[mc.j] > half_cols(col_len[mc.j]))
             MB_CUDA(waitf(c, c->flags + F_FINAL2 + h[1] * MAX_PAIR + pair_slot[mc.id], e, S));
     }
 
     // ---- 5. my tiles may not be overwritten / freed until everyone has finished pulling them ----
-    for (int p = 0; p < world; ++p)
-        if (consumer[p]) MB_CUDA(waitf(c, flag_ch(c, rank, CH_DONE, p), e, S));
+    if ((rc = wait_consumers(c, consumer, e, S)) != MB_OK) return rc;
     // surface a timed-out wait of an EARLIER call (this call's status is read by the next one / mb_comm_check)
-    if (*c->status_host != 0)
-        return fail(MB_ERR_TIMEOUT, "mb_matmul_blocked_dist: a device-side wait for a peer timed out in an earlier call");
-    MB_CUDA(cudaMemcpyAsync(c->status_host, c->flags + F_STATUS, 8, cudaMemcpyDeviceToHost, S));
-    (void)esz;
+    if ((rc = check_status(c, "mb_matmul_blocked_dist")) != MB_OK) return rc;
+    MB_CUDA(read_status(c, S));
     return MB_OK;
 }
 
@@ -1084,22 +1144,17 @@ int32_t mb_host_free_shared(const char* name, void* ptr, int64_t bytes, int32_t 
 int32_t mb_matmul_blocked_dist_host(mb_comm* c, const double* const* A_host, const int32_t* a_home, const double* const* B_host,
                                     const int32_t* b_home, int32_t m, int32_t k, int32_t n, const int32_t* row_len,
                                     const int32_t* k_len, const int32_t* col_len, double* const* C_host) {
-    if (!c) return fail(MB_ERR_INVALID_ARG, "null communicator");
+    int32_t rc = check_call(c, "mb_matmul_blocked_dist_host", A_host && B_host && C_host && a_home && b_home && row_len && k_len && col_len &&
+                                                              m > 0 && k > 0 && n > 0);
+    if (rc) return rc;
     mb_ctx* ctx = c->ctx;
-    MB_CTX(ctx);
     MB_LOCK(ctx);
-    if (!A_host || !B_host || !C_host || !a_home || !b_home || !row_len || !k_len || !col_len || m <= 0 || k <= 0 || n <= 0)
-        return fail(MB_ERR_INVALID_ARG, "mb_matmul_blocked_dist_host: bad argument");
-    if (c->aborted) return fail(MB_ERR_TIMEOUT, "mb_comm: the communicator was aborted after a peer stopped answering");
     const int rank = c->rank, world = c->world;
     if (k > mb::G2_MAX_SEG) return fail(MB_ERR_UNSUPPORTED, "mb_matmul_blocked_dist_host: k = %d > %d", k, mb::G2_MAX_SEG);
     for (int i = 0; i < m; ++i) if (row_len[i] <= 0) return fail(MB_ERR_UNSUPPORTED, "mb_matmul_blocked_dist_host: empty block row");
     for (int kk = 0; kk < k; ++kk) if (k_len[kk] <= 0) return fail(MB_ERR_UNSUPPORTED, "mb_matmul_blocked_dist_host: empty k segment");
     for (int j = 0; j < n; ++j) if (col_len[j] <= 0) return fail(MB_ERR_UNSUPPORTED, "mb_matmul_blocked_dist_host: empty block column");
-    if (!ctx->h2d_stream) {
-        MB_CUDA(cudaStreamCreateWithFlags(&ctx->h2d_stream, cudaStreamNonBlocking));
-        MB_CUDA(cudaStreamCreateWithFlags(&ctx->d2h_stream, cudaStreamNonBlocking));
-    }
+    MB_CUDA(ensure_copy_streams(ctx));
     cudaStream_t S = ctx->stream, X = c->X, U = ctx->h2d_stream, R = c->R;
     const Plan plan = make_plan(m, k, n, world);
     // ---- global feasibility (the same verdict on every rank) ----
@@ -1108,77 +1163,54 @@ int32_t mb_matmul_blocked_dist_host(mb_comm* c, const double* const* A_host, con
     for (int t = 0; t < k * n; ++t) { if (b_home[t] < 0 || b_home[t] >= world) return fail(MB_ERR_INVALID_ARG, "bad b_home"); ++ups[b_home[t]]; }
     for (int r = 0; r < world; ++r) if (ups[r] > UP_SLOTS) return fail(MB_ERR_UNSUPPORTED, "mb_matmul_blocked_dist_host: rank %d would upload %d tiles (limit %d)", r, ups[r], UP_SLOTS);
     for (int id = 0; id < m * n; ++id) if (plan.holders[id].size() > 2) return fail(MB_ERR_UNSUPPORTED, "mb_matmul_blocked_dist_host: C tile %d has %d holders (limit 2)", id, (int)plan.holders[id].size());
-    auto bands_of = [](int extent, int& band, int& nb) {
-        nb = extent >= 1024 ? MAX_BANDS : 1;
-        band = ((extent + nb - 1) / nb + 127) / 128 * 128;
-        nb = (extent + band - 1) / band;
-    };
+    // one grouped launch per rank: one entry per sub-block
     for (int r = 0; r < world; ++r) {
-        std::vector<char> ua(m * k, 0), ub(k * n, 0);
-        int na = 0, nb = 0, subs = 0;
+        const std::vector<MyC> cs = plan.c_tiles_of(r);
+        int subs = 0;
         std::map<int, int> pair_subs;
-        for (int i = 0; i < m; ++i)
-            for (int j = 0; j < n; ++j) {
-                bool mine_ = false;
-                for (int kk = 0; kk < k; ++kk)
-                    if (plan.prod_rank[i * n * k + j * k + kk] == r) {
-                        mine_ = true;
-                        if (!ua[i * k + kk]) { ua[i * k + kk] = 1; ++na; }
-                        if (!ub[kk * n + j]) { ub[kk * n + j] = 1; ++nb; }
-                    }
-                if (mine_) {
-                    int ba, nba, bb, nbb;
-                    bands_of(row_len[i], ba, nba); bands_of(col_len[j], bb, nbb);
-                    subs += nba * nbb;
-                    const auto& h = plan.holders[i * n + j];
-                    if (h.size() == 2) pair_subs[h[0] == r ? h[1] : h[0]] += nba * nbb;
-                }
-            }
-        if (na > mb::G2_MAX_OPS || nb > mb::G2_MAX_OPS || subs > mb::G2_MAX_ENTRIES)
+        for (const MyC& mc : cs) {
+            int ba, nba, bb, nbb;
+            bands_of(row_len[mc.i], MAX_BANDS, ba, nba); bands_of(col_len[mc.j], MAX_BANDS, bb, nbb);
+            subs += nba * nbb;
+            const auto& h = plan.holders[mc.id];
+            if (h.size() == 2) pair_subs[h[0] == r ? h[1] : h[0]] += nba * nbb;
+        }
+        if (!operands_fit(plan, cs) || subs > mb::G2_MAX_ENTRIES)
             return fail(MB_ERR_UNSUPPORTED, "mb_matmul_blocked_dist_host: rank %d's share (%d sub-blocks) does not fit one grouped launch", r, subs);
         for (auto& kv : pair_subs) if (kv.second > SUB_SLOTS) return fail(MB_ERR_UNSUPPORTED, "mb_matmul_blocked_dist_host: too many shared sub-blocks");
     }
     // ---- local checks ----
     for (int t = 0; t < m * k; ++t) if (a_home[t] == rank && !A_host[t]) return fail(MB_ERR_INVALID_ARG, "mb_matmul_blocked_dist_host: A tile %d is homed here but NULL", t);
     for (int t = 0; t < k * n; ++t) if (b_home[t] == rank && !B_host[t]) return fail(MB_ERR_INVALID_ARG, "mb_matmul_blocked_dist_host: B tile %d is homed here but NULL", t);
-    struct MyC { int id, i, j; std::vector<int> kks; };
-    std::vector<MyC> myc;
-    for (int i = 0; i < m; ++i)
-        for (int j = 0; j < n; ++j) {
-            MyC mc{i * n + j, i, j, {}};
-            for (int kk = 0; kk < k; ++kk) if (plan.prod_rank[i * n * k + j * k + kk] == rank) mc.kks.push_back(kk);
-            if (!mc.kks.empty()) {
-                if (!C_host[mc.id]) return fail(MB_ERR_INVALID_ARG, "mb_matmul_blocked_dist_host: C tile %d is computed here but NULL", mc.id);
-                myc.push_back(mc);
-            }
-        }
+    const std::vector<MyC> myc = plan.c_tiles_of(rank);
+    for (const MyC& mc : myc)
+        if (!C_host[mc.id]) return fail(MB_ERR_INVALID_ARG, "mb_matmul_blocked_dist_host: C tile %d is computed here but NULL", mc.id);
     const unsigned long long e = ++c->epoch;
     c->events_used = 0;
-    int32_t rc = MB_OK;
 
     // ---- device layout in the arena: tiles I upload, tiles I pull, my C tiles ----
-    struct HTile { size_t off = 0; int rows = 0, cols = 0, ld = 0, home = -1, band = 0, nbands = 1, slot = -1, ready_base = -1, op = -1; bool need = false; char* peer = nullptr; };
-    std::vector<HTile> tA(m * k), tB(k * n);
+    std::vector<Tile> tA(m * k), tB(k * n);
+    for (const MyC& mc : myc)
+        for (int kk : mc.kks) { tA[mc.i * k + kk].need = true; tB[kk * n + mc.j].need = true; }
     size_t total = 0;
     int nflag = 0;
     std::vector<int> slot_ctr(world, 0);
-    for (int t = 0; t < m * k; ++t) { tA[t].rows = row_len[t / k]; tA[t].cols = k_len[t % k]; tA[t].home = a_home[t]; tA[t].slot = slot_ctr[a_home[t]]++; }
-    for (int t = 0; t < k * n; ++t) { tB[t].rows = k_len[t / n]; tB[t].cols = col_len[t % n]; tB[t].home = b_home[t]; tB[t].slot = slot_ctr[b_home[t]]++; }
-    for (const MyC& mc : myc)
-        for (int kk : mc.kks) { tA[mc.i * k + kk].need = true; tB[kk * n + mc.j].need = true; }
-    auto place = [&](HTile& t, bool is_a) {
-        t.ld = std::max(2, even(t.rows));
-        bands_of(is_a ? t.rows : t.cols, t.band, t.nbands);
-        if (t.home == rank || t.need) { t.off = total; total += up256((size_t)t.ld * t.cols * 8); }
+    auto place = [&](Tile& t, int rows, int cols, int home, bool is_a) {
+        t.blk.rows = rows; t.blk.cols = cols; t.blk.ld = std::max(2, even(rows)); t.blk.dtype = MB_F64;
+        t.src = home; t.up_slot = slot_ctr[home]++;
+        bands_of(is_a ? rows : cols, MAX_BANDS, t.band, t.nbands);
+        if (home == rank || t.need) { t.blk.offset = (long long)(total / 8); total += up256((size_t)t.blk.ld * cols * 8); }
         if (t.need) { t.ready_base = nflag * MAX_BANDS; ++nflag; }
     };
-    for (auto& t : tA) place(t, true);
-    for (auto& t : tB) place(t, false);
+    for (int t = 0; t < m * k; ++t) place(tA[t], row_len[t / k], k_len[t % k], a_home[t], true);
+    for (int t = 0; t < k * n; ++t) place(tB[t], k_len[t / n], col_len[t % n], b_home[t], false);
     std::vector<size_t> coff(m * n, 0);
     for (const MyC& mc : myc) { coff[mc.id] = total; total += up256((size_t)even(row_len[mc.i]) * col_len[mc.j] * 8); }
     // The arena may be regrown (device sync inside): peers cannot still be pulling from the old one, because every call
     // orders the DONE flags of its consumers on S before it ends.
     if ((rc = ensure_arena(c, total)) != MB_OK) return rc;
+    for (Tile& t : tA) t.blk.data = c->arena;          // the tiles' offsets are arena offsets
+    for (Tile& t : tB) t.blk.data = c->arena;
 
     // ---- staging: the partner's partial of a whole tile footprint per shared C tile ----
     std::vector<size_t> slot_off(m * n, 0);
@@ -1194,7 +1226,7 @@ int32_t mb_matmul_blocked_dist_host(mb_comm* c, const double* const* A_host, con
             slot_off[id] = used[key];
             used[key] += up256((size_t)even(row_len[id / n]) * col_len[id % n] * 8);
             int ba, nba, bb, nbb;
-            bands_of(row_len[id / n], ba, nba); bands_of(col_len[id % n], bb, nbb);
+            bands_of(row_len[id / n], MAX_BANDS, ba, nba); bands_of(col_len[id % n], MAX_BANDS, bb, nbb);
             pair_base[id] = subs[key];
             subs[key] += nba * nbb;
         }
@@ -1204,33 +1236,17 @@ int32_t mb_matmul_blocked_dist_host(mb_comm* c, const double* const* A_host, con
 
     // ---- publish my upload buffers, read everybody's ----
     std::vector<ShmEntry> mine;
-    auto pub = [&](const HTile& t, int kind, int idx) {
-        mb_block b;
-        b.data = c->arena + t.off; b.rows = t.rows; b.cols = t.cols; b.ld = t.ld; b.dtype = MB_F64;
-        ShmEntry en;
-        int32_t r = export_block(&b, kind, idx, &en);
-        if (r == MB_OK) mine.push_back(en);
-        return r;
-    };
-    for (int t = 0; t < m * k; ++t) if (tA[t].home == rank && (rc = pub(tA[t], 0, t)) != MB_OK) return rc;
-    for (int t = 0; t < k * n; ++t) if (tB[t].home == rank && (rc = pub(tB[t], 1, t)) != MB_OK) return rc;
-    if ((rc = publish(c, e, mine)) != MB_OK) return rc;
+    for (int t = 0; t < m * k; ++t)
+        if (tA[t].src == rank) { ShmEntry en; if ((rc = export_block(&tA[t].blk, 0, t, &en)) != MB_OK) return rc; mine.push_back(en); }
+    for (int t = 0; t < k * n; ++t)
+        if (tB[t].src == rank) { ShmEntry en; if ((rc = export_block(&tB[t].blk, 1, t, &en)) != MB_OK) return rc; mine.push_back(en); }
     std::vector<std::vector<ShmEntry>> dir;
-    if ((rc = read_all(c, e, dir)) != MB_OK) return rc;
-    for (int attempt = 0; attempt < 3; ++attempt) {
-        const unsigned long long gen = mb::ipc_evictions();
-        for (int p = 0; p < world; ++p) {
-            if (p == rank) continue;
-            for (const ShmEntry& en : dir[p]) {
-                HTile* t = en.kind == 0 ? (en.idx >= 0 && en.idx < m * k ? &tA[en.idx] : nullptr) : (en.kind == 1 && en.idx >= 0 && en.idx < k * n ? &tB[en.idx] : nullptr);
-                if (!t || !t->need || t->home != p) continue;
-                if ((rc = open_entry(en, &t->peer)) != MB_OK) return rc;
-            }
-        }
-        if (mb::ipc_evictions() == gen) break;
-    }
-    for (auto& t : tA) if (t.need && t.home != rank && !t.peer) return fail(MB_ERR_INVALID_ARG, "mb_matmul_blocked_dist_host: a peer did not publish an A tile");
-    for (auto& t : tB) if (t.need && t.home != rank && !t.peer) return fail(MB_ERR_INVALID_ARG, "mb_matmul_blocked_dist_host: a peer did not publish a B tile");
+    if ((rc = exchange_directory(c, e, mine, dir)) != MB_OK) return rc;
+    const std::vector<const ShmEntry*> entA = entries_of(dir, 0, m * k, a_home), entB = entries_of(dir, 1, k * n, b_home);
+    for (int t = 0; t < m * k; ++t)
+        if (tA[t].need && tA[t].src != rank && !(tA[t].ent = entA[t])) return fail(MB_ERR_INVALID_ARG, "mb_matmul_blocked_dist_host: a peer did not publish an A tile");
+    for (int t = 0; t < k * n; ++t)
+        if (tB[t].need && tB[t].src != rank && !(tB[t].ent = entB[t])) return fail(MB_ERR_INVALID_ARG, "mb_matmul_blocked_dist_host: a peer did not publish a B tile");
 
     // everything of the previous call that touches the arena / my uploads is ordered on S: fan that out
     MB_CUDA(cudaEventRecord(c->ev_tmp, S));
@@ -1253,20 +1269,13 @@ int32_t mb_matmul_blocked_dist_host(mb_comm* c, const double* const* A_host, con
         for (int pass = 0; pass < 2; ++pass) {
             const int cnt = pass == 0 ? m * k : k * n;
             for (int t = 0; t < cnt; ++t) {
-                HTile& ht = pass == 0 ? tA[t] : tB[t];
-                if (ht.home != rank || b >= ht.nbands) continue;
+                Tile& ht = pass == 0 ? tA[t] : tB[t];
+                if (ht.src != rank || b >= ht.nbands) continue;
                 const double* src = pass == 0 ? A_host[t] : B_host[t];
-                char* dst = c->arena + ht.off;
-                const int lo = b * ht.band, hi = std::min(pass == 0 ? ht.rows : ht.cols, lo + ht.band);
-                if (pass == 0)      // A: row band [lo, hi) of every column
-                    MB_CUDA(cudaMemcpy2DAsync(dst + (size_t)lo * 8, (size_t)ht.ld * 8, src + lo, (size_t)ht.rows * 8, (size_t)(hi - lo) * 8, ht.cols,
-                                              cudaMemcpyHostToDevice, U));
-                else                // B: column band [lo, hi)
-                    MB_CUDA(cudaMemcpy2DAsync(dst + (size_t)lo * ht.ld * 8, (size_t)ht.ld * 8, src + (size_t)lo * ht.rows, (size_t)ht.rows * 8,
-                                              (size_t)ht.rows * 8, hi - lo, cudaMemcpyHostToDevice, U));
+                MB_CUDA(copy_band(ht, pass == 0, b, reinterpret_cast<const char*>(src), ht.blk.rows, cudaMemcpyHostToDevice, U));
                 if (ht.need) MB_CUDA(sig(c, c->flags + F_BAND + ht.ready_base + b, e, U));
                 for (int r : (pass == 0 ? consumers_a[t] : consumers_b[t])) {
-                    MB_CUDA(sig(c, c->flags_peer[r] + F_UPREADY + (rank * UP_SLOTS + ht.slot) * MAX_BANDS + b, e, U));
+                    MB_CUDA(sig(c, c->flags_peer[r] + F_UPREADY + (rank * UP_SLOTS + ht.up_slot) * MAX_BANDS + b, e, U));
                     consumer[r] = 1;
                 }
             }
@@ -1277,18 +1286,18 @@ int32_t mb_matmul_blocked_dist_host(mb_comm* c, const double* const* A_host, con
         for (int pass = 0; pass < 2; ++pass) {
             const int cnt = pass == 0 ? m * k : k * n;
             for (int t = 0; t < cnt; ++t) {
-                HTile& ht = pass == 0 ? tA[t] : tB[t];
-                if (!ht.need || ht.home == rank || b >= ht.nbands) continue;
-                source[ht.home] = 1;
-                MB_CUDA(waitf(c, c->flags + F_UPREADY + (ht.home * UP_SLOTS + ht.slot) * MAX_BANDS + b, e, X));
-                char* dst = c->arena + ht.off;
-                const int lo = b * ht.band, hi = std::min(pass == 0 ? ht.rows : ht.cols, lo + ht.band);
-                if (pass == 0)
-                    MB_CUDA(cudaMemcpy2DAsync(dst + (size_t)lo * 8, (size_t)ht.ld * 8, ht.peer + (size_t)lo * 8, (size_t)ht.ld * 8, (size_t)(hi - lo) * 8,
-                                              ht.cols, cudaMemcpyDeviceToDevice, X));
-                else
-                    MB_CUDA(cudaMemcpyAsync(dst + (size_t)lo * ht.ld * 8, ht.peer + (size_t)lo * ht.ld * 8, (size_t)(hi - lo) * ht.ld * 8,
-                                            cudaMemcpyDeviceToDevice, X));
+                Tile& ht = pass == 0 ? tA[t] : tB[t];
+                if (!ht.need || ht.src == rank || b >= ht.nbands) continue;
+                source[ht.src] = 1;
+                MB_CUDA(waitf(c, c->flags + F_UPREADY + (ht.src * UP_SLOTS + ht.up_slot) * MAX_BANDS + b, e, X));
+                char* peer = nullptr;
+                if ((rc = open_entry(*ht.ent, &peer)) != MB_OK) return rc;
+                if (pass == 0) {
+                    MB_CUDA(copy_band(ht, true, b, peer, ht.blk.ld, cudaMemcpyDeviceToDevice, X));
+                } else {            // a column band of the uploader's packed copy is one contiguous range
+                    const size_t lo = (size_t)b * ht.band, hi = std::min((size_t)ht.blk.cols, lo + ht.band), ld = ht.blk.ld;
+                    MB_CUDA(cudaMemcpyAsync(elem_ptr(&ht.blk) + lo * ld * 8, peer + lo * ld * 8, (hi - lo) * ld * 8, cudaMemcpyDeviceToDevice, X));
+                }
                 MB_CUDA(sig(c, c->flags + F_BAND + ht.ready_base + b, e, X));
             }
         }
@@ -1306,26 +1315,18 @@ int32_t mb_matmul_blocked_dist_host(mb_comm* c, const double* const* A_host, con
     // it must have consumed what I pushed there last time
     for (int p = 0; p < world; ++p)
         if (writes_to[p] && c->last_write_epoch[p]) MB_CUDA(waitf(c, flag_ch(c, rank, CH_FREE, p), c->last_write_epoch[p], R));
-    static thread_local mb::G2Launch L;
+    mb::G2Launch& L = launch_tables[0];
     L = mb::G2Launch();
-    auto op_of = [&](HTile& t, bool is_a) {
-        if (t.op >= 0) return t.op;
-        int& cnt = is_a ? L.na : L.nb;
-        mb::G2Operand& o = (is_a ? L.A : L.B)[cnt];
-        o.ptr = reinterpret_cast<const double*>(c->arena + t.off); o.ld = t.ld; o.rows = t.rows; o.cols = t.cols;
-        o.band = t.band; o.ready_base = t.ready_base;
-        return t.op = cnt++;
-    };
-    struct Sub { int id, p, q, m_off, n_off, M, N, wave, sub_idx; bool mine; int entry; };
+    struct Sub { const MyC* mc; int p, q, m_off, n_off, M, N, wave, sub_idx; bool mine; int entry; };
     std::vector<Sub> subs;
     for (const MyC& mc : myc) {
         int ba, nba, bb, nbb;
-        bands_of(row_len[mc.i], ba, nba); bands_of(col_len[mc.j], bb, nbb);
+        bands_of(row_len[mc.i], MAX_BANDS, ba, nba); bands_of(col_len[mc.j], MAX_BANDS, bb, nbb);
         const auto& h = plan.holders[mc.id];
         const int my_pos = h[0] == rank ? 0 : 1;
         for (int p = 0; p < nba; ++p)
             for (int q = 0; q < nbb; ++q) {
-                Sub sb{mc.id, p, q, p * ba, q * bb, std::min(ba, row_len[mc.i] - p * ba), std::min(bb, col_len[mc.j] - q * bb), std::max(p, q),
+                Sub sb{&mc, p, q, p * ba, q * bb, std::min(ba, row_len[mc.i] - p * ba), std::min(bb, col_len[mc.j] - q * bb), std::max(p, q),
                        pair_base[mc.id] + p * nbb + q, true, -1};
                 if (h.size() == 2) sb.mine = ((p + q) % 2) == my_pos;        // checkerboard: both links carry half of the tile
                 subs.push_back(sb);
@@ -1337,32 +1338,30 @@ int32_t mb_matmul_blocked_dist_host(mb_comm* c, const double* const* A_host, con
     std::stable_sort(subs.begin(), subs.end(), [](const Sub& a, const Sub& b) {
         if (a.wave != b.wave) return a.wave < b.wave;
         if (a.mine != b.mine) return !a.mine;
-        return a.id != b.id ? a.id < b.id : (a.p != b.p ? a.p < b.p : a.q < b.q);
+        return a.mc->id != b.mc->id ? a.mc->id < b.mc->id : (a.p != b.p ? a.p < b.p : a.q < b.q);
     });
     for (Sub& sb : subs) {
-        const int i = sb.id / n, j = sb.id % n;
-        const MyC* mc = nullptr;
-        for (const MyC& qq : myc) if (qq.id == sb.id) mc = &qq;
+        const MyC& mc = *sb.mc;
         sb.entry = L.ne;
         mb::G2Entry& en = L.E[L.ne++];
-        en.nseg = (int)mc->kks.size();
+        en.nseg = (int)mc.kks.size();
         for (int sg = 0; sg < en.nseg; ++sg) {
-            en.a_op[sg] = op_of(tA[i * k + mc->kks[sg]], true);
-            en.b_op[sg] = op_of(tB[mc->kks[sg] * n + j], false);
+            en.a_op[sg] = op_of(L, tA[mc.i * k + mc.kks[sg]], true);
+            en.b_op[sg] = op_of(L, tB[mc.kks[sg] * n + mc.j], false);
         }
         en.m_off = sb.m_off; en.n_off = sb.n_off; en.M = sb.M; en.N = sb.N;
-        const int ldc = even(row_len[i]);
+        const int ldc = even(row_len[mc.i]);
         en.done_ctr = c->flags + F_CTR + sb.entry;
         en.sig_val = e;
-        const auto& h = plan.holders[sb.id];
+        const auto& h = plan.holders[mc.id];
         if (sb.mine) {
-            en.D = reinterpret_cast<double*>(c->arena + coff[sb.id]) + (size_t)sb.n_off * ldc + sb.m_off; en.ldd = ldc;
+            en.D = reinterpret_cast<double*>(c->arena + coff[mc.id]) + (size_t)sb.n_off * ldc + sb.m_off; en.ldd = ldc;
             en.sig_local = c->flags + F_SIG + sb.entry;
             if (h.size() == 2) {
                 // reduce in the epilogue: my partial + the peer's staged partial (no separate add kernel: a kernel launched
                 // while this GEMM is resident might not be scheduled before it ends)
                 const int peer = h[0] == rank ? h[1] : h[0];
-                en.Cin = reinterpret_cast<const double*>(c->staging + (size_t)peer * c->slot_bytes + slot_off[sb.id]) + (size_t)sb.n_off * ldc + sb.m_off;
+                en.Cin = reinterpret_cast<const double*>(c->staging + (size_t)peer * c->slot_bytes + slot_off[mc.id]) + (size_t)sb.n_off * ldc + sb.m_off;
                 en.ldcin = ldc;
                 en.cin_flag = c->flags + F_SUBDONE + peer * SUB_SLOTS + sb.sub_idx;
                 en.cin_val = e;
@@ -1371,7 +1370,7 @@ int32_t mb_matmul_blocked_dist_host(mb_comm* c, const double* const* A_host, con
             // a sub-block the PEER reduces: my partial goes to the same place in my own C buffer (local stores: completion
             // counting next to peer stores proved unreliable, see mb_matmul_blocked_dist) and is pushed from there by the
             // copy engine once the entry's completion flag is up
-            en.D = reinterpret_cast<double*>(c->arena + coff[sb.id]) + (size_t)sb.n_off * ldc + sb.m_off; en.ldd = ldc;
+            en.D = reinterpret_cast<double*>(c->arena + coff[mc.id]) + (size_t)sb.n_off * ldc + sb.m_off; en.ldd = ldc;
             en.sig_local = c->flags + F_SIG + sb.entry;
         }
     }
@@ -1390,17 +1389,17 @@ int32_t mb_matmul_blocked_dist_host(mb_comm* c, const double* const* A_host, con
     // ---- copy-out stream, in entry order: a finished sub-block is either mine (already reduced in the epilogue) -> host,
     //      or the peer's -> pushed into its staging buffer over NVLink + its flag; all hidden behind the rest of the GEMM ----
     for (const Sub& sb : subs) {
-        const int i = sb.id / n;
+        const int id = sb.mc->id, i = sb.mc->i;
         const int ldc = even(row_len[i]);
         MB_CUDA(waitf(c, c->flags + F_SIG + sb.entry, e, R));
-        const double* src = reinterpret_cast<const double*>(c->arena + coff[sb.id]) + (size_t)sb.n_off * ldc + sb.m_off;
+        const double* src = reinterpret_cast<const double*>(c->arena + coff[id]) + (size_t)sb.n_off * ldc + sb.m_off;
         if (sb.mine) {
-            MB_CUDA(cudaMemcpy2DAsync(C_host[sb.id] + (size_t)sb.n_off * row_len[i] + sb.m_off, (size_t)row_len[i] * 8, src, (size_t)ldc * 8,
+            MB_CUDA(cudaMemcpy2DAsync(C_host[id] + (size_t)sb.n_off * row_len[i] + sb.m_off, (size_t)row_len[i] * 8, src, (size_t)ldc * 8,
                                       (size_t)sb.M * 8, sb.N, cudaMemcpyDeviceToHost, R));
         } else {
-            const auto& h = plan.holders[sb.id];
+            const auto& h = plan.holders[id];
             const int peer = h[0] == rank ? h[1] : h[0];
-            double* dst = reinterpret_cast<double*>(c->staging_peer[peer] + (size_t)rank * c->slot_bytes + slot_off[sb.id]) + (size_t)sb.n_off * ldc + sb.m_off;
+            double* dst = reinterpret_cast<double*>(c->staging_peer[peer] + (size_t)rank * c->slot_bytes + slot_off[id]) + (size_t)sb.n_off * ldc + sb.m_off;
             MB_CUDA(cudaMemcpy2DAsync(dst, (size_t)ldc * 8, src, (size_t)ldc * 8, (size_t)sb.M * 8, sb.N, cudaMemcpyDeviceToDevice, R));
             MB_CUDA(sig(c, c->flags_peer[peer] + F_SUBDONE + rank * SUB_SLOTS + sb.sub_idx, e, R));
         }
@@ -1409,18 +1408,15 @@ int32_t mb_matmul_blocked_dist_host(mb_comm* c, const double* const* A_host, con
     for (int p = 0; p < world; ++p)
         if (reads_from[p]) MB_CUDA(sig(c, flag_ch(c, p, CH_FREE, rank), e, S));
     // ---- my upload buffers may not be overwritten until everyone has pulled them; S is ordered behind R ----
-    for (int p = 0; p < world; ++p)
-        if (consumer[p]) MB_CUDA(waitf(c, flag_ch(c, rank, CH_DONE, p), e, S));
+    if ((rc = wait_consumers(c, consumer, e, S)) != MB_OK) return rc;
     MB_CUDA(cudaEventRecord(c->ev_tmp, R));
     MB_CUDA(cudaStreamWaitEvent(S, c->ev_tmp, 0));
     MB_CUDA(cudaEventRecord(c->ev_tmp, U));
     MB_CUDA(cudaStreamWaitEvent(S, c->ev_tmp, 0));
-    MB_CUDA(cudaMemcpyAsync(c->status_host, c->flags + F_STATUS, 8, cudaMemcpyDeviceToHost, S));
+    MB_CUDA(read_status(c, S));
     if ((rc = sync_bounded(c, R, "mb_matmul_blocked_dist_host")) != MB_OK) return rc;
     if ((rc = sync_bounded(c, S, "mb_matmul_blocked_dist_host")) != MB_OK) return rc;
-    if (*c->status_host != 0)
-        return fail(MB_ERR_TIMEOUT, "mb_matmul_blocked_dist_host: a device-side wait for a peer timed out (status 0x%llx: a rank died or fell out of step)", *c->status_host);
-    return MB_OK;
+    return check_status(c, "mb_matmul_blocked_dist_host");
 }
 
 }  // extern "C"

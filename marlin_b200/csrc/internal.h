@@ -120,3 +120,10 @@ inline int32_t check_ctx(mb_ctx* ctx) {
     } while (0)
 #define MB_LOCK(ctx) std::lock_guard<std::recursive_mutex> _mb_lock((ctx)->mu)
 
+// The copy streams of the host pipelines, created on first use.
+inline cudaError_t ensure_copy_streams(mb_ctx* ctx) {
+    if (ctx->h2d_stream) return cudaSuccess;
+    cudaError_t e = cudaStreamCreateWithFlags(&ctx->h2d_stream, cudaStreamNonBlocking);
+    return e == cudaSuccess ? cudaStreamCreateWithFlags(&ctx->d2h_stream, cudaStreamNonBlocking) : e;
+}
+
