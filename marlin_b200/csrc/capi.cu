@@ -43,6 +43,19 @@ int32_t same_shape(const mb_block* a, const mb_block* b, const char* what) {
     return MB_OK;
 }
 
+// The transpose of a block: a non-owning view of the same storage.
+mb_block transposed(const mb_block& b) {
+    mb_block t = b;
+    t.owns = 0;
+    std::swap(t.rows, t.cols);
+    t.is_transpose = !b.is_transpose;
+    return t;
+}
+
+// Element-wise kernels iterate in the output's storage order so the store side is contiguous: with a transposed output
+// every operand is walked through its transpose.
+mb_block in_out_order(const mb_block* b, const mb_block* out) { return out->is_transpose ? transposed(*b) : *b; }
+
 int32_t binary_op(mb_ctx* ctx, int op, const mb_block* A, const mb_block* B, mb_block* out, const char* name) {
     MB_CTX(ctx);
     if (!A || !B || !out) return fail(MB_ERR_INVALID_ARG, "%s: null block", name);
@@ -53,21 +66,16 @@ int32_t binary_op(mb_ctx* ctx, int op, const mb_block* A, const mb_block* B, mb_
     const bool all_f32 = A->dtype == MB_F32 && B->dtype == MB_F32 && out->dtype == MB_F32;
     if (!all_f32 && (A->dtype != MB_F64 || B->dtype != MB_F64 || out->dtype != MB_F64))
         return fail(MB_ERR_UNSUPPORTED, "%s: fp64 (or all-fp32) blocks only (convert bf16 blocks with mb_block_copy)", name);
-    // iterate in the output's storage order so the store side is contiguous
-    int rows = A->rows, cols = A->cols;
-    long long ars = rs(A), acs = cs(A), brs = rs(B), bcs = cs(B), ors = rs(out), ocs = cs(out);
-    if (out->is_transpose) {
-        std::swap(rows, cols);
-        std::swap(ars, acs); std::swap(brs, bcs); std::swap(ors, ocs);
-    }
+    const mb_block a = in_out_order(A, out), b = in_out_order(B, out), o = in_out_order(out, out);
     if (all_f32) {
-        MB_CUDA(mb::ew_binary_f32(op, rows, cols, reinterpret_cast<const float*>(elem_ptr(A)), ars, acs,
-                                  reinterpret_cast<const float*>(elem_ptr(B)), brs, bcs, reinterpret_cast<float*>(elem_ptr(out)), ors,
-                                  ocs, ctx->stream));
+        MB_CUDA(mb::ew_binary_f32(op, a.rows, a.cols, reinterpret_cast<const float*>(elem_ptr(&a)), rs(&a), cs(&a),
+                                  reinterpret_cast<const float*>(elem_ptr(&b)), rs(&b), cs(&b), reinterpret_cast<float*>(elem_ptr(&o)),
+                                  rs(&o), cs(&o), ctx->stream));
         ctx->launches++;
         return MB_OK;
     }
-    MB_CUDA(mb::ew_binary(op, rows, cols, f64_ptr(A), ars, acs, f64_ptr(B), brs, bcs, f64_ptr(out), ors, ocs, ctx->stream));
+    MB_CUDA(mb::ew_binary(op, a.rows, a.cols, f64_ptr(&a), rs(&a), cs(&a), f64_ptr(&b), rs(&b), cs(&b), f64_ptr(&o), rs(&o), cs(&o),
+                          ctx->stream));
     ctx->launches++;
     return MB_OK;
 }
@@ -79,25 +87,17 @@ int32_t unary_op(mb_ctx* ctx, int op, const mb_block* A, mb_block* out, double a
     if (r) return r;
     if (A->dtype != MB_F64 || out->dtype != MB_F64)
         return fail(MB_ERR_UNSUPPORTED, "%s: fp64 blocks only", name);
-    int rows = A->rows, cols = A->cols;
-    long long ars = rs(A), acs = cs(A), ors = rs(out), ocs = cs(out);
-    if (out->is_transpose) {
-        std::swap(rows, cols);
-        std::swap(ars, acs); std::swap(ors, ocs);
-    }
-    MB_CUDA(mb::ew_unary(op, rows, cols, f64_ptr(A), ars, acs, f64_ptr(out), ors, ocs, alpha, beta, ctx->stream));
+    const mb_block a = in_out_order(A, out), o = in_out_order(out, out);
+    MB_CUDA(mb::ew_unary(op, a.rows, a.cols, f64_ptr(&a), rs(&a), cs(&a), f64_ptr(&o), rs(&o), cs(&o), alpha, beta, ctx->stream));
     ctx->launches++;
     return MB_OK;
 }
 
 // out (col-major packed or strided, same logical shape as `A` view) = A, with dtype conversion.
 int32_t copy_convert(mb_ctx* ctx, const mb_block* A, mb_block* out) {
-    int rows = A->rows, cols = A->cols;
-    long long ars = rs(A), acs = cs(A), ors = rs(out), ocs = cs(out);
-    if (out->is_transpose) {
-        std::swap(rows, cols);
-        std::swap(ars, acs); std::swap(ors, ocs);
-    }
+    const mb_block a = in_out_order(A, out), o = in_out_order(out, out);
+    const int rows = a.rows, cols = a.cols;
+    const long long ars = rs(&a), acs = cs(&a), ors = rs(&o), ocs = cs(&o);
     if (A->dtype == MB_F64 && out->dtype == MB_F64) {
         if (ars == 1 && ors == 1) {
             MB_CUDA(mb::ew_unary(mb::EW_COPY, rows, cols, f64_ptr(A), ars, acs, f64_ptr(out), ors, ocs, 1.0, 0.0, ctx->stream));
@@ -188,6 +188,7 @@ int32_t mb_shutdown(mb_ctx* ctx) {
     if (ctx->host_scalar) cudaFreeHost(ctx->host_scalar);
     if (ctx->ev0) cudaEventDestroy(ctx->ev0);
     if (ctx->ev1) cudaEventDestroy(ctx->ev1);
+    for (cudaEvent_t ev : ctx->events) cudaEventDestroy(ev);
     if (ctx->own_stream) cudaStreamDestroy(ctx->own_stream);
     if (ctx->h2d_stream) cudaStreamDestroy(ctx->h2d_stream);
     if (ctx->d2h_stream) cudaStreamDestroy(ctx->d2h_stream);
@@ -296,10 +297,7 @@ int32_t mb_block_view_t(mb_ctx* ctx, const mb_block* blk, mb_block** out) {
     if (!ctx || !blk || !out) return fail(MB_ERR_INVALID_ARG, "mb_block_view_t: null argument");
     int32_t r = new_block(out);
     if (r) return r;
-    **out = *blk;
-    (*out)->owns = 0;
-    std::swap((*out)->rows, (*out)->cols);
-    (*out)->is_transpose = !blk->is_transpose;
+    **out = transposed(*blk);
     return MB_OK;
 }
 
@@ -397,14 +395,10 @@ static int32_t dgemm_device_impl(mb_ctx* ctx, char transa, char transb, int32_t 
     int launches = 0;
     if (ctx->fp64_mode != MB_FP64_NATIVE && !force_generic && !ta && !tb && alpha == 1.0 && (beta == 0.0 || beta == 1.0) &&
         m >= 256 && n >= 256 && k >= 256 && mb::ozaki_supported(m, n, k, ctx->fp64_slices, ctx->fp64_bits)) {
-        const size_t need = mb::ozaki_workspace_bytes(m, n, k, ctx->fp64_slices);
-        if (need > ctx->ozaki_ws_bytes) {
-            if (ctx->ozaki_ws) { MB_CUDA(cudaStreamSynchronize(ctx->stream)); cudaFree(ctx->ozaki_ws); ctx->ozaki_ws = nullptr; ctx->ozaki_ws_bytes = 0; }
-            MB_CUDA(cudaMalloc(&ctx->ozaki_ws, need));
-            ctx->ozaki_ws_bytes = need;
-        }
-        cudaError_t e = mb::gemm_f64_ozaki(m, n, k, A, lda, B, ldb, C, ldc, beta == 1.0, ctx->fp64_slices, ctx->fp64_bits, ctx->ozaki_ws,
-                                           ctx->num_sms, ctx->stream, &launches);
+        cudaError_t e = grow(&ctx->ozaki_ws, &ctx->ozaki_ws_bytes, mb::ozaki_workspace_bytes(m, n, k, ctx->fp64_slices), &ctx->stream);
+        if (e != cudaSuccess) return cuda_fail(e, "dgemm: int8-split workspace");
+        e = mb::gemm_f64_ozaki(m, n, k, A, lda, B, ldb, C, ldc, beta == 1.0, ctx->fp64_slices, ctx->fp64_bits, ctx->ozaki_ws,
+                               ctx->num_sms, ctx->stream, &launches);
         if (e == cudaSuccess) { ctx->launches += launches; return MB_OK; }
         if (e != cudaErrorNotSupported) return cuda_fail(e, "gemm_f64_ozaki");
         cudaGetLastError();
@@ -584,10 +578,7 @@ int32_t mb_block_gemm(mb_ctx* ctx, const mb_block* A, const mb_block* B, mb_bloc
         // degenerate shapes are HBM-bound vector kernels, not tensor-core tiles
         if (N == 1 && M > 1) return mb_block_gemv(ctx, A, B, C, accumulate);                 // matrix x column
         if (M == 1 && N > 1) {                                                              // row x matrix = (B^T a^T)^T
-            mb_block bt = *B;
-            bt.is_transpose = !B->is_transpose;
-            std::swap(bt.rows, bt.cols);
-            bt.owns = 0;
+            const mb_block bt = transposed(*B);
             return mb_block_gemv(ctx, &bt, A, C, accumulate);
         }
         if (K == 1 && !accumulate && M > 1 && N > 1) return mb_block_ger(ctx, A, B, C);     // column x row
@@ -703,6 +694,35 @@ int32_t mb_matmul_blocked(mb_ctx* ctx, mb_block* const* A_tiles, mb_block* const
     return mb_matmul_blocked_subset(ctx, A_tiles, B_tiles, m, k, n, C_tiles, ids.data(), m * n);
 }
 
+// How mb_matmul_blocked_host cuts one block product so that the tensor cores start before its tiles have crossed PCIe.
+// Piece q multiplies k in [k0, k1) of A(i,kk) B(kk,j) into the C columns [c0, c1); it needs only columns [k0, k1) of A
+// and that part of B.
+//  * along K: the first product, unless it is also the last, when k_len >= 1024 and the tile is non-empty.  The rest of
+//    both uploads hides behind the partial products, which accumulate in place.  The cuts are at k_len * q / 4 rounded
+//    down to a multiple of 16; the last is k_len.
+//  * along the columns: the first and the last product when col_len >= 1024.  The first starts after A and a quarter
+//    of B have landed; the last hands each finished column range of C to the D2H stream at once (`download`).
+//  * whole: every other product.
+struct Piece { int k0, k1, c0, c1; };
+struct ProductCut {
+    int count = 1;
+    Piece piece[4];
+    bool along_k = false, download = false;
+};
+static ProductCut cut_product(bool first, bool last, int rows, int k_len, int cols) {
+    ProductCut s;
+    s.piece[0] = {0, k_len, 0, cols};
+    s.along_k = first && !last && k_len >= 1024 && rows > 0 && cols > 0;
+    if (!s.along_k && !((first || last) && cols >= 1024)) return s;
+    s.count = 4;
+    s.download = last;
+    auto kcut = [&](int q) { return q == 4 ? k_len : (int)(((long long)k_len * q / 4) & ~15ll); };
+    auto ccut = [&](int q) { return (int)((long long)cols * q / 4); };
+    for (int q = 0; q < 4; ++q)
+        s.piece[q] = s.along_k ? Piece{kcut(q), kcut(q + 1), 0, cols} : Piece{0, k_len, ccut(q), ccut(q + 1)};
+    return s;
+}
+
 int32_t mb_matmul_blocked_host(mb_ctx* ctx, const double* const* A_host, const double* const* B_host, int32_t m,
                                int32_t k, int32_t n, const int32_t* row_len, const int32_t* k_len, const int32_t* col_len,
                                double* const* C_host) {
@@ -711,6 +731,7 @@ int32_t mb_matmul_blocked_host(mb_ctx* ctx, const double* const* A_host, const d
     if (!A_host || !B_host || !C_host || !row_len || !k_len || !col_len || m <= 0 || k <= 0 || n <= 0)
         return fail(MB_ERR_INVALID_ARG, "mb_matmul_blocked_host: bad argument");
     MB_CUDA(ensure_copy_streams(ctx));
+    ctx->events_used = 0;
     // device layout: every tile gets an even leading dimension and a 256-byte aligned slot (TMA eligibility)
     auto even = [](int x) { return (x + 1) & ~1; };
     auto slot = [](size_t bytes) { return (bytes + 255) & ~size_t(255); };
@@ -722,161 +743,87 @@ int32_t mb_matmul_blocked_host(mb_ctx* ctx, const double* const* A_host, const d
         for (int j = 0; j < n; ++j) { offB[kk * n + j] = total; total += slot((size_t)even(k_len[kk]) * col_len[j] * 8); }
     for (int i = 0; i < m; ++i)
         for (int j = 0; j < n; ++j) { offC[i * n + j] = total; total += slot((size_t)even(row_len[i]) * col_len[j] * 8); }
-    if (total > ctx->workspace_bytes) {
-        if (ctx->workspace) { MB_CUDA(cudaDeviceSynchronize()); cudaFree(ctx->workspace); ctx->workspace = nullptr; ctx->workspace_bytes = 0; }
-        MB_CUDA(cudaMalloc(&ctx->workspace, total));
-        ctx->workspace_bytes = total;
-    }
+    const cudaError_t ge = grow(&ctx->workspace, &ctx->workspace_bytes, total, nullptr);
+    if (ge != cudaSuccess) return cuda_fail(ge, "mb_matmul_blocked_host: workspace");
     char* base = static_cast<char*>(ctx->workspace);
-    std::vector<cudaEvent_t> evA(m * k, nullptr), evB(k * n, nullptr), evC(m * n, nullptr);
-    cudaEvent_t ev_start = nullptr, ev_done = nullptr;
-    int32_t rc = MB_OK;
-    cudaError_t e = cudaSuccess;
-    auto upload = [&](bool isA, int idx, int rows, int cols, const double* host, size_t off, cudaEvent_t& ev) {
-        if (ev || e != cudaSuccess) return;
-        e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
-        if (e != cudaSuccess) return;
-        if (rows > 0 && cols > 0)
-            e = cudaMemcpy2DAsync(base + off, (size_t)even(rows) * 8, host, (size_t)rows * 8, (size_t)rows * 8, cols,
-                                  cudaMemcpyHostToDevice, ctx->h2d_stream);
-        if (e == cudaSuccess) e = cudaEventRecord(ev, ctx->h2d_stream);
-        (void)isA; (void)idx;
+    cudaStream_t const S = ctx->stream, h2d = ctx->h2d_stream, d2h = ctx->d2h_stream;
+    // `to` waits for everything issued to `from` so far; *at is the event recorded there
+    auto handoff = [&](cudaStream_t from, cudaStream_t to, cudaEvent_t* at) {
+        cudaError_t e = next_event(ctx, at);
+        if (e == cudaSuccess) e = cudaEventRecord(*at, from);
+        return e == cudaSuccess ? cudaStreamWaitEvent(to, *at, 0) : e;
     };
-    // the workspace may still be read by a previous call on ctx->stream / d2h_stream: order behind them
-    e = cudaEventCreateWithFlags(&ev_start, cudaEventDisableTiming);
-    if (e == cudaSuccess) e = cudaEventRecord(ev_start, ctx->stream);
-    if (e == cudaSuccess) e = cudaStreamWaitEvent(ctx->h2d_stream, ev_start, 0);
-    // one block product restricted to columns [c0, c1) of B(kk,j) / C(i,j)
-    auto gemm_cols = [&](int i, int j, int kk, int c0, int c1) {
-        const int lda8 = even(row_len[i]) > 0 ? even(row_len[i]) : 1, ldb8 = even(k_len[kk]) > 0 ? even(k_len[kk]) : 1;
-        rc = dgemm_device_impl(ctx, 'N', 'N', row_len[i], c1 - c0, k_len[kk], 1.0, reinterpret_cast<double*>(base + offA[i * k + kk]), lda8,
-                               reinterpret_cast<double*>(base + offB[kk * n + j]) + (size_t)c0 * ldb8, ldb8, kk > 0 ? 1.0 : 0.0,
-                               reinterpret_cast<double*>(base + offC[i * n + j]) + (size_t)c0 * lda8, lda8, false);
+    // a rows x cols column-major part of a tile between the host and the workspace (leading dimensions in doubles)
+    auto copy = [](double* dst, int dld, const double* src, int sld, int rows, int cols, cudaMemcpyKind kind, cudaStream_t st) {
+        if (rows <= 0 || cols <= 0) return cudaSuccess;
+        return cudaMemcpy2DAsync(dst, (size_t)dld * 8, src, (size_t)sld * 8, (size_t)rows * 8, cols, kind, st);
     };
-    std::vector<cudaEvent_t> chunk_events;
-    for (int i = 0; i < m && e == cudaSuccess && rc == MB_OK; ++i)
-        for (int j = 0; j < n && e == cudaSuccess && rc == MB_OK; ++j) {
-            for (int kk = 0; kk < k && e == cudaSuccess && rc == MB_OK; ++kk) {
-                const bool first_product = (i == 0 && j == 0 && kk == 0);
-                const bool last_product = (i == m - 1 && j == n - 1 && kk == k - 1);
-                if (first_product && !last_product && k_len[kk] >= 1024 && row_len[i] > 0 && col_len[j] > 0) {
-                    // The first product is split along K: the GEMM on chunk q needs only columns [k0,k1) of A and rows
-                    // [k0,k1) of B, so the tensor cores start after a quarter of each tile has crossed PCIe and the rest
-                    // of both uploads hides behind the partial products (accumulated in place, beta = 1).
-                    const int nk = 4;
-                    const int lda8 = even(row_len[i]), ldb8 = even(k_len[kk]);
-                    for (int q = 0; q < nk && e == cudaSuccess && rc == MB_OK; ++q) {
-                        const int k0 = q == 0 ? 0 : (int)(((long long)k_len[kk] * q / nk) & ~15ll);
-                        const int k1 = q == nk - 1 ? k_len[kk] : (int)(((long long)k_len[kk] * (q + 1) / nk) & ~15ll);
-                        cudaEvent_t ev = nullptr;
-                        e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
-                        if (e != cudaSuccess) break;
-                        chunk_events.push_back(ev);
-                        e = cudaMemcpy2DAsync(base + offA[i * k + kk] + (size_t)k0 * lda8 * 8, (size_t)lda8 * 8,
-                                              A_host[i * k + kk] + (size_t)k0 * row_len[i], (size_t)row_len[i] * 8,
-                                              (size_t)row_len[i] * 8, k1 - k0, cudaMemcpyHostToDevice, ctx->h2d_stream);
-                        if (e == cudaSuccess)
-                            e = cudaMemcpy2DAsync(base + offB[kk * n + j] + (size_t)k0 * 8, (size_t)ldb8 * 8, B_host[kk * n + j] + k0,
-                                                  (size_t)k_len[kk] * 8, (size_t)(k1 - k0) * 8, col_len[j], cudaMemcpyHostToDevice,
-                                                  ctx->h2d_stream);
-                        if (e == cudaSuccess) e = cudaEventRecord(ev, ctx->h2d_stream);
-                        if (e == cudaSuccess) e = cudaStreamWaitEvent(ctx->stream, ev, 0);
-                        if (e != cudaSuccess) break;
-                        rc = dgemm_device_impl(ctx, 'N', 'N', row_len[i], col_len[j], k1 - k0, 1.0,
-                                               reinterpret_cast<double*>(base + offA[i * k + kk]) + (size_t)k0 * lda8, lda8,
-                                               reinterpret_cast<double*>(base + offB[kk * n + j]) + k0, ldb8, (kk > 0 || q > 0) ? 1.0 : 0.0,
-                                               reinterpret_cast<double*>(base + offC[i * n + j]), lda8, false);
-                    }
-                    if (e != cudaSuccess || rc != MB_OK) break;
-                    // later users of these two tiles wait for the whole of them
-                    e = cudaEventCreateWithFlags(&evA[i * k + kk], cudaEventDisableTiming);
-                    if (e == cudaSuccess) e = cudaEventRecord(evA[i * k + kk], ctx->h2d_stream);
-                    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&evB[kk * n + j], cudaEventDisableTiming);
-                    if (e == cudaSuccess) e = cudaEventRecord(evB[kk * n + j], ctx->h2d_stream);
-                    continue;
-                }
-                const int nch = ((first_product || last_product) && col_len[j] >= 1024) ? 4 : 1;
-                // uploads in first-use order (seq = i*n*k + j*k + kk)
-                upload(true, i * k + kk, row_len[i], k_len[kk], A_host[i * k + kk], offA[i * k + kk], evA[i * k + kk]);
-                if (e != cudaSuccess) break;
-                e = cudaStreamWaitEvent(ctx->stream, evA[i * k + kk], 0);
-                if (e != cudaSuccess) break;
-                if (nch == 1) {
-                    upload(false, kk * n + j, k_len[kk], col_len[j], B_host[kk * n + j], offB[kk * n + j], evB[kk * n + j]);
-                    if (e == cudaSuccess) e = cudaStreamWaitEvent(ctx->stream, evB[kk * n + j], 0);
-                    if (e != cudaSuccess) break;
-                    gemm_cols(i, j, kk, 0, col_len[j]);
-                    continue;
-                }
-                // The first product starts after A + a quarter of B has landed (B uploaded and multiplied in column
-                // chunks); the last product hands each finished column chunk of C to the D2H stream at once.
-                const bool b_pending = (evB[kk * n + j] == nullptr);
-                const int ldb8 = even(k_len[kk]), ldc8 = even(row_len[i]);
-                for (int q = 0; q < nch && e == cudaSuccess && rc == MB_OK; ++q) {
-                    const int c0 = (int)((long long)col_len[j] * q / nch), c1 = (int)((long long)col_len[j] * (q + 1) / nch);
-                    if (b_pending) {
-                        cudaEvent_t ev = nullptr;
-                        e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
-                        if (e != cudaSuccess) break;
-                        chunk_events.push_back(ev);
-                        e = cudaMemcpy2DAsync(base + offB[kk * n + j] + (size_t)c0 * ldb8 * 8, (size_t)ldb8 * 8,
-                                              B_host[kk * n + j] + (size_t)c0 * k_len[kk], (size_t)k_len[kk] * 8, (size_t)k_len[kk] * 8,
-                                              c1 - c0, cudaMemcpyHostToDevice, ctx->h2d_stream);
-                        if (e == cudaSuccess) e = cudaEventRecord(ev, ctx->h2d_stream);
-                        if (e == cudaSuccess) e = cudaStreamWaitEvent(ctx->stream, ev, 0);
-                        if (e != cudaSuccess) break;
-                        if (q == nch - 1) {          // later users of this B tile wait for the whole of it
-                            e = cudaEventCreateWithFlags(&evB[kk * n + j], cudaEventDisableTiming);
-                            if (e == cudaSuccess) e = cudaEventRecord(evB[kk * n + j], ctx->h2d_stream);
+    std::vector<cudaEvent_t> evA(m * k, nullptr), evB(k * n, nullptr);     // the tile's upload, once all of it is issued
+    // every copy, wait and product of the call in issue order; the first failure ends it
+    auto issue = [&]() -> int32_t {
+        cudaEvent_t ev = nullptr;
+        // the workspace may still be read by a previous call on ctx->stream / d2h_stream: order behind them
+        MB_CUDA(handoff(S, h2d, &ev));
+        for (int i = 0; i < m; ++i)
+            for (int j = 0; j < n; ++j)
+                for (int kk = 0; kk < k; ++kk) {
+                    const int ia = i * k + kk, ib = kk * n + j, ic = i * n + j;
+                    const int rows = row_len[i], depth = k_len[kk], cols = col_len[j];
+                    const int lda = std::max(1, even(rows)), ldb = std::max(1, even(depth));     // C has A's leading dimension
+                    double *dA = reinterpret_cast<double*>(base + offA[ia]), *dB = reinterpret_cast<double*>(base + offB[ib]),
+                           *dC = reinterpret_cast<double*>(base + offC[ic]);
+                    const ProductCut cut =
+                        cut_product(i == 0 && j == 0 && kk == 0, i == m - 1 && j == n - 1 && kk == k - 1, rows, depth, cols);
+                    const bool a_new = !evA[ia], b_new = !evB[ib];
+                    for (int q = 0; q < cut.count; ++q) {
+                        const Piece& p = cut.piece[q];
+                        // uploads in first-use order (seq = i*n*k + j*k + kk); A is cut along K only, B along K or its columns
+                        const bool up_a = a_new && (cut.along_k || q == 0);
+                        if (up_a)
+                            MB_CUDA(copy(dA + (size_t)p.k0 * lda, lda, A_host[ia] + (size_t)p.k0 * rows, rows, rows, p.k1 - p.k0,
+                                         cudaMemcpyHostToDevice, h2d));
+                        if (b_new)
+                            MB_CUDA(copy(dB + (size_t)p.c0 * ldb + p.k0, ldb, B_host[ib] + (size_t)p.c0 * depth + p.k0, depth,
+                                         p.k1 - p.k0, p.c1 - p.c0, cudaMemcpyHostToDevice, h2d));
+                        // the GEMM waits for this piece's uploads; without any, the first piece waits for the tiles' uploads
+                        if (up_a || b_new) {
+                            MB_CUDA(handoff(h2d, S, &ev));
+                            // a tile whose last part is now issued is complete for the later products
+                            if (up_a && p.k1 == depth) evA[ia] = ev;
+                            if (b_new && p.k1 == depth && p.c1 == cols) evB[ib] = ev;
+                        } else if (q == 0) {
+                            MB_CUDA(cudaStreamWaitEvent(S, evA[ia], 0));
+                            MB_CUDA(cudaStreamWaitEvent(S, evB[ib], 0));
                         }
-                    } else if (q == 0) {
-                        e = cudaStreamWaitEvent(ctx->stream, evB[kk * n + j], 0);
+                        const int32_t rc = dgemm_device_impl(ctx, 'N', 'N', rows, p.c1 - p.c0, p.k1 - p.k0, 1.0, dA + (size_t)p.k0 * lda,
+                                                             lda, dB + (size_t)p.c0 * ldb + p.k0, ldb, (kk > 0 || p.k0 > 0) ? 1.0 : 0.0,
+                                                             dC + (size_t)p.c0 * lda, lda, false);
+                        if (rc != MB_OK) return rc;
+                        if (cut.download) {
+                            MB_CUDA(handoff(S, d2h, &ev));
+                            MB_CUDA(copy(C_host[ic] + (size_t)p.c0 * rows, rows, dC + (size_t)p.c0 * lda, lda, rows, p.c1 - p.c0,
+                                         cudaMemcpyDeviceToHost, d2h));
+                        }
                     }
-                    if (e != cudaSuccess) break;
-                    gemm_cols(i, j, kk, c0, c1);
-                    if (rc != MB_OK) break;
-                    if (last_product) {
-                        cudaEvent_t ev = nullptr;
-                        e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
-                        if (e != cudaSuccess) break;
-                        chunk_events.push_back(ev);
-                        e = cudaEventRecord(ev, ctx->stream);
-                        if (e == cudaSuccess) e = cudaStreamWaitEvent(ctx->d2h_stream, ev, 0);
-                        if (e == cudaSuccess && row_len[i] > 0 && c1 > c0)
-                            e = cudaMemcpy2DAsync(C_host[i * n + j] + (size_t)c0 * row_len[i], (size_t)row_len[i] * 8,
-                                                  base + offC[i * n + j] + (size_t)c0 * ldc8 * 8, (size_t)ldc8 * 8, (size_t)row_len[i] * 8,
-                                                  c1 - c0, cudaMemcpyDeviceToHost, ctx->d2h_stream);
+                    // C(i,j) goes to the host after its last kk, unless the last product sent it piece by piece
+                    if (kk == k - 1 && !cut.download) {
+                        MB_CUDA(handoff(S, d2h, &ev));
+                        MB_CUDA(copy(C_host[ic], rows, dC, lda, rows, cols, cudaMemcpyDeviceToHost, d2h));
                     }
                 }
-            }
-            if (e != cudaSuccess || rc != MB_OK) break;
-            const bool chunked_out = (i == m - 1 && j == n - 1 && col_len[j] >= 1024);
-            if (chunked_out) continue;               // already downloaded chunk by chunk
-            e = cudaEventCreateWithFlags(&evC[i * n + j], cudaEventDisableTiming);
-            if (e == cudaSuccess) e = cudaEventRecord(evC[i * n + j], ctx->stream);
-            if (e == cudaSuccess) e = cudaStreamWaitEvent(ctx->d2h_stream, evC[i * n + j], 0);
-            if (e == cudaSuccess && row_len[i] > 0 && col_len[j] > 0)
-                e = cudaMemcpy2DAsync(C_host[i * n + j], (size_t)row_len[i] * 8, base + offC[i * n + j], (size_t)even(row_len[i]) * 8,
-                                      (size_t)row_len[i] * 8, col_len[j], cudaMemcpyDeviceToHost, ctx->d2h_stream);
-        }
-    if (e == cudaSuccess && rc == MB_OK) {
+        return MB_OK;
+    };
+    int32_t rc = issue();
+    if (rc == MB_OK) {
         // the call returns when every C tile is on the host; ctx->stream is ordered behind the downloads too
-        e = cudaEventCreateWithFlags(&ev_done, cudaEventDisableTiming);
-        if (e == cudaSuccess) e = cudaEventRecord(ev_done, ctx->d2h_stream);
-        if (e == cudaSuccess) e = cudaStreamWaitEvent(ctx->stream, ev_done, 0);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->d2h_stream);
+        cudaEvent_t ev = nullptr;
+        cudaError_t e = handoff(d2h, S, &ev);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(d2h);
+        if (e != cudaSuccess) rc = cuda_fail(e, "mb_matmul_blocked_host");
     } else {
-        cudaStreamSynchronize(ctx->h2d_stream); cudaStreamSynchronize(ctx->stream); cudaStreamSynchronize(ctx->d2h_stream);
+        cudaStreamSynchronize(h2d); cudaStreamSynchronize(S); cudaStreamSynchronize(d2h);
     }
-    for (auto ev : evA) if (ev) cudaEventDestroy(ev);
-    for (auto ev : evB) if (ev) cudaEventDestroy(ev);
-    for (auto ev : evC) if (ev) cudaEventDestroy(ev);
-    for (auto ev : chunk_events) if (ev) cudaEventDestroy(ev);
-    if (ev_start) cudaEventDestroy(ev_start);
-    if (ev_done) cudaEventDestroy(ev_done);
-    if (rc != MB_OK) return rc;
-    if (e != cudaSuccess) return cuda_fail(e, "mb_matmul_blocked_host");
-    return MB_OK;
+    return rc;
 }
 
 // DenseVecMatrix.multiply(B: BDM) for one row shard (matrix/DenseVecMatrix.scala:1660-1680): C_rows = A_rows * B with
@@ -902,6 +849,7 @@ int32_t mb_matmul_rowsharded_host(mb_ctx* ctx, const double* A_host, int64_t row
         return fail(MB_ERR_INVALID_ARG, "mb_matmul_rowsharded_host: bad argument");
     if (rows == 0 || n == 0) return MB_OK;
     MB_CUDA(ensure_copy_streams(ctx));
+    ctx->events_used = 0;
     constexpr int SLOTS = 3;
     // ~256 MiB of A (or C, whichever is wider) per chunk, a multiple of 128 rows (whole GEMM tiles), at least one tile;
     // MARLIN_B200_ROWSHARD_CHUNK_MIB overrides the size (the tests use it to run many chunks on small inputs)
@@ -913,20 +861,15 @@ int32_t mb_matmul_rowsharded_host(mb_ctx* ctx, const double* A_host, int64_t row
     const int kk = std::max(k, 1);
     auto slot = [](size_t bytes) { return (bytes + 255) & ~size_t(255); };
     const size_t bytesB = slot((size_t)kk * n * 8), bytesA = slot((size_t)chunk * kk * 8), bytesC = slot((size_t)chunk * n * 8);
-    const size_t total = bytesB + SLOTS * (bytesA + bytesC);
-    if (total > ctx->workspace_bytes) {
-        if (ctx->workspace) { MB_CUDA(cudaDeviceSynchronize()); cudaFree(ctx->workspace); ctx->workspace = nullptr; ctx->workspace_bytes = 0; }
-        MB_CUDA(cudaMalloc(&ctx->workspace, total));
-        ctx->workspace_bytes = total;
-    }
+    cudaError_t e = grow(&ctx->workspace, &ctx->workspace_bytes, bytesB + SLOTS * (bytesA + bytesC), nullptr);
+    if (e != cudaSuccess) return cuda_fail(e, "mb_matmul_rowsharded_host: workspace");
     char* base = static_cast<char*>(ctx->workspace);
     double* dB = reinterpret_cast<double*>(base);
     auto dA = [&](int s_) { return reinterpret_cast<double*>(base + bytesB + (size_t)s_ * (bytesA + bytesC)); };
     auto dC = [&](int s_) { return reinterpret_cast<double*>(base + bytesB + (size_t)s_ * (bytesA + bytesC) + bytesA); };
     cudaEvent_t ev_start = nullptr, ev_b = nullptr, ev_up[SLOTS] = {}, ev_gemm[SLOTS] = {}, ev_down[SLOTS] = {};
-    cudaError_t e = cudaSuccess;
     int32_t rc = MB_OK;
-    auto mk = [&](cudaEvent_t& ev) { if (e == cudaSuccess && !ev) e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming); };
+    auto mk = [&](cudaEvent_t& ev) { if (e == cudaSuccess) e = next_event(ctx, &ev); };
     mk(ev_start); mk(ev_b);
     for (int s_ = 0; s_ < SLOTS; ++s_) { mk(ev_up[s_]); mk(ev_gemm[s_]); mk(ev_down[s_]); }
     // the workspace may still be in use by an earlier call on ctx->stream
@@ -964,13 +907,6 @@ int32_t mb_matmul_rowsharded_host(mb_ctx* ctx, const double* A_host, int64_t row
         if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->d2h_stream);
     } else {
         cudaStreamSynchronize(ctx->h2d_stream); cudaStreamSynchronize(ctx->stream); cudaStreamSynchronize(ctx->d2h_stream);
-    }
-    if (ev_start) cudaEventDestroy(ev_start);
-    if (ev_b) cudaEventDestroy(ev_b);
-    for (int s_ = 0; s_ < SLOTS; ++s_) {
-        if (ev_up[s_]) cudaEventDestroy(ev_up[s_]);
-        if (ev_gemm[s_]) cudaEventDestroy(ev_gemm[s_]);
-        if (ev_down[s_]) cudaEventDestroy(ev_down[s_]);
     }
     if (rc != MB_OK) return rc;
     if (e != cudaSuccess) return cuda_fail(e, "mb_matmul_rowsharded_host");
@@ -1061,10 +997,7 @@ int32_t mb_block_transpose(mb_ctx* ctx, const mb_block* A, mb_block* out) {
     if (!A || !out) return fail(MB_ERR_INVALID_ARG, "mb_block_transpose: null block");
     if (out->rows != A->cols || out->cols != A->rows)
         return fail(MB_ERR_DIM_MISMATCH, "transpose: result block is %dx%d, expected %dx%d", out->rows, out->cols, A->cols, A->rows);
-    mb_block view = *A;     // A^T as a view, then materialise it (denseBlock.t.copy)
-    view.owns = 0;
-    std::swap(view.rows, view.cols);
-    view.is_transpose = !A->is_transpose;
+    const mb_block view = transposed(*A);     // A^T as a view, then materialise it (denseBlock.t.copy)
     return copy_convert(ctx, &view, out);
 }
 
@@ -1097,12 +1030,8 @@ int32_t mb_block_gemv(mb_ctx* ctx, const mb_block* A, const mb_block* x, mb_bloc
     // a transposed view is the column-major (cols x rows) array underneath: y = S^T x
     const bool trans = A->is_transpose != 0;
     const int m = trans ? A->cols : A->rows, n = trans ? A->rows : A->cols;
-    const size_t need = mb::gemv_workspace_doubles(trans, m, n);
-    if (need > ctx->vec_ws_doubles) {
-        if (ctx->vec_ws) { MB_CUDA(cudaStreamSynchronize(ctx->stream)); MB_CUDA(cudaFree(ctx->vec_ws)); ctx->vec_ws = nullptr; ctx->vec_ws_doubles = 0; }
-        MB_CUDA(cudaMalloc(&ctx->vec_ws, need * sizeof(double)));
-        ctx->vec_ws_doubles = need;
-    }
+    const cudaError_t e = grow(&ctx->vec_ws, &ctx->vec_ws_bytes, mb::gemv_workspace_doubles(trans, m, n) * sizeof(double), &ctx->stream);
+    if (e != cudaSuccess) return cuda_fail(e, "mb_block_gemv: workspace");
     int launches = 0;
     MB_CUDA(mb::gemv_f64(trans, m, n, f64_ptr(A), A->ld, xv.p, xv.inc, yv.p, yv.inc, accumulate != 0, ctx->vec_ws, ctx->stream,
                          &launches));
@@ -1144,11 +1073,8 @@ int32_t mb_block_ger(mb_ctx* ctx, const mb_block* x, const mb_block* y, mb_block
 
 // ---------------------------------------------------------------------- factorizations (SURVEY 8 f4)
 static int32_t int_scratch(mb_ctx* ctx, size_t count) {
-    if (count > ctx->int_ws_count) {
-        if (ctx->int_ws) { MB_CUDA(cudaStreamSynchronize(ctx->stream)); cudaFree(ctx->int_ws); ctx->int_ws = nullptr; ctx->int_ws_count = 0; }
-        MB_CUDA(cudaMalloc(&ctx->int_ws, count * sizeof(int)));
-        ctx->int_ws_count = count;
-    }
+    const cudaError_t e = grow(&ctx->int_ws, &ctx->int_ws_bytes, count * sizeof(int), &ctx->stream);
+    if (e != cudaSuccess) return cuda_fail(e, "factorization workspace");
     if (count > ctx->int_host_count) {
         if (ctx->int_host) { cudaFreeHost(ctx->int_host); ctx->int_host = nullptr; ctx->int_host_count = 0; }
         MB_CUDA(cudaMallocHost(&ctx->int_host, count * sizeof(int)));
@@ -1449,13 +1375,9 @@ int32_t mb_sparse_upload(mb_ctx* ctx, int32_t rows, int32_t cols, const int32_t*
     if (r) return r;
     const long long nnz = colptr[cols];
     if (nnz > 0 && !values) return fail(MB_ERR_INVALID_ARG, "mb_sparse_upload: null values");
-    mb_sparse* S = new (std::nothrow) mb_sparse();
-    if (!S) return fail(MB_ERR_OOM, "host allocation failed");
-    S->rows = rows; S->cols = cols; S->nnz = nnz; S->owns = 1; S->device = ctx->device;
-    cudaError_t e = cudaMalloc(&S->colptr, sizeof(int) * ((size_t)cols + 1));
-    if (e == cudaSuccess && nnz) e = cudaMalloc(&S->rowidx, sizeof(int) * (size_t)nnz);
-    if (e == cudaSuccess && nnz) e = cudaMalloc(&S->values, sizeof(double) * (size_t)nnz);
-    if (e == cudaSuccess) e = cudaMemcpy(S->colptr, colptr, sizeof(int) * ((size_t)cols + 1), cudaMemcpyHostToDevice);
+    mb_sparse* S = nullptr;
+    if ((r = mb_sparse_alloc(ctx, rows, cols, nnz, &S)) != MB_OK) return r;
+    cudaError_t e = cudaMemcpy(S->colptr, colptr, sizeof(int) * ((size_t)cols + 1), cudaMemcpyHostToDevice);
     if (e == cudaSuccess && nnz) e = cudaMemcpy(S->rowidx, rowidx, sizeof(int) * (size_t)nnz, cudaMemcpyHostToDevice);
     if (e == cudaSuccess && nnz) e = cudaMemcpy(S->values, values, sizeof(double) * (size_t)nnz, cudaMemcpyHostToDevice);
     if (e != cudaSuccess) { sparse_release(S); return cuda_fail(e, "mb_sparse_upload"); }

@@ -123,8 +123,6 @@ struct mb_comm {
     bool have_half[2] = {false, false};
     unsigned long long* status_host = nullptr;       // pinned copy of flags[F_STATUS]
     double timeout_s = 120.0;
-    std::vector<cudaEvent_t> events;                 // pool, reused every call
-    size_t events_used = 0;
     bool aborted = false;                            // abort_local() ran: every later call fails
     bool remote_write_ok = true;                     // cuStreamWriteValue64 accepted a peer address (else: 8-byte copies)
     unsigned long long* ring = nullptr;              // pinned host values for the copy-based flag writes
@@ -241,14 +239,6 @@ int32_t sync_bounded(mb_comm* c, cudaStream_t st, const char* what) {
         }
     }
 }
-cudaEvent_t next_event(mb_comm* c) {
-    if (c->events_used == c->events.size()) {
-        cudaEvent_t ev = nullptr;
-        if (cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) != cudaSuccess) return nullptr;
-        c->events.push_back(ev);
-    }
-    return c->events[c->events_used++];
-}
 
 // ---------------------------------------------------------------------------------------- plan
 struct MyC { int id, i, j; std::vector<int> kks; };   // a C tile (id = i*n + j) with the kk of one rank's products of it
@@ -351,14 +341,8 @@ int32_t ensure_staging(mb_comm* c, size_t need_slot) {
 }
 
 int32_t ensure_arena(mb_comm* c, size_t bytes) {
-    if (bytes <= c->arena_bytes) return MB_OK;
-    MB_CUDA(cudaDeviceSynchronize());
-    if (c->arena) cudaFree(c->arena);
-    c->arena = nullptr;
-    c->arena_bytes = 0;
-    MB_CUDA(cudaMalloc(&c->arena, bytes));
-    c->arena_bytes = bytes;
-    return MB_OK;
+    const cudaError_t e = grow(&c->arena, &c->arena_bytes, bytes, nullptr);
+    return e == cudaSuccess ? MB_OK : cuda_fail(e, "mb_comm: arena");
 }
 
 // ---------------------------------------------------------------------------------------- metadata exchange
@@ -730,7 +714,6 @@ int32_t mb_comm_destroy(mb_comm* c) {
     if (c->flags) cudaFree(c->flags);
     if (c->status_host) cudaFreeHost(c->status_host);
     if (c->ring) cudaFreeHost(c->ring);
-    for (auto ev : c->events) cudaEventDestroy(ev);
     if (c->ev_compute) cudaEventDestroy(c->ev_compute);
     if (c->ev_tmp) cudaEventDestroy(c->ev_tmp);
     if (c->X) cudaStreamDestroy(c->X);
@@ -810,7 +793,7 @@ int32_t mb_matmul_blocked_dist(mb_comm* c, mb_block* const* A_tiles, const int32
                             row_len[t / n], col_len[t % n]);
         }
     const unsigned long long e = ++c->epoch;
-    c->events_used = 0;
+    ctx->events_used = 0;
 
     // ---- 0. publish the tiles I own, read everybody's ----
     std::vector<ShmEntry> mine;
@@ -978,8 +961,7 @@ int32_t mb_matmul_blocked_dist(mb_comm* c, mb_block* const* A_tiles, const int32
                     MB_CUDA(copy_band(t, is_a, b, src, t.ent->ld, cudaMemcpyDeviceToDevice, X));
                     if (t.ready_base >= 0) MB_CUDA(sig(c, c->flags + F_BAND + t.ready_base + b, e, X));
                     if (b == t.nbands - 1) {
-                        t.landed = next_event(c);
-                        if (!t.landed) return fail(MB_ERR_CUDA, "cudaEventCreate failed");
+                        MB_CUDA(next_event(ctx, &t.landed));
                         MB_CUDA(cudaEventRecord(t.landed, X));
                     }
                 }
@@ -1186,7 +1168,7 @@ int32_t mb_matmul_blocked_dist_host(mb_comm* c, const double* const* A_host, con
     for (const MyC& mc : myc)
         if (!C_host[mc.id]) return fail(MB_ERR_INVALID_ARG, "mb_matmul_blocked_dist_host: C tile %d is computed here but NULL", mc.id);
     const unsigned long long e = ++c->epoch;
-    c->events_used = 0;
+    ctx->events_used = 0;
 
     // ---- device layout in the arena: tiles I upload, tiles I pull, my C tiles ----
     std::vector<Tile> tA(m * k), tB(k * n);

@@ -9,6 +9,7 @@
 #include <cstdarg>
 #include <cstdio>
 #include <mutex>
+#include <vector>
 
 struct mb_ctx {
     int device = 0;
@@ -32,12 +33,16 @@ struct mb_ctx {
     size_t ozaki_ws_bytes = 0;
     // partial vectors of the matrix x vector kernels (grow-only)
     double* vec_ws = nullptr;
-    size_t vec_ws_doubles = 0;
+    size_t vec_ws_bytes = 0;
     // pivots / permutation / info of the factorization entries (grow-only) + a pinned mirror for the results
     int* int_ws = nullptr;
-    size_t int_ws_count = 0;
+    size_t int_ws_bytes = 0;
     int* int_host = nullptr;
     size_t int_host_count = 0;
+    // Events of the host pipelines and the multi-GPU entries (next_event).  An entry resets events_used when it starts,
+    // under the lock; re-recording an event is safe because a stream wait binds to the record current when it is issued.
+    std::vector<cudaEvent_t> events;
+    size_t events_used = 0;
     // Entry points that use the context's own scratch buffers, workspaces, events or copy streams take this lock, so
     // threads sharing one context (Spark local[N] task threads) serialise there; kernel-only entries (gemm, element-wise,
     // transpose, fill) touch no shared host state and need none.  Threads that want concurrency use one context each.
@@ -125,5 +130,34 @@ inline cudaError_t ensure_copy_streams(mb_ctx* ctx) {
     if (ctx->h2d_stream) return cudaSuccess;
     cudaError_t e = cudaStreamCreateWithFlags(&ctx->h2d_stream, cudaStreamNonBlocking);
     return e == cudaSuccess ? cudaStreamCreateWithFlags(&ctx->d2h_stream, cudaStreamNonBlocking) : e;
+}
+
+// The next unused event of the context's pool, created when the pool runs out.
+inline cudaError_t next_event(mb_ctx* ctx, cudaEvent_t* ev) {
+    if (ctx->events_used == ctx->events.size()) {
+        cudaEvent_t fresh = nullptr;
+        cudaError_t e = cudaEventCreateWithFlags(&fresh, cudaEventDisableTiming);
+        if (e != cudaSuccess) return e;
+        ctx->events.push_back(fresh);
+    }
+    *ev = ctx->events[ctx->events_used++];
+    return cudaSuccess;
+}
+
+// A grow-only device buffer: when `need` exceeds *have bytes, the old buffer is freed once the work that may still use
+// it has finished (*sync, or the whole device when sync is null) and a buffer of `need` bytes takes its place.
+template <class T>
+cudaError_t grow(T** p, size_t* have, size_t need, const cudaStream_t* sync) {
+    if (need <= *have) return cudaSuccess;
+    if (*p) {
+        cudaError_t e = sync ? cudaStreamSynchronize(*sync) : cudaDeviceSynchronize();
+        if (e != cudaSuccess) return e;
+        cudaFree(*p);
+        *p = nullptr;
+        *have = 0;
+    }
+    cudaError_t e = cudaMalloc(p, need);
+    if (e == cudaSuccess) *have = need;
+    return e;
 }
 
