@@ -226,6 +226,73 @@ int32_t mb_lr_gradient(mb_ctx* ctx, const mb_block* rows, const double* w, doubl
  * (max row id + 1) and must be positive.  Blocking. */
 int32_t mb_lr_train(mb_ctx* ctx, const mb_block* rows, int64_t data_size, double step, int32_t iters, double* w_out);
 
+/* ---- CoordinateMatrix.ALS (matrix/CoordinateMatrix.scala:88-98, ml/ALSHelp.scala:34-382).  One side of the problem is the
+ *      users (row ids), the other the products (column ids); an entity of a side has a POSITION: block 0's distinct ids
+ *      ascending, then block 1's, ... with block = id mod num_blocks (Spark's HashPartitioner).  A side's factors are a
+ *      row-major fp64 view (is_transpose = 1, or one column) with one row per position and `rank` columns.
+ *      The arithmetic of one entity u is updateBlock's (:292-382), in its order:
+ *        A_u = sum of fl(y_i y_j) over u's terms (partner block ascending, partner id ascending, then input order), each
+ *              element one sequential sum from 0.0 with separate roundings; implicit: sum of fl(fl(c - 1) fl(y_i y_j)) with
+ *              c = fl(1 + fl(alpha |r|));
+ *        b_u = sum of fl(r y_i); implicit: sum of fl(c y_i) over the ratings r > 0;
+ *        A_u(i, i) += fl(numRatings * lambda), then (implicit) A_u += YtY, the Gramian of the fixed side's factors;
+ *        x_u = A_u^-1 b_u by Cholesky (the reference inverts and multiplies: equal within rounding, not bitwise).
+ *      A_u never leaves the kernel.  rank < 1 or lambda < 0: MB_ERR_INVALID_ARG; rank > MB_ALS_MAX_RANK: MB_ERR_UNSUPPORTED.
+ *      A non-positive pivot (only possible with lambda = 0) is MB_ERR_CUDA "not positive definite" naming the lowest
+ *      such entity id. ---- */
+#define MB_ALS_MAX_RANK 128
+/* Pure host logic (makeOutLinkBlock / makeInLinkBlock, :101-165) for the side whose ids are ent[] (partner[] the other
+ * side's ids of the same ratings).  Every id must lie in [0, 2^31 - 1] (MB_ERR_INVALID_ARG otherwise; the reference
+ * truncates with toInt).  Writes, with n = the side's distinct ids (returned in *count_out, n <= nnz):
+ *   ids_out[n]                 the id of each position
+ *   block_offsets_out[nb + 1]  block b holds positions [block_offsets_out[b], block_offsets_out[b + 1])
+ *   offsets_out[n + 1]         position p's terms are q in [offsets_out[p], offsets_out[p + 1]), in the order above,
+ *   partners_out[nnz], ratings_out[nnz]  the partner's position on the other side and the rating of term q
+ *   work_out[n]                positions by rating count descending, ties by position (heaviest first)
+ * Duplicated (row, col) entries are kept, each a term of its own, in input order.  Output arrays are sized by nnz. */
+int32_t mb_als_links(int64_t nnz, const int64_t* ent, const int64_t* partner, const float* values, int32_t num_blocks,
+                     int32_t num_partner_blocks, int64_t* ids_out, int64_t* block_offsets_out, int64_t* offsets_out,
+                     int32_t* partners_out, float* ratings_out, int32_t* work_out, int64_t* count_out);
+/* Pure host logic (:60-74, randomFactor :170-179): the initial factors of `count` consecutive positions of block `block`
+ * of side 0 (users, seed1) or side 1 (products, seed2), row-major into out[count * rank].  seed1 and seed2 are the first
+ * two nextInt() of java.util.Random(seed); the block draws from Random(byteswap32(seedN ^ block)). */
+int32_t mb_als_init_factors(int64_t seed, int32_t side, int32_t block, int32_t rank, int64_t count, double* out);
+/* The device-resident links of one side (the arrays of mb_als_links, ids narrowed to int32, on the device), restricted
+ * to the `count` positions of `work`.  The ctx stream must see them filled. */
+typedef struct mb_als_side {
+    int64_t count;
+    const int32_t* ids;
+    const int64_t* offsets;
+    const int32_t* partners;
+    const float* ratings;
+    const int32_t* work;
+} mb_als_side;
+/* The assembly alone: for every position p in side->work, the packed lower triangle of A_p (row-major, element (i, j) at
+ * i (i + 1) / 2 + j, regularisation and YtY included) to the DEVICE array A_out + p * rank (rank + 1) / 2 and b_p to
+ * b_out + p * rank.  Y: the fixed side's factors.  YtY (rank x rank) is read when implicit; NULL computes it from Y. */
+int32_t mb_als_normal_equations(mb_ctx* ctx, const mb_als_side* side, const mb_block* Y, double lambda, double alpha,
+                                int32_t implicit, const mb_block* YtY, double* A_out, double* b_out);
+/* One half-step: row p of X gets x_p for every position p in side->work; other rows are left as they are.  YtY as above.
+ * Blocking (the pivot check reads back one int). */
+int32_t mb_als_update(mb_ctx* ctx, const mb_als_side* side, const mb_block* Y, double lambda, double alpha, int32_t implicit,
+                      const mb_block* YtY, mb_block* X);
+/* The whole loop on one device (:77-82): `iterations` times, products from users then users from products, YtY computed on
+ * the device each half-step when implicit (mb_block_gramian), no host synchronisation between half-steps.  U and P hold
+ * the initial factors on entry and the result on return; iterations <= 0 leaves them as they are.  Blocking. */
+int32_t mb_als_train(mb_ctx* ctx, const mb_als_side* users, const mb_als_side* products, int32_t iterations, double lambda,
+                     double alpha, int32_t implicit, mb_block* U, mb_block* P);
+/* updateBlock (:292-382) on HOST arrays, for the JVM: n positions with offsets[n + 1] / partners / ratings as from
+ * mb_als_links and ids[n]; Y: n_fixed x rank row-major; YtY: rank x rank row-major or NULL (computed when implicit);
+ * X: n x rank row-major.  Uploads, solves and frees inside the call. */
+int32_t mb_als_update_host(mb_ctx* ctx, int32_t rank, int64_t n_fixed, const double* Y, int64_t n, const int64_t* ids,
+                           const int64_t* offsets, const int32_t* partners, const float* ratings, double lambda,
+                           double alpha, int32_t implicit, const double* YtY, double* X);
+/* CoordinateMatrix.toDenseVecMatrix (matrix/CoordinateMatrix.scala:51-64): out (a row-major fp64 view) is zeroed and
+ * gets out(row_pos[e], cols[e]) = values[e] from HOST arrays.  A repeated (row, col) is MB_ERR_INVALID_ARG
+ * "requirement failed: Found duplicate indices: j." before anything is written, as Vectors.sparse fails. */
+int32_t mb_coo_to_dense_rows(mb_ctx* ctx, int64_t nnz, const int32_t* row_pos, const int32_t* cols, const float* values,
+                             mb_block* out);
+
 /* ---- a11: MTUtils.randomDenVecMatrix / randomBlockMatrix input generation
  *      (utils/MTUtils.scala:34-73, rdd/RandomRDD.scala:28-101, utils/RandomDataGenerator.scala:53-65,113-131).
  * Fills `count` consecutive values of partition stream `partition_seed` (one XORShift stream per

@@ -11,12 +11,15 @@
 #include "marlin_b200.h"
 
 #include <algorithm>
+#include <charconv>
+#include <chrono>
 #include <cctype>
 #include <cmath>
 #include <cstdint>
 #include <fstream>
 #include <map>
 #include <memory>
+#include <regex>
 #include <sstream>
 #include <stdexcept>
 #include <string>
@@ -1096,7 +1099,144 @@ inline DistributedVector DenseVecMatrix::multiply(DistributedVector& vector, std
 }
 
 // ---------------------------------------------------------------------------------------------- MTUtils
+// ---- CoordinateMatrix (matrix/CoordinateMatrix.scala) and its ALS (ml/ALSHelp.scala:34-403), one process.  The links and
+//      the initial factors come from the library's host logic; every half-step is one mb_als_update_host call (the
+//      kernel that assembles and Cholesky-solves each entity's normal equations).  Deviations as in DESIGN 3.10. ----
+class CoordinateMatrix {
+public:
+    struct Entry { long row, col; float value; };
+    explicit CoordinateMatrix(std::vector<Entry> entries, long nRows = 0, long nCols = 0)
+        : e_(std::move(entries)), nRows_(nRows), nCols_(nCols) {}
+    const std::vector<Entry>& entries() const { return e_; }
+    long numRows() { size(); return nRows_; }                                          // :42-48
+    long numCols() { size(); return nCols_; }                                          // :35-40
+    DenseMatrix toBreeze() {                                                           // :78-86
+        DenseMatrix m((int)numRows(), (int)numCols());
+        for (const Entry& x : e_) m((int)x.row, (int)x.col) = (double)x.value;
+        return m;
+    }
+    // :51-64 — one row per row id with entries (ascending); a repeated (row, col) fails as Vectors.sparse does
+    DenseVecMatrix toDenseVecMatrix();
+    // :88-98 -> (user factors, product factors): row ids are the user (row) / product (column) ids
+    std::pair<DenseVecMatrix, DenseVecMatrix> ALS(int rank, int iterations, double lambda = 1.0, int numUserBlock = 10,
+                                                  int numProductBlock = 10, bool implicitPrefs = false, double alpha = 1.0,
+                                                  long seed = (long)std::chrono::steady_clock::now().time_since_epoch().count());
+
+private:
+    struct Side {
+        std::vector<int64_t> ids, blockOffsets, offsets;
+        std::vector<int32_t> partners, work;
+        std::vector<float> ratings;
+        long n = 0;
+        Side(const std::vector<int64_t>& ent, const std::vector<int64_t>& partner, const std::vector<float>& vals, int nb, int npb) {
+            const size_t cap = std::max<size_t>(1, ent.size());
+            ids.resize(cap); blockOffsets.resize((size_t)nb + 1); offsets.resize(cap + 1);
+            partners.resize(cap); work.resize(cap); ratings.resize(cap);
+            int64_t count = 0;
+            check(mb_als_links((int64_t)ent.size(), ent.data(), partner.data(), vals.data(), nb, npb, ids.data(), blockOffsets.data(),
+                               offsets.data(), partners.data(), ratings.data(), work.data(), &count));
+            n = (long)count;
+        }
+        std::vector<double> initFactors(long seed, int side, int rank) const {
+            std::vector<double> out((size_t)n * rank);
+            for (size_t b = 0; b + 1 < blockOffsets.size(); ++b)
+                if (blockOffsets[b + 1] > blockOffsets[b])
+                    check(mb_als_init_factors(seed, side, (int32_t)b, rank, blockOffsets[b + 1] - blockOffsets[b],
+                                              out.data() + (size_t)blockOffsets[b] * rank));
+            return out;
+        }
+        // updateBlock (:292-382) for every entity of this side from the other side's factors Y
+        void update(int rank, const std::vector<double>& Y, long nFixed, double lambda, double alpha, bool implicitPrefs,
+                    std::vector<double>& X) const {
+            check(mb_als_update_host(Context::get(), rank, nFixed, Y.data(), n, ids.data(), offsets.data(), partners.data(),
+                                     ratings.data(), lambda, alpha, implicitPrefs ? 1 : 0, nullptr, X.data()));
+        }
+        DenseVecMatrix factors(const std::vector<double>& X, int rank) const;
+    };
+    void size() {                                                                      // computeSize :67-75
+        if (nRows_ > 0 && nCols_ > 0) return;
+        if (e_.empty()) throw std::runtime_error("empty collection");
+        long m = 0, c = 0;
+        for (const Entry& x : e_) { m = std::max(m, x.row); c = std::max(c, x.col); }
+        nRows_ = std::max(nRows_, m + 1);
+        nCols_ = std::max(nCols_, c + 1);
+    }
+    std::vector<Entry> e_;
+    long nRows_, nCols_;
+};
+
+inline DenseVecMatrix CoordinateMatrix::Side::factors(const std::vector<double>& X, int rank) const {
+    std::vector<DenseVecMatrix::Row> rows;
+    for (long p = 0; p < n; ++p) rows.emplace_back((long)ids[p], std::vector<double>(X.begin() + p * rank, X.begin() + (p + 1) * rank));
+    return DenseVecMatrix(rows, 0, rank);
+}
+
+inline DenseVecMatrix CoordinateMatrix::toDenseVecMatrix() {
+    const long n = numCols(), m = numRows();
+    if (n > 2147483647L)
+        throw std::invalid_argument("Cannot convert to a row-oriented format because the number of columns " + std::to_string(n) + " is too large.");
+    std::vector<long> ids;
+    for (const Entry& x : e_) ids.push_back(x.row);
+    std::sort(ids.begin(), ids.end());
+    ids.erase(std::unique(ids.begin(), ids.end()), ids.end());
+    std::vector<int32_t> pos, cols;
+    std::vector<float> vals;
+    for (const Entry& x : e_) {
+        pos.push_back((int32_t)(std::lower_bound(ids.begin(), ids.end(), x.row) - ids.begin()));
+        cols.push_back((int32_t)x.col);
+        vals.push_back(x.value);
+    }
+    SubMatrix shard = SubMatrix::empty((int)n, (int)ids.size()).t();                   // row-major ids x n
+    check(mb_coo_to_dense_rows(Context::get(), (int64_t)pos.size(), pos.data(), cols.data(), vals.data(), shard.handle()));
+    return DenseVecMatrix(ids, shard, m, n);
+}
+
+inline std::pair<DenseVecMatrix, DenseVecMatrix> CoordinateMatrix::ALS(int rank, int iterations, double lambda, int numUserBlock,
+                                                                         int numProductBlock, bool implicitPrefs, double alpha, long seed) {
+    if (rank < 1) throw std::invalid_argument("ALS: rank " + std::to_string(rank) + " must be at least 1");
+    if (rank > MB_ALS_MAX_RANK) throw std::invalid_argument("ALS: rank " + std::to_string(rank) + " is above the kernel's cap");
+    if (!(lambda >= 0.0)) throw std::invalid_argument("ALS: lambda must be non-negative");
+    const int nub = numUserBlock == -1 ? 1 : numUserBlock, npb = numProductBlock == -1 ? 1 : numProductBlock;   // one process
+    if (e_.empty()) throw std::runtime_error("empty collection");
+    std::vector<int64_t> rows, cols;
+    std::vector<float> vals;
+    for (const Entry& x : e_) { rows.push_back(x.row); cols.push_back(x.col); vals.push_back(x.value); }
+    const Side users(rows, cols, vals, nub, npb), products(cols, rows, vals, npb, nub);
+    std::vector<double> U = users.initFactors(seed, 0, rank), P = products.initFactors(seed, 1, rank);
+    for (int it = 0; it < iterations; ++it) {                                          // :77-82
+        products.update(rank, U, users.n, lambda, alpha, implicitPrefs, P);
+        users.update(rank, P, products.n, lambda, alpha, implicitPrefs, U);
+    }
+    return {users.factors(U, rank), products.factors(P, rank)};
+}
+
 struct MTUtils {
+    // utils/MTUtils.scala:228-243 — `row col value [timestamp]`, fields split on `,\s?|\s+`; the value is rounded once to
+    // float32 (std::from_chars, locale-independent, as Float.parseFloat); blank lines are skipped
+    static CoordinateMatrix loadCoordinateMatrix(const std::string& path) {
+        if (!(path.rfind("hdfs://", 0) == 0 || path.rfind("tachyon://", 0) == 0 || path.rfind("/", 0) == 0 || path.rfind("~/", 0) == 0))
+            throw std::invalid_argument("the path is not in local file System, HDFS or Tachyon");
+        std::ifstream in(path);
+        if (!in) throw std::runtime_error("cannot open " + path);
+        static const std::regex sep(",\\s?|\\s+");
+        std::vector<CoordinateMatrix::Entry> entries;
+        std::string line;
+        while (std::getline(in, line)) {
+            if (!line.empty() && line.back() == '\r') line.pop_back();
+            if (line.find_first_not_of(" \t") == std::string::npos) continue;
+            std::vector<std::string> f(std::sregex_token_iterator(line.begin(), line.end(), sep, -1), std::sregex_token_iterator());
+            while (!f.empty() && f.back().empty()) f.pop_back();
+            if (f.size() != 3 && f.size() != 4) throw std::invalid_argument("scala.MatchError: a line of " + std::to_string(f.size()) + " fields");
+            float v = 0.0f;
+            const std::string& s = f[2];
+            const char* b = s.data() + (s.size() && s[0] == '+' ? 1 : 0);
+            const auto r = std::from_chars(b, s.data() + s.size(), v);
+            if (r.ec != std::errc() || r.ptr != s.data() + s.size())
+                throw std::invalid_argument("java.lang.NumberFormatException: For input string: \"" + s + "\"");
+            entries.push_back({std::stol(f[0]), std::stol(f[1]), v});
+        }
+        return CoordinateMatrix(std::move(entries));
+    }
     static std::tuple<int, int, int> splitMethod(long m, long k, long n, int cores) {   // utils/MTUtils.scala:150-175
         int32_t out[3];
         check(mb_choose_split(m, k, n, cores, out));

@@ -13,6 +13,7 @@
 typedef int32_t jint;
 typedef int64_t jlong;
 typedef double jdouble;
+typedef float jfloat;
 typedef uint8_t jboolean;
 typedef jint jsize;
 typedef void* jobject;
@@ -22,6 +23,7 @@ typedef jobject jarray;
 typedef jarray jdoubleArray;
 typedef jarray jintArray;
 typedef jarray jlongArray;
+typedef jarray jfloatArray;
 struct JNINativeInterface_;
 typedef const struct JNINativeInterface_* JNIEnv;
 struct JNINativeInterface_ {
@@ -37,6 +39,9 @@ struct JNINativeInterface_ {
     void (*SetLongArrayRegion)(JNIEnv*, jlongArray, jsize, jsize, const jlong*);
     void (*GetIntArrayRegion)(JNIEnv*, jintArray, jsize, jsize, jint*);
     void (*GetLongArrayRegion)(JNIEnv*, jlongArray, jsize, jsize, jlong*);
+    void (*GetFloatArrayRegion)(JNIEnv*, jfloatArray, jsize, jsize, jfloat*);
+    void (*GetDoubleArrayRegion)(JNIEnv*, jdoubleArray, jsize, jsize, jdouble*);
+    void (*SetDoubleArrayRegion)(JNIEnv*, jdoubleArray, jsize, jsize, const jdouble*);
     const char* (*GetStringUTFChars)(JNIEnv*, jstring, jboolean*);
     void (*ReleaseStringUTFChars)(JNIEnv*, jstring, const char*);
     jstring (*NewStringUTF)(JNIEnv*, const char*);

@@ -200,6 +200,45 @@ NATIVE(void, lrGradient)(JNIEnv* e, jobject o, jlong ctx, jdoubleArray rows, jin
     free(buf);
     raise(e, rc);
 }
+/* ---- CoordinateMatrix.ALS (ml/ALSHelp.scala:292-382): updateBlock for one block on host arrays ---- */
+NATIVE(void, alsUpdateBlock)(JNIEnv* e, jobject o, jlong ctx, jint rank, jdoubleArray y, jlongArray ids, jlongArray offsets,
+                             jintArray partners, jfloatArray ratings, jdouble lambda, jdouble alpha, jboolean implicitPrefs,
+                             jdoubleArray yty, jdoubleArray xOut) {
+    /* y: the received factors, rank doubles per row; ids: the block's entity ids; offsets (ids.length + 1), partners and
+     * ratings: each entity's terms (rows of y) in updateBlock's order; yty: rank x rank or null; xOut: rank doubles per
+     * entity.  The arrays are copied out before the (blocking) device call and the result copied back after it. */
+    const jsize n = (*e)->GetArrayLength(e, ids), ny = (*e)->GetArrayLength(e, y), nnz = (*e)->GetArrayLength(e, partners);
+    if (rank < 1 || ny % rank != 0 || (*e)->GetArrayLength(e, offsets) != n + 1 || (*e)->GetArrayLength(e, ratings) != nnz ||
+        (*e)->GetArrayLength(e, xOut) != (jlong)n * rank || (yty && (*e)->GetArrayLength(e, yty) != rank * rank)) {
+        (*e)->ThrowNew(e, (*e)->FindClass(e, "java/lang/IllegalArgumentException"),
+                       "Dimension mismatch: alsUpdateBlock needs rank doubles per factor row, ids.length + 1 offsets, one rating "
+                       "per partner, rank doubles per entity out and a rank x rank YtY");
+        return;
+    }
+    double* Y = (double*)malloc(sizeof(double) * (size_t)(ny > 0 ? ny : 1));
+    double* X = (double*)malloc(sizeof(double) * (size_t)((jlong)n * rank > 0 ? (jlong)n * rank : 1));
+    double* G = yty ? (double*)malloc(sizeof(double) * (size_t)rank * rank) : NULL;
+    int64_t* I = (int64_t*)malloc(sizeof(int64_t) * (size_t)(n > 0 ? n : 1));
+    int64_t* O = (int64_t*)malloc(sizeof(int64_t) * (size_t)n + sizeof(int64_t));
+    int32_t* P = ints(e, partners);
+    float* R = (float*)malloc(sizeof(float) * (size_t)(nnz > 0 ? nnz : 1));
+    int32_t rc = MB_ERR_OOM;
+    if (Y && X && (G || !yty) && I && O && R) {
+        (*e)->GetDoubleArrayRegion(e, y, 0, ny, Y);
+        if (yty) (*e)->GetDoubleArrayRegion(e, yty, 0, rank * rank, G);
+        (*e)->GetLongArrayRegion(e, ids, 0, n, (jlong*)I);
+        (*e)->GetLongArrayRegion(e, offsets, 0, n + 1, (jlong*)O);
+        (*e)->GetFloatArrayRegion(e, ratings, 0, nnz, R);
+        rc = (n > 0 && O[n] != nnz) ? MB_ERR_DIM_MISMATCH
+                                    : mb_als_update_host(CTX(ctx), rank, ny / rank, Y, n, I, O, P, R, lambda, alpha,
+                                                         implicitPrefs ? 1 : 0, G, X);
+        if (rc == MB_ERR_DIM_MISMATCH && O[n] != nnz)
+            (*e)->ThrowNew(e, (*e)->FindClass(e, "java/lang/IllegalArgumentException"), "alsUpdateBlock: offsets[n] != partners.length");
+        if (rc == MB_OK && n > 0) (*e)->SetDoubleArrayRegion(e, xOut, 0, n * rank, X);
+    }
+    free(Y); free(X); free(G); free(I); free(O); free(P); free(R);
+    raise(e, rc);
+}
 NATIVE(jint, svdMode)(JNIEnv* e, jobject o, jlong n, jint k, jstring mode) {
     const char* m = (*e)->GetStringUTFChars(e, mode, NULL);
     int32_t cm = 0;

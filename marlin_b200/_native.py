@@ -22,6 +22,7 @@ MB_ERR_NO_CONVERGENCE = -8
 
 MB_F64, MB_BF16, MB_F32 = 0, 1, 2
 MB_SVD_LOCAL_LAPACK, MB_SVD_LOCAL_ARPACK, MB_SVD_DIST_ARPACK = 0, 1, 2
+MB_ALS_MAX_RANK = 128
 
 _LIB_PATH = Path(__file__).resolve().parent / "lib" / "libmarlin_b200.so"
 
@@ -87,6 +88,15 @@ SIGNATURES = {
     "mb_svd_rank": (c_i32, [c_dp, c_i32, c_i32, c_f64]),
     "mb_lr_gradient": (c_i32, [c_ctx, c_blk, c_dp, c_dp]),
     "mb_lr_train": (c_i32, [c_ctx, c_blk, c_i64, c_f64, c_i32, c_dp]),
+    "mb_als_links": (c_i32, [c_i64, C.c_void_p, C.c_void_p, C.c_void_p, c_i32, c_i32, C.c_void_p, C.c_void_p, C.c_void_p,
+                             C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(c_i64)]),
+    "mb_als_init_factors": (c_i32, [c_i64, c_i32, c_i32, c_i32, c_i64, C.c_void_p]),
+    "mb_als_normal_equations": (c_i32, [c_ctx, C.c_void_p, c_blk, c_f64, c_f64, c_i32, c_blk, C.c_void_p, C.c_void_p]),
+    "mb_als_update": (c_i32, [c_ctx, C.c_void_p, c_blk, c_f64, c_f64, c_i32, c_blk, c_blk]),
+    "mb_als_train": (c_i32, [c_ctx, C.c_void_p, C.c_void_p, c_i32, c_f64, c_f64, c_i32, c_blk, c_blk]),
+    "mb_als_update_host": (c_i32, [c_ctx, c_i32, c_i64, C.c_void_p, c_i64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                   c_f64, c_f64, c_i32, C.c_void_p, C.c_void_p]),
+    "mb_coo_to_dense_rows": (c_i32, [c_ctx, c_i64, C.c_void_p, C.c_void_p, C.c_void_p, c_blk]),
     "mb_fill_uniform": (c_i32, [c_ctx, c_blk, c_i64, c_i64, c_f64, c_f64, c_i32]),
     "mb_sparse_check": (c_i32, [c_i32, c_i32, C.c_void_p, C.c_void_p]),
     "mb_sparse_wrap": (c_i32, [c_ctx, c_i32, c_i32, c_i64, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(c_sp)]),
@@ -140,6 +150,12 @@ SIGNATURES = {
     "mb_matmul_blocked_dist": (c_i32, [C.c_void_p, C.POINTER(c_blk), C.POINTER(c_i32), C.POINTER(c_blk), C.POINTER(c_i32), c_i32, c_i32,
                                        c_i32, C.POINTER(c_i32), C.POINTER(c_i32), C.POINTER(c_i32), c_i32, C.POINTER(c_blk)]),
 }
+
+
+class AlsSide(C.Structure):
+    """mb_als_side: one side's device-resident ALS links (device pointers)."""
+    _fields_ = [("count", c_i64), ("ids", C.c_void_p), ("offsets", C.c_void_p), ("partners", C.c_void_p),
+                ("ratings", C.c_void_p), ("work", C.c_void_p)]
 
 
 class MarlinError(RuntimeError):

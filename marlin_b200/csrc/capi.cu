@@ -11,8 +11,10 @@
 #include "eigen.h"
 #include "sparse.h"
 #include "logistic.h"
+#include "als.h"
 
 #include <cuda_runtime.h>
+#include <climits>
 #include <algorithm>
 #include <cmath>
 #include <cstdarg>
@@ -1319,6 +1321,252 @@ int32_t mb_lr_train(mb_ctx* ctx, const mb_block* rows, int64_t data_size, double
         ctx->launches += 2;
     }
     MB_CUDA(cudaMemcpyAsync(w_out, b.w, sizeof(double) * b.n, cudaMemcpyDeviceToHost, ctx->stream));
+    MB_CUDA(cudaStreamSynchronize(ctx->stream));
+    return MB_OK;
+}
+
+// ------------------------------------------------------------------------------------------- ALS (CoordinateMatrix.ALS)
+// Row i of a row-major fp64 view (a row shard's transposed view, or a single column) at p + i * ld.
+static int32_t als_rows(const mb_block* b, const char* what, const double** p, long long* ld) {
+    if (!b) return fail(MB_ERR_INVALID_ARG, "ALS: null %s", what);
+    if (b->dtype != MB_F64) return fail(MB_ERR_UNSUPPORTED, "ALS: %s must be fp64", what);
+    if (!b->is_transpose && b->cols != 1) return fail(MB_ERR_UNSUPPORTED, "ALS: %s must be a row-major view", what);
+    *p = f64_ptr(b);
+    *ld = b->is_transpose ? b->ld : 1;
+    return MB_OK;
+}
+
+static int32_t als_check(const mb_als_side* side, int rank, double lambda) {
+    if (!side) return fail(MB_ERR_INVALID_ARG, "ALS: null links");
+    if (rank < 1) return fail(MB_ERR_INVALID_ARG, "ALS: rank %d must be at least 1", rank);
+    if (rank > MB_ALS_MAX_RANK) return fail(MB_ERR_UNSUPPORTED, "ALS: rank %d is above the kernel's cap of %d", rank, MB_ALS_MAX_RANK);
+    if (!(lambda >= 0.0)) return fail(MB_ERR_INVALID_ARG, "ALS: lambda %g must be non-negative", lambda);
+    if (side->count > 0 && (!side->ids || !side->offsets || !side->partners || !side->ratings || !side->work))
+        return fail(MB_ERR_INVALID_ARG, "ALS: null links array");
+    return MB_OK;
+}
+
+static mb::AlsLinks als_links(const mb_als_side* s) {
+    return mb::AlsLinks{s->ids, reinterpret_cast<const long long*>(s->offsets), s->partners, s->ratings, s->work, (long long)s->count};
+}
+
+// YtY for implicit mode: the caller's, or the Gramian of Y into `own` (rank x rank, stream-ordered, freed by the caller)
+static int32_t als_yty(mb_ctx* ctx, const mb_block* Yb, const mb_block* YtY, int rank, double** own, const double** p,
+                       long long* ld) {
+    if (YtY) {
+        if (YtY->dtype != MB_F64 || YtY->rows != rank || YtY->cols != rank)
+            return fail(MB_ERR_DIM_MISMATCH, "ALS: YtY is %dx%d, expected %dx%d fp64", YtY->rows, YtY->cols, rank, rank);
+        *p = f64_ptr(YtY);
+        *ld = YtY->ld;          // symmetric: either storage order reads the same element
+        return MB_OK;
+    }
+    MB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(own), sizeof(double) * rank * rank, ctx->stream));
+    mb_block g;
+    g.data = *own; g.rows = rank; g.cols = rank; g.ld = rank; g.dtype = MB_F64; g.device = ctx->device;
+    const int32_t r = mb_block_gramian(ctx, Yb, &g);
+    if (r) return r;
+    *p = *own;
+    *ld = rank;
+    return MB_OK;
+}
+
+// One half-step on the ctx stream; *bad (device) collects the lowest failing entity id
+static int32_t als_half_step(mb_ctx* ctx, const mb_als_side* side, const mb_block* Yb, double lambda, double alpha,
+                             int32_t implicit, const mb_block* YtY, mb_block* Xb, int* bad) {
+    const double *Y, *X, *yty = nullptr;
+    long long ldy, ldx, ldyty = 0;
+    int32_t r = als_rows(Yb, "fixed-side factors", &Y, &ldy);
+    if (!r) r = als_rows(Xb, "solved-side factors", &X, &ldx);
+    if (r) return r;
+    const int rank = Yb->cols;
+    if (Xb->cols != rank)
+        return fail(MB_ERR_DIM_MISMATCH, "ALS: factors of rank %d and %d", rank, Xb->cols);
+    r = als_check(side, rank, lambda);
+    if (r) return r;
+    double* own = nullptr;
+    if (implicit) r = als_yty(ctx, Yb, YtY, rank, &own, &yty, &ldyty);
+    if (!r) {
+        const cudaError_t e = mb::als_solve(als_links(side), rank, Y, ldy, lambda, alpha, implicit != 0, yty, ldyty,
+                                            const_cast<double*>(X), ldx, bad, ctx->stream);
+        if (e != cudaSuccess) r = cuda_fail(e, "ALS update");
+        else ctx->launches++;
+    }
+    if (own) cudaFreeAsync(own, ctx->stream);
+    return r;
+}
+
+// The pivot flag of the half-steps enqueued since it was set to INT32_MAX
+static int32_t als_pivots(mb_ctx* ctx, int* bad) {
+    MB_CUDA(cudaMemcpyAsync(ctx->int_host, bad, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    MB_CUDA(cudaStreamSynchronize(ctx->stream));
+    if (ctx->int_host[0] != INT_MAX)      // Breeze's inv: MatrixSingularException -> RuntimeException
+        return fail(MB_ERR_CUDA, "ALS: the normal equations of entity %d are not positive definite", ctx->int_host[0]);
+    return MB_OK;
+}
+
+static int32_t als_flag(mb_ctx* ctx, int** bad) {
+    int32_t r = int_scratch(ctx, 8);
+    if (r) return r;
+    *bad = ctx->int_ws;
+    const int init = INT_MAX;
+    MB_CUDA(cudaMemcpyAsync(*bad, &init, sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+    MB_CUDA(cudaStreamSynchronize(ctx->stream));          // `init` lives on this frame
+    return MB_OK;
+}
+
+int32_t mb_als_normal_equations(mb_ctx* ctx, const mb_als_side* side, const mb_block* Yb, double lambda, double alpha,
+                                int32_t implicit, const mb_block* YtY, double* A_out, double* b_out) {
+    MB_CTX(ctx);
+    MB_LOCK(ctx);
+    const double *Y, *yty = nullptr;
+    long long ldy, ldyty = 0;
+    int32_t r = als_rows(Yb, "fixed-side factors", &Y, &ldy);
+    if (r) return r;
+    const int rank = Yb->cols;
+    r = als_check(side, rank, lambda);
+    if (r) return r;
+    if (side->count > 0 && (!A_out || !b_out)) return fail(MB_ERR_INVALID_ARG, "mb_als_normal_equations: null output");
+    double* own = nullptr;
+    if (implicit) r = als_yty(ctx, Yb, YtY, rank, &own, &yty, &ldyty);
+    if (!r) {
+        const cudaError_t e = mb::als_assemble(als_links(side), rank, Y, ldy, lambda, alpha, implicit != 0, yty, ldyty, A_out,
+                                               b_out, ctx->stream);
+        if (e != cudaSuccess) r = cuda_fail(e, "mb_als_normal_equations");
+        else ctx->launches++;
+    }
+    if (own) cudaFreeAsync(own, ctx->stream);
+    if (!r) MB_CUDA(cudaStreamSynchronize(ctx->stream));
+    return r;
+}
+
+int32_t mb_als_update(mb_ctx* ctx, const mb_als_side* side, const mb_block* Y, double lambda, double alpha, int32_t implicit,
+                      const mb_block* YtY, mb_block* X) {
+    MB_CTX(ctx);
+    MB_LOCK(ctx);
+    int* bad = nullptr;
+    int32_t r = als_flag(ctx, &bad);
+    if (!r) r = als_half_step(ctx, side, Y, lambda, alpha, implicit, YtY, X, bad);
+    return r ? r : als_pivots(ctx, bad);
+}
+
+int32_t mb_als_train(mb_ctx* ctx, const mb_als_side* users, const mb_als_side* products, int32_t iterations, double lambda,
+                     double alpha, int32_t implicit, mb_block* U, mb_block* P) {
+    MB_CTX(ctx);
+    MB_LOCK(ctx);
+    if (!U || !P) return fail(MB_ERR_INVALID_ARG, "mb_als_train: null factors");
+    int32_t r = als_check(users, U->cols, lambda);
+    if (!r) r = als_check(products, P->cols, lambda);
+    if (r || iterations <= 0) return r;
+    int* bad = nullptr;
+    r = als_flag(ctx, &bad);
+    for (int it = 0; it < iterations && !r; ++it) {
+        r = als_half_step(ctx, products, U, lambda, alpha, implicit, nullptr, P, bad);      // products from the users
+        if (!r) r = als_half_step(ctx, users, P, lambda, alpha, implicit, nullptr, U, bad); // then users from the products
+    }
+    return r ? r : als_pivots(ctx, bad);
+}
+
+// Device copies of host arrays, stream-ordered, freed by the destructor
+struct AlsUpload {
+    std::vector<void*> bufs;
+    cudaStream_t st;
+    explicit AlsUpload(cudaStream_t s) : st(s) {}
+    ~AlsUpload() { for (void* b : bufs) cudaFreeAsync(b, st); }
+    cudaError_t put(const void* host, size_t bytes, void* dev_ptr_out) {
+        void* d = nullptr;
+        cudaError_t e = cudaMallocAsync(&d, bytes ? bytes : 8, st);
+        if (e != cudaSuccess) return e;
+        bufs.push_back(d);
+        *static_cast<void**>(dev_ptr_out) = d;
+        return bytes ? cudaMemcpyAsync(d, host, bytes, cudaMemcpyHostToDevice, st) : cudaSuccess;
+    }
+};
+
+int32_t mb_als_update_host(mb_ctx* ctx, int32_t rank, int64_t n_fixed, const double* Y, int64_t n, const int64_t* ids,
+                           const int64_t* offsets, const int32_t* partners, const float* ratings, double lambda,
+                           double alpha, int32_t implicit, const double* YtY, double* X) {
+    MB_CTX(ctx);
+    MB_LOCK(ctx);
+    if (n < 0 || n_fixed < 0 || (n > 0 && (!ids || !offsets || !X)) || (n_fixed > 0 && !Y) || (n > 0 && offsets[n] > 0 && (!partners || !ratings)))
+        return fail(MB_ERR_INVALID_ARG, "mb_als_update_host: bad argument");
+    if (n == 0) return MB_OK;
+    const mb_als_side none{};
+    int32_t r = als_check(&none, rank, lambda);
+    if (r) return r;
+    if (n > INT32_MAX) return fail(MB_ERR_UNSUPPORTED, "mb_als_update_host: %lld entities", (long long)n);
+    if (offsets[0] != 0) return fail(MB_ERR_INVALID_ARG, "mb_als_update_host: offsets[0] is %lld, not 0", (long long)offsets[0]);
+    for (int64_t p = 0; p < n; ++p)
+        if (offsets[p + 1] < offsets[p])
+            return fail(MB_ERR_INVALID_ARG, "mb_als_update_host: offsets decrease at entity %lld", (long long)p);
+    const int64_t nnz = offsets[n];
+    for (int64_t q = 0; q < nnz; ++q)
+        if (partners[q] < 0 || partners[q] >= n_fixed)
+            return fail(MB_ERR_INVALID_ARG, "mb_als_update_host: partner %d outside the %lld fixed rows", partners[q], (long long)n_fixed);
+    std::vector<int32_t> ids32(n), work(n);
+    for (int64_t p = 0; p < n; ++p) {
+        if (ids[p] < 0 || ids[p] > INT32_MAX) return fail(MB_ERR_INVALID_ARG, "ALS: id %lld is outside [0, 2147483647]", (long long)ids[p]);
+        ids32[p] = int32_t(ids[p]);
+        work[p] = int32_t(p);
+    }
+    std::stable_sort(work.begin(), work.end(), [&](int32_t a, int32_t b) { return offsets[a + 1] - offsets[a] > offsets[b + 1] - offsets[b]; });
+    AlsUpload up(ctx->stream);
+    mb_als_side side{n, nullptr, nullptr, nullptr, nullptr, nullptr};
+    int32_t *d_ids, *d_partners, *d_work;
+    int64_t* d_off;
+    float* d_r;
+    double *d_y, *d_x, *d_yty = nullptr;
+    MB_CUDA(up.put(ids32.data(), sizeof(int32_t) * n, &d_ids));
+    MB_CUDA(up.put(offsets, sizeof(int64_t) * (n + 1), &d_off));
+    MB_CUDA(up.put(partners, sizeof(int32_t) * nnz, &d_partners));
+    MB_CUDA(up.put(ratings, sizeof(float) * nnz, &d_r));
+    MB_CUDA(up.put(work.data(), sizeof(int32_t) * n, &d_work));
+    MB_CUDA(up.put(Y, sizeof(double) * n_fixed * rank, &d_y));
+    MB_CUDA(up.put(X, sizeof(double) * n * rank, &d_x));
+    if (YtY) MB_CUDA(up.put(YtY, sizeof(double) * rank * rank, &d_yty));
+    side.ids = d_ids; side.offsets = d_off; side.partners = d_partners; side.ratings = d_r; side.work = d_work;
+    mb_block yb, xb, gb;
+    yb.data = d_y; yb.rows = (int)n_fixed; yb.cols = rank; yb.ld = rank; yb.is_transpose = 1; yb.dtype = MB_F64; yb.device = ctx->device;
+    xb = yb; xb.data = d_x; xb.rows = (int)n;
+    gb = yb; gb.data = d_yty; gb.rows = rank;
+    r = mb_als_update(ctx, &side, &yb, lambda, alpha, implicit, YtY ? &gb : nullptr, &xb);
+    if (r) return r;
+    MB_CUDA(cudaMemcpyAsync(X, d_x, sizeof(double) * n * rank, cudaMemcpyDeviceToHost, ctx->stream));
+    MB_CUDA(cudaStreamSynchronize(ctx->stream));
+    return MB_OK;
+}
+
+int32_t mb_coo_to_dense_rows(mb_ctx* ctx, int64_t nnz, const int32_t* row_pos, const int32_t* cols, const float* values,
+                             mb_block* out) {
+    MB_CTX(ctx);
+    MB_LOCK(ctx);
+    const double* p;
+    long long ld;
+    int32_t r = als_rows(out, "toDenseVecMatrix output", &p, &ld);
+    if (r) return r;
+    if (nnz < 0 || (nnz > 0 && (!row_pos || !cols || !values))) return fail(MB_ERR_INVALID_ARG, "mb_coo_to_dense_rows: bad argument");
+    std::vector<int64_t> keys((size_t)nnz);
+    for (int64_t e = 0; e < nnz; ++e) {
+        if (row_pos[e] < 0 || row_pos[e] >= out->rows || cols[e] < 0 || cols[e] >= out->cols)
+            return fail(MB_ERR_INVALID_ARG, "toDenseVecMatrix: entry (%d, %d) is outside the %dx%d rows", row_pos[e], cols[e],
+                        out->rows, out->cols);
+        keys[e] = (int64_t)row_pos[e] * out->cols + cols[e];
+    }
+    std::sort(keys.begin(), keys.end());
+    for (size_t e = 1; e < keys.size(); ++e)      // Vectors.sparse (matrix/Vectors.scala:92-104)
+        if (keys[e] == keys[e - 1])
+            return fail(MB_ERR_INVALID_ARG, "requirement failed: Found duplicate indices: %lld.", (long long)(keys[e] % out->cols));
+    if (ld == out->cols || out->rows == 1)
+        MB_CUDA(cudaMemsetAsync(const_cast<double*>(p), 0, sizeof(double) * out->rows * out->cols, ctx->stream));
+    else
+        MB_CUDA(cudaMemset2DAsync(const_cast<double*>(p), sizeof(double) * ld, 0, sizeof(double) * out->cols, out->rows, ctx->stream));
+    AlsUpload up(ctx->stream);
+    int32_t *d_row, *d_col;
+    float* d_val;
+    MB_CUDA(up.put(row_pos, sizeof(int32_t) * nnz, &d_row));
+    MB_CUDA(up.put(cols, sizeof(int32_t) * nnz, &d_col));
+    MB_CUDA(up.put(values, sizeof(float) * nnz, &d_val));
+    MB_CUDA(mb::coo_scatter_rows(nnz, d_row, d_col, d_val, const_cast<double*>(p), ld, ctx->stream));
+    ctx->launches++;
     MB_CUDA(cudaStreamSynchronize(ctx->stream));
     return MB_OK;
 }

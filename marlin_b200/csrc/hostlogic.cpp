@@ -2,9 +2,11 @@
 // Each function cites the reference code it mirrors (src/main/scala/edu/nju/pasalab/marlin/...).
 #include "../../include/marlin_b200.h"
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstdint>
 #include <cstring>
+#include <vector>
 
 namespace {
 
@@ -57,6 +59,80 @@ uint32_t mm3_bytes_hash(const uint8_t* data, int len, uint32_t seed) {
     }
     return mm3_finalize(h, uint32_t(len));
 }
+
+// java.lang.StrictMath.log (fdlibm e_log.c) for positive normal x, the only inputs nextGaussian gives it.  The C library's
+// log differs from it in the last bit for some inputs (Random(42).nextGaussian() is one), and the JVM's factors are these.
+double fdlibm_log(double x) {
+    const double ln2_hi = 6.93147180369123816490e-01, ln2_lo = 1.90821492927058770002e-10;
+    const double Lg1 = 6.666666666666735130e-01, Lg2 = 3.999999999940941908e-01, Lg3 = 2.857142874366239149e-01,
+                 Lg4 = 2.222219843214978396e-01, Lg5 = 1.818357216161805012e-01, Lg6 = 1.531383769920937332e-01,
+                 Lg7 = 1.479819860511658591e-01;
+    uint64_t bits;
+    std::memcpy(&bits, &x, 8);
+    int32_t hx = int32_t(bits >> 32);
+    int32_t k = (hx >> 20) - 1023;
+    hx &= 0x000fffff;
+    int32_t i = (hx + 0x95f64) & 0x100000;
+    bits = (uint64_t(uint32_t(hx | (i ^ 0x3ff00000))) << 32) | (bits & 0xffffffffull);   // x or x / 2 normalised
+    std::memcpy(&x, &bits, 8);
+    k += i >> 20;
+    const double f = x - 1.0, dk = double(k);
+    if ((0x000fffff & (2 + hx)) < 3) {
+        if (f == 0.0) return k == 0 ? 0.0 : dk * ln2_hi + dk * ln2_lo;
+        const double R = f * f * (0.5 - 0.33333333333333333 * f);
+        return k == 0 ? f - R : dk * ln2_hi - ((R - dk * ln2_lo) - f);
+    }
+    const double s = f / (2.0 + f), z = s * s, w = z * z;
+    i = hx - 0x6147a;
+    const int32_t j = 0x6b851 - hx;
+    const double t1 = w * (Lg2 + w * (Lg4 + w * Lg6));
+    const double t2 = z * (Lg1 + w * (Lg3 + w * (Lg5 + w * Lg7)));
+    i |= j;
+    const double R = t2 + t1;
+    if (i > 0) {
+        const double hfsq = 0.5 * f * f;
+        return k == 0 ? f - (hfsq - s * (hfsq + R)) : dk * ln2_hi - ((hfsq - (s * (hfsq + R) + dk * ln2_lo)) - f);
+    }
+    return k == 0 ? f - s * (f - R) : dk * ln2_hi - ((s * (f - R) - dk * ln2_lo) - f);
+}
+
+// java.util.Random: the 48-bit LCG, next(bits), nextInt(), nextDouble() and nextGaussian() with its cached second value
+struct JavaRandom {
+    uint64_t s;
+    bool have_next = false;
+    double next_next = 0.0;
+    explicit JavaRandom(int64_t seed) : s((uint64_t(seed) ^ 0x5DEECE66Dull) & ((1ull << 48) - 1)) {}
+    int32_t next(int bits) {
+        s = (s * 0x5DEECE66Dull + 0xBull) & ((1ull << 48) - 1);
+        return int32_t(int64_t(s) >> (48 - bits));
+    }
+    double next_double() { return double((int64_t(next(26)) << 27) + next(27)) * 0x1.0p-53; }
+    double next_gaussian() {
+        if (have_next) {
+            have_next = false;
+            return next_next;
+        }
+        double v1, v2, q;
+        do {
+            v1 = 2 * next_double() - 1;
+            v2 = 2 * next_double() - 1;
+            q = v1 * v1 + v2 * v2;
+        } while (q >= 1 || q == 0);
+        const double multiplier = std::sqrt(-2 * fdlibm_log(q) / q);
+        next_next = v2 * multiplier;
+        have_next = true;
+        return v1 * multiplier;
+    }
+};
+
+// scala.util.hashing.byteswap32: v * 0x9e3775cd, Integer.reverseBytes, * 0x9e3775cd (Int arithmetic, wrapping)
+int32_t byteswap32(int32_t v) {
+    uint32_t hc = uint32_t(v) * 0x9e3775cdu;
+    hc = (hc >> 24) | ((hc >> 8) & 0xff00u) | ((hc << 8) & 0xff0000u) | (hc << 24);
+    return int32_t(hc * 0x9e3775cdu);
+}
+
+int32_t hash_block(int64_t id, int32_t n) { return int32_t(id % n); }   // HashPartitioner on a non-negative Int
 
 }  // namespace
 
@@ -224,6 +300,87 @@ int32_t mb_svd_rank(const double* sigmas, int32_t count, int32_t k, double rcond
     int32_t i = 0;
     while (i < std::min(k, count) && sigmas[i] >= threshold) ++i;
     return i;
+}
+
+// ml/ALSHelp.scala:34-58,101-165 (ratings keyed by block with HashPartitioner, makeOutLinkBlock / makeInLinkBlock, the
+// grouping and sorting of updateBlock's loop at :319-357), for the side whose ids are ent[]:
+//   positions: block 0's distinct ids ascending, then block 1's, ...  (block = id mod num_blocks)
+//   a position's terms: partner block ascending, partner id ascending, then input order -- i.e. the partner's position on
+//   the other side ascending, ties in input order
+//   work list: positions by rating count descending, ties by position
+int32_t mb_als_links(int64_t nnz, const int64_t* ent, const int64_t* partner, const float* values, int32_t num_blocks,
+                     int32_t num_partner_blocks, int64_t* ids_out, int64_t* block_offsets_out, int64_t* offsets_out,
+                     int32_t* partners_out, float* ratings_out, int32_t* work_out, int64_t* count_out) {
+    if (nnz < 0 || num_blocks < 1 || num_partner_blocks < 1 || !count_out || !block_offsets_out || !offsets_out ||
+        (nnz > 0 && (!ent || !partner || !values || !ids_out || !partners_out || !ratings_out || !work_out)))
+        return mb_fail(MB_ERR_INVALID_ARG, "mb_als_links: bad argument");
+    if (nnz > INT32_MAX) return mb_fail(MB_ERR_UNSUPPORTED, "mb_als_links: %lld ratings (at most 2^31 - 1)", (long long)nnz);
+    for (int64_t e = 0; e < nnz; ++e)
+        for (int64_t id : {ent[e], partner[e]})
+            if (id < 0 || id > INT32_MAX)
+                return mb_fail(MB_ERR_INVALID_ARG, "ALS: id %lld of entry %lld is outside [0, 2147483647]", (long long)id,
+                               (long long)e);
+    // positions of both sides: distinct ids ordered by (block, id), as one monotone key (block << 31 | id)
+    auto keyed = [nnz](const int64_t* ids, int32_t nb) {
+        std::vector<int64_t> k((size_t)nnz);
+        for (int64_t e = 0; e < nnz; ++e) k[e] = (int64_t(hash_block(ids[e], nb)) << 31) | ids[e];
+        return k;
+    };
+    const std::vector<int64_t> ekey = keyed(ent, num_blocks), pkey = keyed(partner, num_partner_blocks);
+    auto distinct = [](std::vector<int64_t> v) {
+        std::sort(v.begin(), v.end());
+        v.erase(std::unique(v.begin(), v.end()), v.end());
+        return v;
+    };
+    const std::vector<int64_t> mine = distinct(ekey), theirs = distinct(pkey);
+    // (entity position, partner position, input index): sorting these is the stable sort by the first two
+    std::vector<std::pair<uint64_t, int32_t>> terms((size_t)nnz);
+    for (int64_t e = 0; e < nnz; ++e) {
+        const uint64_t ep = uint64_t(std::lower_bound(mine.begin(), mine.end(), ekey[e]) - mine.begin());
+        const uint64_t pp = uint64_t(std::lower_bound(theirs.begin(), theirs.end(), pkey[e]) - theirs.begin());
+        terms[e] = {(ep << 32) | pp, int32_t(e)};
+    }
+    std::sort(terms.begin(), terms.end());
+    const int64_t n = int64_t(mine.size());
+    std::fill(offsets_out, offsets_out + n + 1, 0);
+    for (int64_t q = 0; q < nnz; ++q) {
+        offsets_out[(terms[q].first >> 32) + 1]++;
+        partners_out[q] = int32_t(terms[q].first & 0xffffffffu);
+        ratings_out[q] = values[terms[q].second];
+    }
+    for (int64_t p = 0; p < n; ++p) offsets_out[p + 1] += offsets_out[p];
+    std::fill(block_offsets_out, block_offsets_out + num_blocks + 1, 0);
+    for (int64_t p = 0; p < n; ++p) {
+        ids_out[p] = mine[p] & INT32_MAX;
+        block_offsets_out[(mine[p] >> 31) + 1]++;
+        work_out[p] = int32_t(p);
+    }
+    for (int32_t b = 0; b < num_blocks; ++b) block_offsets_out[b + 1] += block_offsets_out[b];
+    std::stable_sort(work_out, work_out + n, [&](int32_t a, int32_t b) {
+        return offsets_out[a + 1] - offsets_out[a] > offsets_out[b + 1] - offsets_out[b];
+    });
+    *count_out = n;
+    return MB_OK;
+}
+
+// ml/ALSHelp.scala:60-74,170-179: seed1 / seed2 are the first two nextInt() of Random(seed); block b of the users (side 0)
+// or products (side 1) draws from Random(byteswap32(seed1 or seed2 ^ b)), and its p-th position gets the p-th
+// randomFactor: rank draws of |nextGaussian()| over the square root of their in-order sum of squares.
+int32_t mb_als_init_factors(int64_t seed, int32_t side, int32_t block, int32_t rank, int64_t count, double* out) {
+    if ((side != 0 && side != 1) || block < 0 || rank < 1 || count < 0 || (count > 0 && !out))
+        return mb_fail(MB_ERR_INVALID_ARG, "mb_als_init_factors: bad argument");
+    JavaRandom gen(seed);
+    const int32_t seed1 = gen.next(32), seed2 = gen.next(32);
+    JavaRandom rand(int64_t(byteswap32((side == 0 ? seed1 : seed2) ^ block)));
+    for (int64_t p = 0; p < count; ++p) {
+        double* f = out + p * rank;
+        double sum = 0.0;
+        for (int32_t i = 0; i < rank; ++i) f[i] = std::fabs(rand.next_gaussian());
+        for (int32_t i = 0; i < rank; ++i) sum += f[i] * f[i];
+        const double norm = std::sqrt(sum);
+        for (int32_t i = 0; i < rank; ++i) f[i] = f[i] / norm;
+    }
+    return MB_OK;
 }
 
 }  // extern "C"

@@ -11,6 +11,7 @@ import math
 import os
 import re
 import time
+from fractions import Fraction
 from typing import List, Optional, Sequence, Tuple
 
 import numpy as np
@@ -20,6 +21,7 @@ from .. import _native as nat
 from .. import comm
 from ..matrix.block import BlockID
 from ..matrix.block_matrix import BlockMatrix
+from ..matrix.coordinate_matrix import CoordinateMatrix
 from ..matrix.dense_vec_matrix import DenseVecMatrix
 from ..matrix.sparse_matrix import SparseBlock, column_count
 from ..matrix.sub_matrix import SubMatrix
@@ -54,6 +56,38 @@ def _jdouble(v: float) -> str:
             whole, frac = "0", "0" * (-lead - 1) + digits
         return f"{neg}{whole}.{frac}"
     return f"{neg}{digits[0]}.{digits[1:] or '0'}E{lead}"
+
+
+# java.lang.Float.valueOf's decimal syntax (FloatingDecimal): optional sign, digits with an optional point, an optional
+# exponent, an optional f / F / d / D suffix; or NaN / Infinity
+_JFLOAT = re.compile(r"[+-]?(NaN|Infinity|((\d+\.?\d*|\.\d+)([eE][+-]?\d+)?)[fFdD]?)")
+_F32_MAX_HALF_UP = Fraction(2 ** 128 - 2 ** 103, 1)      # float32 max + half an ulp: from here the value rounds to infinity
+
+
+def _parse_float32(s: str) -> np.float32:
+    """java.lang.Float.parseFloat: the decimal string rounded once, to nearest even, to float32.  Exact rational arithmetic,
+    so it depends on no locale; going through a double (float(s), np.float32(s)) rounds twice and can land one float32 ulp
+    off ("1.00000005960464477550" gives 1.0 that way, 1.0000001192092896 correctly)."""
+    t = s.strip()
+    m = _JFLOAT.fullmatch(t)
+    if not m:
+        raise nat.MarlinArgumentError(nat.MB_ERR_INVALID_ARG, f"java.lang.NumberFormatException: For input string: \"{s}\"")
+    neg = t.startswith("-")
+    if m.group(1) == "NaN":
+        return np.float32("nan")
+    if m.group(1) == "Infinity":
+        return np.float32("-inf" if neg else "inf")
+    q = abs(Fraction(m.group(2)))
+    if q >= _F32_MAX_HALF_UP:
+        v = np.float32("inf")
+    else:
+        # float32(float(q)) is within one float32 ulp of the correctly rounded value: pick the nearest of it and its two
+        # neighbours, ties to the even significand
+        c = np.float32(float(q))
+        cands = [np.nextafter(c, np.float32(0)), c, np.nextafter(c, np.float32("inf"))]
+        v = min((x for x in cands if np.isfinite(x)),
+                key=lambda x: (abs(Fraction(float(x)) - q), int(np.array(x).view(np.uint32)) & 1))
+    return np.float32(-v) if neg else np.float32(v)
 
 
 def _check_path(path: str) -> None:
@@ -275,6 +309,34 @@ class MTUtils:
                 body = body[len("DenseVector("):-1]
             rows.append((int(head), np.array([float(t) for t in _SEP.split(body) if t != ""], dtype=np.float64)))
         return DenseVecMatrix(rows)
+
+    @staticmethod
+    def loadCoordinateMatrix(sc, path: str, minPartitions: int = 4) -> CoordinateMatrix:
+        """utils/MTUtils.scala:228-243 — `row col value` or `row col value timestamp` (MovieLens), fields split on
+        `,\\s?|\\s+`; the timestamp is ignored.  value.toFloat rounds the decimal string once, straight to float32
+        (Float.parseFloat, C strtof), not through a double.  Lines are dealt to ranks in contiguous chunks; blank lines are
+        skipped; any other field count is rejected (a MatchError on the JVM)."""
+        _check_path(path)
+        files = [path] if os.path.isfile(path) else sorted(os.path.join(path, f) for f in os.listdir(path)
+                                                           if not f.startswith((".", "_")))
+        lines = []
+        for f in files:
+            with open(f) as fh:
+                lines.extend(l.rstrip("\r\n") for l in fh if l.strip())
+        rank, ws = world()
+        n = len(lines)
+        lo, hi = (rank * n) // ws, ((rank + 1) * n) // ws
+        rows, cols, vals = [], [], []
+        for line in lines[lo:hi]:
+            fields = _SEP.split(line)
+            while fields and fields[-1] == "":             # java.lang.String.split drops trailing empty strings
+                fields.pop()
+            if len(fields) not in (3, 4):
+                raise nat.MarlinArgumentError(nat.MB_ERR_INVALID_ARG, f"scala.MatchError: a line of {len(fields)} fields: {line!r}")
+            rows.append(int(fields[0]))
+            cols.append(int(fields[1]))
+            vals.append(_parse_float32(fields[2]))
+        return CoordinateMatrix((np.array(rows, np.int64), np.array(cols, np.int64), np.array(vals, np.float32)))
 
     @staticmethod
     def loadSVMDenVecMatrix(sc, path: str, vectorLen: int, minPartitions: int = 4) -> DenseVecMatrix:

@@ -60,6 +60,13 @@ object Native {
   // row-major in `rows` (column 0 = label); the rows live on the device only for the duration of the call
   @native def lrGradient(ctx: Long, rows: Array[Double], numRows: Int, w: Array[Double], gradOut: Array[Double]): Unit
 
+  // CoordinateMatrix.ALS: updateBlock of one block.  y holds the received factor rows (rank doubles each); the block's
+  // entities (ids) have the terms [offsets(u), offsets(u + 1)) of partners (rows of y) and ratings; yty (rank x rank) is
+  // required for implicitPrefs (null otherwise); xOut gets rank doubles per entity
+  @native def alsUpdateBlock(ctx: Long, rank: Int, y: Array[Double], ids: Array[Long], offsets: Array[Long], partners: Array[Int],
+                             ratings: Array[Float], lambda: Double, alpha: Double, implicitPrefs: Boolean, yty: Array[Double],
+                             xOut: Array[Double]): Unit
+
   // sparse blocks: a CSC block in HBM (SparseMatrix / LibMatrixMult / SparseMatrix.rand on the device)
   @native def sparseUpload(ctx: Long, rows: Int, cols: Int, colptr: Array[Int], rowidx: Array[Int],
                            values: Array[Double]): Long
