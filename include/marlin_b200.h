@@ -361,6 +361,50 @@ int32_t mb_sparse_column_count(int32_t rows, int32_t cols, double density, int32
  * exactly s sorted rows, every s-subset equally likely.  rows * cols draws per block whatever the density. */
 int32_t mb_fill_sparse_uniform(mb_ctx* ctx, mb_sparse* S, int64_t partition_seed);
 
+/* ---- SparseVecMatrix (matrix/SparseVecMatrix.scala).  A row shard (nloc rows of nCols columns) is CSR, held as the
+ *      CSC handle of its transpose: an mb_sparse with rows = nCols and cols = nloc, whose colptr is the row pointer array
+ *      and whose rowidx holds each row's column ids, strictly increasing (mb_sparse_check applies unchanged).
+ *      toDenseVecMatrix (:56-65) is mb_sparse_to_dense into the transposed view of a row-major shard. ---- */
+/* Row bins of mb_spvec_multiply by a row's product count u = sum over its stored k of nnz(B(k, :)): u <= WARP_BOUND is
+ * one warp with a shared-memory hash, u <= CTA_BOUND one CTA with a larger hash, anything above one CTA walking windows
+ * of MB_SPVEC_WINDOW columns.  The bin never changes a result. */
+#define MB_SPVEC_WARP_BOUND 256
+#define MB_SPVEC_CTA_BOUND  4096
+#define MB_SPVEC_WINDOW     16384
+/* multiplySparse (:22-50): C = A * B row by row.  A: the shard of A (handle rows = A.nCols), B: all of B laid out as one CSR
+ * over row ids [0, B.nRows) (handle cols = B.nRows).  *out receives a new library-owned handle of C's rows in the same
+ * form (rows = B.nCols, cols = A's local rows), columns ascending within each row; free it with mb_sparse_free.
+ * Arithmetic: a = (float)A(i,k), b = (float)B(k,j), p = a * b in float32; C(i,j) is the first product of the row's k order
+ * (A's stored order, k ascending), every later one added in float32, separately rounded, no flush to zero.  Entries are
+ * the structural product: every (i, j) with at least one k stored on both sides, stored zeros and cancellations included.
+ * The float32 results are stored widened to double in the values array (exact), so mb_sparse_download, mb_sparse_to_dense
+ * and mb_sparse_free apply unchanged.  A.nCols != B.nRows is MB_ERR_DIM_MISMATCH (the reference drops the unmatched k);
+ * more than 2^31 - 1 output entries is MB_ERR_UNSUPPORTED naming the count.  Synchronises the stream twice (bin sizes,
+ * total count). */
+int32_t mb_spvec_multiply(mb_ctx* ctx, const mb_sparse* A, const mb_sparse* B, mb_sparse** out);
+/* The same product on HOST CSR arrays, for callers holding rows on the host (the JVM, the C++ mirror): A is a_rows rows of
+ * k columns (a_rowptr[a_rows + 1], a_colidx, a_values), B is k rows of n columns (absent row ids empty).  Both are checked
+ * as mb_sparse_upload checks a block (MB_ERR_INVALID_ARG on unsorted or repeated columns).  Uploads, multiplies and frees
+ * the inputs; *out receives a library-owned handle of C's rows as from mb_spvec_multiply.  Blocking. */
+int32_t mb_spvec_multiply_host(mb_ctx* ctx, int32_t a_rows, int32_t k, const int32_t* a_rowptr, const int32_t* a_colidx,
+                               const double* a_values, int32_t n, const int32_t* b_rowptr, const int32_t* b_colidx,
+                               const double* b_values, mb_sparse** out);
+/* The entries of a row handle (from mb_spvec_multiply / _host) as HOST COO arrays of nnz elements (mb_sparse_info): the
+ * local row position, the column and the float32 value, rows ascending and columns ascending within a row.  Blocking. */
+int32_t mb_spvec_coo(mb_ctx* ctx, const mb_sparse* C, int32_t* rows_out, int32_t* cols_out, float* values_out);
+/* DenseVecMatrix.toSparseVecMatrix (DenseVecMatrix.scala:1333-1353): the rows of an fp64 view (one matrix row per shard
+ * row, any ld) to a new library-owned handle (rows = view cols, cols = view rows) keeping the entries v != 0.0 in column
+ * order: NaN is kept, +-0.0 dropped.  Blocking (one synchronisation to size the result). */
+int32_t mb_dense_rows_to_sparse(mb_ctx* ctx, const mb_block* rows, mb_sparse** out);
+/* randomSpaVecMatrix (utils/MTUtils.scala:75-85, rdd/RandomRDD.scala:136-159) for one partition of P rows: S (rows =
+ * nColumns, cols = P, nnz = s * P with s from mb_sparse_column_count(nColumns, nColumns, density)) gets
+ *   values: positions [0, s*P) of the partition's XORShift stream as U[lo, hi) (row r takes [r*s, (r+1)*s)), bit-identical
+ *           to randomDenVecMatrix's stream for the same partition seed;
+ *   columns: ONE sorted set of s distinct columns shared by all P rows, as in the reference, drawn by selection sampling
+ *           (mb_fill_sparse_uniform's sampler) over positions [s*P, s*P + nColumns) of the same stream.
+ * The reference draws the set from an unseeded java.util.Random; here it is a function of (seed, partition). */
+int32_t mb_fill_spvec_uniform(mb_ctx* ctx, mb_sparse* S, int64_t partition_seed, double lo, double hi);
+
 /* ---- a7/a8: strategy + partitioning (pure integer logic) --------------------------------- */
 /* MTUtils.splitMethod(m,k,n,cores) (utils/MTUtils.scala:150-175, dimToSplit :204-213) */
 int32_t mb_choose_split(int64_t m, int64_t k, int64_t n, int32_t cores, int32_t out_mkn[3]);

@@ -340,6 +340,7 @@ struct LibMatrixMult {
 
 class DenseVecMatrix;
 class DistributedVector;
+class SparseVecMatrix;
 
 // ---------------------------------------------------------------------------------------------- BlockMatrix
 class BlockMatrix {
@@ -670,6 +671,8 @@ public:
     DenseVecMatrix(std::vector<long> ids, SubMatrix data, long nRows, long nCols) : ids_(std::move(ids)), data_(std::move(data)), nRows_(nRows), nCols_(nCols) {}
 
     long numCols() { if (nCols_ <= 0) { if (ids_.empty()) throw std::runtime_error("empty collection"); nCols_ = data_.cols(); } return nCols_; }   // :55-61
+    // :1333-1353 — the entries != 0.0 of each row (NaN kept, +-0.0 dropped) on the device (mb_dense_rows_to_sparse)
+    SparseVecMatrix toSparseVecMatrix();
     long numRows() { if (nRows_ <= 0) { if (ids_.empty()) throw std::runtime_error("empty collection"); nRows_ = *std::max_element(ids_.begin(), ids_.end()) + 1; } return nRows_; }  // :63-69
     const std::vector<long>& rowIds() const { return ids_; }
     const SubMatrix& shard() const { return data_; }
@@ -1210,6 +1213,117 @@ inline std::pair<DenseVecMatrix, DenseVecMatrix> CoordinateMatrix::ALS(int rank,
     return {users.factors(U, rank), products.factors(P, rank)};
 }
 
+// ---- SparseVecMatrix (matrix/SparseVecMatrix.scala), one process: rows on the host, each product one
+//      mb_spvec_multiply_host call (the row-wise float32 SpGEMM).  Deviations as in DESIGN 3.11. ----
+class SparseVecMatrix {
+public:
+    struct Row { long id; std::vector<int32_t> indices; std::vector<double> values; };
+    // Ids must lie in [0, nRows) and appear once; columns are checked (sorted, distinct, < nCols) by the library.
+    SparseVecMatrix(std::vector<Row> rows, long nRows, long nCols) : rows_(std::move(rows)), nRows_(nRows), nCols_(nCols) {
+        if (nRows < 0 || nCols < 0 || nCols > 2147483647L) throw std::invalid_argument("SparseVecMatrix: bad dimensions");
+        std::vector<long> ids;
+        for (const Row& r : rows_) {
+            if (r.id < 0 || r.id >= nRows) throw std::invalid_argument("SparseVecMatrix: row id " + std::to_string(r.id) + " is outside [0, " + std::to_string(nRows) + ")");
+            if (r.indices.size() != r.values.size()) throw std::invalid_argument("SparseVecMatrix: indices and values differ in length");
+            ids.push_back(r.id);
+        }
+        std::sort(ids.begin(), ids.end());
+        for (size_t i = 1; i < ids.size(); ++i)
+            if (ids[i] == ids[i - 1]) throw std::invalid_argument("SparseVecMatrix: repeated row id " + std::to_string(ids[i]));
+    }
+    long nRows() const { return nRows_; }
+    long nCols() const { return nCols_; }
+    const std::vector<Row>& rows() const { return rows_; }
+    long elementsCount() const { return (long)rows_.size(); }                            // :67-69: rows.count()
+    // :22-50 -> CoordinateMatrix(entries, nRows, other.nCols), float32 values summed in this row's stored order
+    CoordinateMatrix multiplySparse(const SparseVecMatrix& other) const {
+        if (nCols_ != other.nRows_)
+            throw std::invalid_argument("multiplySparse: this.nCols " + std::to_string(nCols_) + " does not match other.nRows " + std::to_string(other.nRows_));
+        std::vector<int32_t> arp, aci, brp((size_t)other.nRows_ + 1, 0), bci;
+        std::vector<double> ava, bva;
+        csr(rows_, arp, aci, ava);
+        std::vector<const Row*> byId((size_t)other.nRows_, nullptr);                     // B over ids [0, nRows), absent ids empty
+        for (const Row& r : other.rows_) byId[(size_t)r.id] = &r;
+        for (long k = 0; k < other.nRows_; ++k) {
+            const Row* r = byId[(size_t)k];
+            if (r) { bci.insert(bci.end(), r->indices.begin(), r->indices.end()); bva.insert(bva.end(), r->values.begin(), r->values.end()); }
+            brp[(size_t)k + 1] = (int32_t)bci.size();
+        }
+        mb_sparse* c = nullptr;
+        check(mb_spvec_multiply_host(Context::get(), (int32_t)rows_.size(), (int32_t)nCols_, arp.data(), aci.data(), ava.data(),
+                                     (int32_t)other.nCols_, brp.data(), bci.data(), bva.data(), &c));
+        int64_t nnz = 0;
+        mb_sparse_info(c, nullptr, nullptr, &nnz);
+        std::vector<int32_t> pos((size_t)std::max<int64_t>(1, nnz)), col((size_t)std::max<int64_t>(1, nnz));
+        std::vector<float> val((size_t)std::max<int64_t>(1, nnz));
+        const int32_t rc = mb_spvec_coo(Context::get(), c, pos.data(), col.data(), val.data());
+        mb_sparse_free(Context::get(), c);
+        check(rc);
+        std::vector<CoordinateMatrix::Entry> e;
+        for (int64_t q = 0; q < nnz; ++q) e.push_back({rows_[(size_t)pos[q]].id, (long)col[q], val[q]});
+        return CoordinateMatrix(std::move(e), nRows_, other.nCols_);
+    }
+    // :56-65 — every id in [0, nRows): the stored rows densified on the device (mb_sparse_to_dense), the others zero
+    DenseVecMatrix toDenseVecMatrix() const {
+        std::vector<int32_t> rp, ci;
+        std::vector<double> va;
+        csr(rows_, rp, ci, va);
+        std::vector<long> ids;
+        std::vector<char> held((size_t)nRows_, 0);
+        for (const Row& r : rows_) { ids.push_back(r.id); held[(size_t)r.id] = 1; }
+        for (long i = 0; i < nRows_; ++i) if (!held[(size_t)i]) ids.push_back(i);
+        if (ids.empty() || nCols_ == 0) return DenseVecMatrix(std::vector<DenseVecMatrix::Row>(), nRows_, nCols_);
+        SubMatrix shardT = SubMatrix::empty((int)nCols_, (int)ids.size());             // column-major (nCols x rows) == row-major rows
+        check(mb_block_fill(Context::get(), shardT.handle(), 0.0));
+        if (!rows_.empty()) {
+            mb_sparse* s = nullptr;
+            check(mb_sparse_upload(Context::get(), (int32_t)nCols_, (int32_t)rows_.size(), rp.data(), ci.data(), va.data(), &s));
+            SubMatrix own = shardT.slice(0, (int)nCols_, 0, (int)rows_.size());
+            const int32_t rc = mb_sparse_to_dense(Context::get(), s, own.handle());
+            mb_sparse_free(Context::get(), s);
+            check(rc);
+        }
+        return DenseVecMatrix(ids, shardT.t(), nRows_, nCols_);
+    }
+
+private:
+    static void csr(const std::vector<Row>& rows, std::vector<int32_t>& rp, std::vector<int32_t>& ci, std::vector<double>& va) {
+        rp.assign(1, 0);
+        for (const Row& r : rows) {
+            ci.insert(ci.end(), r.indices.begin(), r.indices.end());
+            va.insert(va.end(), r.values.begin(), r.values.end());
+            if (ci.size() > 2147483647UL) throw std::invalid_argument("SparseVecMatrix: more than 2^31 - 1 non-zeros");
+            rp.push_back((int32_t)ci.size());
+        }
+    }
+    static SparseVecMatrix fromHandle(mb_sparse* s, const std::vector<long>& ids, long nRows, long nCols) {
+        int32_t cols = 0;
+        int64_t nnz = 0;
+        mb_sparse_info(s, nullptr, &cols, &nnz);
+        std::vector<int32_t> rp((size_t)cols + 1), ci((size_t)std::max<int64_t>(1, nnz));
+        std::vector<double> va((size_t)std::max<int64_t>(1, nnz));
+        const int32_t rc = mb_sparse_download(Context::get(), s, rp.data(), ci.data(), va.data());
+        mb_sparse_free(Context::get(), s);
+        check(rc);
+        std::vector<Row> rows;
+        for (int32_t i = 0; i < cols; ++i)
+            rows.push_back({ids[(size_t)i], std::vector<int32_t>(ci.begin() + rp[i], ci.begin() + rp[i + 1]),
+                            std::vector<double>(va.begin() + rp[i], va.begin() + rp[i + 1])});
+        return SparseVecMatrix(std::move(rows), nRows, nCols);
+    }
+    friend class DenseVecMatrix;
+    friend struct MTUtils;
+    std::vector<Row> rows_;
+    long nRows_, nCols_;
+};
+
+inline SparseVecMatrix DenseVecMatrix::toSparseVecMatrix() {
+    const long m = numRows(), n = numCols();
+    mb_sparse* s = nullptr;
+    check(mb_dense_rows_to_sparse(Context::get(), data_.handle(), &s));
+    return SparseVecMatrix::fromHandle(s, ids_, m, n);
+}
+
 struct MTUtils {
     // utils/MTUtils.scala:228-243 — `row col value [timestamp]`, fields split on `,\s?|\s+`; the value is rounded once to
     // float32 (std::from_chars, locale-independent, as Float.parseFloat); blank lines are skipped
@@ -1262,7 +1376,34 @@ struct MTUtils {
         for (long i = 0; i < nRows; ++i) ids[i] = i;
         return DenseVecMatrix(ids, shard, nRows, nCols);
     }
-    // randomBlockMatrix (:34-50): one partition per block in row-major BlockID order, column-major fill
+    // randomSpaVecMatrix (:75-85): randomDenVecMatrix's partitions and seeds; partition p's rows share one column set and
+    // take successive values of its stream (mb_fill_spvec_uniform)
+    static SparseVecMatrix randomSpaVecMatrix(long nRows, int nColumns, double density, int numPartitions, long seed,
+                                              double lo = 0.0, double hi = 1.0) {
+        if (nRows <= 0 || nColumns <= 0 || numPartitions <= 0) throw std::invalid_argument("randomSpaVecMatrix: bad dimensions");
+        int32_t s = 0;
+        check(mb_sparse_column_count(nColumns, nColumns, density, &s));
+        std::vector<int64_t> seeds(numPartitions);
+        check(mb_partition_seeds(seed, numPartitions, seeds.data()));
+        std::vector<SparseVecMatrix::Row> rows;
+        long start = 0;
+        for (int p = 0; p < numPartitions; ++p) {
+            const long end = ((long)(p + 1) * nRows) / numPartitions;
+            if (end > start) {
+                mb_sparse* blk = nullptr;
+                check(mb_sparse_alloc(Context::get(), nColumns, (int)(end - start), (long)s * (end - start), &blk));
+                const int32_t rc = mb_fill_spvec_uniform(Context::get(), blk, seeds[p], lo, hi);
+                if (rc != MB_OK) { mb_sparse_free(Context::get(), blk); check(rc); }
+                std::vector<long> ids;
+                for (long i = start; i < end; ++i) ids.push_back(i);
+                SparseVecMatrix part = SparseVecMatrix::fromHandle(blk, ids, nRows, nColumns);
+                for (auto& r : part.rows_) rows.push_back(std::move(r));
+            }
+            start = end;
+        }
+        return SparseVecMatrix(std::move(rows), nRows, nColumns);
+    }
+    // randomBlockMatrix (:34-50): one partition per block    // randomBlockMatrix (:34-50): one partition per block in row-major BlockID order, column-major fill
     static BlockMatrix randomBlockMatrix(long nRows, long nCols, int numByRow, int numByCol, long seed, double lo = 0.0, double hi = 1.0) {
         const int brs = ceilLen(nRows, numByRow), bcs = ceilLen(nCols, numByCol);
         const int byRow = (int)std::ceil((double)nRows / brs), byCol = (int)std::ceil((double)nCols / bcs);

@@ -398,6 +398,43 @@ NATIVE(void, sparseDownload)(JNIEnv* e, jobject o, jlong ctx, jlong sp, jintArra
     (*e)->ReleasePrimitiveArrayCritical(e, colptr, cp, 0);
     raise(e, rc);
 }
+/* ---- SparseVecMatrix.multiplySparse (matrix/SparseVecMatrix.scala:22-50) on host CSR rows: A (aRows rows of k columns) and
+ *      B (k rows of n columns, absent row ids empty).  Returns the library-owned handle of C's rows; spvecCoo copies its
+ *      sparseNnz entries out as (local row, column, float32 value); sparseFree releases it. ---- */
+NATIVE(jlong, spvecMultiply)(JNIEnv* e, jobject o, jlong ctx, jint aRows, jint k, jintArray aRowptr, jintArray aColidx,
+                             jdoubleArray aValues, jint n, jintArray bRowptr, jintArray bColidx, jdoubleArray bValues) {
+    if ((*e)->GetArrayLength(e, aRowptr) != aRows + 1 || (*e)->GetArrayLength(e, bRowptr) != k + 1 ||
+        (*e)->GetArrayLength(e, aColidx) != (*e)->GetArrayLength(e, aValues) ||
+        (*e)->GetArrayLength(e, bColidx) != (*e)->GetArrayLength(e, bValues)) {
+        (*e)->ThrowNew(e, (*e)->FindClass(e, "java/lang/IllegalArgumentException"),
+                       "Dimension mismatch: spvecMultiply needs rows + 1 row pointers and one value per column index");
+        return 0;
+    }
+    const jsize na = (*e)->GetArrayLength(e, aValues), nb = (*e)->GetArrayLength(e, bValues);
+    int32_t *arp = ints(e, aRowptr), *aci = ints(e, aColidx), *brp = ints(e, bRowptr), *bci = ints(e, bColidx);
+    double* ava = (double*)malloc(sizeof(double) * (size_t)(na > 0 ? na : 1));
+    double* bva = (double*)malloc(sizeof(double) * (size_t)(nb > 0 ? nb : 1));
+    mb_sparse* out = NULL;
+    int32_t rc = MB_ERR_OOM;
+    if (arp && aci && brp && bci && ava && bva) {
+        (*e)->GetDoubleArrayRegion(e, aValues, 0, na, ava);
+        (*e)->GetDoubleArrayRegion(e, bValues, 0, nb, bva);
+        rc = mb_spvec_multiply_host(CTX(ctx), aRows, k, arp, aci, ava, n, brp, bci, bva, &out);
+    }
+    free(arp); free(aci); free(brp); free(bci); free(ava); free(bva);
+    raise(e, rc);
+    return (jlong)(intptr_t)out;
+}
+NATIVE(void, spvecCoo)(JNIEnv* e, jobject o, jlong ctx, jlong sp, jintArray rowsOut, jintArray colsOut, jfloatArray valuesOut) {
+    jint* r = (jint*)(*e)->GetPrimitiveArrayCritical(e, rowsOut, NULL);
+    jint* c = (jint*)(*e)->GetPrimitiveArrayCritical(e, colsOut, NULL);
+    jfloat* v = (jfloat*)(*e)->GetPrimitiveArrayCritical(e, valuesOut, NULL);
+    const int32_t rc = mb_spvec_coo(CTX(ctx), SP(sp), (int32_t*)r, (int32_t*)c, v);
+    (*e)->ReleasePrimitiveArrayCritical(e, valuesOut, v, 0);
+    (*e)->ReleasePrimitiveArrayCritical(e, colsOut, c, 0);
+    (*e)->ReleasePrimitiveArrayCritical(e, rowsOut, r, 0);
+    raise(e, rc);
+}
 NATIVE(jlong, sparseNnz)(JNIEnv* e, jobject o, jlong sp) {
     int64_t nnz = 0;
     raise(e, mb_sparse_info(SP(sp), NULL, NULL, &nnz));

@@ -1,7 +1,7 @@
 """marlin_b200 — H100-native engine for the dense block-matrix hot path of PasaLab/marlin.
 
 Public surface mirrors edu.nju.pasalab.marlin.{matrix,utils,rdd} for that path only:
-BlockMatrix / DenseVecMatrix / CoordinateMatrix / DistributedVector / SubMatrix / BlockID, MTUtils, MatrixMultPartitioner /
+BlockMatrix / DenseVecMatrix / CoordinateMatrix / SparseVecMatrix / DistributedVector / SubMatrix / BlockID, MTUtils, MatrixMultPartitioner /
 MatrixElemOpPartitioner.  All arithmetic runs in libmarlin_b200.so (hand-written sm_90a kernels).
 """
 import os as _os
@@ -13,10 +13,10 @@ _os.environ.setdefault("CUDA_DEVICE_MAX_CONNECTIONS", "32")
 
 from ._native import MarlinArgumentError, MarlinError
 from .matrix import (BlockID, BlockMatrix, CoordinateMatrix, DenseVecMatrix, DistributedMatrix, DistributedVector, SparseMatrix, SparseVector,
-                     SubMatrix)
+                     SparseVecMatrix, SubMatrix)
 from .rdd import MatrixElemOpPartitioner, MatrixMultPartitioner
 from .runtime import Runtime
 from .utils import MTUtils
 
 __all__ = ["BlockID", "BlockMatrix", "CoordinateMatrix", "DenseVecMatrix", "DistributedMatrix", "DistributedVector", "SparseMatrix", "SparseVector",
-           "SubMatrix", "MTUtils", "MatrixElemOpPartitioner", "MatrixMultPartitioner", "Runtime", "MarlinError", "MarlinArgumentError"]
+           "SparseVecMatrix", "SubMatrix", "MTUtils", "MatrixElemOpPartitioner", "MatrixMultPartitioner", "Runtime", "MarlinError", "MarlinArgumentError"]

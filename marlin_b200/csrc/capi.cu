@@ -12,6 +12,7 @@
 #include "sparse.h"
 #include "logistic.h"
 #include "als.h"
+#include "spvec.h"
 
 #include <cuda_runtime.h>
 #include <climits>
@@ -1793,8 +1794,125 @@ int32_t mb_fill_sparse_uniform(mb_ctx* ctx, mb_sparse* S, int64_t partition_seed
     if (S->nnz) {
         MB_CUDA(mb::fill_uniform_f64(S->values, 1, S->nnz, (int)S->nnz, 1, 0, state0, 0, 0.0, 1.0, ctx->stream, &launches));
     }
-    MB_CUDA(mb::sparse_sample_rows(S->rows, S->cols, s, state0, S->colptr, S->rowidx, ctx->stream));
+    MB_CUDA(mb::sparse_sample_rows(S->rows, S->cols, s, state0, S->nnz, S->colptr, S->rowidx, ctx->stream));
     ctx->launches += launches + 1;
+    return MB_OK;
+}
+
+// ------------------------------------------------------------------------------- SparseVecMatrix (matrix/SparseVecMatrix.scala)
+// A row shard is the CSC handle of its transpose: colptr = row pointers, rowidx = column ids.
+static mb::CsrView rows_of(const mb_sparse* S) { return mb::CsrView{S->cols, S->rows, S->colptr, S->rowidx, S->values}; }
+
+// Gives the handle made by mb_sparse_alloc(nnz = 0) room for nnz entries.
+static cudaError_t sparse_reserve(mb_sparse* S, long long nnz) {
+    S->nnz = nnz;
+    if (!nnz) return cudaSuccess;
+    cudaError_t e = cudaMalloc(&S->rowidx, sizeof(int) * (size_t)nnz);
+    return e == cudaSuccess ? cudaMalloc(&S->values, sizeof(double) * (size_t)nnz) : e;
+}
+
+int32_t mb_spvec_multiply(mb_ctx* ctx, const mb_sparse* A, const mb_sparse* B, mb_sparse** out) {
+    MB_CTX(ctx);
+    if (!A || !B || !out) return fail(MB_ERR_INVALID_ARG, "mb_spvec_multiply: null argument");
+    if (A->rows != B->cols)
+        return fail(MB_ERR_DIM_MISMATCH, "multiplySparse: this.nCols %d does not match other.nRows %d", A->rows, B->cols);
+    mb_sparse* R = nullptr;
+    int32_t r = mb_sparse_alloc(ctx, B->rows, A->cols, 0, &R);
+    if (r) return r;
+    mb::SpvecWork w;
+    long long total = 0;
+    int launches = 0, more = 0;
+    cudaError_t e = mb::spvec_count(rows_of(A), rows_of(B), R->colptr, &total, &w, ctx->stream, &launches);
+    if (e == cudaSuccess && total > 0x7fffffffLL) {
+        mb::spvec_release(&w, ctx->stream);
+        mb_sparse_free(ctx, R);
+        return fail(MB_ERR_UNSUPPORTED, "multiplySparse: the product has %lld entries, more than 2^31 - 1", total);
+    }
+    if (e == cudaSuccess) e = sparse_reserve(R, total);
+    if (e == cudaSuccess && total) e = mb::spvec_fill(rows_of(A), rows_of(B), w, R->colptr, R->rowidx, R->values, ctx->stream, &more);
+    mb::spvec_release(&w, ctx->stream);
+    ctx->launches += launches + more;
+    if (e != cudaSuccess) { mb_sparse_free(ctx, R); return cuda_fail(e, "multiplySparse"); }
+    *out = R;
+    return MB_OK;
+}
+
+int32_t mb_spvec_multiply_host(mb_ctx* ctx, int32_t a_rows, int32_t k, const int32_t* a_rowptr, const int32_t* a_colidx,
+                               const double* a_values, int32_t n, const int32_t* b_rowptr, const int32_t* b_colidx,
+                               const double* b_values, mb_sparse** out) {
+    MB_CTX(ctx);
+    if (!out || !a_rowptr || !b_rowptr) return fail(MB_ERR_INVALID_ARG, "mb_spvec_multiply_host: null argument");
+    mb_sparse *A = nullptr, *B = nullptr;
+    int32_t r = mb_sparse_upload(ctx, k, a_rows, a_rowptr, a_colidx, a_values, &A);     // the CSC of A's transpose
+    if (r == MB_OK) r = mb_sparse_upload(ctx, n, k, b_rowptr, b_colidx, b_values, &B);
+    if (r == MB_OK) r = mb_spvec_multiply(ctx, A, B, out);
+    if (r == MB_OK) r = mb_synchronize(ctx);
+    mb_sparse_free(ctx, A);
+    mb_sparse_free(ctx, B);
+    return r;
+}
+
+int32_t mb_spvec_coo(mb_ctx* ctx, const mb_sparse* C, int32_t* rows_out, int32_t* cols_out, float* values_out) {
+    MB_CTX(ctx);
+    if (!C || (C->nnz > 0 && (!rows_out || !cols_out || !values_out))) return fail(MB_ERR_INVALID_ARG, "mb_spvec_coo: null argument");
+    std::vector<int32_t> rowptr((size_t)C->cols + 1);
+    std::vector<double> vals((size_t)C->nnz);
+    int32_t r = mb_sparse_download(ctx, C, rowptr.data(), cols_out, vals.data());
+    if (r) return r;
+    for (int32_t i = 0; i < C->cols; ++i)
+        for (int32_t q = rowptr[i]; q < rowptr[i + 1]; ++q) rows_out[q] = i;
+    for (long long q = 0; q < C->nnz; ++q) values_out[q] = (float)vals[q];      // exact: the values are float32 widened
+    return MB_OK;
+}
+
+int32_t mb_dense_rows_to_sparse(mb_ctx* ctx, const mb_block* rows, mb_sparse** out) {
+    MB_CTX(ctx);
+    if (!rows || !out) return fail(MB_ERR_INVALID_ARG, "mb_dense_rows_to_sparse: null argument");
+    if (rows->dtype != MB_F64) return fail(MB_ERR_UNSUPPORTED, "toSparseVecMatrix: fp64 blocks only");
+    mb_sparse* R = nullptr;
+    int32_t r = mb_sparse_alloc(ctx, rows->cols, rows->rows, 0, &R);
+    if (r) return r;
+    long long total = 0;
+    int launches = 0;
+    cudaError_t e = mb::dense_rows_count(dview(rows), rows->rows, rows->cols, R->colptr, &total, ctx->stream, &launches);
+    if (e == cudaSuccess && total > 0x7fffffffLL) {
+        mb_sparse_free(ctx, R);
+        return fail(MB_ERR_UNSUPPORTED, "toSparseVecMatrix: %lld non-zeros, more than 2^31 - 1", total);
+    }
+    if (e == cudaSuccess) e = sparse_reserve(R, total);
+    if (e == cudaSuccess && total) {
+        e = mb::dense_rows_compact(dview(rows), rows->rows, rows->cols, R->colptr, R->rowidx, R->values, ctx->stream);
+        ++launches;
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+    ctx->launches += launches;
+    if (e != cudaSuccess) { mb_sparse_free(ctx, R); return cuda_fail(e, "toSparseVecMatrix"); }
+    *out = R;
+    return MB_OK;
+}
+
+int32_t mb_fill_spvec_uniform(mb_ctx* ctx, mb_sparse* S, int64_t partition_seed, double lo, double hi) {
+    MB_CTX(ctx);
+    if (!S) return fail(MB_ERR_INVALID_ARG, "mb_fill_spvec_uniform: null block");
+    if (S->cols == 0 || S->nnz == 0) {
+        if (S->nnz != 0) return fail(MB_ERR_INVALID_ARG, "mb_fill_spvec_uniform: %lld non-zeros in 0 rows", (long long)S->nnz);
+        MB_CUDA(cudaMemsetAsync(S->colptr, 0, sizeof(int) * ((size_t)S->cols + 1), ctx->stream));     // s = 0: empty rows
+        return MB_OK;
+    }
+    if (S->nnz % S->cols != 0)
+        return fail(MB_ERR_INVALID_ARG, "mb_fill_spvec_uniform: nnz %lld is not a multiple of %d rows", (long long)S->nnz, S->cols);
+    const int s = (int)(S->nnz / S->cols);
+    if (s > S->rows) return fail(MB_ERR_INVALID_ARG, "mb_fill_spvec_uniform: %d columns per row of %d", s, S->rows);
+    if (S->nnz + S->rows >= (1LL << 39))
+        return fail(MB_ERR_UNSUPPORTED, "mb_fill_spvec_uniform: %d rows of %d columns exceed the generator's 2^39 stream positions",
+                    S->cols, S->rows);
+    const unsigned long long state0 = (unsigned long long)mb_hash_seed(partition_seed);
+    int launches = 0;
+    MB_CUDA(mb::fill_uniform_f64(S->values, 1, S->nnz, (int)S->nnz, 1, 0, state0, 0, lo, hi, ctx->stream, &launches));
+    // row 0's columns: one "column" of the sampler over nColumns positions, from position s*P
+    MB_CUDA(mb::sparse_sample_rows(S->rows, 1, s, state0, S->nnz, S->colptr, S->rowidx, ctx->stream));
+    MB_CUDA(mb::spvec_replicate_columns(S->cols, s, S->colptr, S->rowidx, ctx->stream));
+    ctx->launches += launches + 2;
     return MB_OK;
 }
 

@@ -180,18 +180,19 @@ __device__ __forceinline__ unsigned long long xs_step(unsigned long long s) {
     return s;
 }
 
-// Column j jumps straight to stream position s*cols + j*rows (two XORShift steps per position) and takes row t when
+// Column j jumps straight to stream position first + j*rows (two XORShift steps per position) and takes row t when
 // x * (rows - t) < q * 2^53, x the 53-bit integer behind that position's nextDouble and q the rows still needed: select with
 // probability q / (rows - t), in exact 128-bit integer arithmetic.  When q == rows - t the test always passes, so every
 // column gets exactly s sorted rows.
 __global__ void __launch_bounds__(128) sample_rows_kernel(int rows, int cols, int s, unsigned long long state0,
-                                                          const unsigned long long* tab, int* colptr, int* rowidx) {
+                                                          unsigned long long first, const unsigned long long* tab,
+                                                          int* colptr, int* rowidx) {
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j > cols) return;
     colptr[j] = j * s;
     if (j == cols || s == 0) return;
     unsigned long long st = state0;
-    unsigned long long steps = 2ull * ((unsigned long long)s * cols + (unsigned long long)j * rows);
+    unsigned long long steps = 2ull * (first + (unsigned long long)j * rows);
     for (int lv = 0; steps; ++lv, steps >>= 1) {
         if (steps & 1ull) {
             unsigned long long t = 0, x = st;
@@ -273,12 +274,13 @@ cudaError_t spgemm_dense_out(const CscView& A, const CscView& B, DView C, bool a
     return cudaGetLastError();
 }
 
-cudaError_t sparse_sample_rows(int rows, int cols, int s, unsigned long long state0, int* colptr, int* rowidx,
-                               cudaStream_t st) {
+cudaError_t sparse_sample_rows(int rows, int cols, int s, unsigned long long state0, long long first, int* colptr,
+                               int* rowidx, cudaStream_t st) {
     const unsigned long long* tab = nullptr;
     cudaError_t e = fill_jump_tables(&tab);
     if (e != cudaSuccess) return e;
-    sample_rows_kernel<<<(cols + 1 + 127) / 128, 128, 0, st>>>(rows, cols, s, state0, tab, colptr, rowidx);
+    sample_rows_kernel<<<(cols + 1 + 127) / 128, 128, 0, st>>>(rows, cols, s, state0, (unsigned long long)first, tab,
+                                                               colptr, rowidx);
     return cudaGetLastError();
 }
 

@@ -34,8 +34,8 @@ cudaError_t spmm_sparse_dense(const CsrView& A, int n, DView B, DView C, bool ac
 // C (m x n, dense) [+]= A (m x K, CSC) * B (K x n, CSC); each C(r, j) summed over B's column j in stored order.
 cudaError_t spgemm_dense_out(const CscView& A, const CscView& B, DView C, bool accumulate, cudaStream_t st);
 // Row indices of the sparse generator: column j takes s rows by selection sampling from stream positions
-// [s*cols + j*rows, s*cols + (j+1)*rows) of the XORShift stream state0; colptr[j] = j*s.
-cudaError_t sparse_sample_rows(int rows, int cols, int s, unsigned long long state0, int* colptr, int* rowidx,
-                               cudaStream_t st);
+// [first + j*rows, first + (j+1)*rows) of the XORShift stream state0; colptr[j] = j*s.
+cudaError_t sparse_sample_rows(int rows, int cols, int s, unsigned long long state0, long long first, int* colptr,
+                               int* rowidx, cudaStream_t st);
 
 }  // namespace mb

@@ -1,6 +1,7 @@
 """examples/SparseMultiply.scala:10-81 — `sparse_multiply <A rows> <A cols / B rows> <B cols> <density> <mode> [<seed>]`:
-BlockMatrix multiplies on a 6 x 6 grid with sparse blocks (modes 3 to 6).  Modes 1 and 2 need SparseVecMatrix, which
-this library does not have."""
+mode 1 multiplies two random SparseVecMatrix row by row into a CoordinateMatrix (multiplySparse) and prints its entries
+count; mode 2 densifies the same two matrices and multiplies them as DenseVecMatrix on a 6 x 6 x 6 split; modes 3 to 6
+are BlockMatrix multiplies on a 6 x 6 grid with sparse blocks."""
 import sys
 import time
 
@@ -16,6 +17,18 @@ MODES = {
 }
 
 
+def _entries_count(result) -> int:
+    """entries.count(): every rank's entries (an object gather, which NCCL-only groups support)."""
+    from ..runtime import world
+    _, ws = world()
+    if ws == 1:
+        return len(result.rows)
+    import torch.distributed as dist
+    counts = [None] * ws
+    dist.all_gather_object(counts, len(result.rows))
+    return sum(counts)
+
+
 def main(args):
     if len(args) < 5:
         sys.stderr.write("usage: sparse_multiply <matrixA row length> <matrixA column length> <matrixB column length> "
@@ -25,10 +38,30 @@ def main(args):
         sys.exit(1)
     rowA, colA, colB, density, mode = int(args[0]), int(args[1]), int(args[2]), float(args[3]), int(args[4])
     seed = int(args[5]) if len(args) > 5 else None
-    if mode in (1, 2):
-        print(f"mode {mode} ({MODES[mode]}) is not supported: SparseVecMatrix is not part of marlin_b200")
-        return
     mb, rank = start()
+    if mode in (1, 2):
+        s2 = None if seed is None else seed + 1
+        A = mb.MTUtils.randomSpaVecMatrix(None, rowA, colA, density, seed=seed)
+        B = mb.MTUtils.randomSpaVecMatrix(None, colA, colB, density, seed=s2)
+        if mode == 1:
+            t0 = time.perf_counter()
+            result = A.multiplySparse(B)
+            count = _entries_count(result)
+            if rank == 0:
+                print(f"result entries count: {count}")
+                print(f"sparse-multiply used time: {(time.perf_counter() - t0) * 1e3:.1f} ms")
+        else:
+            denA, denB = A.toDenseVecMatrix(), B.toDenseVecMatrix()
+            mb.MTUtils.evaluate(denB)
+            t0 = time.perf_counter()
+            result = denA.multiply(denB, (6, 6, 6))
+            count = result.elementsCount()
+            mb.MTUtils.evaluate(result)
+            if rank == 0:
+                print(f"result blocks count: {count}")
+                print(f"dense-multiply used time: {(time.perf_counter() - t0) * 1e3:.1f} ms")
+        stop()
+        return
     rnd = mb.MTUtils.randomBlockMatrix
     s2 = None if seed is None else seed + 1
     if mode == 3:

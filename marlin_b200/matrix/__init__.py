@@ -5,7 +5,8 @@ from .dense_vec_matrix import DenseVecMatrix
 from .distributed_matrix import DistributedMatrix
 from .distributed_vector import DistributedVector
 from .sparse_matrix import SparseMatrix, SparseVector
+from .sparse_vec_matrix import SparseVecMatrix
 from .sub_matrix import SubMatrix
 
 __all__ = ["BlockID", "BlockMatrix", "CoordinateMatrix", "DenseVecMatrix", "DistributedMatrix", "DistributedVector", "SparseMatrix", "SparseVector",
-           "SubMatrix"]
+           "SparseVecMatrix", "SubMatrix"]

@@ -480,6 +480,12 @@ class DenseVecMatrix(DistributedMatrix):
         return self.toBlockMatrix(min(par, self.numRows() // 2), 1).transpose()
 
     # ------------------------------------------------------------------ rows -> blocks (:1084-1328)
+    def toSparseVecMatrix(self):
+        """:1333-1353 — the entries != 0.0 of every row (NaN kept, +-0.0 dropped) as a SparseVecMatrix, built on the
+        device; its vectors have length numCols (the reference gives them length nnz)."""
+        from .sparse_vec_matrix import SparseVecMatrix
+        return SparseVecMatrix._from_dense(self)
+
     def toBlockMatrix(self, numByRow: int, numByCol: int):
         """:1259-1328 — ceil-sized blocks; the strided `mat(r, ::) := vec.t` fills become strided device copies
         of whole row runs, and the groupByKey becomes one grouped exchange of the pieces that change GPU."""

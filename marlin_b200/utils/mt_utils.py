@@ -24,6 +24,7 @@ from ..matrix.block_matrix import BlockMatrix
 from ..matrix.coordinate_matrix import CoordinateMatrix
 from ..matrix.dense_vec_matrix import DenseVecMatrix
 from ..matrix.sparse_matrix import SparseBlock, column_count
+from ..matrix.sparse_vec_matrix import SparseVecMatrix
 from ..matrix.sub_matrix import SubMatrix
 from ..runtime import Runtime, world
 
@@ -162,6 +163,52 @@ class MTUtils:
             off += e - s
         ids_arr = np.concatenate(ids) if ids else np.zeros(0, dtype=np.int64)
         return DenseVecMatrix(ids=ids_arr, data=data, nRows=nRows, nCols=nColumns)
+
+    @staticmethod
+    def randomSpaVecMatrix(sc, nRows: int, nColumns: int, density: float, numPartitions: int = 0,
+                           distribution: Optional[UniformGenerator] = None, seed: Optional[int] = None) -> SparseVecMatrix:
+        """utils/MTUtils.scala:75-85 -> RandomSpaVecRDD (rdd/RandomRDD.scala:47-65, 136-159): the partitions, seeds and rank
+        placement of randomDenVecMatrix.  Every row of partition p has the same s = (int)(nColumns * density) sorted columns
+        and takes the next s values of the partition's stream, bit-identical to randomDenVecMatrix's values at the same
+        stream positions.  The reference draws the column set from an unseeded java.util.Random; here it is drawn by
+        selection sampling from the same stream, after the values (mb_fill_spvec_uniform), so it is a function of
+        (seed, partition).  density <= 0 and s > nColumns (where the reference never ends) are rejected."""
+        dist_ = distribution or UniformGenerator(0.0, 1.0)
+        if nRows <= 0 or nColumns <= 0:
+            raise nat.MarlinArgumentError(nat.MB_ERR_INVALID_ARG, f"randomSpaVecMatrix: {nRows} x {nColumns}")
+        s = column_count(nColumns, nColumns, density)
+        rank, ws = world()
+        P = numPartitions if numPartitions > 0 else max(ws, 2 if ws == 1 else ws)
+        if seed is None:
+            seed = time.time_ns()
+        seeds = MTUtils._partition_seeds(seed, P)
+        bounds = [(p * nRows) // P for p in range(P + 1)]
+        for r in range(ws):                                 # every rank checks every rank's shard, so all raise together
+            if s * sum(bounds[p + 1] - bounds[p] for p in range(r, P, ws)) > 2 ** 31 - 1:
+                raise nat.MarlinArgumentError(nat.MB_ERR_UNSUPPORTED, f"randomSpaVecMatrix: a rank's rows would hold more "
+                                              f"than 2^31 - 1 non-zeros ({s} per row)")
+        rt = Runtime.get()
+        rt.sync_stream()
+        ids, rps, cis, vas = [], [], [], []
+        start, base = 0, 0
+        for p in range(P):
+            end = ((p + 1) * nRows) // P
+            if p % ws == rank and end > start:
+                blk = SparseBlock.empty(nColumns, end - start, s * (end - start))
+                nat.check(rt.lib.mb_fill_spvec_uniform(rt.ctx, blk.handle(), seeds[p], dist_.start, dist_.end))
+                ids.append(np.arange(start, end, dtype=np.int64))
+                rps.append(blk.colptr[(1 if rps else 0):] + base)
+                cis.append(blk.rowidx)
+                vas.append(blk.values)
+                base += blk.nnz
+            start = end
+        if not ids:
+            block = SparseBlock(nColumns, 0, torch.zeros(1, dtype=torch.int32, device=rt.device),
+                                torch.empty(0, dtype=torch.int32, device=rt.device),
+                                torch.empty(0, dtype=torch.float64, device=rt.device))
+            return SparseVecMatrix._from_block(np.zeros(0, np.int64), block, nRows, nColumns)
+        block = SparseBlock(nColumns, sum(len(i) for i in ids), torch.cat(rps), torch.cat(cis), torch.cat(vas))
+        return SparseVecMatrix._from_block(np.concatenate(ids), block, nRows, nColumns)
 
     @staticmethod
     def randomBlockMatrix(sc, nRows: int, nColumns: int, numByRow: int, numByCol: int, sparseInfo=(False, 1.0),

@@ -67,6 +67,12 @@ object Native {
                              ratings: Array[Float], lambda: Double, alpha: Double, implicitPrefs: Boolean, yty: Array[Double],
                              xOut: Array[Double]): Unit
 
+  // SparseVecMatrix.multiplySparse on host CSR rows: returns the handle of C's rows (sparseNnz entries, freed by
+  // sparseFree); spvecCoo copies them out as local row, column and float32 value
+  @native def spvecMultiply(ctx: Long, aRows: Int, k: Int, aRowptr: Array[Int], aColidx: Array[Int], aValues: Array[Double],
+                            n: Int, bRowptr: Array[Int], bColidx: Array[Int], bValues: Array[Double]): Long
+  @native def spvecCoo(ctx: Long, sp: Long, rowsOut: Array[Int], colsOut: Array[Int], valuesOut: Array[Float]): Unit
+
   // sparse blocks: a CSC block in HBM (SparseMatrix / LibMatrixMult / SparseMatrix.rand on the device)
   @native def sparseUpload(ctx: Long, rows: Int, cols: Int, colptr: Array[Int], rowidx: Array[Int],
                            values: Array[Double]): Long
