@@ -405,6 +405,46 @@ int32_t mb_dense_rows_to_sparse(mb_ctx* ctx, const mb_block* rows, mb_sparse** o
  * The reference draws the set from an unseeded java.util.Random; here it is a function of (seed, partition). */
 int32_t mb_fill_spvec_uniform(mb_ctx* ctx, mb_sparse* S, int64_t partition_seed, double lo, double hi);
 
+/* ---- PageRank (examples/PageRank.scala).  The link matrix is held as the in-link CSR of the target pages: the CSC handle
+ *      of its transpose, an mb_sparse with rows = n (source pages) and cols = the number of target rows, whose colptr is the
+ *      row pointer array and whose rowidx holds each target's sources, strictly increasing (mb_sparse_check applies).
+ *      One iteration of the example (links.multiply(ranks) over the 1 x numBlocks block grid of
+ *      linkRows.transpose(numBlocks).multiply(0.85), BlockMatrix.scala:240-259, then .reduce(add).add(0.15 * ones)) is,
+ *      for every target row i,
+ *        y_i = fl(fl(P_0 + P_1 + ...) + addend),
+ *      P_s = 0.0 + fl(w_ij x_j) + ... over the stored sources j in [s * seg_len, (s + 1) * seg_len), ascending, each
+ *      multiply and add rounded separately (F2J dgemv per block column), the partials folded left in segment order.  With
+ *      finite x >= 0 the terms of the non-links the dense blocks hold are +0.0, so the result is the dense composition's
+ *      bit for bit.  Errors: seg_len <= 0 is MB_ERR_INVALID_ARG; x or y of the wrong length MB_ERR_DIM_MISMATCH. ---- */
+/* In-degree above which a target row gets a warp of its own instead of one lane.  The bin never changes a result. */
+#define MB_PAGERANK_LIGHT_BOUND 256
+/* Pure host logic (loadLinksMatrix :13-27 and transpose, DenseVecMatrix.scala:1420-1436): the in-link CSR of targets
+ * [t0, t1) from the link rows in source-major CSR.  Row r is source page ids[r] (in [0, n), distinct) with targets
+ * targets[rowptr[r] .. rowptr[r + 1]) (strictly increasing, in [0, n)) and values values[...].  Writes
+ *   in_rowptr_out[t1 - t0 + 1]        target t0 + k holds entries [in_rowptr_out[k], in_rowptr_out[k + 1])
+ *   sources_out[nnz], weights_out[nnz] the source ids ascending (a stable counting sort by target over the rows taken
+ *                                      in ascending source order) and fl(value * damping)
+ * with nnz (<= rowptr[num_rows]) in *nnz_out.  Anything out of range is MB_ERR_INVALID_ARG naming it; more than
+ * 2^31 - 1 entries is MB_ERR_UNSUPPORTED. */
+int32_t mb_pagerank_links(int32_t n, int64_t num_rows, const int64_t* ids, const int64_t* rowptr, const int32_t* targets,
+                          const double* values, int32_t t0, int32_t t1, double damping, int32_t* in_rowptr_out,
+                          int32_t* sources_out, double* weights_out, int64_t* nnz_out);
+/* One iteration: y (in_links->cols x 1) = the step above applied to x (in_links->rows x 1).  x and y are contiguous fp64
+ * blocks of one column; y must not overlap x.  The first step or train call on a handle bins its rows by in-degree and
+ * keeps the list with the handle (one stream synchronisation); later calls only enqueue. */
+int32_t mb_pagerank_step(mb_ctx* ctx, mb_sparse* in_links, const mb_block* x, int64_t seg_len, double addend, mb_block* y);
+/* The whole loop on one device: `iterations` steps of a square in_links (rows == cols == n), ping-ponging x_inout (n x 1)
+ * and one scratch vector with no host synchronisation between steps; x_inout holds the initial ranks on entry and the
+ * result on return.  iterations <= 0 leaves x_inout as it is.  Blocking. */
+int32_t mb_pagerank_train(mb_ctx* ctx, mb_sparse* in_links, int64_t seg_len, double addend, int32_t iterations,
+                          mb_block* x_inout);
+/* The same loop on HOST arrays, for callers holding the link rows on the host (the JVM, the C++ mirror): the link rows as
+ * for mb_pagerank_links over all n targets and the damping factor; ranks_inout (n doubles) holds the initial ranks on
+ * entry and the result on return.  Builds the in-links, uploads, runs and frees inside the call.  Blocking. */
+int32_t mb_pagerank_host(mb_ctx* ctx, int32_t n, int64_t num_rows, const int64_t* ids, const int64_t* rowptr,
+                         const int32_t* targets, const double* values, double damping, int64_t seg_len, double addend,
+                         int32_t iterations, double* ranks_inout);
+
 /* ---- a7/a8: strategy + partitioning (pure integer logic) --------------------------------- */
 /* MTUtils.splitMethod(m,k,n,cores) (utils/MTUtils.scala:150-175, dimToSplit :204-213) */
 int32_t mb_choose_split(int64_t m, int64_t k, int64_t n, int32_t cores, int32_t out_mkn[3]);

@@ -1475,4 +1475,31 @@ struct MTUtils {
     }
 };
 
+// examples/PageRank.scala:41-59 over the link rows of loadLinksMatrix (row `page - 1`: its targets ascending, 1.0 / size
+// each): the final ranks as the example's 2 pieces of ceil(n / 2), the last taking the rest.  The in-links, the upload and
+// the whole loop run in mb_pagerank_host, so the ranks are the Python API's bit for bit.  iterations <= 0 gives ones;
+// fewer than 4 pages with iterations >= 1 throws, as the reference's check of the block grid against the 2 pieces does.
+inline std::vector<std::vector<double>> pageRank(const SparseVecMatrix& linkRows, int iterations) {
+    const long n = linkRows.nRows();
+    if (linkRows.nCols() != n || n < 1 || n > 2147483647L) throw std::invalid_argument("PageRank: the link rows must be a square matrix");
+    const long seg = (n + 1) / 2;
+    std::vector<double> ranks((size_t)n, 1.0);
+    if (iterations > 0) {
+        if (n < 4) throw std::invalid_argument("not supported matrix or vector");
+        std::vector<int64_t> ids, rowptr{0};
+        std::vector<int32_t> targets;
+        std::vector<double> values;
+        for (const auto& r : linkRows.rows()) {
+            if (r.indices.size() != r.values.size()) throw std::invalid_argument("PageRank: a link row's indices and values differ in length");
+            ids.push_back(r.id);
+            targets.insert(targets.end(), r.indices.begin(), r.indices.end());
+            values.insert(values.end(), r.values.begin(), r.values.end());
+            rowptr.push_back((int64_t)targets.size());
+        }
+        check(mb_pagerank_host(Context::get(), (int32_t)n, (int64_t)ids.size(), ids.data(), rowptr.data(), targets.data(),
+                               values.data(), 0.85, seg, 0.15, iterations, ranks.data()));
+    }
+    return {std::vector<double>(ranks.begin(), ranks.begin() + seg), std::vector<double>(ranks.begin() + seg, ranks.end())};
+}
+
 }  // namespace marlin

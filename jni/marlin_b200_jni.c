@@ -435,6 +435,39 @@ NATIVE(void, spvecCoo)(JNIEnv* e, jobject o, jlong ctx, jlong sp, jintArray rows
     (*e)->ReleasePrimitiveArrayCritical(e, rowsOut, r, 0);
     raise(e, rc);
 }
+/* ---- examples/PageRank.scala on host link rows: row r is page ids[r] (0-based) with targets
+ *      targets[rowptr[r] .. rowptr[r + 1]) (ascending) and values (1.0 / size each).  ranks (n doubles) holds the initial
+ *      ranks on entry and the ranks after `iterations` steps of 0.85 * links^T * ranks + 0.15 on return, the two block
+ *      columns split at segLen. ---- */
+NATIVE(void, pageRank)(JNIEnv* e, jobject o, jlong ctx, jint n, jlongArray ids, jlongArray rowptr, jintArray targets,
+                       jdoubleArray values, jlong segLen, jint iterations, jdoubleArray ranks) {
+    const jsize rows = (*e)->GetArrayLength(e, ids), nnz = (*e)->GetArrayLength(e, targets);
+    if ((*e)->GetArrayLength(e, rowptr) != rows + 1 || (*e)->GetArrayLength(e, values) != nnz ||
+        (*e)->GetArrayLength(e, ranks) != n) {
+        (*e)->ThrowNew(e, (*e)->FindClass(e, "java/lang/IllegalArgumentException"),
+                       "Dimension mismatch: pageRank needs rows + 1 row pointers, one value per target and n ranks");
+        return;
+    }
+    int64_t* I = (int64_t*)malloc(sizeof(int64_t) * (size_t)(rows > 0 ? rows : 1));
+    int64_t* P = (int64_t*)malloc(sizeof(int64_t) * (size_t)rows + sizeof(int64_t));
+    int32_t* T = ints(e, targets);
+    double* V = (double*)malloc(sizeof(double) * (size_t)(nnz > 0 ? nnz : 1));
+    double* X = (double*)malloc(sizeof(double) * (size_t)(n > 0 ? n : 1));
+    int32_t rc = MB_ERR_OOM;
+    if (I && P && T && V && X) {
+        (*e)->GetLongArrayRegion(e, ids, 0, rows, (jlong*)I);
+        (*e)->GetLongArrayRegion(e, rowptr, 0, rows + 1, (jlong*)P);
+        (*e)->GetDoubleArrayRegion(e, values, 0, nnz, V);
+        (*e)->GetDoubleArrayRegion(e, ranks, 0, n, X);
+        rc = P[rows] != nnz ? MB_ERR_DIM_MISMATCH
+                            : mb_pagerank_host(CTX(ctx), n, rows, I, P, T, V, 0.85, segLen, 0.15, iterations, X);
+        if (rc == MB_ERR_DIM_MISMATCH && P[rows] != nnz)
+            (*e)->ThrowNew(e, (*e)->FindClass(e, "java/lang/IllegalArgumentException"), "pageRank: rowptr[rows] != targets.length");
+        if (rc == MB_OK && n > 0) (*e)->SetDoubleArrayRegion(e, ranks, 0, n, X);
+    }
+    free(I); free(P); free(T); free(V); free(X);
+    raise(e, rc);
+}
 NATIVE(jlong, sparseNnz)(JNIEnv* e, jobject o, jlong sp) {
     int64_t nnz = 0;
     raise(e, mb_sparse_info(SP(sp), NULL, NULL, &nnz));

@@ -24,6 +24,7 @@ MB_F64, MB_BF16, MB_F32 = 0, 1, 2
 MB_SVD_LOCAL_LAPACK, MB_SVD_LOCAL_ARPACK, MB_SVD_DIST_ARPACK = 0, 1, 2
 MB_ALS_MAX_RANK = 128
 MB_SPVEC_WARP_BOUND, MB_SPVEC_CTA_BOUND, MB_SPVEC_WINDOW = 256, 4096, 16384
+MB_PAGERANK_LIGHT_BOUND = 256
 
 _LIB_PATH = Path(__file__).resolve().parent / "lib" / "libmarlin_b200.so"
 
@@ -119,6 +120,12 @@ SIGNATURES = {
     "mb_spvec_coo": (c_i32, [c_ctx, c_sp, C.c_void_p, C.c_void_p, C.c_void_p]),
     "mb_dense_rows_to_sparse": (c_i32, [c_ctx, c_blk, C.POINTER(c_sp)]),
     "mb_fill_spvec_uniform": (c_i32, [c_ctx, c_sp, c_i64, c_f64, c_f64]),
+    "mb_pagerank_links": (c_i32, [c_i32, c_i64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, c_i32, c_i32, c_f64, C.c_void_p,
+                                  C.c_void_p, C.c_void_p, C.POINTER(c_i64)]),
+    "mb_pagerank_step": (c_i32, [c_ctx, c_sp, c_blk, c_i64, c_f64, c_blk]),
+    "mb_pagerank_train": (c_i32, [c_ctx, c_sp, c_i64, c_f64, c_i32, c_blk]),
+    "mb_pagerank_host": (c_i32, [c_ctx, c_i32, c_i64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, c_f64, c_i64, c_f64, c_i32,
+                                 C.c_void_p]),
     "mb_hash_seed": (c_i64, [c_i64]),
     "mb_partition_seeds": (c_i32, [c_i64, c_i32, C.POINTER(c_i64)]),
     "mb_choose_split": (c_i32, [c_i64, c_i64, c_i64, c_i32, C.POINTER(c_i32)]),

@@ -13,6 +13,7 @@
 #include "logistic.h"
 #include "als.h"
 #include "spvec.h"
+#include "pagerank.h"
 
 #include <cuda_runtime.h>
 #include <climits>
@@ -1599,6 +1600,7 @@ static void sparse_release(mb_sparse* S) {
     cudaFree(S->csr_rowptr);
     cudaFree(S->csr_colidx);
     cudaFree(S->csr_values);
+    cudaFree(S->pagerank_heavy);
     delete S;
 }
 
@@ -1914,6 +1916,118 @@ int32_t mb_fill_spvec_uniform(mb_ctx* ctx, mb_sparse* S, int64_t partition_seed,
     MB_CUDA(mb::spvec_replicate_columns(S->cols, s, S->colptr, S->rowidx, ctx->stream));
     ctx->launches += launches + 2;
     return MB_OK;
+}
+
+// ------------------------------------------------------------------------------------------ PageRank (examples/PageRank.scala)
+// A vector of the step: an fp64 block of `len` rows and one column, element i at p[i * stride].
+static int32_t pagerank_vector(const mb_block* v, int len, const char* what, double** p) {
+    if (!v) return fail(MB_ERR_INVALID_ARG, "PageRank: null %s", what);
+    if (v->dtype != MB_F64) return fail(MB_ERR_UNSUPPORTED, "PageRank: %s must be fp64", what);
+    if (v->cols != 1 || v->rows != len)
+        return fail(MB_ERR_DIM_MISMATCH, "PageRank: %s is %dx%d, expected %dx1", what, v->rows, v->cols, len);
+    if (len > 1 && rs(v) != 1) return fail(MB_ERR_UNSUPPORTED, "PageRank: %s must be contiguous", what);
+    *p = f64_ptr(v);
+    return MB_OK;
+}
+
+// The in-link rows of a handle, binned on first use (the list stays with the handle: blocks are immutable values).
+static int32_t pagerank_links_of(mb_ctx* ctx, mb_sparse* L, int64_t seg_len, mb::PagerankPlan* plan) {
+    if (!L) return fail(MB_ERR_INVALID_ARG, "PageRank: null in-links");
+    if (seg_len <= 0) return fail(MB_ERR_INVALID_ARG, "PageRank: segment length %lld must be positive", (long long)seg_len);
+    if (L->pagerank_nheavy < 0) {
+        mb::PagerankPlan p;
+        cudaError_t e = mb::pagerank_plan(rows_of(L), L->nnz, &p, ctx->stream);
+        if (e != cudaSuccess) {
+            cudaFree(p.heavy);
+            return cuda_fail(e, "PageRank: binning the in-links");
+        }
+        ctx->launches++;
+        L->pagerank_heavy = p.heavy;
+        L->pagerank_nheavy = p.nheavy;
+    }
+    plan->heavy = L->pagerank_heavy;
+    plan->nheavy = L->pagerank_nheavy;
+    return MB_OK;
+}
+
+int32_t mb_pagerank_step(mb_ctx* ctx, mb_sparse* in_links, const mb_block* x, int64_t seg_len, double addend, mb_block* y) {
+    MB_CTX(ctx);
+    MB_LOCK(ctx);
+    if (!in_links) return fail(MB_ERR_INVALID_ARG, "PageRank: null in-links");
+    double *xp = nullptr, *yp = nullptr;
+    int32_t r = pagerank_vector(x, in_links->rows, "x", &xp);
+    if (r == MB_OK) r = pagerank_vector(y, in_links->cols, "y", &yp);
+    if (r) return r;
+    if (in_links->rows && in_links->cols && xp < yp + in_links->cols && yp < xp + in_links->rows)
+        return fail(MB_ERR_INVALID_ARG, "PageRank: y overlaps x");
+    mb::PagerankPlan plan;
+    if ((r = pagerank_links_of(ctx, in_links, seg_len, &plan)) != MB_OK) return r;
+    int launches = 0;
+    MB_CUDA(mb::pagerank_step(rows_of(in_links), plan, xp, seg_len, addend, yp, ctx->stream, &launches));
+    ctx->launches += launches;
+    return MB_OK;
+}
+
+int32_t mb_pagerank_train(mb_ctx* ctx, mb_sparse* in_links, int64_t seg_len, double addend, int32_t iterations,
+                          mb_block* x_inout) {
+    MB_CTX(ctx);
+    MB_LOCK(ctx);
+    if (!in_links) return fail(MB_ERR_INVALID_ARG, "PageRank: null in-links");
+    if (in_links->rows != in_links->cols)
+        return fail(MB_ERR_DIM_MISMATCH, "PageRank: %d target rows over %d sources: the loop needs a square link matrix",
+                    in_links->cols, in_links->rows);
+    double* xp = nullptr;
+    int32_t r = pagerank_vector(x_inout, in_links->rows, "x", &xp);
+    if (r) return r;
+    mb::PagerankPlan plan;
+    if ((r = pagerank_links_of(ctx, in_links, seg_len, &plan)) != MB_OK) return r;
+    const int n = in_links->rows;
+    if (iterations <= 0 || n == 0) return MB_OK;
+    double* scratch = nullptr;
+    MB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&scratch), sizeof(double) * (size_t)n, ctx->stream));
+    double *cur = xp, *next = scratch;
+    cudaError_t e = cudaSuccess;
+    for (int it = 0; it < iterations && e == cudaSuccess; ++it) {
+        int launches = 0;
+        e = mb::pagerank_step(rows_of(in_links), plan, cur, seg_len, addend, next, ctx->stream, &launches);
+        ctx->launches += launches;
+        std::swap(cur, next);
+    }
+    if (e == cudaSuccess && cur != xp) e = cudaMemcpyAsync(xp, cur, sizeof(double) * (size_t)n, cudaMemcpyDeviceToDevice, ctx->stream);
+    cudaFreeAsync(scratch, ctx->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+    return e == cudaSuccess ? MB_OK : cuda_fail(e, "mb_pagerank_train");
+}
+
+int32_t mb_pagerank_host(mb_ctx* ctx, int32_t n, int64_t num_rows, const int64_t* ids, const int64_t* rowptr,
+                         const int32_t* targets, const double* values, double damping, int64_t seg_len, double addend,
+                         int32_t iterations, double* ranks_inout) {
+    MB_CTX(ctx);
+    if (n < 0 || num_rows < 0 || !rowptr || (n > 0 && !ranks_inout)) return fail(MB_ERR_INVALID_ARG, "mb_pagerank_host: bad argument");
+    if (num_rows > 0 && rowptr[num_rows] < 0) return fail(MB_ERR_INVALID_ARG, "mb_pagerank_host: bad row pointers");
+    const size_t cap = num_rows > 0 ? (size_t)std::max<int64_t>(rowptr[num_rows], 0) : 0;
+    std::vector<int32_t> in_rowptr((size_t)n + 1), sources(std::max<size_t>(cap, 1));
+    std::vector<double> weights(std::max<size_t>(cap, 1));
+    int64_t nnz = 0;
+    int32_t r = mb_pagerank_links(n, num_rows, ids, rowptr, targets, values, 0, n, damping, in_rowptr.data(), sources.data(),
+                                  weights.data(), &nnz);
+    if (r || n == 0) return r;
+    mb_sparse* L = nullptr;
+    mb_block* x = nullptr;
+    if ((r = mb_sparse_upload(ctx, n, n, in_rowptr.data(), sources.data(), weights.data(), &L)) != MB_OK) return r;
+    r = mb_block_alloc(ctx, n, 1, MB_F64, &x);
+    if (r == MB_OK) {
+        cudaError_t e = cudaMemcpy(f64_ptr(x), ranks_inout, sizeof(double) * (size_t)n, cudaMemcpyHostToDevice);
+        if (e != cudaSuccess) r = cuda_fail(e, "mb_pagerank_host");
+    }
+    if (r == MB_OK) r = mb_pagerank_train(ctx, L, seg_len, addend, iterations, x);
+    if (r == MB_OK) {
+        cudaError_t e = cudaMemcpy(ranks_inout, f64_ptr(x), sizeof(double) * (size_t)n, cudaMemcpyDeviceToHost);
+        if (e != cudaSuccess) r = cuda_fail(e, "mb_pagerank_host");
+    }
+    mb_block_free(ctx, x);
+    mb_sparse_free(ctx, L);
+    return r;
 }
 
 }  // extern "C"

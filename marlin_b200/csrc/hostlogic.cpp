@@ -383,4 +383,58 @@ int32_t mb_als_init_factors(int64_t seed, int32_t side, int32_t block, int32_t r
     return MB_OK;
 }
 
+// examples/PageRank.scala:13-27 (the link rows) and DenseVecMatrix.scala:1420-1436 (their transpose): the in-link rows of
+// targets [t0, t1), sources ascending.  A stable counting sort by target over the link rows taken in ascending source id:
+// count, scan, place.
+int32_t mb_pagerank_links(int32_t n, int64_t num_rows, const int64_t* ids, const int64_t* rowptr, const int32_t* targets,
+                          const double* values, int32_t t0, int32_t t1, double damping, int32_t* in_rowptr_out,
+                          int32_t* sources_out, double* weights_out, int64_t* nnz_out) {
+    if (n < 0 || num_rows < 0 || !rowptr || !in_rowptr_out || !nnz_out || (num_rows > 0 && !ids))
+        return mb_fail(MB_ERR_INVALID_ARG, "mb_pagerank_links: bad argument");
+    if (t0 < 0 || t1 < t0 || t1 > n)
+        return mb_fail(MB_ERR_INVALID_ARG, "PageRank: target range [%d, %d) is outside [0, %d]", t0, t1, n);
+    if (rowptr[0] != 0) return mb_fail(MB_ERR_INVALID_ARG, "PageRank: rowptr[0] is %lld, not 0", (long long)rowptr[0]);
+    std::vector<int64_t> order((size_t)num_rows);
+    for (int64_t r = 0; r < num_rows; ++r) {
+        if (ids[r] < 0 || ids[r] >= n)
+            return mb_fail(MB_ERR_INVALID_ARG, "PageRank: source page %lld is outside [0, %d)", (long long)ids[r], n);
+        if (rowptr[r + 1] < rowptr[r])
+            return mb_fail(MB_ERR_INVALID_ARG, "PageRank: rowptr decreases at row %lld", (long long)r);
+        if (rowptr[r + 1] > rowptr[r] && (!targets || !values))
+            return mb_fail(MB_ERR_INVALID_ARG, "mb_pagerank_links: null targets or values");
+        for (int64_t q = rowptr[r]; q < rowptr[r + 1]; ++q) {
+            if (targets[q] < 0 || targets[q] >= n)
+                return mb_fail(MB_ERR_INVALID_ARG, "PageRank: target page %d of source page %lld is outside [0, %d)",
+                               targets[q], (long long)ids[r], n);
+            if (q > rowptr[r] && targets[q] <= targets[q - 1])
+                return mb_fail(MB_ERR_INVALID_ARG, "PageRank: the targets of source page %lld are not strictly increasing",
+                               (long long)ids[r]);
+        }
+        order[r] = r;
+    }
+    std::sort(order.begin(), order.end(), [ids](int64_t a, int64_t b) { return ids[a] < ids[b]; });
+    for (int64_t r = 1; r < num_rows; ++r)
+        if (ids[order[r]] == ids[order[r - 1]])
+            return mb_fail(MB_ERR_INVALID_ARG, "PageRank: source page %lld has two link rows", (long long)ids[order[r]]);
+    const int32_t m = t1 - t0;
+    std::vector<int64_t> count((size_t)m + 1, 0);
+    for (int64_t q = 0; q < (num_rows ? rowptr[num_rows] : 0); ++q)
+        if (targets[q] >= t0 && targets[q] < t1) ++count[targets[q] - t0 + 1];
+    for (int32_t k = 0; k < m; ++k) count[k + 1] += count[k];
+    if (count[m] > INT32_MAX)
+        return mb_fail(MB_ERR_UNSUPPORTED, "PageRank: %lld in-links in one range, at most 2^31 - 1", (long long)count[m]);
+    if (count[m] > 0 && (!sources_out || !weights_out)) return mb_fail(MB_ERR_INVALID_ARG, "mb_pagerank_links: null output");
+    for (int32_t k = 0; k <= m; ++k) in_rowptr_out[k] = (int32_t)count[k];
+    for (int64_t r : order)
+        for (int64_t q = rowptr[r]; q < rowptr[r + 1]; ++q) {
+            const int32_t t = targets[q];
+            if (t < t0 || t >= t1) continue;
+            const int64_t at = count[t - t0]++;
+            sources_out[at] = (int32_t)ids[r];
+            weights_out[at] = values[q] * damping;
+        }
+    *nnz_out = in_rowptr_out[m];
+    return MB_OK;
+}
+
 }  // extern "C"

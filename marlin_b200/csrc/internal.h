@@ -74,6 +74,8 @@ struct mb_sparse {
     int* csr_rowptr = nullptr;      // owned by the handle
     int* csr_colidx = nullptr;
     double* csr_values = nullptr;
+    int* pagerank_heavy = nullptr;  // owned by the handle: the rows mb_pagerank_step gives a warp each (mb::pagerank_plan)
+    int pagerank_nheavy = -1;       // -1: not binned yet
 };
 
 namespace mb {

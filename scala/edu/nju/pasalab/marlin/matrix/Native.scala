@@ -73,6 +73,11 @@ object Native {
                             n: Int, bRowptr: Array[Int], bColidx: Array[Int], bValues: Array[Double]): Long
   @native def spvecCoo(ctx: Long, sp: Long, rowsOut: Array[Int], colsOut: Array[Int], valuesOut: Array[Float]): Unit
 
+  // examples/PageRank.scala: `iterations` steps of 0.85 * links^T * ranks + 0.15 over host link rows (page ids, CSR targets
+  // ascending, values 1.0 / size); ranks (n doubles) holds the initial ranks and gets the result
+  @native def pageRank(ctx: Long, n: Int, ids: Array[Long], rowptr: Array[Long], targets: Array[Int], values: Array[Double],
+                       segLen: Long, iterations: Int, ranks: Array[Double]): Unit
+
   // sparse blocks: a CSC block in HBM (SparseMatrix / LibMatrixMult / SparseMatrix.rand on the device)
   @native def sparseUpload(ctx: Long, rows: Int, cols: Int, colptr: Array[Int], rowidx: Array[Int],
                            values: Array[Double]): Long
