@@ -11,7 +11,8 @@
  *
  * Conventions
  *   - plain C, no torch / C++ types; all functions return int32 status (0 = MB_OK, <0 = error);
- *     mb_last_error() returns a thread-local message for the last failing call.
+ *     mb_last_error() returns a thread-local message for the last failing call.  An entry that returns a
+ *     new block or sparse handle through *out sets *out to NULL on failure and leaves nothing allocated.
  *   - one mb_ctx per process and GPU (one process per GPU, like one Spark executor per device).
  *   - a block (mb_block) is the device-resident analogue of SubMatrix.denseBlock: Breeze
  *     DenseMatrix semantics (data, offset, rows, cols, majorStride, isTranspose), column-major:

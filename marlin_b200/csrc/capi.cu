@@ -25,6 +25,7 @@
 #include <cstring>
 #include <new>
 #include <atomic>
+#include <memory>
 #include <mutex>
 #include <vector>
 
@@ -39,6 +40,12 @@ int32_t new_block(mb_block** out) {
     if (!*out) return fail(MB_ERR_OOM, "host allocation failed");
     return MB_OK;
 }
+
+// A new handle until its entry returns it: freed on every failure path, handed to *out by release() on success.
+struct BlockFree { mb_ctx* ctx; void operator()(mb_block* b) const { mb_block_free(ctx, b); } };
+struct SparseFree { mb_ctx* ctx; void operator()(mb_sparse* s) const { mb_sparse_free(ctx, s); } };
+using BlockPtr = std::unique_ptr<mb_block, BlockFree>;
+using SparsePtr = std::unique_ptr<mb_sparse, SparseFree>;
 
 int32_t same_shape(const mb_block* a, const mb_block* b, const char* what) {
     if (a->rows != b->rows || a->cols != b->cols)
@@ -240,22 +247,24 @@ int32_t mb_timer_stop(mb_ctx* ctx, float* ms_out) {
 
 // ---------------------------------------------------------------------------------- blocks
 int32_t mb_block_alloc(mb_ctx* ctx, int32_t rows, int32_t cols, mb_dtype dtype, mb_block** out) {
+    if (out) *out = nullptr;
     MB_CTX(ctx);
     if (!out || rows < 0 || cols < 0 || dtype < 0 || dtype > 2) return fail(MB_ERR_INVALID_ARG, "mb_block_alloc: bad argument");
-    int32_t r = new_block(out);
-    if (r) return r;
-    mb_block* b = *out;
+    BlockPtr b(new (std::nothrow) mb_block(), BlockFree{ctx});
+    if (!b) return fail(MB_ERR_OOM, "host allocation failed");
     b->rows = rows; b->cols = cols; b->ld = rows > 0 ? rows : 1; b->dtype = dtype; b->owns = 1; b->device = ctx->device;
     const size_t bytes = (size_t)rows * (size_t)cols * elem_size(dtype);
     if (bytes) {
         cudaError_t e = cudaMalloc(&b->data, bytes);
-        if (e != cudaSuccess) { delete b; *out = nullptr; return cuda_fail(e, "cudaMalloc(block)"); }
+        if (e != cudaSuccess) return cuda_fail(e, "cudaMalloc(block)");
     }
+    *out = b.release();
     return MB_OK;
 }
 
 int32_t mb_block_wrap(mb_ctx* ctx, void* device_ptr, int64_t offset, int32_t rows, int32_t cols, int32_t ld,
                       int32_t is_transpose, mb_dtype dtype, mb_block** out) {
+    if (out) *out = nullptr;
     if (!ctx) return fail(MB_ERR_INVALID_ARG, "null context");
     if (!out || rows < 0 || cols < 0 || offset < 0 || dtype < 0 || dtype > 2)
         return fail(MB_ERR_INVALID_ARG, "mb_block_wrap: bad argument");
@@ -298,6 +307,7 @@ int32_t mb_block_set_ready_event(mb_block* blk, void* cuda_event) {
 }
 
 int32_t mb_block_view_t(mb_ctx* ctx, const mb_block* blk, mb_block** out) {
+    if (out) *out = nullptr;
     if (!ctx || !blk || !out) return fail(MB_ERR_INVALID_ARG, "mb_block_view_t: null argument");
     int32_t r = new_block(out);
     if (r) return r;
@@ -306,6 +316,7 @@ int32_t mb_block_view_t(mb_ctx* ctx, const mb_block* blk, mb_block** out) {
 }
 
 int32_t mb_block_slice(mb_ctx* ctx, const mb_block* blk, int32_t r0, int32_t r1, int32_t c0, int32_t c1, mb_block** out) {
+    if (out) *out = nullptr;
     if (!ctx || !blk || !out) return fail(MB_ERR_INVALID_ARG, "mb_block_slice: null argument");
     if (r0 < 0 || r1 < r0 || r1 > blk->rows || c0 < 0 || c1 < c0 || c1 > blk->cols)
         return fail(MB_ERR_INVALID_ARG, "mb_block_slice: range [%d,%d)x[%d,%d) outside %dx%d", r0, r1, c0, c1, blk->rows, blk->cols);
@@ -321,35 +332,32 @@ int32_t mb_block_slice(mb_ctx* ctx, const mb_block* blk, int32_t r0, int32_t r1,
 
 int32_t mb_block_upload(mb_ctx* ctx, const double* host, int64_t offset, int32_t rows, int32_t cols, int32_t ld,
                         int32_t is_transpose, mb_dtype store_as, mb_block** out) {
+    if (out) *out = nullptr;
     MB_CTX(ctx);
     if (!host || !out || rows < 0 || cols < 0 || offset < 0) return fail(MB_ERR_INVALID_ARG, "mb_block_upload: bad argument");
     const int minor = is_transpose ? cols : rows, major = is_transpose ? rows : cols;
     if (ld < (minor > 0 ? minor : 1)) return fail(MB_ERR_INVALID_ARG, "mb_block_upload: ld %d < %d", ld, minor);
-    int32_t r = mb_block_alloc(ctx, rows, cols, store_as, out);
+    mb_block* raw = nullptr;
+    int32_t r = mb_block_alloc(ctx, rows, cols, store_as, &raw);
     if (r) return r;
-    if (rows == 0 || cols == 0) return MB_OK;
-    // stage the raw (minor x major) host array, then one device kernel packs / transposes / rounds it
-    mb_block* dst = *out;
-    const bool direct = (store_as == MB_F64) && !is_transpose;
-    if (direct) {
-        cudaError_t e = cudaMemcpy2DAsync(dst->data, (size_t)rows * 8, host + offset, (size_t)ld * 8, (size_t)rows * 8,
-                                          (size_t)cols, cudaMemcpyHostToDevice, ctx->stream);
-        if (e != cudaSuccess) { mb_block_free(ctx, dst); *out = nullptr; return cuda_fail(e, "cudaMemcpy2DAsync(H2D)"); }
-        MB_CUDA(cudaStreamSynchronize(ctx->stream));
-        return MB_OK;
+    BlockPtr dst(raw, BlockFree{ctx});
+    if (rows > 0 && cols > 0) {
+        // the raw (minor x major) host array lands in the block, or in a stage one kernel packs / transposes / rounds
+        const bool direct = store_as == MB_F64 && !is_transpose;
+        mb::StreamBuffer stage;
+        if (!direct) MB_CUDA(stage.alloc((size_t)minor * major * 8, ctx->stream));
+        MB_CUDA(cudaMemcpy2DAsync(direct ? dst->data : stage.as<void>(), (size_t)minor * 8, host + offset, (size_t)ld * 8,
+                                  (size_t)minor * 8, (size_t)major, cudaMemcpyHostToDevice, ctx->stream));
+        if (!direct) {
+            const mb_block src = block_view(stage.as<void>(), rows, cols, minor, is_transpose, MB_F64, ctx->device);
+            r = copy_convert(ctx, &src, dst.get());
+        }
+        const cudaError_t e = cudaStreamSynchronize(ctx->stream);      // the copy reads the caller's array
+        if (r) return r;
+        if (e != cudaSuccess) return cuda_fail(e, "mb_block_upload");
     }
-    double* stage = nullptr;
-    MB_CUDA(cudaMalloc(&stage, (size_t)minor * major * 8));
-    cudaError_t e = cudaMemcpy2DAsync(stage, (size_t)minor * 8, host + offset, (size_t)ld * 8, (size_t)minor * 8,
-                                      (size_t)major, cudaMemcpyHostToDevice, ctx->stream);
-    if (e != cudaSuccess) { cudaFree(stage); mb_block_free(ctx, dst); *out = nullptr; return cuda_fail(e, "cudaMemcpy2DAsync(H2D)"); }
-    mb_block src;
-    src.data = stage; src.rows = rows; src.cols = cols; src.ld = minor; src.is_transpose = is_transpose ? 1 : 0; src.dtype = MB_F64;
-    r = copy_convert(ctx, &src, dst);
-    cudaStreamSynchronize(ctx->stream);
-    cudaFree(stage);
-    if (r) { mb_block_free(ctx, dst); *out = nullptr; }
-    return r;
+    *out = dst.release();
+    return MB_OK;
 }
 
 int32_t mb_block_download(mb_ctx* ctx, const mb_block* blk, double* host, int32_t ld) {
@@ -357,25 +365,18 @@ int32_t mb_block_download(mb_ctx* ctx, const mb_block* blk, double* host, int32_
     if (!blk || !host) return fail(MB_ERR_INVALID_ARG, "mb_block_download: null argument");
     if (ld < blk->rows) return fail(MB_ERR_INVALID_ARG, "mb_block_download: ld %d < rows %d", ld, blk->rows);
     if (blk->rows == 0 || blk->cols == 0) return MB_OK;
-    const double* src = nullptr;
-    size_t src_pitch = 0;
-    double* stage = nullptr;
-    if (blk->dtype == MB_F64 && !blk->is_transpose) {
-        src = f64_ptr(blk);
-        src_pitch = (size_t)blk->ld * 8;
-    } else {
-        MB_CUDA(cudaMalloc(&stage, (size_t)blk->rows * blk->cols * 8));
-        mb_block tmp;
-        tmp.data = stage; tmp.rows = blk->rows; tmp.cols = blk->cols; tmp.ld = blk->rows; tmp.dtype = MB_F64;
-        int32_t r = copy_convert(ctx, blk, &tmp);
-        if (r) { cudaFree(stage); return r; }
-        src = stage;
-        src_pitch = (size_t)blk->rows * 8;
+    // fp64 column-major blocks are copied out as they are, others through a packed fp64 copy
+    mb_block src = *blk;
+    mb::StreamBuffer stage;
+    if (blk->dtype != MB_F64 || blk->is_transpose) {
+        MB_CUDA(stage.alloc((size_t)blk->rows * blk->cols * 8, ctx->stream));
+        src = block_view(stage.as<void>(), blk->rows, blk->cols, blk->rows, false, MB_F64, ctx->device);
+        int32_t r = copy_convert(ctx, blk, &src);
+        if (r) return r;
     }
-    cudaError_t e = cudaMemcpy2DAsync(host, (size_t)ld * 8, src, src_pitch, (size_t)blk->rows * 8, (size_t)blk->cols,
-                                      cudaMemcpyDeviceToHost, ctx->stream);
+    cudaError_t e = cudaMemcpy2DAsync(host, (size_t)ld * 8, f64_ptr(&src), (size_t)src.ld * 8, (size_t)blk->rows * 8,
+                                      (size_t)blk->cols, cudaMemcpyDeviceToHost, ctx->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    if (stage) cudaFree(stage);
     if (e != cudaSuccess) return cuda_fail(e, "cudaMemcpy2DAsync(D2H)");
     return MB_OK;
 }
@@ -453,14 +454,14 @@ int32_t mb_dgemm_host(mb_ctx* ctx, char transa, char transb, int32_t m, int32_t 
     // device staging is packed with an even leading dimension so the TMA path is always eligible
     auto even = [](int x) { return (x + 1) & ~1; };
     const int dlda = even(ra > 0 ? ra : 1), dldb = even(rb > 0 ? rb : 1), dldc = even(m);
-    double *dA = nullptr, *dB = nullptr, *dC = nullptr;
-    cudaError_t e = cudaSuccess;
-    auto cleanup = [&]() { if (dA) cudaFree(dA); if (dB) cudaFree(dB); if (dC) cudaFree(dC); };
+    mb::StreamBuffer bufA, bufB, bufC;
     if (k > 0) {
-        if ((e = cudaMalloc(&dA, (size_t)dlda * ca * 8)) != cudaSuccess) { cleanup(); return cuda_fail(e, "cudaMalloc(A)"); }
-        if ((e = cudaMalloc(&dB, (size_t)dldb * cb * 8)) != cudaSuccess) { cleanup(); return cuda_fail(e, "cudaMalloc(B)"); }
+        MB_CUDA(bufA.alloc((size_t)dlda * ca * 8, ctx->stream));
+        MB_CUDA(bufB.alloc((size_t)dldb * cb * 8, ctx->stream));
     }
-    if ((e = cudaMalloc(&dC, (size_t)dldc * n * 8)) != cudaSuccess) { cleanup(); return cuda_fail(e, "cudaMalloc(C)"); }
+    MB_CUDA(bufC.alloc((size_t)dldc * n * 8, ctx->stream));
+    double *dA = bufA.as<double>(), *dB = bufB.as<double>(), *dC = bufC.as<double>();
+    cudaError_t e = cudaSuccess;
     if (k > 0) {
         e = cudaMemcpy2DAsync(dA, (size_t)dlda * 8, a + a_offset, (size_t)lda * 8, (size_t)ra * 8, ca, cudaMemcpyHostToDevice, ctx->stream);
         if (e == cudaSuccess)
@@ -468,14 +469,15 @@ int32_t mb_dgemm_host(mb_ctx* ctx, char transa, char transb, int32_t m, int32_t 
     }
     if (e == cudaSuccess && beta != 0.0)
         e = cudaMemcpy2DAsync(dC, (size_t)dldc * 8, c + c_offset, (size_t)ldc * 8, (size_t)m * 8, n, cudaMemcpyHostToDevice, ctx->stream);
-    if (e != cudaSuccess) { cleanup(); return cuda_fail(e, "H2D copy"); }
-    int32_t r = dgemm_device_impl(ctx, transa, transb, m, n, k, alpha, dA, dlda, dB, dldb, beta, dC, dldc, false);
+    int32_t r = e == cudaSuccess ? dgemm_device_impl(ctx, transa, transb, m, n, k, alpha, dA, dlda, dB, dldb, beta, dC, dldc, false)
+                                 : cuda_fail(e, "H2D copy");
     if (r == MB_OK) {
         e = cudaMemcpy2DAsync(c + c_offset, (size_t)ldc * 8, dC, (size_t)dldc * 8, (size_t)m * 8, n, cudaMemcpyDeviceToHost, ctx->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
         if (e != cudaSuccess) r = cuda_fail(e, "D2H copy");
     }
-    cleanup();
+    // the copies read and write the caller's arrays: they have finished when the call returns, whether it failed or not
+    e = cudaStreamSynchronize(ctx->stream);
+    if (r == MB_OK && e != cudaSuccess) r = cuda_fail(e, "D2H copy");
     return r;
 }
 
@@ -532,15 +534,14 @@ static int32_t bf16_gemm(mb_ctx* ctx, bool ta, bool tb, int M, int N, int nseg, 
         return MB_OK;
     }
     auto misaligned = [](const char* p, long long ld) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0 || ld % 8 != 0; };
-    std::vector<void*> staged;
-    auto release = [&]() { for (void* p : staged) cudaFreeAsync(p, ctx->stream); staged.clear(); };
+    std::vector<mb::StreamBuffer> staged;     // the copies of the launch being issued
     // the stored (rows x cols) array of an operand -> a packed copy with ld rounded up to 8 (256-byte aligned base)
     auto stage = [&](const char*& p, long long& ld, int rows, int cols) -> cudaError_t {
         const long long ld8 = (rows + 7) / 8 * 8;
-        void* dst = nullptr;
-        cudaError_t e = cudaMallocAsync(&dst, (size_t)ld8 * cols * 2, ctx->stream);
+        staged.emplace_back();
+        cudaError_t e = staged.back().alloc((size_t)ld8 * cols * 2, ctx->stream);
         if (e != cudaSuccess) return e;
-        staged.push_back(dst);
+        void* dst = staged.back().as<void>();
         if ((e = mb::convert_strided(MB_BF16, MB_BF16, rows, cols, p, 1, ld, dst, 1, ld8, ctx->stream)) != cudaSuccess) return e;
         ctx->launches++;
         p = static_cast<const char*>(dst);
@@ -562,7 +563,7 @@ static int32_t bf16_gemm(mb_ctx* ctx, bool ta, bool tb, int M, int N, int nseg, 
         if (e == cudaSuccess)
             e = mb::gemm_bf16_segments(ta, tb, M, N, ns, ks, pa, la, pb, lb, C, ldc, c_f32, accumulate || g > 0, ctx->num_sms,
                                        ctx->stream, &launches);
-        release();
+        staged.clear();
         if (e == cudaErrorNotSupported) return fail(MB_ERR_UNSUPPORTED, "bf16 GEMM: cuTensorMapEncodeTiled is not available");
         if (e != cudaSuccess) return cuda_fail(e, "gemm_bf16_segments");
         ctx->launches += launches;
@@ -1151,24 +1152,20 @@ int32_t mb_block_inverse(mb_ctx* ctx, const mb_block* A, mb_block* out) {
     if (r) return r;
     // working copy of A for the factors (packed, even leading dimension)
     const int ld = (n + 1) & ~1;
-    double* lu = nullptr;
-    MB_CUDA(cudaMalloc(&lu, (size_t)ld * n * sizeof(double)));
-    mb_block tmp;
-    tmp.data = lu; tmp.rows = n; tmp.cols = n; tmp.ld = ld; tmp.dtype = MB_F64; tmp.device = ctx->device;
+    mb::StreamBuffer lu;
+    MB_CUDA(lu.alloc((size_t)ld * n * sizeof(double), ctx->stream));
+    mb_block tmp = block_view(lu.as<void>(), n, n, ld, false, MB_F64, ctx->device);
     r = copy_convert(ctx, A, &tmp);
-    if (r) { cudaFree(lu); return r; }
+    if (r) return r;
     int *piv = ctx->int_ws, *info = ctx->int_ws + 2 * n;
     int launches = 0;
     cudaError_t e = mb::getrf(fview(&tmp), piv, nullptr, info, ctx->num_sms, ctx->stream, &launches);
     if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->int_host, info, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    if (e == cudaSuccess && ctx->int_host[0] != 0) {
-        cudaFree(lu);
+    if (e == cudaSuccess && ctx->int_host[0] != 0)
         return fail(MB_ERR_CUDA, "matrix is singular (zero pivot in column %d)", ctx->int_host[0] - 1);   // Breeze: MatrixSingularException
-    }
     if (e == cudaSuccess) e = mb::inverse_from_lu(fview(&tmp), piv, fview(out), ctx->num_sms, ctx->stream, &launches);
     if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    cudaFree(lu);
     ctx->launches += launches;
     if (e != cudaSuccess) return cuda_fail(e, "mb_block_inverse");
     return MB_OK;
@@ -1206,11 +1203,11 @@ int32_t mb_block_gramian(mb_ctx* ctx, const mb_block* A, mb_block* G) {
     // split-K partials only when the triangle is too small for the SMs (at most 256 MiB), stream-ordered and returned
     // after the call; with one split the product is written into G directly
     const size_t need = mb::gemm_f64_tma_eligible(f64_ptr(A), A->ld, f64_ptr(A), A->ld) ? mb::gram_workspace_doubles(n, m, ctx->num_sms) : 0;
-    double* ws = nullptr;
-    if (need) MB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&ws), need * sizeof(double), ctx->stream));
+    mb::StreamBuffer ws;
+    if (need) MB_CUDA(ws.alloc(need * sizeof(double), ctx->stream));
     int launches = 0;
-    const cudaError_t e = mb::gram_f64(trans, n, m, f64_ptr(A), A->ld, f64_ptr(G), G->ld, ws, ctx->num_sms, ctx->stream, &launches);
-    if (ws) cudaFreeAsync(ws, ctx->stream);
+    const cudaError_t e = mb::gram_f64(trans, n, m, f64_ptr(A), A->ld, f64_ptr(G), G->ld, ws.as<double>(), ctx->num_sms,
+                                       ctx->stream, &launches);
     ctx->launches += launches;
     if (e != cudaSuccess) return cuda_fail(e, "mb_block_gramian");
     return MB_OK;
@@ -1249,44 +1246,24 @@ int32_t mb_block_syev(mb_ctx* ctx, const mb_block* G, mb_block* V, double* w_out
 }
 
 // ------------------------------------------------------------------------------------ logistic regression (DenseVecMatrix.lr)
-// Device buffers of one lr call: the rows as the kernel reads them (row-major, in place or staged), w, the gradient and the
-// per-CTA partials.  Stream-ordered; freed when the call's work completes.
-struct LrBuffers {
-    const double* x = nullptr;
-    long long ld = 0;
-    double* staged = nullptr;
-    double* w = nullptr;          // n weights, then n gradient values, then the partials
-    int m = 0, n = 0;
-    cudaStream_t st = nullptr;
-    ~LrBuffers() {
-        if (staged) cudaFreeAsync(staged, st);
-        if (w) cudaFreeAsync(w, st);
-    }
-};
-
-static int32_t lr_setup(mb_ctx* ctx, const mb_block* A, const char* name, LrBuffers* b) {
+// The rows of one lr call as the kernel reads them: *v, with row r at f64_ptr(v) + r * rs(v), is A itself when A is a
+// row-major view or one column, else a row-major copy in `staged`.  `ws`: n weights, then n gradient values, then the
+// per-CTA partials.
+static int32_t lr_setup(mb_ctx* ctx, const mb_block* A, const char* name, mb::StreamBuffer* staged, mb::StreamBuffer* ws,
+                        mb_block* v) {
     if (!A) return fail(MB_ERR_INVALID_ARG, "%s: null block", name);
     if (A->dtype != MB_F64) return fail(MB_ERR_UNSUPPORTED, "%s: fp64 rows only", name);
     if (A->rows == 0) return fail(MB_ERR_EMPTY, "empty collection");       // numRows() / numCols() on an empty RDD
     if (A->cols == 0) return fail(MB_ERR_INVALID_ARG, "%s: a row needs at least its label (0 columns)", name);
-    b->m = A->rows;
-    b->n = A->cols;
-    b->st = ctx->stream;
-    if (A->is_transpose || A->cols == 1) {          // row r at data + r * ld (an m x 1 column: ld 1)
-        b->x = f64_ptr(A);
-        b->ld = A->is_transpose ? A->ld : 1;
-    } else {
-        MB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&b->staged), (size_t)b->m * b->n * sizeof(double), ctx->stream));
-        mb_block tmp;
-        tmp.data = b->staged; tmp.rows = b->m; tmp.cols = b->n; tmp.ld = b->n; tmp.is_transpose = 1; tmp.dtype = MB_F64;
-        tmp.device = ctx->device;
-        const int32_t r = copy_convert(ctx, A, &tmp);
+    const int m = A->rows, n = A->cols;
+    *v = *A;
+    if (!A->is_transpose && n > 1) {
+        MB_CUDA(staged->alloc((size_t)m * n * sizeof(double), ctx->stream));
+        *v = block_view(staged->as<void>(), m, n, n, true, MB_F64, ctx->device);
+        const int32_t r = copy_convert(ctx, A, v);
         if (r) return r;
-        b->x = b->staged;
-        b->ld = b->n;
     }
-    const size_t ws = (size_t)2 * b->n + (size_t)mb::lr_parts(b->m, ctx->num_sms) * b->n;
-    MB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&b->w), ws * sizeof(double), ctx->stream));
+    MB_CUDA(ws->alloc(((size_t)2 * n + (size_t)mb::lr_parts(m, ctx->num_sms) * n) * sizeof(double), ctx->stream));
     return MB_OK;
 }
 
@@ -1294,14 +1271,16 @@ int32_t mb_lr_gradient(mb_ctx* ctx, const mb_block* rows, const double* w, doubl
     MB_CTX(ctx);
     MB_LOCK(ctx);
     if (!w || !grad) return fail(MB_ERR_INVALID_ARG, "mb_lr_gradient: null weights or gradient");
-    LrBuffers b;
-    int32_t r = lr_setup(ctx, rows, "mb_lr_gradient", &b);
+    mb::StreamBuffer staged, ws;
+    mb_block v;
+    int32_t r = lr_setup(ctx, rows, "mb_lr_gradient", &staged, &ws, &v);
     if (r) return r;
-    double* g = b.w + b.n;
-    MB_CUDA(cudaMemcpyAsync(b.w, w, sizeof(double) * b.n, cudaMemcpyHostToDevice, ctx->stream));
-    MB_CUDA(mb::lr_gradient_f64(b.x, b.ld, b.m, b.n, b.w, g + b.n, g, false, 0.0, ctx->num_sms, ctx->stream));
+    const int n = v.cols;
+    double *wd = ws.as<double>(), *g = wd + n;
+    MB_CUDA(cudaMemcpyAsync(wd, w, sizeof(double) * n, cudaMemcpyHostToDevice, ctx->stream));
+    MB_CUDA(mb::lr_gradient_f64(f64_ptr(&v), rs(&v), v.rows, n, wd, g + n, g, false, 0.0, ctx->num_sms, ctx->stream));
     ctx->launches += 2;
-    MB_CUDA(cudaMemcpyAsync(grad, g, sizeof(double) * b.n, cudaMemcpyDeviceToHost, ctx->stream));
+    MB_CUDA(cudaMemcpyAsync(grad, g, sizeof(double) * n, cudaMemcpyDeviceToHost, ctx->stream));
     MB_CUDA(cudaStreamSynchronize(ctx->stream));
     return MB_OK;
 }
@@ -1312,17 +1291,21 @@ int32_t mb_lr_train(mb_ctx* ctx, const mb_block* rows, int64_t data_size, double
     if (!w_out) return fail(MB_ERR_INVALID_ARG, "mb_lr_train: null output");
     if (rows && rows->rows > 0 && data_size <= 0)
         return fail(MB_ERR_INVALID_ARG, "mb_lr_train: data size %lld must be positive", (long long)data_size);
-    LrBuffers b;
-    int32_t r = lr_setup(ctx, rows, "mb_lr_train", &b);
+    mb::StreamBuffer staged, ws;
+    mb_block v;
+    int32_t r = lr_setup(ctx, rows, "mb_lr_train", &staged, &ws, &v);
     if (r) return r;
-    MB_CUDA(cudaMemsetAsync(b.w, 0, sizeof(double) * b.n, ctx->stream));          // BDV(Array.fill(featureSize)(0.0))
+    const int n = v.cols;
+    double* wd = ws.as<double>();
+    MB_CUDA(cudaMemsetAsync(wd, 0, sizeof(double) * n, ctx->stream));          // BDV(Array.fill(featureSize)(0.0))
     for (int i = 1; i <= iters; ++i) {
         // weights - delta * (stepSize / dataSize / math.sqrt(i)), the scalar evaluated in that order
         const double scale = step / (double)data_size / std::sqrt((double)i);
-        MB_CUDA(mb::lr_gradient_f64(b.x, b.ld, b.m, b.n, b.w, b.w + 2 * b.n, nullptr, true, scale, ctx->num_sms, ctx->stream));
+        MB_CUDA(mb::lr_gradient_f64(f64_ptr(&v), rs(&v), v.rows, n, wd, wd + 2 * n, nullptr, true, scale, ctx->num_sms,
+                                    ctx->stream));
         ctx->launches += 2;
     }
-    MB_CUDA(cudaMemcpyAsync(w_out, b.w, sizeof(double) * b.n, cudaMemcpyDeviceToHost, ctx->stream));
+    MB_CUDA(cudaMemcpyAsync(w_out, wd, sizeof(double) * n, cudaMemcpyDeviceToHost, ctx->stream));
     MB_CUDA(cudaStreamSynchronize(ctx->stream));
     return MB_OK;
 }
@@ -1352,9 +1335,9 @@ static mb::AlsLinks als_links(const mb_als_side* s) {
     return mb::AlsLinks{s->ids, reinterpret_cast<const long long*>(s->offsets), s->partners, s->ratings, s->work, (long long)s->count};
 }
 
-// YtY for implicit mode: the caller's, or the Gramian of Y into `own` (rank x rank, stream-ordered, freed by the caller)
-static int32_t als_yty(mb_ctx* ctx, const mb_block* Yb, const mb_block* YtY, int rank, double** own, const double** p,
-                       long long* ld) {
+// YtY for implicit mode: the caller's, or the Gramian of Y into `own` (rank x rank)
+static int32_t als_yty(mb_ctx* ctx, const mb_block* Yb, const mb_block* YtY, int rank, mb::StreamBuffer* own,
+                       const double** p, long long* ld) {
     if (YtY) {
         if (YtY->dtype != MB_F64 || YtY->rows != rank || YtY->cols != rank)
             return fail(MB_ERR_DIM_MISMATCH, "ALS: YtY is %dx%d, expected %dx%d fp64", YtY->rows, YtY->cols, rank, rank);
@@ -1362,12 +1345,11 @@ static int32_t als_yty(mb_ctx* ctx, const mb_block* Yb, const mb_block* YtY, int
         *ld = YtY->ld;          // symmetric: either storage order reads the same element
         return MB_OK;
     }
-    MB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(own), sizeof(double) * rank * rank, ctx->stream));
-    mb_block g;
-    g.data = *own; g.rows = rank; g.cols = rank; g.ld = rank; g.dtype = MB_F64; g.device = ctx->device;
+    MB_CUDA(own->alloc(sizeof(double) * rank * rank, ctx->stream));
+    mb_block g = block_view(own->as<void>(), rank, rank, rank, false, MB_F64, ctx->device);
     const int32_t r = mb_block_gramian(ctx, Yb, &g);
     if (r) return r;
-    *p = *own;
+    *p = own->as<double>();
     *ld = rank;
     return MB_OK;
 }
@@ -1385,7 +1367,7 @@ static int32_t als_half_step(mb_ctx* ctx, const mb_als_side* side, const mb_bloc
         return fail(MB_ERR_DIM_MISMATCH, "ALS: factors of rank %d and %d", rank, Xb->cols);
     r = als_check(side, rank, lambda);
     if (r) return r;
-    double* own = nullptr;
+    mb::StreamBuffer own;
     if (implicit) r = als_yty(ctx, Yb, YtY, rank, &own, &yty, &ldyty);
     if (!r) {
         const cudaError_t e = mb::als_solve(als_links(side), rank, Y, ldy, lambda, alpha, implicit != 0, yty, ldyty,
@@ -1393,7 +1375,6 @@ static int32_t als_half_step(mb_ctx* ctx, const mb_als_side* side, const mb_bloc
         if (e != cudaSuccess) r = cuda_fail(e, "ALS update");
         else ctx->launches++;
     }
-    if (own) cudaFreeAsync(own, ctx->stream);
     return r;
 }
 
@@ -1428,7 +1409,7 @@ int32_t mb_als_normal_equations(mb_ctx* ctx, const mb_als_side* side, const mb_b
     r = als_check(side, rank, lambda);
     if (r) return r;
     if (side->count > 0 && (!A_out || !b_out)) return fail(MB_ERR_INVALID_ARG, "mb_als_normal_equations: null output");
-    double* own = nullptr;
+    mb::StreamBuffer own;
     if (implicit) r = als_yty(ctx, Yb, YtY, rank, &own, &yty, &ldyty);
     if (!r) {
         const cudaError_t e = mb::als_assemble(als_links(side), rank, Y, ldy, lambda, alpha, implicit != 0, yty, ldyty, A_out,
@@ -1436,7 +1417,6 @@ int32_t mb_als_normal_equations(mb_ctx* ctx, const mb_als_side* side, const mb_b
         if (e != cudaSuccess) r = cuda_fail(e, "mb_als_normal_equations");
         else ctx->launches++;
     }
-    if (own) cudaFreeAsync(own, ctx->stream);
     if (!r) MB_CUDA(cudaStreamSynchronize(ctx->stream));
     return r;
 }
@@ -1468,22 +1448,6 @@ int32_t mb_als_train(mb_ctx* ctx, const mb_als_side* users, const mb_als_side* p
     return r ? r : als_pivots(ctx, bad);
 }
 
-// Device copies of host arrays, stream-ordered, freed by the destructor
-struct AlsUpload {
-    std::vector<void*> bufs;
-    cudaStream_t st;
-    explicit AlsUpload(cudaStream_t s) : st(s) {}
-    ~AlsUpload() { for (void* b : bufs) cudaFreeAsync(b, st); }
-    cudaError_t put(const void* host, size_t bytes, void* dev_ptr_out) {
-        void* d = nullptr;
-        cudaError_t e = cudaMallocAsync(&d, bytes ? bytes : 8, st);
-        if (e != cudaSuccess) return e;
-        bufs.push_back(d);
-        *static_cast<void**>(dev_ptr_out) = d;
-        return bytes ? cudaMemcpyAsync(d, host, bytes, cudaMemcpyHostToDevice, st) : cudaSuccess;
-    }
-};
-
 int32_t mb_als_update_host(mb_ctx* ctx, int32_t rank, int64_t n_fixed, const double* Y, int64_t n, const int64_t* ids,
                            const int64_t* offsets, const int32_t* partners, const float* ratings, double lambda,
                            double alpha, int32_t implicit, const double* YtY, double* X) {
@@ -1511,28 +1475,23 @@ int32_t mb_als_update_host(mb_ctx* ctx, int32_t rank, int64_t n_fixed, const dou
         work[p] = int32_t(p);
     }
     std::stable_sort(work.begin(), work.end(), [&](int32_t a, int32_t b) { return offsets[a + 1] - offsets[a] > offsets[b + 1] - offsets[b]; });
-    AlsUpload up(ctx->stream);
-    mb_als_side side{n, nullptr, nullptr, nullptr, nullptr, nullptr};
-    int32_t *d_ids, *d_partners, *d_work;
-    int64_t* d_off;
-    float* d_r;
-    double *d_y, *d_x, *d_yty = nullptr;
-    MB_CUDA(up.put(ids32.data(), sizeof(int32_t) * n, &d_ids));
-    MB_CUDA(up.put(offsets, sizeof(int64_t) * (n + 1), &d_off));
-    MB_CUDA(up.put(partners, sizeof(int32_t) * nnz, &d_partners));
-    MB_CUDA(up.put(ratings, sizeof(float) * nnz, &d_r));
-    MB_CUDA(up.put(work.data(), sizeof(int32_t) * n, &d_work));
-    MB_CUDA(up.put(Y, sizeof(double) * n_fixed * rank, &d_y));
-    MB_CUDA(up.put(X, sizeof(double) * n * rank, &d_x));
-    if (YtY) MB_CUDA(up.put(YtY, sizeof(double) * rank * rank, &d_yty));
-    side.ids = d_ids; side.offsets = d_off; side.partners = d_partners; side.ratings = d_r; side.work = d_work;
-    mb_block yb, xb, gb;
-    yb.data = d_y; yb.rows = (int)n_fixed; yb.cols = rank; yb.ld = rank; yb.is_transpose = 1; yb.dtype = MB_F64; yb.device = ctx->device;
-    xb = yb; xb.data = d_x; xb.rows = (int)n;
-    gb = yb; gb.data = d_yty; gb.rows = rank;
+    mb::StreamBuffer d_ids, d_off, d_partners, d_r, d_work, d_y, d_x, d_yty;
+    MB_CUDA(d_ids.upload(ids32.data(), sizeof(int32_t) * n, ctx->stream));
+    MB_CUDA(d_off.upload(offsets, sizeof(int64_t) * (n + 1), ctx->stream));
+    MB_CUDA(d_partners.upload(partners, sizeof(int32_t) * nnz, ctx->stream));
+    MB_CUDA(d_r.upload(ratings, sizeof(float) * nnz, ctx->stream));
+    MB_CUDA(d_work.upload(work.data(), sizeof(int32_t) * n, ctx->stream));
+    MB_CUDA(d_y.upload(Y, sizeof(double) * n_fixed * rank, ctx->stream));
+    MB_CUDA(d_x.upload(X, sizeof(double) * n * rank, ctx->stream));
+    if (YtY) MB_CUDA(d_yty.upload(YtY, sizeof(double) * rank * rank, ctx->stream));
+    const mb_als_side side{n, d_ids.as<int32_t>(), d_off.as<int64_t>(), d_partners.as<int32_t>(), d_r.as<float>(),
+                           d_work.as<int32_t>()};
+    const mb_block yb = block_view(d_y.as<void>(), (int)n_fixed, rank, rank, true, MB_F64, ctx->device);
+    const mb_block gb = block_view(d_yty.as<void>(), rank, rank, rank, true, MB_F64, ctx->device);
+    mb_block xb = block_view(d_x.as<void>(), (int)n, rank, rank, true, MB_F64, ctx->device);
     r = mb_als_update(ctx, &side, &yb, lambda, alpha, implicit, YtY ? &gb : nullptr, &xb);
     if (r) return r;
-    MB_CUDA(cudaMemcpyAsync(X, d_x, sizeof(double) * n * rank, cudaMemcpyDeviceToHost, ctx->stream));
+    MB_CUDA(cudaMemcpyAsync(X, d_x.as<void>(), sizeof(double) * n * rank, cudaMemcpyDeviceToHost, ctx->stream));
     MB_CUDA(cudaStreamSynchronize(ctx->stream));
     return MB_OK;
 }
@@ -1561,13 +1520,12 @@ int32_t mb_coo_to_dense_rows(mb_ctx* ctx, int64_t nnz, const int32_t* row_pos, c
         MB_CUDA(cudaMemsetAsync(const_cast<double*>(p), 0, sizeof(double) * out->rows * out->cols, ctx->stream));
     else
         MB_CUDA(cudaMemset2DAsync(const_cast<double*>(p), sizeof(double) * ld, 0, sizeof(double) * out->cols, out->rows, ctx->stream));
-    AlsUpload up(ctx->stream);
-    int32_t *d_row, *d_col;
-    float* d_val;
-    MB_CUDA(up.put(row_pos, sizeof(int32_t) * nnz, &d_row));
-    MB_CUDA(up.put(cols, sizeof(int32_t) * nnz, &d_col));
-    MB_CUDA(up.put(values, sizeof(float) * nnz, &d_val));
-    MB_CUDA(mb::coo_scatter_rows(nnz, d_row, d_col, d_val, const_cast<double*>(p), ld, ctx->stream));
+    mb::StreamBuffer d_row, d_col, d_val;
+    MB_CUDA(d_row.upload(row_pos, sizeof(int32_t) * nnz, ctx->stream));
+    MB_CUDA(d_col.upload(cols, sizeof(int32_t) * nnz, ctx->stream));
+    MB_CUDA(d_val.upload(values, sizeof(float) * nnz, ctx->stream));
+    MB_CUDA(mb::coo_scatter_rows(nnz, d_row.as<int32_t>(), d_col.as<int32_t>(), d_val.as<float>(), const_cast<double*>(p), ld,
+                                 ctx->stream));
     ctx->launches++;
     MB_CUDA(cudaStreamSynchronize(ctx->stream));
     return MB_OK;
@@ -1591,21 +1549,9 @@ int32_t mb_fill_uniform(mb_ctx* ctx, mb_block* blk, int64_t partition_seed, int6
 static mb::CscView csc(const mb_sparse* S) { return mb::CscView{S->rows, S->cols, S->colptr, S->rowidx, S->values}; }
 static mb::DView dview(const mb_block* b) { return mb::DView{f64_ptr(b), rs(b), cs(b)}; }
 
-static void sparse_release(mb_sparse* S) {
-    if (S->owns) {
-        cudaFree(S->colptr);
-        cudaFree(S->rowidx);
-        cudaFree(S->values);
-    }
-    cudaFree(S->csr_rowptr);
-    cudaFree(S->csr_colidx);
-    cudaFree(S->csr_values);
-    cudaFree(S->pagerank_heavy);
-    delete S;
-}
-
 int32_t mb_sparse_wrap(mb_ctx* ctx, int32_t rows, int32_t cols, int64_t nnz, void* colptr, void* rowidx, void* values,
                        mb_sparse** out) {
+    if (out) *out = nullptr;
     if (!ctx) return fail(MB_ERR_INVALID_ARG, "null context");
     if (!out || rows < 0 || cols < 0 || nnz < 0 || !colptr || (nnz > 0 && (!rowidx || !values)))
         return fail(MB_ERR_INVALID_ARG, "mb_sparse_wrap: bad argument");
@@ -1620,19 +1566,21 @@ int32_t mb_sparse_wrap(mb_ctx* ctx, int32_t rows, int32_t cols, int64_t nnz, voi
 
 int32_t mb_sparse_upload(mb_ctx* ctx, int32_t rows, int32_t cols, const int32_t* colptr, const int32_t* rowidx,
                          const double* values, mb_sparse** out) {
+    if (out) *out = nullptr;
     MB_CTX(ctx);
     if (!out || !colptr) return fail(MB_ERR_INVALID_ARG, "mb_sparse_upload: null argument");
     int32_t r = mb_sparse_check(rows, cols, colptr, rowidx);
     if (r) return r;
     const long long nnz = colptr[cols];
     if (nnz > 0 && !values) return fail(MB_ERR_INVALID_ARG, "mb_sparse_upload: null values");
-    mb_sparse* S = nullptr;
-    if ((r = mb_sparse_alloc(ctx, rows, cols, nnz, &S)) != MB_OK) return r;
+    mb_sparse* raw = nullptr;
+    if ((r = mb_sparse_alloc(ctx, rows, cols, nnz, &raw)) != MB_OK) return r;
+    SparsePtr S(raw, SparseFree{ctx});
     cudaError_t e = cudaMemcpy(S->colptr, colptr, sizeof(int) * ((size_t)cols + 1), cudaMemcpyHostToDevice);
     if (e == cudaSuccess && nnz) e = cudaMemcpy(S->rowidx, rowidx, sizeof(int) * (size_t)nnz, cudaMemcpyHostToDevice);
     if (e == cudaSuccess && nnz) e = cudaMemcpy(S->values, values, sizeof(double) * (size_t)nnz, cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) { sparse_release(S); return cuda_fail(e, "mb_sparse_upload"); }
-    *out = S;
+    if (e != cudaSuccess) return cuda_fail(e, "mb_sparse_upload");
+    *out = S.release();
     return MB_OK;
 }
 
@@ -1657,26 +1605,29 @@ int32_t mb_sparse_info(const mb_sparse* S, int32_t* rows, int32_t* cols, int64_t
 }
 
 int32_t mb_sparse_alloc(mb_ctx* ctx, int32_t rows, int32_t cols, int64_t nnz, mb_sparse** out) {
+    if (out) *out = nullptr;
     MB_CTX(ctx);
     if (!out || rows < 0 || cols < 0 || nnz < 0) return fail(MB_ERR_INVALID_ARG, "mb_sparse_alloc: bad argument");
     if (nnz > 0x7fffffffLL) return fail(MB_ERR_INVALID_ARG, "sparse block with %lld non-zeros: at most 2^31 - 1", (long long)nnz);
-    mb_sparse* S = new (std::nothrow) mb_sparse();
+    SparsePtr S(new (std::nothrow) mb_sparse(), SparseFree{ctx});
     if (!S) return fail(MB_ERR_OOM, "host allocation failed");
     S->rows = rows; S->cols = cols; S->nnz = nnz; S->owns = 1; S->device = ctx->device;
     cudaError_t e = cudaMalloc(&S->colptr, sizeof(int) * ((size_t)cols + 1));
     if (e == cudaSuccess && nnz) e = cudaMalloc(&S->rowidx, sizeof(int) * (size_t)nnz);
     if (e == cudaSuccess && nnz) e = cudaMalloc(&S->values, sizeof(double) * (size_t)nnz);
-    if (e != cudaSuccess) { sparse_release(S); return cuda_fail(e, "mb_sparse_alloc"); }
-    *out = S;
+    if (e != cudaSuccess) return cuda_fail(e, "mb_sparse_alloc");
+    *out = S.release();
     return MB_OK;
 }
 
 int32_t mb_sparse_values_op(mb_ctx* ctx, const mb_sparse* S, int32_t op, double b, mb_sparse** out) {
+    if (out) *out = nullptr;
     MB_CTX(ctx);
     if (!S || !out || op < MB_SPARSE_ADD || op > MB_SPARSE_DIV) return fail(MB_ERR_INVALID_ARG, "mb_sparse_values_op: bad argument");
-    mb_sparse* R = nullptr;
-    int32_t r = mb_sparse_alloc(ctx, S->rows, S->cols, S->nnz, &R);
+    mb_sparse* raw = nullptr;
+    int32_t r = mb_sparse_alloc(ctx, S->rows, S->cols, S->nnz, &raw);
     if (r) return r;
+    SparsePtr R(raw, SparseFree{ctx});
     cudaError_t e = cudaMemcpyAsync(R->colptr, S->colptr, sizeof(int) * ((size_t)S->cols + 1), cudaMemcpyDeviceToDevice, ctx->stream);
     if (e == cudaSuccess && S->nnz)
         e = cudaMemcpyAsync(R->rowidx, S->rowidx, sizeof(int) * (size_t)S->nnz, cudaMemcpyDeviceToDevice, ctx->stream);
@@ -1691,8 +1642,8 @@ int32_t mb_sparse_values_op(mb_ctx* ctx, const mb_sparse* S, int32_t op, double 
         }
         ctx->launches++;
     }
-    if (e != cudaSuccess) { mb_sparse_free(ctx, R); return cuda_fail(e, "mb_sparse_values_op"); }
-    *out = R;
+    if (e != cudaSuccess) return cuda_fail(e, "mb_sparse_values_op");
+    *out = R.release();
     return MB_OK;
 }
 
@@ -1702,7 +1653,16 @@ int32_t mb_sparse_free(mb_ctx* ctx, mb_sparse* S) {
         cudaSetDevice(ctx->device);
         cudaStreamSynchronize(ctx->stream);      // a product may still read the CSR copy
     }
-    sparse_release(S);
+    if (S->owns) {
+        cudaFree(S->colptr);
+        cudaFree(S->rowidx);
+        cudaFree(S->values);
+    }
+    cudaFree(S->csr_rowptr);
+    cudaFree(S->csr_colidx);
+    cudaFree(S->csr_values);
+    cudaFree(S->pagerank_heavy);
+    delete S;
     return MB_OK;
 }
 
@@ -1814,43 +1774,43 @@ static cudaError_t sparse_reserve(mb_sparse* S, long long nnz) {
 }
 
 int32_t mb_spvec_multiply(mb_ctx* ctx, const mb_sparse* A, const mb_sparse* B, mb_sparse** out) {
+    if (out) *out = nullptr;
     MB_CTX(ctx);
     if (!A || !B || !out) return fail(MB_ERR_INVALID_ARG, "mb_spvec_multiply: null argument");
     if (A->rows != B->cols)
         return fail(MB_ERR_DIM_MISMATCH, "multiplySparse: this.nCols %d does not match other.nRows %d", A->rows, B->cols);
-    mb_sparse* R = nullptr;
-    int32_t r = mb_sparse_alloc(ctx, B->rows, A->cols, 0, &R);
+    mb_sparse* raw = nullptr;
+    int32_t r = mb_sparse_alloc(ctx, B->rows, A->cols, 0, &raw);
     if (r) return r;
+    SparsePtr R(raw, SparseFree{ctx});
     mb::SpvecWork w;
     long long total = 0;
     int launches = 0, more = 0;
     cudaError_t e = mb::spvec_count(rows_of(A), rows_of(B), R->colptr, &total, &w, ctx->stream, &launches);
-    if (e == cudaSuccess && total > 0x7fffffffLL) {
-        mb::spvec_release(&w, ctx->stream);
-        mb_sparse_free(ctx, R);
+    if (e == cudaSuccess && total > 0x7fffffffLL)
         return fail(MB_ERR_UNSUPPORTED, "multiplySparse: the product has %lld entries, more than 2^31 - 1", total);
-    }
-    if (e == cudaSuccess) e = sparse_reserve(R, total);
+    if (e == cudaSuccess) e = sparse_reserve(R.get(), total);
     if (e == cudaSuccess && total) e = mb::spvec_fill(rows_of(A), rows_of(B), w, R->colptr, R->rowidx, R->values, ctx->stream, &more);
-    mb::spvec_release(&w, ctx->stream);
     ctx->launches += launches + more;
-    if (e != cudaSuccess) { mb_sparse_free(ctx, R); return cuda_fail(e, "multiplySparse"); }
-    *out = R;
+    if (e != cudaSuccess) return cuda_fail(e, "multiplySparse");
+    *out = R.release();
     return MB_OK;
 }
 
 int32_t mb_spvec_multiply_host(mb_ctx* ctx, int32_t a_rows, int32_t k, const int32_t* a_rowptr, const int32_t* a_colidx,
                                const double* a_values, int32_t n, const int32_t* b_rowptr, const int32_t* b_colidx,
                                const double* b_values, mb_sparse** out) {
+    if (out) *out = nullptr;
     MB_CTX(ctx);
     if (!out || !a_rowptr || !b_rowptr) return fail(MB_ERR_INVALID_ARG, "mb_spvec_multiply_host: null argument");
-    mb_sparse *A = nullptr, *B = nullptr;
-    int32_t r = mb_sparse_upload(ctx, k, a_rows, a_rowptr, a_colidx, a_values, &A);     // the CSC of A's transpose
-    if (r == MB_OK) r = mb_sparse_upload(ctx, n, k, b_rowptr, b_colidx, b_values, &B);
-    if (r == MB_OK) r = mb_spvec_multiply(ctx, A, B, out);
+    mb_sparse *a = nullptr, *b = nullptr, *c = nullptr;
+    int32_t r = mb_sparse_upload(ctx, k, a_rows, a_rowptr, a_colidx, a_values, &a);     // the CSC of A's transpose
+    if (r == MB_OK) r = mb_sparse_upload(ctx, n, k, b_rowptr, b_colidx, b_values, &b);
+    if (r == MB_OK) r = mb_spvec_multiply(ctx, a, b, &c);
+    const SparsePtr A(a, SparseFree{ctx}), B(b, SparseFree{ctx});
+    SparsePtr C(c, SparseFree{ctx});
     if (r == MB_OK) r = mb_synchronize(ctx);
-    mb_sparse_free(ctx, A);
-    mb_sparse_free(ctx, B);
+    if (r == MB_OK) *out = C.release();
     return r;
 }
 
@@ -1868,28 +1828,28 @@ int32_t mb_spvec_coo(mb_ctx* ctx, const mb_sparse* C, int32_t* rows_out, int32_t
 }
 
 int32_t mb_dense_rows_to_sparse(mb_ctx* ctx, const mb_block* rows, mb_sparse** out) {
+    if (out) *out = nullptr;
     MB_CTX(ctx);
     if (!rows || !out) return fail(MB_ERR_INVALID_ARG, "mb_dense_rows_to_sparse: null argument");
     if (rows->dtype != MB_F64) return fail(MB_ERR_UNSUPPORTED, "toSparseVecMatrix: fp64 blocks only");
-    mb_sparse* R = nullptr;
-    int32_t r = mb_sparse_alloc(ctx, rows->cols, rows->rows, 0, &R);
+    mb_sparse* raw = nullptr;
+    int32_t r = mb_sparse_alloc(ctx, rows->cols, rows->rows, 0, &raw);
     if (r) return r;
+    SparsePtr R(raw, SparseFree{ctx});
     long long total = 0;
     int launches = 0;
     cudaError_t e = mb::dense_rows_count(dview(rows), rows->rows, rows->cols, R->colptr, &total, ctx->stream, &launches);
-    if (e == cudaSuccess && total > 0x7fffffffLL) {
-        mb_sparse_free(ctx, R);
+    if (e == cudaSuccess && total > 0x7fffffffLL)
         return fail(MB_ERR_UNSUPPORTED, "toSparseVecMatrix: %lld non-zeros, more than 2^31 - 1", total);
-    }
-    if (e == cudaSuccess) e = sparse_reserve(R, total);
+    if (e == cudaSuccess) e = sparse_reserve(R.get(), total);
     if (e == cudaSuccess && total) {
         e = mb::dense_rows_compact(dview(rows), rows->rows, rows->cols, R->colptr, R->rowidx, R->values, ctx->stream);
         ++launches;
     }
     if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
     ctx->launches += launches;
-    if (e != cudaSuccess) { mb_sparse_free(ctx, R); return cuda_fail(e, "toSparseVecMatrix"); }
-    *out = R;
+    if (e != cudaSuccess) return cuda_fail(e, "toSparseVecMatrix");
+    *out = R.release();
     return MB_OK;
 }
 
@@ -1983,9 +1943,9 @@ int32_t mb_pagerank_train(mb_ctx* ctx, mb_sparse* in_links, int64_t seg_len, dou
     if ((r = pagerank_links_of(ctx, in_links, seg_len, &plan)) != MB_OK) return r;
     const int n = in_links->rows;
     if (iterations <= 0 || n == 0) return MB_OK;
-    double* scratch = nullptr;
-    MB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&scratch), sizeof(double) * (size_t)n, ctx->stream));
-    double *cur = xp, *next = scratch;
+    mb::StreamBuffer scratch;
+    MB_CUDA(scratch.alloc(sizeof(double) * (size_t)n, ctx->stream));
+    double *cur = xp, *next = scratch.as<double>();
     cudaError_t e = cudaSuccess;
     for (int it = 0; it < iterations && e == cudaSuccess; ++it) {
         int launches = 0;
@@ -1994,7 +1954,6 @@ int32_t mb_pagerank_train(mb_ctx* ctx, mb_sparse* in_links, int64_t seg_len, dou
         std::swap(cur, next);
     }
     if (e == cudaSuccess && cur != xp) e = cudaMemcpyAsync(xp, cur, sizeof(double) * (size_t)n, cudaMemcpyDeviceToDevice, ctx->stream);
-    cudaFreeAsync(scratch, ctx->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
     return e == cudaSuccess ? MB_OK : cuda_fail(e, "mb_pagerank_train");
 }
@@ -2012,22 +1971,17 @@ int32_t mb_pagerank_host(mb_ctx* ctx, int32_t n, int64_t num_rows, const int64_t
     int32_t r = mb_pagerank_links(n, num_rows, ids, rowptr, targets, values, 0, n, damping, in_rowptr.data(), sources.data(),
                                   weights.data(), &nnz);
     if (r || n == 0) return r;
-    mb_sparse* L = nullptr;
-    mb_block* x = nullptr;
-    if ((r = mb_sparse_upload(ctx, n, n, in_rowptr.data(), sources.data(), weights.data(), &L)) != MB_OK) return r;
-    r = mb_block_alloc(ctx, n, 1, MB_F64, &x);
-    if (r == MB_OK) {
-        cudaError_t e = cudaMemcpy(f64_ptr(x), ranks_inout, sizeof(double) * (size_t)n, cudaMemcpyHostToDevice);
-        if (e != cudaSuccess) r = cuda_fail(e, "mb_pagerank_host");
-    }
-    if (r == MB_OK) r = mb_pagerank_train(ctx, L, seg_len, addend, iterations, x);
-    if (r == MB_OK) {
-        cudaError_t e = cudaMemcpy(ranks_inout, f64_ptr(x), sizeof(double) * (size_t)n, cudaMemcpyDeviceToHost);
-        if (e != cudaSuccess) r = cuda_fail(e, "mb_pagerank_host");
-    }
-    mb_block_free(ctx, x);
-    mb_sparse_free(ctx, L);
-    return r;
+    mb_sparse* l = nullptr;
+    mb_block* xb = nullptr;
+    if ((r = mb_sparse_upload(ctx, n, n, in_rowptr.data(), sources.data(), weights.data(), &l)) != MB_OK) return r;
+    const SparsePtr L(l, SparseFree{ctx});
+    if ((r = mb_block_alloc(ctx, n, 1, MB_F64, &xb)) != MB_OK) return r;
+    const BlockPtr x(xb, BlockFree{ctx});
+    cudaError_t e = cudaMemcpy(f64_ptr(xb), ranks_inout, sizeof(double) * (size_t)n, cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) return cuda_fail(e, "mb_pagerank_host");
+    if ((r = mb_pagerank_train(ctx, l, seg_len, addend, iterations, xb)) != MB_OK) return r;
+    e = cudaMemcpy(ranks_inout, f64_ptr(xb), sizeof(double) * (size_t)n, cudaMemcpyDeviceToHost);
+    return e == cudaSuccess ? MB_OK : cuda_fail(e, "mb_pagerank_host");
 }
 
 }  // extern "C"

@@ -3,6 +3,7 @@
 #pragma once
 #include "../../include/marlin_b200.h"
 #include "gemm_f64.h"
+#include "stream_buffer.h"
 
 #include <cuda_runtime.h>
 #include <atomic>
@@ -112,6 +113,12 @@ inline double* f64_ptr(const mb_block* b) { return reinterpret_cast<double*>(ele
 // strides of the logical (rows x cols) view
 inline long long rs(const mb_block* b) { return b->is_transpose ? b->ld : 1; }
 inline long long cs(const mb_block* b) { return b->is_transpose ? 1 : b->ld; }
+// A block record over device memory the call holds: it owns nothing and lives on the caller's frame.
+inline mb_block block_view(void* data, int rows, int cols, int ld, bool row_major, int dtype, int device) {
+    mb_block b;
+    b.data = data; b.rows = rows; b.cols = cols; b.ld = ld; b.is_transpose = row_major; b.dtype = dtype; b.device = device;
+    return b;
+}
 
 inline int32_t check_ctx(mb_ctx* ctx) {
     if (!ctx) return fail(MB_ERR_INVALID_ARG, "null context");

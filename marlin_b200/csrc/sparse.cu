@@ -8,6 +8,7 @@
 // of BlockMatrix.multiply (matrix/BlockMatrix.scala:177).
 #include "sparse.h"
 #include "elementwise.h"
+#include "stream_buffer.h"
 
 #include <algorithm>
 
@@ -244,15 +245,14 @@ cudaError_t csc_to_csr(const CscView& S, long long nnz, int* rowptr, int* colidx
         const int g = (int)std::min<long long>((nnz + 255) / 256, 4096);
         csr_count_kernel<<<g, 256, 0, st>>>(S.rowidx, nnz, rowptr + 1);
         scan_inplace_kernel<<<1, 1024, 0, st>>>(rowptr + 1, S.rows);
-        int* cursor = nullptr;
-        if ((e = cudaMallocAsync(reinterpret_cast<void**>(&cursor), sizeof(int) * (size_t)S.rows, st)) != cudaSuccess) return e;
-        e = cudaMemcpyAsync(cursor, rowptr, sizeof(int) * (size_t)S.rows, cudaMemcpyDeviceToDevice, st);
+        StreamBuffer cursor;
+        if ((e = cursor.alloc(sizeof(int) * (size_t)S.rows, st)) != cudaSuccess) return e;
+        e = cudaMemcpyAsync(cursor.as<int>(), rowptr, sizeof(int) * (size_t)S.rows, cudaMemcpyDeviceToDevice, st);
         if (e == cudaSuccess) {
-            csr_scatter_kernel<<<g, 256, 0, st>>>(S, nnz, cursor, colidx, vals);
+            csr_scatter_kernel<<<g, 256, 0, st>>>(S, nnz, cursor.as<int>(), colidx, vals);
             csr_sort_kernel<<<(S.rows + 127) / 128, 128, 0, st>>>(S.rows, rowptr, colidx, vals);
             *launches = 4;
         }
-        cudaFreeAsync(cursor, st);
     }
     return e != cudaSuccess ? e : cudaGetLastError();
 }

@@ -340,33 +340,34 @@ cudaError_t spvec_count(const CsrView& A, const CsrView& B, int* rowptr, long lo
     *total = 0;
     cudaError_t e = cudaMemsetAsync(rowptr, 0, sizeof(int) * ((size_t)A.rows + 1), st);
     if (e != cudaSuccess || A.rows == 0) return e;
-    if ((e = cudaMallocAsync(reinterpret_cast<void**>(&w->lists), sizeof(int) * 3 * (size_t)A.rows, st)) != cudaSuccess) return e;
-    if ((e = cudaMallocAsync(reinterpret_cast<void**>(&w->range), sizeof(int2) * (size_t)A.rows, st)) != cudaSuccess) return e;
-    if ((e = cudaMallocAsync(reinterpret_cast<void**>(&w->bin_size), 32, st)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(w->bin_size, 0, 32, st)) != cudaSuccess) return e;
-    spvec_bound_kernel<<<warps_grid(A.rows), 256, 0, st>>>(A, B, w->lists, w->bin_size, w->range);
+    if ((e = w->lists.alloc(sizeof(int) * 3 * (size_t)A.rows, st)) != cudaSuccess) return e;
+    if ((e = w->range.alloc(sizeof(int2) * (size_t)A.rows, st)) != cudaSuccess) return e;
+    if ((e = w->bin_size.alloc(32, st)) != cudaSuccess) return e;
+    int *lists = w->lists.as<int>(), *bin_size = w->bin_size.as<int>();
+    if ((e = cudaMemsetAsync(bin_size, 0, 32, st)) != cudaSuccess) return e;
+    spvec_bound_kernel<<<warps_grid(A.rows), 256, 0, st>>>(A, B, lists, bin_size, w->range.as<int2>());
     ++*launches;
-    if ((e = cudaMemcpyAsync(w->bins, w->bin_size, sizeof(w->bins), cudaMemcpyDeviceToHost, st)) != cudaSuccess) return e;
+    if ((e = cudaMemcpyAsync(w->bins, bin_size, sizeof(w->bins), cudaMemcpyDeviceToHost, st)) != cudaSuccess) return e;
     if ((e = cudaStreamSynchronize(st)) != cudaSuccess) return e;
     const long long n = A.rows;
     if (w->bins[0]) {
-        spvec_warp_kernel<false><<<(w->bins[0] + ROW_WARPS - 1) / ROW_WARPS, 32 * ROW_WARPS, 0, st>>>(A, B, w->lists, w->bins[0],
+        spvec_warp_kernel<false><<<(w->bins[0] + ROW_WARPS - 1) / ROW_WARPS, 32 * ROW_WARPS, 0, st>>>(A, B, lists, w->bins[0],
                                                                                                       rowptr, nullptr, nullptr);
         ++*launches;
     }
     if (w->bins[1]) {
-        spvec_cta_kernel<false><<<w->bins[1], CTA_THREADS, sizeof(int) * CTA_SLOTS, st>>>(A, B, w->lists + n, rowptr, nullptr,
+        spvec_cta_kernel<false><<<w->bins[1], CTA_THREADS, sizeof(int) * CTA_SLOTS, st>>>(A, B, lists + n, rowptr, nullptr,
                                                                                           nullptr);
         ++*launches;
     }
     if (w->bins[2]) {
         const size_t smem = sizeof(unsigned) * (WINDOW / 32) + sizeof(int) * CTA_THREADS;
-        spvec_window_kernel<false><<<w->bins[2], CTA_THREADS, smem, st>>>(A, B, w->lists + 2 * n, w->range, rowptr, nullptr,
+        spvec_window_kernel<false><<<w->bins[2], CTA_THREADS, smem, st>>>(A, B, lists + 2 * n, w->range.as<int2>(), rowptr, nullptr,
                                                                           nullptr);
         ++*launches;
     }
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    return scan(rowptr, A.rows, reinterpret_cast<long long*>(w->bin_size + 4), total, st, launches);
+    return scan(rowptr, A.rows, reinterpret_cast<long long*>(bin_size + 4), total, st, launches);
 }
 
 cudaError_t spvec_fill(const CsrView& A, const CsrView& B, const SpvecWork& w, const int* rowptr, int* colidx, double* vals,
@@ -374,8 +375,9 @@ cudaError_t spvec_fill(const CsrView& A, const CsrView& B, const SpvecWork& w, c
     *launches = 0;
     const long long n = A.rows;
     int* rp = const_cast<int*>(rowptr);
+    const int* lists = w.lists.as<int>();
     if (w.bins[0]) {
-        spvec_warp_kernel<true><<<(w.bins[0] + ROW_WARPS - 1) / ROW_WARPS, 32 * ROW_WARPS, 0, st>>>(A, B, w.lists, w.bins[0], rp,
+        spvec_warp_kernel<true><<<(w.bins[0] + ROW_WARPS - 1) / ROW_WARPS, 32 * ROW_WARPS, 0, st>>>(A, B, lists, w.bins[0], rp,
                                                                                                     colidx, vals);
         ++*launches;
     }
@@ -383,24 +385,17 @@ cudaError_t spvec_fill(const CsrView& A, const CsrView& B, const SpvecWork& w, c
         const size_t smem = (sizeof(int) + sizeof(float)) * CTA_SLOTS;
         cudaError_t e = cudaFuncSetAttribute(spvec_cta_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
-        spvec_cta_kernel<true><<<w.bins[1], CTA_THREADS, smem, st>>>(A, B, w.lists + n, rp, colidx, vals);
+        spvec_cta_kernel<true><<<w.bins[1], CTA_THREADS, smem, st>>>(A, B, lists + n, rp, colidx, vals);
         ++*launches;
     }
     if (w.bins[2]) {
         const size_t smem = sizeof(unsigned) * (WINDOW / 32) + sizeof(int) * CTA_THREADS + sizeof(float) * WINDOW;
         cudaError_t e = cudaFuncSetAttribute(spvec_window_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
-        spvec_window_kernel<true><<<w.bins[2], CTA_THREADS, smem, st>>>(A, B, w.lists + 2 * n, w.range, rp, colidx, vals);
+        spvec_window_kernel<true><<<w.bins[2], CTA_THREADS, smem, st>>>(A, B, lists + 2 * n, w.range.as<int2>(), rp, colidx, vals);
         ++*launches;
     }
     return cudaGetLastError();
-}
-
-void spvec_release(SpvecWork* w, cudaStream_t st) {
-    if (w->lists) cudaFreeAsync(w->lists, st);
-    if (w->range) cudaFreeAsync(w->range, st);
-    if (w->bin_size) cudaFreeAsync(w->bin_size, st);
-    *w = SpvecWork{};
 }
 
 cudaError_t dense_rows_count(DView D, int rows, int cols, int* rowptr, long long* total, cudaStream_t st, int* launches) {
@@ -408,14 +403,12 @@ cudaError_t dense_rows_count(DView D, int rows, int cols, int* rowptr, long long
     *total = 0;
     cudaError_t e = cudaMemsetAsync(rowptr, 0, sizeof(int) * ((size_t)rows + 1), st);
     if (e != cudaSuccess || rows == 0) return e;
-    long long* total_d = nullptr;
-    if ((e = cudaMallocAsync(reinterpret_cast<void**>(&total_d), sizeof(long long), st)) != cudaSuccess) return e;
+    StreamBuffer total_d;
+    if ((e = total_d.alloc(sizeof(long long), st)) != cudaSuccess) return e;
     dense_rows_kernel<false><<<warps_grid(rows), 256, 0, st>>>(D, rows, cols, rowptr, nullptr, nullptr);
     ++*launches;
     e = cudaGetLastError();
-    if (e == cudaSuccess) e = scan(rowptr, rows, total_d, total, st, launches);
-    cudaFreeAsync(total_d, st);
-    return e;
+    return e == cudaSuccess ? scan(rowptr, rows, total_d.as<long long>(), total, st, launches) : e;
 }
 
 cudaError_t dense_rows_compact(DView D, int rows, int cols, const int* rowptr, int* colidx, double* vals, cudaStream_t st) {

@@ -1,14 +1,15 @@
 #pragma once
 #include "sparse.h"
+#include "stream_buffer.h"
 
 namespace mb {
 
 // Device scratch of one row-wise product, made by spvec_count and used by spvec_fill: the rows of each bin and each row's
-// candidate column range.  spvec_release returns it (stream-ordered).
+// candidate column range.
 struct SpvecWork {
-    int* lists = nullptr;        // bin b's rows at lists[b * rows .. + bins[b])
-    int2* range = nullptr;       // lowest and highest column any product of the row can reach
-    int* bin_size = nullptr;     // 3 counters, then the int64 total
+    StreamBuffer lists;          // int: bin b's rows at lists[b * rows .. + bins[b])
+    StreamBuffer range;          // int2: lowest and highest column any product of the row can reach
+    StreamBuffer bin_size;       // int: 3 counters, then the int64 total
     int bins[3] = {0, 0, 0};
 };
 
@@ -21,7 +22,6 @@ cudaError_t spvec_count(const CsrView& A, const CsrView& B, int* rowptr, long lo
 // to double.
 cudaError_t spvec_fill(const CsrView& A, const CsrView& B, const SpvecWork& w, const int* rowptr, int* colidx, double* vals,
                        cudaStream_t st, int* launches);
-void spvec_release(SpvecWork* w, cudaStream_t st);
 
 // Row-major dense rows (rows x cols view D) -> CSR keeping v != 0.0.  The count pass writes rowptr (rows + 1) and *total
 // (one stream synchronisation); the compact pass fills colidx / vals.
