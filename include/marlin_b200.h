@@ -446,6 +446,36 @@ int32_t mb_pagerank_host(mb_ctx* ctx, int32_t n, int64_t num_rows, const int64_t
                          const int32_t* targets, const double* values, double damping, int64_t seg_len, double addend,
                          int32_t iterations, double* ranks_inout);
 
+/* ---- The NeuralNetwork example (examples/NeuralNetwork.scala): mini-batch SGD on a two-layer sigmoid network with ten
+ *      output units.  For the selected row blocks X_b (r_b x V) of one iteration, with W1 (V x H) and W2 (H x 10):
+ *        Z1_b = X_b W1 (:222-225); A1_b = sigmoid(Z1_b), A2_b = sigmoid(A1_b W2) (:226-231);
+ *        D2_b = (1 - A2_b) A2_b (A2_b - onehot(labels_b)) (:119-128, :152-162); D1_b = (1 - A1_b) A1_b (D2_b W2^T) (:240-241);
+ *        dW2 = sum_b fl(scale * A1_b^T D2_b), dW1 = sum_b fl(scale * X_b^T D1_b), blocks in the order given
+ *        (computeWeightUpd :171-183 with scale = learningRate / batchSize; the reference's treeReduce order is not fixed).
+ *      Z1_b and X_b^T D1_b run on the fp64 DMMA GEMM; everything between them is one fused kernel per block, so the
+ *      activations never reach device memory and the hidden layer is written once (Z1) and replaced once (D1).  XT[b] is
+ *      X_b^T materialised (V x r_b, column-major): with it, X_b^T D1_b is split over its r_b-long inner dimension into
+ *      chunks that run as entries of one grouped launch, which fills the SMs where one GEMM of (V/128) x (H/128) tiles
+ *      cannot.  XT, or any XT[b], may be NULL, and an XT[b] that is not 16-byte aligned with an even leading dimension (an
+ *      odd V) is not used: that block's product is then one transposed-A GEMM over X_b.  W1, W2 and the outputs are
+ *      column-major fp64 blocks; a bf16 or fp32 block anywhere is MB_ERR_UNSUPPORTED, a shape that does not fit
+ *      MB_ERR_DIM_MISMATCH.  Sums run in a fixed order: the same call gives the same bits.  Nothing here synchronises with
+ *      the host; device temporaries are returned in stream order. ---- */
+/* `count` labels of one block (DistributedIntVector piece, :71-80) as a device array for the two entries below.  A label
+ * outside 0..9 is MB_ERR_INVALID_ARG naming its row (ArrayIndexOutOfBounds in computeOutputError on the JVM). */
+int32_t mb_nn_labels_upload(mb_ctx* ctx, const int32_t* labels, int64_t count, void** labels_out);
+int32_t mb_nn_labels_free(mb_ctx* ctx, void* labels);
+/* The two scaled gradient sums of the nsel blocks one rank holds: dW1_out (V x H) and dW2_out (H x 10).  labels[b] comes
+ * from mb_nn_labels_upload and holds X[b]->rows labels.  D1_out is NULL or nsel blocks (each NULL or r_b x H, column-major)
+ * that receive D1_b; without one, D1_b replaces Z1_b in the call's workspace. */
+int32_t mb_nn_gradient(mb_ctx* ctx, const mb_block* const* X, const mb_block* const* XT, const void* const* labels,
+                       int32_t nsel, const mb_block* W1, const mb_block* W2, double scale, mb_block* dW1_out,
+                       mb_block* dW2_out, mb_block* const* D1_out);
+/* One iteration on one rank (:219-248): the same, then W1 -= dW1 and W2 -= dW2, both from the W2 before the step.  The
+ * weights stay on the device between steps. */
+int32_t mb_nn_step(mb_ctx* ctx, const mb_block* const* X, const mb_block* const* XT, const void* const* labels, int32_t nsel,
+                   mb_block* W1, mb_block* W2, double scale);
+
 /* ---- a7/a8: strategy + partitioning (pure integer logic) --------------------------------- */
 /* MTUtils.splitMethod(m,k,n,cores) (utils/MTUtils.scala:150-175, dimToSplit :204-213) */
 int32_t mb_choose_split(int64_t m, int64_t k, int64_t n, int32_t cores, int32_t out_mkn[3]);

@@ -1502,4 +1502,44 @@ inline std::vector<std::vector<double>> pageRank(const SparseVecMatrix& linkRows
     return {std::vector<double>(ranks.begin(), ranks.begin() + seg), std::vector<double>(ranks.begin() + seg, ranks.end())};
 }
 
+namespace examples {
+// One iteration of examples/NeuralNetwork.scala:219-248 over the selected blocks (mb_nn_step): the row blocks X_b with their
+// labels, the materialised transposes X_b^T (made once: the data never changes) and the two weights, which stay on the
+// device between steps.  learningRate / batchSize scales each block's product as computeWeightUpd does.
+class NeuralNetwork {
+public:
+    NeuralNetwork(const DenseMatrix& hiddenWeight, const DenseMatrix& outputWeight) : w1_(hiddenWeight), w2_(outputWeight) {}
+    ~NeuralNetwork() { for (void* p : labels_) mb_nn_labels_free(Context::get(), p); }
+    NeuralNetwork(const NeuralNetwork&) = delete;
+    NeuralNetwork& operator=(const NeuralNetwork&) = delete;
+    // A row block and its labels (one in 0..9 per row); returns its index for step().
+    int addBlock(const DenseMatrix& rows, const std::vector<int32_t>& labels) {
+        if ((size_t)rows.rows != labels.size()) throw std::invalid_argument("NeuralNetwork: one label per row");
+        void* p = nullptr;
+        check(mb_nn_labels_upload(Context::get(), labels.data(), (int64_t)labels.size(), &p));
+        labels_.push_back(p);
+        x_.emplace_back(rows);
+        xt_.push_back(x_.back().transpose());
+        return (int)x_.size() - 1;
+    }
+    void step(const std::vector<int>& selected, double learningRate, int batchSize) {
+        std::vector<const mb_block*> x, xt;
+        std::vector<const void*> l;
+        for (int b : selected) {
+            x.push_back(x_.at((size_t)b).handle());
+            xt.push_back(xt_[(size_t)b].handle());
+            l.push_back(labels_[(size_t)b]);
+        }
+        check(mb_nn_step(Context::get(), x.data(), xt.data(), l.data(), (int32_t)x.size(), w1_.handle(), w2_.handle(),
+                         learningRate / batchSize));
+    }
+    DenseMatrix hiddenWeight() const { return w1_.denseBlock(); }
+    DenseMatrix outputWeight() const { return w2_.denseBlock(); }
+private:
+    SubMatrix w1_, w2_;
+    std::vector<SubMatrix> x_, xt_;
+    std::vector<void*> labels_;
+};
+}  // namespace examples
+
 }  // namespace marlin

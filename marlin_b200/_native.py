@@ -126,6 +126,11 @@ SIGNATURES = {
     "mb_pagerank_train": (c_i32, [c_ctx, c_sp, c_i64, c_f64, c_i32, c_blk]),
     "mb_pagerank_host": (c_i32, [c_ctx, c_i32, c_i64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, c_f64, c_i64, c_f64, c_i32,
                                  C.c_void_p]),
+    "mb_nn_labels_upload": (c_i32, [c_ctx, C.c_void_p, c_i64, C.POINTER(C.c_void_p)]),
+    "mb_nn_labels_free": (c_i32, [c_ctx, C.c_void_p]),
+    "mb_nn_gradient": (c_i32, [c_ctx, C.POINTER(c_blk), C.POINTER(c_blk), C.POINTER(C.c_void_p), c_i32, c_blk, c_blk, c_f64, c_blk,
+                               c_blk, C.POINTER(c_blk)]),
+    "mb_nn_step": (c_i32, [c_ctx, C.POINTER(c_blk), C.POINTER(c_blk), C.POINTER(C.c_void_p), c_i32, c_blk, c_blk, c_f64]),
     "mb_hash_seed": (c_i64, [c_i64]),
     "mb_partition_seeds": (c_i32, [c_i64, c_i32, C.POINTER(c_i64)]),
     "mb_choose_split": (c_i32, [c_i64, c_i64, c_i64, c_i32, C.POINTER(c_i32)]),

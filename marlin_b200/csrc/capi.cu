@@ -14,6 +14,7 @@
 #include "als.h"
 #include "spvec.h"
 #include "pagerank.h"
+#include "mlp.h"
 
 #include <cuda_runtime.h>
 #include <climits>
@@ -1982,6 +1983,181 @@ int32_t mb_pagerank_host(mb_ctx* ctx, int32_t n, int64_t num_rows, const int64_t
     if ((r = mb_pagerank_train(ctx, l, seg_len, addend, iterations, xb)) != MB_OK) return r;
     e = cudaMemcpy(ranks_inout, f64_ptr(xb), sizeof(double) * (size_t)n, cudaMemcpyDeviceToHost);
     return e == cudaSuccess ? MB_OK : cuda_fail(e, "mb_pagerank_host");
+}
+
+// ------------------------------------------------------------------------------ NeuralNetwork (examples/NeuralNetwork.scala)
+int32_t mb_nn_labels_upload(mb_ctx* ctx, const int32_t* labels, int64_t count, void** labels_out) {
+    if (labels_out) *labels_out = nullptr;
+    MB_CTX(ctx);
+    if (!labels || !labels_out || count <= 0) return fail(MB_ERR_INVALID_ARG, "mb_nn_labels_upload: null or empty labels");
+    for (int64_t i = 0; i < count; ++i)
+        if (labels[i] < 0 || labels[i] >= mb::NN_CLASSES)
+            return fail(MB_ERR_INVALID_ARG, "NeuralNetwork: label %d of row %lld is outside 0..%d", labels[i], (long long)i, mb::NN_CLASSES - 1);
+    void* d = nullptr;
+    MB_CUDA(cudaMalloc(&d, sizeof(int32_t) * (size_t)count));
+    const cudaError_t e = cudaMemcpy(d, labels, sizeof(int32_t) * (size_t)count, cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) {
+        cudaFree(d);
+        return cuda_fail(e, "mb_nn_labels_upload");
+    }
+    *labels_out = d;
+    return MB_OK;
+}
+
+int32_t mb_nn_labels_free(mb_ctx* ctx, void* labels) {
+    MB_CTX(ctx);
+    MB_CUDA(cudaFree(labels));
+    return MB_OK;
+}
+
+// A column-major fp64 block of the given shape, or the error that says what it is instead.
+static int32_t nn_colmajor(const mb_block* b, int rows, int cols, const char* what) {
+    if (!b) return fail(MB_ERR_INVALID_ARG, "NeuralNetwork: null %s", what);
+    if (b->dtype != MB_F64) return fail(MB_ERR_UNSUPPORTED, "NeuralNetwork: %s must be fp64", what);
+    if (b->rows != rows || b->cols != cols)
+        return fail(MB_ERR_DIM_MISMATCH, "NeuralNetwork: %s is %dx%d, expected %dx%d", what, b->rows, b->cols, rows, cols);
+    if (b->is_transpose) return fail(MB_ERR_UNSUPPORTED, "NeuralNetwork: %s must be column-major", what);
+    return MB_OK;
+}
+
+// Rows [k0, k1) of block b's D1 against columns [k0, k1) of its XT: one entry of the grouped launch, one partial.
+struct NnChunk { int b, k0, k1; };
+
+// Steps 1-5 of an iteration for the blocks given.  out1 / out2 non-null: the gradient sums go there; null: W1 and W2 are updated.
+static int32_t nn_run(mb_ctx* ctx, const mb_block* const* X, const mb_block* const* XT, const void* const* labels, int nsel,
+                      const mb_block* W1, const mb_block* W2, double scale, mb_block* out1, mb_block* out2,
+                      mb_block* const* D1_out, bool update) {
+    if (!X || !labels || nsel <= 0) return fail(MB_ERR_INVALID_ARG, "NeuralNetwork: no selected blocks");
+    if (!W1 || !W2) return fail(MB_ERR_INVALID_ARG, "NeuralNetwork: null weight");
+    const int V = W1->rows, H = W1->cols;
+    if (V <= 0 || H <= 0) return fail(MB_ERR_INVALID_ARG, "NeuralNetwork: the hidden weight is %dx%d", V, H);
+    int32_t r = nn_colmajor(W1, V, H, "the hidden weight");
+    if (r == MB_OK) r = nn_colmajor(W2, H, mb::NN_CLASSES, "the output weight");
+    if (r == MB_OK && !update) r = nn_colmajor(out1, V, H, "the hidden-weight gradient");
+    if (r == MB_OK && !update) r = nn_colmajor(out2, H, mb::NN_CLASSES, "the output-weight gradient");
+    if (r) return r;
+    for (int b = 0; b < nsel; ++b) {
+        if (!X[b] || !labels[b]) return fail(MB_ERR_INVALID_ARG, "NeuralNetwork: block %d or its labels are null", b);
+        if (X[b]->dtype != MB_F64) return fail(MB_ERR_UNSUPPORTED, "NeuralNetwork: fp64 blocks only (block %d)", b);
+        if (X[b]->rows <= 0) return fail(MB_ERR_INVALID_ARG, "NeuralNetwork: block %d has no rows", b);
+        if (X[b]->cols != V)
+            return fail(MB_ERR_DIM_MISMATCH, "NeuralNetwork: block %d has %d columns, the hidden weight %d rows", b, X[b]->cols, V);
+        if (XT && XT[b]) {
+            if (XT[b]->dtype != MB_F64) return fail(MB_ERR_UNSUPPORTED, "NeuralNetwork: fp64 blocks only (transposed block %d)", b);
+            if (XT[b]->rows != V || XT[b]->cols != X[b]->rows)
+                return fail(MB_ERR_DIM_MISMATCH, "NeuralNetwork: transposed block %d is %dx%d, expected %dx%d", b, XT[b]->rows,
+                            XT[b]->cols, V, X[b]->rows);
+        }
+        if (D1_out && D1_out[b] && (r = nn_colmajor(D1_out[b], X[b]->rows, H, "a hidden-delta block")) != MB_OK) return r;
+    }
+    const int sms = ctx->num_sms;
+    const long long ldp = (V + 1) & ~1;                        // leading dimension of a hidden-weight partial
+    // chunks of the inner dimension: enough entries to give every SM a tile, at least 512 rows each, starting at multiples
+    // of 16 rows so that a chunk of D1 is as aligned as the block
+    const int tiles_per = ((V + 127) / 128) * ((H + 127) / 128);
+    const int per_block = std::max(1, ((sms + tiles_per - 1) / tiles_per + nsel - 1) / nsel);
+    std::vector<NnChunk> chunks;
+    std::vector<int> first1(1, 0), first2(1, 0);
+    std::vector<size_t> z_off(nsel), p2_off(nsel);
+    std::vector<char> grouped(nsel);
+    size_t doubles = 0;
+    for (int b = 0; b < nsel; ++b) {
+        const int rb = X[b]->rows;
+        z_off[b] = doubles;
+        doubles += (size_t)((rb + 1) & ~1) * H;
+    }
+    for (int b = 0; b < nsel; ++b) {
+        p2_off[b] = doubles;
+        const int parts = mb::nn_parts(X[b]->rows, sms);
+        doubles += (size_t)parts * H * mb::NN_CLASSES;
+        first2.push_back(first2.back() + parts);
+    }
+    for (int b = 0; b < nsel; ++b) {
+        const int rb = X[b]->rows;
+        const mb_block* d1 = D1_out ? D1_out[b] : nullptr;
+        grouped[b] = XT && XT[b] && !XT[b]->is_transpose && mb::gemm_f64_tma_eligible(f64_ptr(XT[b]), XT[b]->ld, f64_ptr(XT[b]), 2) &&
+                     (!d1 || mb::gemm_f64_tma_eligible(f64_ptr(d1), d1->ld, f64_ptr(d1), 2));
+        const int n = grouped[b] ? std::max(1, std::min(per_block, rb / 512)) : 1;
+        const int len = (((rb + n - 1) / n) + 15) & ~15;
+        for (int k0 = 0; k0 < rb; k0 += len) chunks.push_back(NnChunk{b, k0, std::min(rb, k0 + len)});
+        first1.push_back((int)chunks.size());
+    }
+    const size_t p1_off = doubles;
+    doubles += chunks.size() * (size_t)ldp * H;
+    mb::StreamBuffer ws, idx;
+    MB_CUDA(ws.alloc(doubles * sizeof(double), ctx->stream));
+    std::vector<int> firsts(first1);
+    firsts.insert(firsts.end(), first2.begin(), first2.end());
+    MB_CUDA(idx.upload(firsts.data(), firsts.size() * sizeof(int), ctx->stream));
+    double* base = ws.as<double>();
+    int launches = 0;
+    cudaError_t e = cudaSuccess;
+    // Z1_b = X_b W1, then the fused output layer and both deltas; D1_b replaces Z1_b unless the caller wants it elsewhere
+    for (int b = 0; b < nsel && e == cudaSuccess; ++b) {
+        const int rb = X[b]->rows;
+        const long long ldz = (rb + 1) & ~1;
+        double* z = base + z_off[b];
+        e = mb::gemm_f64(X[b]->is_transpose, false, rb, H, V, 1.0, f64_ptr(X[b]), X[b]->ld, f64_ptr(W1), W1->ld, 0.0, z, ldz, sms,
+                         ctx->stream, false, &launches);
+        if (e != cudaSuccess) break;
+        const mb_block* d1 = D1_out ? D1_out[b] : nullptr;
+        e = mb::nn_backprop_f64(z, ldz, rb, H, f64_ptr(W2), W2->ld, static_cast<const int*>(labels[b]), d1 ? f64_ptr(d1) : z,
+                                d1 ? d1->ld : ldz, base + p2_off[b], sms, ctx->stream);
+        ++launches;
+    }
+    // X_b^T D1_b: the chunks of the blocks with a usable XT as entries of grouped launches, the other blocks one GEMM each
+    static thread_local mb::G2Launch L;
+    L = mb::G2Launch();
+    for (size_t c = 0; c < chunks.size() && e == cudaSuccess; ++c) {
+        const NnChunk& ch = chunks[c];
+        const mb_block* d1b = D1_out ? D1_out[ch.b] : nullptr;
+        const double* d1 = d1b ? f64_ptr(d1b) : base + z_off[ch.b];
+        const long long ldd = d1b ? d1b->ld : (X[ch.b]->rows + 1) & ~1;
+        double* P = base + p1_off + c * (size_t)ldp * H;
+        if (!grouped[ch.b]) {
+            const mb_block* x = X[ch.b];
+            e = mb::gemm_f64(!x->is_transpose, false, V, H, x->rows, 1.0, f64_ptr(x), x->ld, d1, ldd, 0.0, P, ldp, sms, ctx->stream,
+                             false, &launches);
+            continue;
+        }
+        mb::G2Operand& A = L.A[L.na];
+        A.ptr = f64_ptr(XT[ch.b]) + (long long)ch.k0 * XT[ch.b]->ld; A.ld = XT[ch.b]->ld; A.rows = V; A.cols = ch.k1 - ch.k0;
+        mb::G2Operand& B = L.B[L.nb];
+        B.ptr = d1 + ch.k0; B.ld = ldd; B.rows = ch.k1 - ch.k0; B.cols = H;
+        mb::G2Entry& en = L.E[L.ne++];
+        en.nseg = 1; en.a_op[0] = L.na++; en.b_op[0] = L.nb++;
+        en.M = V; en.N = H; en.D = P; en.ldd = ldp;
+        if (L.ne == mb::G2_MAX_OPS) {
+            e = mb::gemm_f64_grouped2(L, sms, ctx->stream, &launches);
+            L = mb::G2Launch();
+        }
+    }
+    if (e == cudaSuccess && L.ne > 0) e = mb::gemm_f64_grouped2(L, sms, ctx->stream, &launches);
+    const int* first = idx.as<int>();
+    if (e == cudaSuccess)
+        e = mb::nn_apply_f64(base + p1_off, ldp, ldp * H, first, nsel, V, H, scale, update ? nullptr : f64_ptr(out1),
+                             update ? 0 : out1->ld, update ? f64_ptr(W1) : nullptr, W1->ld, ctx->stream);
+    if (e == cudaSuccess)
+        e = mb::nn_apply_f64(base + p2_off[0], H, (long long)H * mb::NN_CLASSES, first + nsel + 1, nsel, H, mb::NN_CLASSES, scale,
+                             update ? nullptr : f64_ptr(out2), update ? 0 : out2->ld, update ? f64_ptr(W2) : nullptr, W2->ld,
+                             ctx->stream);
+    ctx->launches += launches + 2;
+    return e == cudaSuccess ? MB_OK : cuda_fail(e, "NeuralNetwork");
+}
+
+int32_t mb_nn_gradient(mb_ctx* ctx, const mb_block* const* X, const mb_block* const* XT, const void* const* labels,
+                       int32_t nsel, const mb_block* W1, const mb_block* W2, double scale, mb_block* dW1_out,
+                       mb_block* dW2_out, mb_block* const* D1_out) {
+    MB_CTX(ctx);
+    MB_LOCK(ctx);
+    return nn_run(ctx, X, XT, labels, nsel, W1, W2, scale, dW1_out, dW2_out, D1_out, false);
+}
+
+int32_t mb_nn_step(mb_ctx* ctx, const mb_block* const* X, const mb_block* const* XT, const void* const* labels, int32_t nsel,
+                   mb_block* W1, mb_block* W2, double scale) {
+    MB_CTX(ctx);
+    MB_LOCK(ctx);
+    return nn_run(ctx, X, XT, labels, nsel, W1, W2, scale, nullptr, nullptr, nullptr, true);
 }
 
 }  // extern "C"

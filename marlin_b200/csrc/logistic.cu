@@ -41,17 +41,6 @@ struct LrShape {
     int ntiles;
 };
 
-// 16-byte-aligned span [a0, a0 + bytes) covering row piece p..p+cw; the piece starts lead doubles into it.
-__device__ __forceinline__ const double* piece_span(const double* p, int cw, uint32_t* bytes, int* lead) {
-    const uintptr_t a = reinterpret_cast<uintptr_t>(p);
-    const uintptr_t a0 = a & ~uintptr_t(15), a1 = (a + uintptr_t(cw) * 8 + 15) & ~uintptr_t(15);
-    *bytes = static_cast<uint32_t>(a1 - a0);
-    *lead = static_cast<int>((a - a0) >> 3);
-    return reinterpret_cast<const double*>(a0);
-}
-
-__device__ __forceinline__ int piece_lead(const double* p) { return static_cast<int>((reinterpret_cast<uintptr_t>(p) & 15) >> 3); }
-
 // Warp 0 (all lanes): issue load k of this CTA's sequence into stage k % LR_STAGES, if it exists.
 __device__ __forceinline__ void lr_issue(const LrShape& s, int k, double* ring, uint64_t* full) {
     const int q = k / s.per_tile;

@@ -60,6 +60,18 @@ __device__ __forceinline__ void bulk_load(uint32_t dst_smem, const void* src, ui
                  ::"r"(dst_smem), "l"(src), "r"(bytes), "r"(bar)
                  : "memory");
 }
+// 16-byte-aligned span [a0, a0 + bytes) covering the cw doubles at p, for a bulk_load of doubles that are only 8-byte
+// aligned; the doubles start lead doubles into it.
+__device__ __forceinline__ const double* piece_span(const double* p, int cw, uint32_t* bytes, int* lead) {
+    const uintptr_t a = reinterpret_cast<uintptr_t>(p);
+    const uintptr_t a0 = a & ~uintptr_t(15), a1 = (a + uintptr_t(cw) * 8 + 15) & ~uintptr_t(15);
+    *bytes = static_cast<uint32_t>(a1 - a0);
+    *lead = static_cast<int>((a - a0) >> 3);
+    return reinterpret_cast<const double*>(a0);
+}
+
+__device__ __forceinline__ int piece_lead(const double* p) { return static_cast<int>((reinterpret_cast<uintptr_t>(p) & 15) >> 3); }
+
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src_smem, int32_t c0, int32_t c1) {
     asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
                  ::"l"(reinterpret_cast<uint64_t>(map)), "r"(src_smem), "r"(c0), "r"(c1)

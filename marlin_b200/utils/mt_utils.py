@@ -103,6 +103,19 @@ class UniformGenerator:
         self.start, self.end = float(start), float(end)
 
 
+def _svm_vector(items, vectorLen: int) -> np.ndarray:
+    """The `i:v` entries of one SVM-format line as a dense vector: entry i sets element i - 1 (a later entry for the same
+    index wins); an index outside 1..vectorLen is rejected (ArrayIndexOutOfBoundsException on the JVM)."""
+    vec = np.zeros(vectorLen)
+    for item in items:
+        ind, val = item.split(":")[:2]
+        i = int(ind) - 1
+        if not 0 <= i < vectorLen:
+            raise nat.MarlinArgumentError(nat.MB_ERR_INVALID_ARG, f"index {i} out of bounds for length {vectorLen}")
+        vec[i] = float(val)
+    return vec
+
+
 class MTUtils:
     # ------------------------------------------------------------------ seeds / RNG plumbing
     @staticmethod
@@ -407,14 +420,7 @@ class MTUtils:
             items = line.split(" ")
             while items and items[-1] == "":                 # java.lang.String.split drops trailing empty strings
                 items.pop()
-            vec = np.zeros(vectorLen)
-            for item in items[1:]:
-                ind, val = item.split(":")[:2]
-                i = int(ind) - 1
-                if not 0 <= i < vectorLen:
-                    raise nat.MarlinArgumentError(nat.MB_ERR_INVALID_ARG, f"index {i} out of bounds for length {vectorLen}")
-                vec[i] = float(val)
-            rows.append((int(items[0]), vec))
+            rows.append((int(items[0]), _svm_vector(items[1:], vectorLen)))
         return DenseVecMatrix(rows, 0, vectorLen)
 
     @staticmethod
