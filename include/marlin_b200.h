@@ -58,7 +58,8 @@ const char* mb_version(void);
 int32_t     mb_set_stream(mb_ctx* ctx, void* cuda_stream);
 int32_t     mb_reset_stream(mb_ctx* ctx);
 int32_t     mb_synchronize(mb_ctx* ctx);
-/* Number of kernels this library has launched on ctx since init (bench.py's gpu_launches). */
+/* Number of kernels enqueued by calls on ctx since init, the kernel nodes of graph launches included (bench.py's
+ * gpu_launches).  Memsets, copies and stream memory operations are not counted; a call that launches nothing adds nothing. */
 int64_t     mb_launch_count(mb_ctx* ctx);
 /* CUDA-event timing on the ctx stream, so callers can time kernels on the launching stream. */
 int32_t     mb_timer_start(mb_ctx* ctx);

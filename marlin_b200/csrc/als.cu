@@ -17,6 +17,7 @@
 // the entity: its row is left unwritten and the lowest such entity id is kept in *bad.
 // The host orders the work list heaviest first, so a long-tailed user starts early instead of ending the launch alone.
 #include "als.h"
+#include "launch.h"
 
 #include <climits>
 
@@ -201,7 +202,7 @@ cudaError_t launch(AlsArgs a, cudaStream_t st) {
     if (e != cudaSuccess) return e;
     const long long grid = (a.L.count + GROUPS - 1) / GROUPS;
     als_kernel<G, EPT, SOLVE><<<(unsigned)grid, ALS_THREADS, smem, st>>>(a);
-    return cudaGetLastError();
+    return launched();
 }
 
 template <bool SOLVE>
@@ -234,7 +235,7 @@ cudaError_t coo_scatter_rows(long long nnz, const int32_t* row, const int32_t* c
                              long long ld, cudaStream_t st) {
     if (nnz <= 0) return cudaSuccess;
     coo_scatter_kernel<<<(unsigned)((nnz + 255) / 256), 256, 0, st>>>(nnz, row, col, val, out, ld);
-    return cudaGetLastError();
+    return launched();
 }
 
 }  // namespace mb

@@ -9,6 +9,7 @@
 // Multiplies and adds round separately (the JVM never contracts to an FMA), so a gemv that fits one column
 // chunk reproduces F2J's dgemv bit for bit.
 #include "blas12.h"
+#include "launch.h"
 
 #include <cstdint>
 
@@ -241,18 +242,15 @@ size_t gemv_workspace_doubles(bool trans, int m, int n) {
 }
 
 cudaError_t gemv_f64(bool trans, int m, int n, const double* a, long long lda, const double* x, long long incx, double* y,
-                     long long incy, bool accumulate, double* workspace, cudaStream_t st, int* launches) {
+                     long long incy, bool accumulate, double* workspace, cudaStream_t st) {
     const int len = trans ? n : m;          // result length
     const int red = trans ? m : n;          // contraction length
-    *launches = 0;
     if (len == 0) return cudaSuccess;
     if (red == 0) {
         // empty contraction: y = 0 (or unchanged when accumulating), like dgemv with beta = 0 / 1
-        if (!accumulate) {
-            fold_partials_kernel<<<(len + 255) / 256, 256, 0, st>>>(workspace, 0, len, y, incy, 0);
-            ++*launches;
-        }
-        return cudaGetLastError();
+        if (accumulate) return cudaSuccess;
+        fold_partials_kernel<<<(len + 255) / 256, 256, 0, st>>>(workspace, 0, len, y, incy, 0);
+        return launched();
     }
     int nparts;
     if (!trans) {
@@ -267,9 +265,9 @@ cudaError_t gemv_f64(bool trans, int m, int n, const double* a, long long lda, c
         dim3 grid((n + GEMV_T_WARPS - 1) / GEMV_T_WARPS, nparts);
         gemv_t_kernel<<<grid, GEMV_T_WARPS * 32, 0, st>>>(a, lda, m, n, x, incx, workspace);
     }
+    if (const cudaError_t e = launched(); e != cudaSuccess) return e;
     fold_partials_kernel<<<(len + 255) / 256, 256, 0, st>>>(workspace, nparts, len, y, incy, accumulate ? 1 : 0);
-    *launches = 2;
-    return cudaGetLastError();
+    return launched();
 }
 
 cudaError_t ger_f64(int m, int n, const double* x, long long incx, const double* y, long long incy, double* out,
@@ -278,7 +276,7 @@ cudaError_t ger_f64(int m, int n, const double* x, long long incx, const double*
     dim3 grid((n + GER_COLS - 1) / GER_COLS, (m + GEMV_ROWS - 1) / GEMV_ROWS);
     if (grid.y > 65535) return cudaErrorInvalidValue;
     ger_kernel<<<grid, GEMV_THREADS, 0, st>>>(m, n, x, incx, y, incy, out, ldo);
-    return cudaGetLastError();
+    return launched();
 }
 
 int dot_scratch_doubles() { return 4096 + 1; }
@@ -288,8 +286,9 @@ cudaError_t dot_f64(long long n, const double* x, long long incx, const double* 
     const long long tiles = (n + DOT_TILE - 1) / DOT_TILE;
     const int nparts = (int)(tiles < 1 ? 1 : (tiles > 4096 ? 4096 : tiles));
     dot_stage1_kernel<<<nparts, 256, 0, st>>>(n, x, incx, y, incy, scratch + 1, nparts);
+    if (const cudaError_t e = launched(); e != cudaSuccess) return e;
     dot_stage2_kernel<<<1, 256, 0, st>>>(scratch + 1, nparts, scratch);
-    return cudaGetLastError();
+    return launched();
 }
 
 }  // namespace mb

@@ -8,7 +8,7 @@ namespace mb {
 // gemv_workspace_doubles(trans, m, n) doubles of partial vectors.
 size_t gemv_workspace_doubles(bool trans, int m, int n);
 cudaError_t gemv_f64(bool trans, int m, int n, const double* a, long long lda, const double* x, long long incx, double* y,
-                     long long incy, bool accumulate, double* workspace, cudaStream_t st, int* launches);
+                     long long incy, bool accumulate, double* workspace, cudaStream_t st);
 // out (column-major m x n, ldo) = x y^T
 cudaError_t ger_f64(int m, int n, const double* x, long long incx, const double* y, long long incy, double* out,
                     long long ldo, cudaStream_t st);

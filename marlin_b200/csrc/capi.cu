@@ -83,12 +83,10 @@ int32_t binary_op(mb_ctx* ctx, int op, const mb_block* A, const mb_block* B, mb_
         MB_CUDA(mb::ew_binary_f32(op, a.rows, a.cols, reinterpret_cast<const float*>(elem_ptr(&a)), rs(&a), cs(&a),
                                   reinterpret_cast<const float*>(elem_ptr(&b)), rs(&b), cs(&b), reinterpret_cast<float*>(elem_ptr(&o)),
                                   rs(&o), cs(&o), ctx->stream));
-        ctx->launches++;
         return MB_OK;
     }
     MB_CUDA(mb::ew_binary(op, a.rows, a.cols, f64_ptr(&a), rs(&a), cs(&a), f64_ptr(&b), rs(&b), cs(&b), f64_ptr(&o), rs(&o), cs(&o),
                           ctx->stream));
-    ctx->launches++;
     return MB_OK;
 }
 
@@ -101,7 +99,6 @@ int32_t unary_op(mb_ctx* ctx, int op, const mb_block* A, mb_block* out, double a
         return fail(MB_ERR_UNSUPPORTED, "%s: fp64 blocks only", name);
     const mb_block a = in_out_order(A, out), o = in_out_order(out, out);
     MB_CUDA(mb::ew_unary(op, a.rows, a.cols, f64_ptr(&a), rs(&a), cs(&a), f64_ptr(&o), rs(&o), cs(&o), alpha, beta, ctx->stream));
-    ctx->launches++;
     return MB_OK;
 }
 
@@ -126,7 +123,6 @@ int32_t copy_convert(mb_ctx* ctx, const mb_block* A, mb_block* out) {
     } else {
         MB_CUDA(mb::convert_strided(A->dtype, out->dtype, rows, cols, elem_ptr(A), ars, acs, elem_ptr(out), ors, ocs, ctx->stream));
     }
-    ctx->launches++;
     return MB_OK;
 }
 
@@ -398,20 +394,17 @@ static int32_t dgemm_device_impl(mb_ctx* ctx, char transa, char transb, int32_t 
         return fail(MB_ERR_INVALID_ARG, "dgemm: leading dimension too small (lda=%d ldb=%d ldc=%d)", lda, ldb, ldc);
     if (m == 0 || n == 0) return MB_OK;
     if (!C || (k > 0 && alpha != 0.0 && (!A || !B))) return fail(MB_ERR_INVALID_ARG, "dgemm: null pointer");
-    int launches = 0;
     if (ctx->fp64_mode != MB_FP64_NATIVE && !force_generic && !ta && !tb && alpha == 1.0 && (beta == 0.0 || beta == 1.0) &&
         m >= 256 && n >= 256 && k >= 256 && mb::ozaki_supported(m, n, k, ctx->fp64_slices, ctx->fp64_bits)) {
         cudaError_t e = grow(&ctx->ozaki_ws, &ctx->ozaki_ws_bytes, mb::ozaki_workspace_bytes(m, n, k, ctx->fp64_slices), &ctx->stream);
         if (e != cudaSuccess) return cuda_fail(e, "dgemm: int8-split workspace");
         e = mb::gemm_f64_ozaki(m, n, k, A, lda, B, ldb, C, ldc, beta == 1.0, ctx->fp64_slices, ctx->fp64_bits, ctx->ozaki_ws,
-                               ctx->num_sms, ctx->stream, &launches);
-        if (e == cudaSuccess) { ctx->launches += launches; return MB_OK; }
+                               ctx->num_sms, ctx->stream);
+        if (e == cudaSuccess) return MB_OK;
         if (e != cudaErrorNotSupported) return cuda_fail(e, "gemm_f64_ozaki");
         cudaGetLastError();
-        launches = 0;
     }
-    MB_CUDA(mb::gemm_f64(ta, tb, m, n, k, alpha, A, lda, B, ldb, beta, C, ldc, ctx->num_sms, ctx->stream, force_generic, &launches));
-    ctx->launches += launches;
+    MB_CUDA(mb::gemm_f64(ta, tb, m, n, k, alpha, A, lda, B, ldb, beta, C, ldc, ctx->num_sms, ctx->stream, force_generic));
     return MB_OK;
 }
 
@@ -544,7 +537,6 @@ static int32_t bf16_gemm(mb_ctx* ctx, bool ta, bool tb, int M, int N, int nseg, 
         if (e != cudaSuccess) return e;
         void* dst = staged.back().as<void>();
         if ((e = mb::convert_strided(MB_BF16, MB_BF16, rows, cols, p, 1, ld, dst, 1, ld8, ctx->stream)) != cudaSuccess) return e;
-        ctx->launches++;
         p = static_cast<const char*>(dst);
         ld = ld8;
         return cudaSuccess;
@@ -560,14 +552,12 @@ static int32_t bf16_gemm(mb_ctx* ctx, bool ta, bool tb, int M, int N, int nseg, 
             if (e == cudaSuccess && misaligned(pc.b, pc.ldb)) e = stage(pc.b, pc.ldb, tb ? N : pc.k, tb ? pc.k : N);
             pa[s] = pc.a; la[s] = pc.lda; pb[s] = pc.b; lb[s] = pc.ldb; ks[s] = pc.k;
         }
-        int launches = 0;
         if (e == cudaSuccess)
             e = mb::gemm_bf16_segments(ta, tb, M, N, ns, ks, pa, la, pb, lb, C, ldc, c_f32, accumulate || g > 0, ctx->num_sms,
-                                       ctx->stream, &launches);
+                                       ctx->stream);
         staged.clear();
         if (e == cudaErrorNotSupported) return fail(MB_ERR_UNSUPPORTED, "bf16 GEMM: cuTensorMapEncodeTiled is not available");
         if (e != cudaSuccess) return cuda_fail(e, "gemm_bf16_segments");
-        ctx->launches += launches;
     }
     return MB_OK;
 }
@@ -657,11 +647,9 @@ int32_t mb_matmul_blocked_subset(mb_ctx* ctx, mb_block* const* A_tiles, mb_block
         }
     }
     if (groupable) {
-        int launches = 0;
         cudaError_t e = mb::gemm_f64_grouped(m, k, n, c_ids, num_c, Ap.data(), lda.data(), Bp.data(), ldb.data(), Cp.data(),
-                                             ldc.data(), row_len.data(), k_len.data(), col_len.data(), ctx->num_sms, ctx->stream,
-                                             &launches);
-        if (e == cudaSuccess) { ctx->launches += launches; return MB_OK; }
+                                             ldc.data(), row_len.data(), k_len.data(), col_len.data(), ctx->num_sms, ctx->stream);
+        if (e == cudaSuccess) return MB_OK;
         if (e != cudaErrorNotSupported) return cuda_fail(e, "gemm_f64_grouped");
         cudaGetLastError();
     }
@@ -958,14 +946,12 @@ int32_t mb_flag_signal(mb_ctx* ctx, void* flag, int64_t value) {
     MB_CTX(ctx);
     if (!flag) return fail(MB_ERR_INVALID_ARG, "mb_flag_signal: null flag");
     MB_CUDA(mb::flag_signal(flag, (unsigned long long)value, ctx->stream));
-    ctx->launches++;
     return MB_OK;
 }
 int32_t mb_flag_wait(mb_ctx* ctx, const void* flag, int64_t value) {
     MB_CTX(ctx);
     if (!flag) return fail(MB_ERR_INVALID_ARG, "mb_flag_wait: null flag");
     MB_CUDA(mb::flag_wait(flag, (unsigned long long)value, ctx->stream));
-    ctx->launches++;
     return MB_OK;
 }
 int32_t mb_memcpy_async(mb_ctx* ctx, void* dst, const void* src, int64_t bytes) {
@@ -1015,7 +1001,6 @@ int32_t mb_block_sum(mb_ctx* ctx, const mb_block* A, double* sum_out) {
     if (A->rows == 0 || A->cols == 0) { *sum_out = 0.0; return MB_OK; }
     const int minor = A->is_transpose ? A->cols : A->rows, major = A->is_transpose ? A->rows : A->cols;
     MB_CUDA(mb::sum_f64(f64_ptr(A), minor, major, A->ld, ctx->scratch, ctx->stream));
-    ctx->launches += 2;
     MB_CUDA(cudaMemcpyAsync(ctx->host_scalar, ctx->scratch, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
     MB_CUDA(cudaStreamSynchronize(ctx->stream));
     *sum_out = *ctx->host_scalar;
@@ -1038,10 +1023,7 @@ int32_t mb_block_gemv(mb_ctx* ctx, const mb_block* A, const mb_block* x, mb_bloc
     const int m = trans ? A->cols : A->rows, n = trans ? A->rows : A->cols;
     const cudaError_t e = grow(&ctx->vec_ws, &ctx->vec_ws_bytes, mb::gemv_workspace_doubles(trans, m, n) * sizeof(double), &ctx->stream);
     if (e != cudaSuccess) return cuda_fail(e, "mb_block_gemv: workspace");
-    int launches = 0;
-    MB_CUDA(mb::gemv_f64(trans, m, n, f64_ptr(A), A->ld, xv.p, xv.inc, yv.p, yv.inc, accumulate != 0, ctx->vec_ws, ctx->stream,
-                         &launches));
-    ctx->launches += launches;
+    MB_CUDA(mb::gemv_f64(trans, m, n, f64_ptr(A), A->ld, xv.p, xv.inc, yv.p, yv.inc, accumulate != 0, ctx->vec_ws, ctx->stream));
     return MB_OK;
 }
 
@@ -1056,7 +1038,6 @@ int32_t mb_block_dot(mb_ctx* ctx, const mb_block* x, const mb_block* y, double* 
         return fail(MB_ERR_DIM_MISMATCH, "the length of these two vectors are not the same: %d vs %d", xv.len, yv.len);
     if (xv.len == 0) { *dot_out = 0.0; return MB_OK; }
     MB_CUDA(mb::dot_f64(xv.len, xv.p, xv.inc, yv.p, yv.inc, ctx->scratch, ctx->stream));
-    ctx->launches += 2;
     MB_CUDA(cudaMemcpyAsync(ctx->host_scalar, ctx->scratch, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
     MB_CUDA(cudaStreamSynchronize(ctx->stream));
     *dot_out = *ctx->host_scalar;
@@ -1073,7 +1054,6 @@ int32_t mb_block_ger(mb_ctx* ctx, const mb_block* x, const mb_block* y, mb_block
         return fail(MB_ERR_DIM_MISMATCH, "mb_block_ger: result block is %dx%d, expected %dx%d", out->rows, out->cols, xv.len, yv.len);
     if (out->is_transpose) std::swap(xv, yv);       // (x y^T)^T = y x^T in the array underneath
     MB_CUDA(mb::ger_f64(xv.len, yv.len, xv.p, xv.inc, yv.p, yv.inc, f64_ptr(out), out->ld, ctx->stream));
-    ctx->launches++;
     return MB_OK;
 }
 
@@ -1100,15 +1080,13 @@ int32_t mb_block_lu(mb_ctx* ctx, mb_block* A, int32_t* perm_out) {
     int32_t r = int_scratch(ctx, (size_t)2 * m + 8);
     if (r) return r;
     int *piv = ctx->int_ws, *perm = ctx->int_ws + m, *info = ctx->int_ws + 2 * m;
-    int launches = 0;
     // rows that are never a pivot position keep themselves: start from the identity interchange
     std::vector<int> ident(m);
     for (int i = 0; i < m; ++i) ident[i] = i;
     std::memcpy(ctx->int_host, ident.data(), sizeof(int) * m);
     MB_CUDA(cudaMemcpyAsync(piv, ctx->int_host, sizeof(int) * m, cudaMemcpyHostToDevice, ctx->stream));
     MB_CUDA(cudaStreamSynchronize(ctx->stream));
-    MB_CUDA(mb::getrf(fview(A), piv, nullptr, info, ctx->num_sms, ctx->stream, &launches));
-    ctx->launches += launches;
+    MB_CUDA(mb::getrf(fview(A), piv, nullptr, info, ctx->num_sms, ctx->stream));
     MB_CUDA(cudaMemcpyAsync(ctx->int_host, piv, sizeof(int) * (2 * (size_t)m + 1), cudaMemcpyDeviceToHost, ctx->stream));
     MB_CUDA(cudaStreamSynchronize(ctx->stream));
     if (perm_out) {
@@ -1130,9 +1108,7 @@ int32_t mb_block_cholesky(mb_ctx* ctx, mb_block* A) {
     if (A->rows == 0) return MB_OK;
     int32_t r = int_scratch(ctx, 8);
     if (r) return r;
-    int launches = 0;
-    MB_CUDA(mb::potrf_lower(fview(A), ctx->int_ws, ctx->num_sms, ctx->stream, &launches));
-    ctx->launches += launches;
+    MB_CUDA(mb::potrf_lower(fview(A), ctx->int_ws, ctx->num_sms, ctx->stream));
     MB_CUDA(cudaMemcpyAsync(ctx->int_host, ctx->int_ws, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
     MB_CUDA(cudaStreamSynchronize(ctx->stream));
     if (ctx->int_host[0] != 0)      // Breeze: NotConvergedException / MatrixNotSymmetricException family -> RuntimeException
@@ -1159,15 +1135,13 @@ int32_t mb_block_inverse(mb_ctx* ctx, const mb_block* A, mb_block* out) {
     r = copy_convert(ctx, A, &tmp);
     if (r) return r;
     int *piv = ctx->int_ws, *info = ctx->int_ws + 2 * n;
-    int launches = 0;
-    cudaError_t e = mb::getrf(fview(&tmp), piv, nullptr, info, ctx->num_sms, ctx->stream, &launches);
+    cudaError_t e = mb::getrf(fview(&tmp), piv, nullptr, info, ctx->num_sms, ctx->stream);
     if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->int_host, info, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
     if (e == cudaSuccess && ctx->int_host[0] != 0)
         return fail(MB_ERR_CUDA, "matrix is singular (zero pivot in column %d)", ctx->int_host[0] - 1);   // Breeze: MatrixSingularException
-    if (e == cudaSuccess) e = mb::inverse_from_lu(fview(&tmp), piv, fview(out), ctx->num_sms, ctx->stream, &launches);
+    if (e == cudaSuccess) e = mb::inverse_from_lu(fview(&tmp), piv, fview(out), ctx->num_sms, ctx->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    ctx->launches += launches;
     if (e != cudaSuccess) return cuda_fail(e, "mb_block_inverse");
     return MB_OK;
 }
@@ -1178,9 +1152,7 @@ int32_t mb_block_trsm(mb_ctx* ctx, const mb_block* T, int32_t lower, int32_t uni
     if (T->dtype != MB_F64 || B->dtype != MB_F64) return fail(MB_ERR_UNSUPPORTED, "mb_block_trsm: fp64 blocks only");
     if (T->rows != T->cols || T->rows != B->rows)
         return fail(MB_ERR_DIM_MISMATCH, "mb_block_trsm: triangle is %dx%d, right-hand side has %d rows", T->rows, T->cols, B->rows);
-    int launches = 0;
-    MB_CUDA(mb::trsm_left(fview(T), lower != 0, unit_diagonal != 0, fview(B), ctx->num_sms, ctx->stream, &launches));
-    ctx->launches += launches;
+    MB_CUDA(mb::trsm_left(fview(T), lower != 0, unit_diagonal != 0, fview(B), ctx->num_sms, ctx->stream));
     return MB_OK;
 }
 
@@ -1206,10 +1178,8 @@ int32_t mb_block_gramian(mb_ctx* ctx, const mb_block* A, mb_block* G) {
     const size_t need = mb::gemm_f64_tma_eligible(f64_ptr(A), A->ld, f64_ptr(A), A->ld) ? mb::gram_workspace_doubles(n, m, ctx->num_sms) : 0;
     mb::StreamBuffer ws;
     if (need) MB_CUDA(ws.alloc(need * sizeof(double), ctx->stream));
-    int launches = 0;
     const cudaError_t e = mb::gram_f64(trans, n, m, f64_ptr(A), A->ld, f64_ptr(G), G->ld, ws.as<double>(), ctx->num_sms,
-                                       ctx->stream, &launches);
-    ctx->launches += launches;
+                                       ctx->stream);
     if (e != cudaSuccess) return cuda_fail(e, "mb_block_gramian");
     return MB_OK;
 }
@@ -1232,11 +1202,9 @@ int32_t mb_block_syev(mb_ctx* ctx, const mb_block* G, mb_block* V, double* w_out
         return fail(MB_ERR_DIM_MISMATCH, "mb_block_syev: eigenvector block is %dx%d, expected %dx%d", V->rows, V->cols, G->rows, G->rows);
     constexpr int MAX_SWEEPS = 30;
     int sweeps = 0;
-    long long launches = 0;
     bool non_finite = false;
     const cudaError_t e = mb::syev_jacobi(G->rows, f64_ptr(G), rs(G), cs(G), f64_ptr(V), rs(V), cs(V), w_out, &sweeps, MAX_SWEEPS,
-                                          ctx->stream, &launches, &non_finite);
-    ctx->launches += launches;
+                                          ctx->stream, &non_finite);
     if (sweeps_out) *sweeps_out = sweeps;
     if (e == cudaSuccess && non_finite)
         return fail(MB_ERR_INVALID_ARG, "mb_block_syev: the matrix holds NaN or Inf (n = %d)", G->rows);
@@ -1280,7 +1248,6 @@ int32_t mb_lr_gradient(mb_ctx* ctx, const mb_block* rows, const double* w, doubl
     double *wd = ws.as<double>(), *g = wd + n;
     MB_CUDA(cudaMemcpyAsync(wd, w, sizeof(double) * n, cudaMemcpyHostToDevice, ctx->stream));
     MB_CUDA(mb::lr_gradient_f64(f64_ptr(&v), rs(&v), v.rows, n, wd, g + n, g, false, 0.0, ctx->num_sms, ctx->stream));
-    ctx->launches += 2;
     MB_CUDA(cudaMemcpyAsync(grad, g, sizeof(double) * n, cudaMemcpyDeviceToHost, ctx->stream));
     MB_CUDA(cudaStreamSynchronize(ctx->stream));
     return MB_OK;
@@ -1304,7 +1271,6 @@ int32_t mb_lr_train(mb_ctx* ctx, const mb_block* rows, int64_t data_size, double
         const double scale = step / (double)data_size / std::sqrt((double)i);
         MB_CUDA(mb::lr_gradient_f64(f64_ptr(&v), rs(&v), v.rows, n, wd, wd + 2 * n, nullptr, true, scale, ctx->num_sms,
                                     ctx->stream));
-        ctx->launches += 2;
     }
     MB_CUDA(cudaMemcpyAsync(w_out, wd, sizeof(double) * n, cudaMemcpyDeviceToHost, ctx->stream));
     MB_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -1374,7 +1340,6 @@ static int32_t als_half_step(mb_ctx* ctx, const mb_als_side* side, const mb_bloc
         const cudaError_t e = mb::als_solve(als_links(side), rank, Y, ldy, lambda, alpha, implicit != 0, yty, ldyty,
                                             const_cast<double*>(X), ldx, bad, ctx->stream);
         if (e != cudaSuccess) r = cuda_fail(e, "ALS update");
-        else ctx->launches++;
     }
     return r;
 }
@@ -1416,7 +1381,6 @@ int32_t mb_als_normal_equations(mb_ctx* ctx, const mb_als_side* side, const mb_b
         const cudaError_t e = mb::als_assemble(als_links(side), rank, Y, ldy, lambda, alpha, implicit != 0, yty, ldyty, A_out,
                                                b_out, ctx->stream);
         if (e != cudaSuccess) r = cuda_fail(e, "mb_als_normal_equations");
-        else ctx->launches++;
     }
     if (!r) MB_CUDA(cudaStreamSynchronize(ctx->stream));
     return r;
@@ -1527,7 +1491,6 @@ int32_t mb_coo_to_dense_rows(mb_ctx* ctx, int64_t nnz, const int32_t* row_pos, c
     MB_CUDA(d_val.upload(values, sizeof(float) * nnz, ctx->stream));
     MB_CUDA(mb::coo_scatter_rows(nnz, d_row.as<int32_t>(), d_col.as<int32_t>(), d_val.as<float>(), const_cast<double*>(p), ld,
                                  ctx->stream));
-    ctx->launches++;
     MB_CUDA(cudaStreamSynchronize(ctx->stream));
     return MB_OK;
 }
@@ -1539,10 +1502,8 @@ int32_t mb_fill_uniform(mb_ctx* ctx, mb_block* blk, int64_t partition_seed, int6
     if (blk->dtype != MB_F64) return fail(MB_ERR_UNSUPPORTED, "mb_fill_uniform: fp64 blocks only (convert afterwards)");
     // generator.setSeed(partition.seed) -> XORShiftRandom.setSeed -> seed = hashSeed(s)
     const unsigned long long state0 = (unsigned long long)mb_hash_seed(partition_seed);
-    int launches = 0;
     MB_CUDA(mb::fill_uniform_f64(f64_ptr(blk), rs(blk), cs(blk), blk->rows, blk->cols, row_major ? 1 : 0, state0, first, lo,
-                                 hi, ctx->stream, &launches));
-    ctx->launches += launches;
+                                 hi, ctx->stream));
     return MB_OK;
 }
 
@@ -1641,7 +1602,6 @@ int32_t mb_sparse_values_op(mb_ctx* ctx, const mb_sparse* S, int32_t op, double 
             const double beta = op == MB_SPARSE_ADD ? b : (op == MB_SPARSE_SUB ? -b : 0.0);
             e = mb::ew_unary(mb::EW_AXPB, n, 1, S->values, 1, n, R->values, 1, n, alpha, beta, ctx->stream);
         }
-        ctx->launches++;
     }
     if (e != cudaSuccess) return cuda_fail(e, "mb_sparse_values_op");
     *out = R.release();
@@ -1680,7 +1640,6 @@ int32_t mb_sparse_to_dense(mb_ctx* ctx, const mb_sparse* S, mb_block* out) {
     int32_t r = dense_f64_out(out, S->rows, S->cols, "toDense");
     if (r) return r;
     MB_CUDA(mb::csc_to_dense(csc(S), dview(out), ctx->stream));
-    ctx->launches++;
     return MB_OK;
 }
 
@@ -1692,7 +1651,6 @@ int32_t mb_spmm_dense_sparse(mb_ctx* ctx, const mb_block* A, const mb_sparse* B,
     int32_t r = dense_f64_out(C, A->rows, B->cols, "multDenseSparse");
     if (r) return r;
     MB_CUDA(mb::spmm_dense_sparse(A->rows, dview(A), csc(B), dview(C), accumulate != 0, ctx->stream));
-    ctx->launches++;
     return MB_OK;
 }
 
@@ -1710,18 +1668,15 @@ int32_t mb_spmm_sparse_dense(mb_ctx* ctx, mb_sparse* A, const mb_block* B, mb_bl
         cudaError_t e = cudaMalloc(&rowptr, sizeof(int) * ((size_t)A->rows + 1));
         if (e == cudaSuccess) e = cudaMalloc(&colidx, sizeof(int) * std::max<size_t>(1, (size_t)A->nnz));
         if (e == cudaSuccess) e = cudaMalloc(&vals, sizeof(double) * std::max<size_t>(1, (size_t)A->nnz));
-        int launches = 0;
-        if (e == cudaSuccess) e = mb::csc_to_csr(csc(A), A->nnz, rowptr, colidx, vals, ctx->stream, &launches);
+        if (e == cudaSuccess) e = mb::csc_to_csr(csc(A), A->nnz, rowptr, colidx, vals, ctx->stream);
         if (e != cudaSuccess) {
             cudaFree(rowptr); cudaFree(colidx); cudaFree(vals);
             return cuda_fail(e, "multSparseDense: CSR copy");
         }
-        ctx->launches += launches;
         A->csr_rowptr = rowptr; A->csr_colidx = colidx; A->csr_values = vals;
     }
     const mb::CsrView csr{A->rows, A->cols, A->csr_rowptr, A->csr_colidx, A->csr_values};
     MB_CUDA(mb::spmm_sparse_dense(csr, B->cols, dview(B), dview(C), accumulate != 0, ctx->stream));
-    ctx->launches++;
     return MB_OK;
 }
 
@@ -1732,7 +1687,6 @@ int32_t mb_spgemm_dense_out(mb_ctx* ctx, const mb_sparse* A, const mb_sparse* B,
     int32_t r = dense_f64_out(C, A->rows, B->cols, "SparseMatrix.multiply");
     if (r) return r;
     MB_CUDA(mb::spgemm_dense_out(csc(A), csc(B), dview(C), accumulate != 0, ctx->stream));
-    ctx->launches++;
     return MB_OK;
 }
 
@@ -1753,12 +1707,10 @@ int32_t mb_fill_sparse_uniform(mb_ctx* ctx, mb_sparse* S, int64_t partition_seed
         return fail(MB_ERR_UNSUPPORTED, "mb_fill_sparse_uniform: a %dx%d block exceeds the generator's 2^39 stream positions",
                     S->rows, S->cols);
     const unsigned long long state0 = (unsigned long long)mb_hash_seed(partition_seed);
-    int launches = 0;
     if (S->nnz) {
-        MB_CUDA(mb::fill_uniform_f64(S->values, 1, S->nnz, (int)S->nnz, 1, 0, state0, 0, 0.0, 1.0, ctx->stream, &launches));
+        MB_CUDA(mb::fill_uniform_f64(S->values, 1, S->nnz, (int)S->nnz, 1, 0, state0, 0, 0.0, 1.0, ctx->stream));
     }
     MB_CUDA(mb::sparse_sample_rows(S->rows, S->cols, s, state0, S->nnz, S->colptr, S->rowidx, ctx->stream));
-    ctx->launches += launches + 1;
     return MB_OK;
 }
 
@@ -1786,13 +1738,11 @@ int32_t mb_spvec_multiply(mb_ctx* ctx, const mb_sparse* A, const mb_sparse* B, m
     SparsePtr R(raw, SparseFree{ctx});
     mb::SpvecWork w;
     long long total = 0;
-    int launches = 0, more = 0;
-    cudaError_t e = mb::spvec_count(rows_of(A), rows_of(B), R->colptr, &total, &w, ctx->stream, &launches);
+    cudaError_t e = mb::spvec_count(rows_of(A), rows_of(B), R->colptr, &total, &w, ctx->stream);
     if (e == cudaSuccess && total > 0x7fffffffLL)
         return fail(MB_ERR_UNSUPPORTED, "multiplySparse: the product has %lld entries, more than 2^31 - 1", total);
     if (e == cudaSuccess) e = sparse_reserve(R.get(), total);
-    if (e == cudaSuccess && total) e = mb::spvec_fill(rows_of(A), rows_of(B), w, R->colptr, R->rowidx, R->values, ctx->stream, &more);
-    ctx->launches += launches + more;
+    if (e == cudaSuccess && total) e = mb::spvec_fill(rows_of(A), rows_of(B), w, R->colptr, R->rowidx, R->values, ctx->stream);
     if (e != cudaSuccess) return cuda_fail(e, "multiplySparse");
     *out = R.release();
     return MB_OK;
@@ -1838,17 +1788,13 @@ int32_t mb_dense_rows_to_sparse(mb_ctx* ctx, const mb_block* rows, mb_sparse** o
     if (r) return r;
     SparsePtr R(raw, SparseFree{ctx});
     long long total = 0;
-    int launches = 0;
-    cudaError_t e = mb::dense_rows_count(dview(rows), rows->rows, rows->cols, R->colptr, &total, ctx->stream, &launches);
+    cudaError_t e = mb::dense_rows_count(dview(rows), rows->rows, rows->cols, R->colptr, &total, ctx->stream);
     if (e == cudaSuccess && total > 0x7fffffffLL)
         return fail(MB_ERR_UNSUPPORTED, "toSparseVecMatrix: %lld non-zeros, more than 2^31 - 1", total);
     if (e == cudaSuccess) e = sparse_reserve(R.get(), total);
-    if (e == cudaSuccess && total) {
+    if (e == cudaSuccess && total)
         e = mb::dense_rows_compact(dview(rows), rows->rows, rows->cols, R->colptr, R->rowidx, R->values, ctx->stream);
-        ++launches;
-    }
     if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    ctx->launches += launches;
     if (e != cudaSuccess) return cuda_fail(e, "toSparseVecMatrix");
     *out = R.release();
     return MB_OK;
@@ -1870,12 +1816,10 @@ int32_t mb_fill_spvec_uniform(mb_ctx* ctx, mb_sparse* S, int64_t partition_seed,
         return fail(MB_ERR_UNSUPPORTED, "mb_fill_spvec_uniform: %d rows of %d columns exceed the generator's 2^39 stream positions",
                     S->cols, S->rows);
     const unsigned long long state0 = (unsigned long long)mb_hash_seed(partition_seed);
-    int launches = 0;
-    MB_CUDA(mb::fill_uniform_f64(S->values, 1, S->nnz, (int)S->nnz, 1, 0, state0, 0, lo, hi, ctx->stream, &launches));
+    MB_CUDA(mb::fill_uniform_f64(S->values, 1, S->nnz, (int)S->nnz, 1, 0, state0, 0, lo, hi, ctx->stream));
     // row 0's columns: one "column" of the sampler over nColumns positions, from position s*P
     MB_CUDA(mb::sparse_sample_rows(S->rows, 1, s, state0, S->nnz, S->colptr, S->rowidx, ctx->stream));
     MB_CUDA(mb::spvec_replicate_columns(S->cols, s, S->colptr, S->rowidx, ctx->stream));
-    ctx->launches += launches + 2;
     return MB_OK;
 }
 
@@ -1902,7 +1846,6 @@ static int32_t pagerank_links_of(mb_ctx* ctx, mb_sparse* L, int64_t seg_len, mb:
             cudaFree(p.heavy);
             return cuda_fail(e, "PageRank: binning the in-links");
         }
-        ctx->launches++;
         L->pagerank_heavy = p.heavy;
         L->pagerank_nheavy = p.nheavy;
     }
@@ -1923,9 +1866,7 @@ int32_t mb_pagerank_step(mb_ctx* ctx, mb_sparse* in_links, const mb_block* x, in
         return fail(MB_ERR_INVALID_ARG, "PageRank: y overlaps x");
     mb::PagerankPlan plan;
     if ((r = pagerank_links_of(ctx, in_links, seg_len, &plan)) != MB_OK) return r;
-    int launches = 0;
-    MB_CUDA(mb::pagerank_step(rows_of(in_links), plan, xp, seg_len, addend, yp, ctx->stream, &launches));
-    ctx->launches += launches;
+    MB_CUDA(mb::pagerank_step(rows_of(in_links), plan, xp, seg_len, addend, yp, ctx->stream));
     return MB_OK;
 }
 
@@ -1949,9 +1890,7 @@ int32_t mb_pagerank_train(mb_ctx* ctx, mb_sparse* in_links, int64_t seg_len, dou
     double *cur = xp, *next = scratch.as<double>();
     cudaError_t e = cudaSuccess;
     for (int it = 0; it < iterations && e == cudaSuccess; ++it) {
-        int launches = 0;
-        e = mb::pagerank_step(rows_of(in_links), plan, cur, seg_len, addend, next, ctx->stream, &launches);
-        ctx->launches += launches;
+        e = mb::pagerank_step(rows_of(in_links), plan, cur, seg_len, addend, next, ctx->stream);
         std::swap(cur, next);
     }
     if (e == cudaSuccess && cur != xp) e = cudaMemcpyAsync(xp, cur, sizeof(double) * (size_t)n, cudaMemcpyDeviceToDevice, ctx->stream);
@@ -2090,7 +2029,6 @@ static int32_t nn_run(mb_ctx* ctx, const mb_block* const* X, const mb_block* con
     firsts.insert(firsts.end(), first2.begin(), first2.end());
     MB_CUDA(idx.upload(firsts.data(), firsts.size() * sizeof(int), ctx->stream));
     double* base = ws.as<double>();
-    int launches = 0;
     cudaError_t e = cudaSuccess;
     // Z1_b = X_b W1, then the fused output layer and both deltas; D1_b replaces Z1_b unless the caller wants it elsewhere
     for (int b = 0; b < nsel && e == cudaSuccess; ++b) {
@@ -2098,12 +2036,11 @@ static int32_t nn_run(mb_ctx* ctx, const mb_block* const* X, const mb_block* con
         const long long ldz = (rb + 1) & ~1;
         double* z = base + z_off[b];
         e = mb::gemm_f64(X[b]->is_transpose, false, rb, H, V, 1.0, f64_ptr(X[b]), X[b]->ld, f64_ptr(W1), W1->ld, 0.0, z, ldz, sms,
-                         ctx->stream, false, &launches);
+                         ctx->stream, false);
         if (e != cudaSuccess) break;
         const mb_block* d1 = D1_out ? D1_out[b] : nullptr;
         e = mb::nn_backprop_f64(z, ldz, rb, H, f64_ptr(W2), W2->ld, static_cast<const int*>(labels[b]), d1 ? f64_ptr(d1) : z,
                                 d1 ? d1->ld : ldz, base + p2_off[b], sms, ctx->stream);
-        ++launches;
     }
     // X_b^T D1_b: the chunks of the blocks with a usable XT as entries of grouped launches, the other blocks one GEMM each
     static thread_local mb::G2Launch L;
@@ -2117,7 +2054,7 @@ static int32_t nn_run(mb_ctx* ctx, const mb_block* const* X, const mb_block* con
         if (!grouped[ch.b]) {
             const mb_block* x = X[ch.b];
             e = mb::gemm_f64(!x->is_transpose, false, V, H, x->rows, 1.0, f64_ptr(x), x->ld, d1, ldd, 0.0, P, ldp, sms, ctx->stream,
-                             false, &launches);
+                             false);
             continue;
         }
         mb::G2Operand& A = L.A[L.na];
@@ -2128,11 +2065,11 @@ static int32_t nn_run(mb_ctx* ctx, const mb_block* const* X, const mb_block* con
         en.nseg = 1; en.a_op[0] = L.na++; en.b_op[0] = L.nb++;
         en.M = V; en.N = H; en.D = P; en.ldd = ldp;
         if (L.ne == mb::G2_MAX_OPS) {
-            e = mb::gemm_f64_grouped2(L, sms, ctx->stream, &launches);
+            e = mb::gemm_f64_grouped2(L, sms, ctx->stream);
             L = mb::G2Launch();
         }
     }
-    if (e == cudaSuccess && L.ne > 0) e = mb::gemm_f64_grouped2(L, sms, ctx->stream, &launches);
+    if (e == cudaSuccess && L.ne > 0) e = mb::gemm_f64_grouped2(L, sms, ctx->stream);
     const int* first = idx.as<int>();
     if (e == cudaSuccess)
         e = mb::nn_apply_f64(base + p1_off, ldp, ldp * H, first, nsel, V, H, scale, update ? nullptr : f64_ptr(out1),
@@ -2141,7 +2078,6 @@ static int32_t nn_run(mb_ctx* ctx, const mb_block* const* X, const mb_block* con
         e = mb::nn_apply_f64(base + p2_off[0], H, (long long)H * mb::NN_CLASSES, first + nsel + 1, nsel, H, mb::NN_CLASSES, scale,
                              update ? nullptr : f64_ptr(out2), update ? 0 : out2->ld, update ? f64_ptr(W2) : nullptr, W2->ld,
                              ctx->stream);
-    ctx->launches += launches + 2;
     return e == cudaSuccess ? MB_OK : cuda_fail(e, "NeuralNetwork");
 }
 

@@ -571,15 +571,13 @@ int32_t products_fused(mb_comm* c, unsigned long long e, const Plan& plan, const
     std::copy_n(L0.B, L0.nb, L2.B);
     L0.ready = L2.ready = c->flags + F_BAND; L0.ready_val = L2.ready_val = e;
     L0.status = L2.status = c->flags + F_STATUS; L0.timeout_ns = L2.timeout_ns = timeout_ns(c);
-    int launches = 0;
-    cudaError_t ce = mb::gemm_f64_grouped2(L0, ctx->num_sms, ctx->stream, &launches);
+    cudaError_t ce = mb::gemm_f64_grouped2(L0, ctx->num_sms, ctx->stream);
     if (ce != cudaSuccess) return cuda_fail(ce, "gemm_f64_grouped2 (first half)");
     for (const Note& w : wrote) MB_CUDA(sig(c, c->flags_peer[w.peer] + F_PART2 + rank * MAX_PAIR + w.slot, e, ctx->stream));
     for (const Note& w : need) MB_CUDA(waitf(c, c->flags + F_PART2 + w.peer * MAX_PAIR + w.slot, e, ctx->stream));
-    ce = mb::gemm_f64_grouped2(L2, ctx->num_sms, ctx->stream, &launches);
+    ce = mb::gemm_f64_grouped2(L2, ctx->num_sms, ctx->stream);
     if (ce != cudaSuccess) return cuda_fail(ce, "gemm_f64_grouped2 (second half)");
     for (const Note& w : final_to) MB_CUDA(sig(c, c->flags_peer[w.peer] + F_FINAL2 + rank * MAX_PAIR + w.slot, e, ctx->stream));
-    ctx->launches += launches;
     return MB_OK;
 }
 
@@ -1358,12 +1356,8 @@ int32_t mb_matmul_blocked_dist_host(mb_comm* c, const double* const* A_host, con
     }
     L.ready = c->flags + F_BAND; L.ready_val = e; L.status = c->flags + F_STATUS; L.timeout_ns = timeout_ns(c);
     MB_CUDA(cudaMemsetAsync(c->flags + F_CTR, 0, sizeof(unsigned long long) * mb::G2_MAX_ENTRIES, S));
-    {
-        int launches = 0;
-        cudaError_t ce = mb::gemm_f64_grouped2(L, ctx->num_sms, S, &launches);
-        if (ce != cudaSuccess) return cuda_fail(ce, "mb_matmul_blocked_dist_host: grouped launch");
-        ctx->launches += launches;
-    }
+    if (const cudaError_t ce = mb::gemm_f64_grouped2(L, ctx->num_sms, S); ce != cudaSuccess)
+        return cuda_fail(ce, "mb_matmul_blocked_dist_host: grouped launch");
     MB_CUDA(cudaEventRecord(c->ev_compute, S));
     c->have_compute = true;
     for (int p = 0; p < world; ++p) if (writes_to[p]) c->last_write_epoch[p] = e;

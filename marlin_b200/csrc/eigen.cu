@@ -18,6 +18,7 @@
 //     after the first sweep that rotated nothing.
 // No atomics, no reductions across threads: the result is bitwise reproducible from run to run.
 #include "eigen.h"
+#include "launch.h"
 
 #include <algorithm>
 #include <cfloat>
@@ -187,7 +188,8 @@ struct Buffers {
     }
 };
 
-// one sweep starting from buffer `from`: clear the flag, N-1 rounds, flag -> host
+// one sweep starting from buffer `from`: clear the flag, N-1 rounds, flag -> host.  Capturing enqueues nothing, so the
+// rounds are not counted here (no launched()) but each time the graph is launched.
 cudaError_t capture_sweep(Buffers& B, int N, int from, cudaGraphExec_t* exec) {
     cudaStream_t cs = nullptr;
     cudaError_t e = cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking);
@@ -215,8 +217,7 @@ cudaError_t capture_sweep(Buffers& B, int N, int from, cudaGraphExec_t* exec) {
 }  // namespace
 
 cudaError_t syev_jacobi(int n, const double* G, long long rs, long long cs, double* V, long long vrs, long long vcs,
-                        double* w_host, int* sweeps, int max_sweeps, cudaStream_t stream, long long* launches,
-                        bool* non_finite) {
+                        double* w_host, int* sweeps, int max_sweeps, cudaStream_t stream, bool* non_finite) {
     if (sweeps) *sweeps = 0;
     if (non_finite) *non_finite = false;
     if (n <= 0) return cudaSuccess;
@@ -238,8 +239,7 @@ cudaError_t syev_jacobi(int n, const double* G, long long rs, long long cs, doub
     if ((e = cudaMemsetAsync(maxbits, 0, sizeof(unsigned long long), stream)) != cudaSuccess) return e;
     const long long nn = (long long)n * n;
     jacobi_maxabs_kernel<<<(unsigned)((nn + 255) / 256), 256, 0, stream>>>(G, rs, cs, n, maxbits);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    if (launches) ++*launches;
+    if ((e = launched()) != cudaSuccess) return e;
     unsigned long long mb_host = 0;
     if ((e = cudaMemcpyAsync(&mb_host, maxbits, sizeof(mb_host), cudaMemcpyDeviceToHost, stream)) != cudaSuccess) return e;
     if ((e = cudaStreamSynchronize(stream)) != cudaSuccess) return e;
@@ -252,14 +252,13 @@ cudaError_t syev_jacobi(int n, const double* G, long long rs, long long cs, doub
     const int shift = gmax > 0.0 ? -std::ilogb(gmax) : 0;
     const long long total = (long long)N * N;
     jacobi_init_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(G, rs, cs, n, N, shift, B.W[0], B.V[0]);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    if (launches) ++*launches;
+    if ((e = launched()) != cudaSuccess) return e;
     int cur = 0, done = 0;
     for (int sw = 1; sw <= max_sweeps; ++sw) {
         if (!B.exec[cur] && (e = capture_sweep(B, N, cur, &B.exec[cur])) != cudaSuccess) return e;
         if ((e = cudaGraphLaunch(B.exec[cur], stream)) != cudaSuccess) return e;
+        count_launches(N - 1);
         if ((e = cudaStreamSynchronize(stream)) != cudaSuccess) return e;
-        if (launches) *launches += N - 1;
         cur ^= (N - 1) & 1;
         if (sweeps) *sweeps = sw;
         if (*B.flag_host == 0) { done = 1; break; }
@@ -278,8 +277,7 @@ cudaError_t syev_jacobi(int n, const double* G, long long rs, long long cs, doub
     for (int j = 0; j < n; ++j) w_host[j] = std::ldexp(w[order[j]], -shift);
     if ((e = cudaMemcpyAsync(B.order, order.data(), sizeof(int) * n, cudaMemcpyHostToDevice, stream)) != cudaSuccess) return e;
     jacobi_gather_kernel<<<(unsigned)((nn + 255) / 256), 256, 0, stream>>>(B.V[cur], N, B.order, n, V, vrs, vcs);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    if (launches) ++*launches;
+    if ((e = launched()) != cudaSuccess) return e;
     return cudaStreamSynchronize(stream);     // the buffers are freed on return
 }
 

@@ -10,7 +10,6 @@ namespace mb {
 // converge (w_host and V are then left unset).  A NaN or +-Inf in the lower triangle of G sets *non_finite, runs no sweep
 // and returns cudaSuccess with w_host and V unset.  Blocking: returns after the result is on the host / in V.
 cudaError_t syev_jacobi(int n, const double* G, long long rs, long long cs, double* V, long long vrs, long long vcs,
-                        double* w_host, int* sweeps, int max_sweeps, cudaStream_t stream, long long* launches,
-                        bool* non_finite);
+                        double* w_host, int* sweeps, int max_sweeps, cudaStream_t stream, bool* non_finite);
 
 }  // namespace mb

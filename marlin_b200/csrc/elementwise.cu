@@ -7,6 +7,7 @@
 // matrix/BlockMatrix.scala:414-452 (subtractBy/divideBy), :467-472 (sum), :494-500 (dotProduct =
 // Hadamard), :514-523 (transpose = denseBlock.t.copy), utils/RandomDataGenerator.scala:53-65,113-131.
 #include "elementwise.h"
+#include "launch.h"
 #include "ptx.cuh"
 #include <cuda_bf16.h>
 #include <atomic>
@@ -559,7 +560,7 @@ cudaError_t ew_binary(int op, int rows, int cols, const double* a, long long ars
     } else {
         binary_strided_kernel<<<ew_grid(total), EW_THREADS, 0, st>>>(op, rows, cols, a, ars, acs, b, brs, bcs, o, ors, ocs);
     }
-    return cudaGetLastError();
+    return launched();
 }
 
 cudaError_t ew_binary_f32(int op, int rows, int cols, const float* a, long long ars, long long acs, const float* b,
@@ -567,7 +568,7 @@ cudaError_t ew_binary_f32(int op, int rows, int cols, const float* a, long long 
     if (rows <= 0 || cols <= 0) return cudaSuccess;
     binary_strided_f32_kernel<<<ew_grid((long long)rows * cols), EW_THREADS, 0, st>>>(op, rows, cols, a, ars, acs, b, brs, bcs, o,
                                                                                     ors, ocs);
-    return cudaGetLastError();
+    return launched();
 }
 
 cudaError_t ew_unary(int op, int rows, int cols, const double* a, long long ars, long long acs, double* o,
@@ -589,7 +590,7 @@ cudaError_t ew_unary(int op, int rows, int cols, const double* a, long long ars,
     } else {
         unary_strided_kernel<<<ew_grid(total), EW_THREADS, 0, st>>>(op, rows, cols, a, ars, acs, o, ors, ocs, alpha, beta);
     }
-    return cudaGetLastError();
+    return launched();
 }
 
 cudaError_t transpose_f64(const double* in, long long ldi, double* out, long long ldo, int rows, int cols,
@@ -600,14 +601,12 @@ cudaError_t transpose_f64(const double* in, long long ldi, double* out, long lon
     if (fast) {
         const int tiles_r = (rows + TT * TT_SUB - 1) / (TT * TT_SUB), tiles_c = (cols + TT - 1) / TT;
         // 64 KiB of dynamic shared memory: above the 48 KiB a launch gets without opting in
-        cudaError_t e = cudaFuncSetAttribute(transpose_f64_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TT_SMEM);
-        if (e != cudaSuccess) return e;
-        transpose_f64_tile_kernel<<<tiles_r * tiles_c, 256, TT_SMEM, st>>>(in, ldi, out, ldo, rows, cols, tiles_r, tiles_c);
-    } else {
-        dim3 grid((rows + 31) / 32, (cols + 31) / 32);
-        transpose_generic_kernel<double><<<grid, 256, 0, st>>>(in, ldi, out, ldo, rows, cols);
+        return launch_with_smem<transpose_f64_tile_kernel>(tiles_r * tiles_c, 256, TT_SMEM, st, in, ldi, out, ldo, rows, cols,
+                                                           tiles_r, tiles_c);
     }
-    return cudaGetLastError();
+    dim3 grid((rows + 31) / 32, (cols + 31) / 32);
+    transpose_generic_kernel<double><<<grid, 256, 0, st>>>(in, ldi, out, ldo, rows, cols);
+    return launched();
 }
 
 cudaError_t transpose_b16(const void* in, long long ldi, void* out, long long ldo, int rows, int cols, cudaStream_t st) {
@@ -615,14 +614,14 @@ cudaError_t transpose_b16(const void* in, long long ldi, void* out, long long ld
     dim3 grid((rows + 31) / 32, (cols + 31) / 32);
     transpose_generic_kernel<unsigned short><<<grid, 256, 0, st>>>(static_cast<const unsigned short*>(in), ldi,
                                                                   static_cast<unsigned short*>(out), ldo, rows, cols);
-    return cudaGetLastError();
+    return launched();
 }
 cudaError_t transpose_b32(const void* in, long long ldi, void* out, long long ldo, int rows, int cols, cudaStream_t st) {
     if (rows <= 0 || cols <= 0) return cudaSuccess;
     dim3 grid((rows + 31) / 32, (cols + 31) / 32);
     transpose_generic_kernel<unsigned int><<<grid, 256, 0, st>>>(static_cast<const unsigned int*>(in), ldi,
                                                                 static_cast<unsigned int*>(out), ldo, rows, cols);
-    return cudaGetLastError();
+    return launched();
 }
 
 int sum_scratch_doubles() { return SUM_BLOCKS + 1; }
@@ -632,8 +631,9 @@ cudaError_t sum_f64(const double* a, int rows, int cols, long long ld, double* s
     const long long total = (long long)rows * cols;
     int blocks = (int)min((long long)SUM_BLOCKS, max(1ll, (total + 2047) / 2048));      // one CTA per 16 KiB tile, capped
     sum_strided_kernel<<<blocks, 256, 0, st>>>(a, rows, cols, ld, scratch + 1);
+    if (const cudaError_t e = launched(); e != cudaSuccess) return e;
     sum_final_kernel<<<1, 256, 0, st>>>(scratch + 1, blocks, scratch);
-    return cudaGetLastError();
+    return launched();
 }
 
 template <typename TI, typename TO>
@@ -642,7 +642,7 @@ static cudaError_t convert_t(int rows, int cols, const void* a, long long ars, l
     if (rows <= 0 || cols <= 0) return cudaSuccess;
     convert_strided_kernel<TI, TO><<<ew_grid((long long)rows * cols), EW_THREADS, 0, st>>>(
         rows, cols, static_cast<const TI*>(a), ars, acs, static_cast<TO*>(o), ors, ocs);
-    return cudaGetLastError();
+    return launched();
 }
 
 // dtype codes follow mb_dtype: 0 = f64, 1 = bf16, 2 = f32
@@ -708,7 +708,8 @@ cudaError_t fill_jump_tables(const unsigned long long** tables) {
 // ONCE per device and process, on the device itself: two CTAs of each kernel at a far, odd stream offset, unit and affine
 // range, compared on the host (about a millisecond).  A mismatch — a compiler or driver that breaks one of the kernel's
 // exactness arguments — disables the fast kernel for the process and says so on stderr; results stay those of the general
-// kernel either way.  Returns 1 (verified) or -1 (disabled).
+// kernel either way.  Returns 1 (verified) or -1 (disabled).  Its launches are not counted (no launched()): they are not
+// the work of the call that happens to run the check.
 static int fast_fill_state(cudaStream_t st) {
     static std::mutex mu;
     static std::atomic<int> state[64];
@@ -747,8 +748,7 @@ static int fast_fill_state(cudaStream_t st) {
 }
 
 cudaError_t fill_uniform_f64(double* out, long long rs, long long cs, int rows, int cols, int row_major,
-                             unsigned long long state0, long long first, double lo, double hi, cudaStream_t st, int* launches) {
-    if (launches) *launches = 0;
+                             unsigned long long state0, long long first, double lo, double hi, cudaStream_t st) {
     if (rows <= 0 || cols <= 0) return cudaSuccess;
     cudaError_t e = fill_uniform_init_tables();
     if (e != cudaSuccess) return e;
@@ -766,15 +766,11 @@ cudaError_t fill_uniform_f64(double* out, long long rs, long long cs, int rows, 
             fill_uniform_fast_kernel<true><<<full, 256, 0, st>>>(out, state0, first, lo, hi, 1u << 21, 1u << 4);
         else
             fill_uniform_fast_kernel<false><<<full, 256, 0, st>>>(out, state0, first, lo, hi, 1u << 21, 1u << 4);
-        cudaError_t e2 = cudaGetLastError();
-        if (e2 != cudaSuccess) return e2;
-        if (launches) ++*launches;
+        if ((e = launched()) != cudaSuccess) return e;
     }
-    if (blocks > full) {
-        fill_uniform_kernel<<<blocks - full, 256, 0, st>>>(out, rs, cs, rows, cols, row_major, state0, first, lo, hi, full);
-        if (launches) ++*launches;
-    }
-    return cudaGetLastError();
+    if (blocks == full) return cudaSuccess;
+    fill_uniform_kernel<<<blocks - full, 256, 0, st>>>(out, rs, cs, rows, cols, row_major, state0, first, lo, hi, full);
+    return launched();
 }
 
 }  // namespace mb

@@ -22,8 +22,7 @@ cudaError_t sum_f64(const double* a, int rows, int cols, long long ld, double* s
 cudaError_t convert_strided(int src_dtype, int dst_dtype, int rows, int cols, const void* a, long long ars,
                             long long acs, void* o, long long ors, long long ocs, cudaStream_t st);
 cudaError_t fill_uniform_f64(double* out, long long rs, long long cs, int rows, int cols, int row_major,
-                             unsigned long long state0, long long first, double lo, double hi, cudaStream_t st,
-                             int* launches = nullptr);      // *launches = kernels launched (fast kernel for full CTAs + general tail)
+                             unsigned long long state0, long long first, double lo, double hi, cudaStream_t st);
 // Device address of the generator's jump tables: 40 x 64 words, row j = the columns of T^(2^j) (T = one XORShift step).
 cudaError_t fill_jump_tables(const unsigned long long** tables);
 

@@ -12,6 +12,7 @@
 // All kernels take element strides (rs, cs), so Breeze views (transposed, sliced) need no copies.
 #include "factor.h"
 #include "gemm_f64.h"
+#include "launch.h"
 
 #include <algorithm>
 #include <cfloat>
@@ -205,7 +206,7 @@ inline int split(int n) {
 }
 
 // C (view) = alpha * A * B + beta * C with arbitrary element strides on all three: routed to the column-major GEMM
-cudaError_t gemm_view(const FView& A, const FView& B, const FView& C, double alpha, double beta, int num_sms, cudaStream_t st, int* launches) {
+cudaError_t gemm_view(const FView& A, const FView& B, const FView& C, double alpha, double beta, int num_sms, cudaStream_t st) {
     // a view is "N" when rs == 1 (column-major, ld = cs) and "T" when cs == 1 (row-major, ld = rs)
     auto form = [](const FView& v, bool* trans, long long* ld) {
         if (v.rs == 1) { *trans = false; *ld = v.cs; return true; }
@@ -219,9 +220,9 @@ cudaError_t gemm_view(const FView& A, const FView& B, const FView& C, double alp
     if (ldb < 1) ldb = 1;
     if (ldc < 1) ldc = 1;
     const int M = C.rows, N = C.cols, K = A.cols;
-    if (!tc) return gemm_f64(ta, tb, M, N, K, alpha, A.p, lda, B.p, ldb, beta, C.p, ldc, num_sms, st, false, launches);
+    if (!tc) return gemm_f64(ta, tb, M, N, K, alpha, A.p, lda, B.p, ldb, beta, C.p, ldc, num_sms, st, false);
     // C^T = B^T * A^T on the column-major array underneath
-    return gemm_f64(!tb, !ta, N, M, K, alpha, B.p, ldb, A.p, lda, beta, C.p, ldc, num_sms, st, false, launches);
+    return gemm_f64(!tb, !ta, N, M, K, alpha, B.p, ldb, A.p, lda, beta, C.p, ldc, num_sms, st, false);
 }
 
 inline FView sub(const FView& v, int r0, int r1, int c0, int c1) {
@@ -232,7 +233,7 @@ inline FView tr(const FView& v) { return FView{v.p, v.cs, v.rs, v.cols, v.rows};
 }  // namespace
 
 // ---- T X = B (left side), T triangular t x t, B t x nrhs, in place -------------------------------------------------
-cudaError_t trsm_left(const FView& T, bool lower, bool unit, const FView& B, int num_sms, cudaStream_t st, int* launches) {
+cudaError_t trsm_left(const FView& T, bool lower, bool unit, const FView& B, int num_sms, cudaStream_t st) {
     const int t = T.rows, nrhs = B.cols;
     if (t <= 0 || nrhs <= 0) return cudaSuccess;
     if (t <= LEAF) {
@@ -241,121 +242,114 @@ cudaError_t trsm_left(const FView& T, bool lower, bool unit, const FView& B, int
         else if (lower) trsm_leaf_kernel<true, false><<<blocks, 128, 0, st>>>(T.p, T.rs, T.cs, t, B.p, B.rs, B.cs, nrhs);
         else if (unit) trsm_leaf_kernel<false, true><<<blocks, 128, 0, st>>>(T.p, T.rs, T.cs, t, B.p, B.rs, B.cs, nrhs);
         else trsm_leaf_kernel<false, false><<<blocks, 128, 0, st>>>(T.p, T.rs, T.cs, t, B.p, B.rs, B.cs, nrhs);
-        if (launches) ++*launches;
-        return cudaGetLastError();
+        return launched();
     }
     const int h = split(t);
     const FView T11 = sub(T, 0, h, 0, h), T22 = sub(T, h, t, h, t);
     const FView B1 = sub(B, 0, h, 0, nrhs), B2 = sub(B, h, t, 0, nrhs);
     cudaError_t e;
     if (lower) {
-        if ((e = trsm_left(T11, true, unit, B1, num_sms, st, launches)) != cudaSuccess) return e;
-        if ((e = gemm_view(sub(T, h, t, 0, h), B1, B2, -1.0, 1.0, num_sms, st, launches)) != cudaSuccess) return e;
-        return trsm_left(T22, true, unit, B2, num_sms, st, launches);
+        if ((e = trsm_left(T11, true, unit, B1, num_sms, st)) != cudaSuccess) return e;
+        if ((e = gemm_view(sub(T, h, t, 0, h), B1, B2, -1.0, 1.0, num_sms, st)) != cudaSuccess) return e;
+        return trsm_left(T22, true, unit, B2, num_sms, st);
     }
-    if ((e = trsm_left(T22, false, unit, B2, num_sms, st, launches)) != cudaSuccess) return e;
-    if ((e = gemm_view(sub(T, 0, h, h, t), B2, B1, -1.0, 1.0, num_sms, st, launches)) != cudaSuccess) return e;
-    return trsm_left(T11, false, unit, B1, num_sms, st, launches);
+    if ((e = trsm_left(T22, false, unit, B2, num_sms, st)) != cudaSuccess) return e;
+    if ((e = gemm_view(sub(T, 0, h, h, t), B2, B1, -1.0, 1.0, num_sms, st)) != cudaSuccess) return e;
+    return trsm_left(T11, false, unit, B1, num_sms, st);
 }
 
 namespace {
 
 // LU of the (m x n) view `a` = columns [c0, c0+n) / rows [r0, ...) of the full matrix `full`; pivots are absolute rows.
-cudaError_t getrf_rec(const FView& full, int r0, int c0, int m, int n, int* piv, int* info, int num_sms, cudaStream_t st, int* launches) {
+cudaError_t getrf_rec(const FView& full, int r0, int c0, int m, int n, int* piv, int* info, int num_sms, cudaStream_t st) {
     if (m <= 0 || n <= 0) return cudaSuccess;
     const FView a = sub(full, r0, r0 + m, c0, c0 + n);
     if (n <= PANEL_W) {
         lu_panel_kernel<<<1, 1024, 0, st>>>(a.p, a.rs, a.cs, m, n, piv + r0, r0, info);
-        if (launches) ++*launches;
-        return cudaGetLastError();
+        return launched();
     }
     const int n1 = std::min(split(n), m);
     const int n2 = n - n1;
     cudaError_t e;
-    if ((e = getrf_rec(full, r0, c0, m, n1, piv, info, num_sms, st, launches)) != cudaSuccess) return e;
+    if ((e = getrf_rec(full, r0, c0, m, n1, piv, info, num_sms, st)) != cudaSuccess) return e;
     const int k1 = std::min(m, n1);
     // apply the left half's interchanges to the right half
     const FView right_full = sub(full, 0, full.rows, c0 + n1, c0 + n);
     laswp_kernel<<<(n2 + 127) / 128, 128, 0, st>>>(right_full.p, right_full.rs, right_full.cs, n2, piv, r0, r0 + k1);
-    if (launches) ++*launches;
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    if ((e = launched()) != cudaSuccess) return e;
     // U12 = L11^-1 A12;  A22 -= L21 U12
     const FView L11 = sub(full, r0, r0 + k1, c0, c0 + k1);
     const FView A12 = sub(full, r0, r0 + k1, c0 + n1, c0 + n);
-    if ((e = trsm_left(L11, true, true, A12, num_sms, st, launches)) != cudaSuccess) return e;
+    if ((e = trsm_left(L11, true, true, A12, num_sms, st)) != cudaSuccess) return e;
     if (m > k1) {
         const FView L21 = sub(full, r0 + k1, r0 + m, c0, c0 + k1);
         const FView A22 = sub(full, r0 + k1, r0 + m, c0 + n1, c0 + n);
-        if ((e = gemm_view(L21, A12, A22, -1.0, 1.0, num_sms, st, launches)) != cudaSuccess) return e;
-        if ((e = getrf_rec(full, r0 + k1, c0 + n1, m - k1, n2, piv, info, num_sms, st, launches)) != cudaSuccess) return e;
+        if ((e = gemm_view(L21, A12, A22, -1.0, 1.0, num_sms, st)) != cudaSuccess) return e;
+        if ((e = getrf_rec(full, r0 + k1, c0 + n1, m - k1, n2, piv, info, num_sms, st)) != cudaSuccess) return e;
         // the right half's interchanges, applied back to the left half
         const int k2 = std::min(m - k1, n2);
         const FView left_full = sub(full, 0, full.rows, c0, c0 + n1);
         laswp_kernel<<<(n1 + 127) / 128, 128, 0, st>>>(left_full.p, left_full.rs, left_full.cs, n1, piv, r0 + k1, r0 + k1 + k2);
-        if (launches) ++*launches;
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+        if ((e = launched()) != cudaSuccess) return e;
     }
     return cudaSuccess;
 }
 
-cudaError_t potrf_rec(const FView& full, int r0, int n, int* info, int num_sms, cudaStream_t st, int* launches) {
+cudaError_t potrf_rec(const FView& full, int r0, int n, int* info, int num_sms, cudaStream_t st) {
     if (n <= 0) return cudaSuccess;
     if (n <= LEAF) {
         const FView a = sub(full, r0, r0 + n, r0, r0 + n);
         potrf_leaf_kernel<<<1, 256, 0, st>>>(a.p, a.rs, a.cs, n, r0, info);
-        if (launches) ++*launches;
-        return cudaGetLastError();
+        return launched();
     }
     const int n1 = split(n), n2 = n - n1;
     cudaError_t e;
-    if ((e = potrf_rec(full, r0, n1, info, num_sms, st, launches)) != cudaSuccess) return e;
+    if ((e = potrf_rec(full, r0, n1, info, num_sms, st)) != cudaSuccess) return e;
     const FView L11 = sub(full, r0, r0 + n1, r0, r0 + n1);
     const FView A21 = sub(full, r0 + n1, r0 + n, r0, r0 + n1);
     // X L11^T = A21  <=>  L11 X^T = A21^T
-    if ((e = trsm_left(L11, true, false, tr(A21), num_sms, st, launches)) != cudaSuccess) return e;
+    if ((e = trsm_left(L11, true, false, tr(A21), num_sms, st)) != cudaSuccess) return e;
     const FView A22 = sub(full, r0 + n1, r0 + n, r0 + n1, r0 + n);
-    if ((e = gemm_view(A21, tr(A21), A22, -1.0, 1.0, num_sms, st, launches)) != cudaSuccess) return e;
+    if ((e = gemm_view(A21, tr(A21), A22, -1.0, 1.0, num_sms, st)) != cudaSuccess) return e;
     (void)n2;
-    return potrf_rec(full, r0 + n1, n - n1, info, num_sms, st, launches);
+    return potrf_rec(full, r0 + n1, n - n1, info, num_sms, st);
 }
 
 }  // namespace
 
-cudaError_t getrf(const FView& a, int* piv_dev, int* perm_dev, int* info_dev, int num_sms, cudaStream_t st, int* launches) {
+cudaError_t getrf(const FView& a, int* piv_dev, int* perm_dev, int* info_dev, int num_sms, cudaStream_t st) {
     const int k = std::min(a.rows, a.cols);
     cudaError_t e = cudaMemsetAsync(info_dev, 0, sizeof(int), st);
     if (e != cudaSuccess) return e;
-    if ((e = getrf_rec(a, 0, 0, a.rows, a.cols, piv_dev, info_dev, num_sms, st, launches)) != cudaSuccess) return e;
+    if ((e = getrf_rec(a, 0, 0, a.rows, a.cols, piv_dev, info_dev, num_sms, st)) != cudaSuccess) return e;
     if (perm_dev) {
         // rows beyond min(m, n) are never pivot positions: identity there
         ipiv_to_perm_kernel<<<1, 1, 0, st>>>(piv_dev, k, perm_dev);
-        if (launches) ++*launches;
-        e = cudaGetLastError();
+        e = launched();
     }
     return e;
 }
 
-cudaError_t potrf_lower(const FView& a, int* info_dev, int num_sms, cudaStream_t st, int* launches) {
+cudaError_t potrf_lower(const FView& a, int* info_dev, int num_sms, cudaStream_t st) {
     cudaError_t e = cudaMemsetAsync(info_dev, 0, sizeof(int), st);
     if (e != cudaSuccess) return e;
-    if ((e = potrf_rec(a, 0, a.rows, info_dev, num_sms, st, launches)) != cudaSuccess) return e;
+    if ((e = potrf_rec(a, 0, a.rows, info_dev, num_sms, st)) != cudaSuccess) return e;
     const long long total = (long long)a.rows * a.rows;
     zero_strict_upper_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(a.p, a.rs, a.cs, a.rows);
-    if (launches) ++*launches;
-    return cudaGetLastError();
+    return launched();
 }
 
 // out = a^-1 : LU of a working copy `lu` (caller-provided, holds a on entry), then L (U X) = P I
-cudaError_t inverse_from_lu(const FView& lu, const int* piv_dev, const FView& out, int num_sms, cudaStream_t st, int* launches) {
+cudaError_t inverse_from_lu(const FView& lu, const int* piv_dev, const FView& out, int num_sms, cudaStream_t st) {
     const int n = lu.rows;
     const long long total = (long long)n * n;
     identity_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(out.p, out.rs, out.cs, n);
-    laswp_kernel<<<(n + 127) / 128, 128, 0, st>>>(out.p, out.rs, out.cs, n, piv_dev, 0, n);
-    if (launches) *launches += 2;
-    cudaError_t e = cudaGetLastError();
+    cudaError_t e = launched();
     if (e != cudaSuccess) return e;
-    if ((e = trsm_left(lu, true, true, out, num_sms, st, launches)) != cudaSuccess) return e;
-    return trsm_left(lu, false, false, out, num_sms, st, launches);
+    laswp_kernel<<<(n + 127) / 128, 128, 0, st>>>(out.p, out.rs, out.cs, n, piv_dev, 0, n);
+    if ((e = launched()) != cudaSuccess) return e;
+    if ((e = trsm_left(lu, true, true, out, num_sms, st)) != cudaSuccess) return e;
+    return trsm_left(lu, false, false, out, num_sms, st);
 }
 
 }  // namespace mb

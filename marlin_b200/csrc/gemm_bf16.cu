@@ -18,6 +18,7 @@
 //   B 'T' (N x K, n contiguous)  -> MN-major B : 4 atoms [64 k-rows][64 n]
 #include "gemm_bf16.h"
 #include "ptx.cuh"
+#include "launch.h"
 #include "tma.h"
 #include <cuda_bf16.h>
 
@@ -221,7 +222,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ SegMaps maps, const Params p) {
 
 cudaError_t gemm_bf16_segments(bool transA, bool transB, int M, int N, int nseg, const int* Kseg, const void* const* A,
                                const long long* lda, const void* const* B, const long long* ldb, void* C, long long ldc,
-                               bool c_is_f32, bool accumulate, int num_sms, cudaStream_t stream, int* launches) {
+                               bool c_is_f32, bool accumulate, int num_sms, cudaStream_t stream) {
     if (M <= 0 || N <= 0) return cudaSuccess;
     if (nseg <= 0 || nseg > MAX_SEG || !tma_encode_fn()) return cudaErrorNotSupported;
     static thread_local SegMaps maps;
@@ -248,7 +249,6 @@ cudaError_t gemm_bf16_segments(bool transA, bool transB, int M, int N, int nseg,
     p.tiles_n = (N + BN - 1) / BN;
     p.c_is_f32 = c_is_f32 ? 1 : 0;
     p.accumulate = accumulate ? 1 : 0;
-    if (launches) ++*launches;
     const int grid = min(p.tiles_m * p.tiles_n, num_sms);
     if (!transA && !transB) return launch_with_smem<gemm_bf16_wgmma_kernel<false, false>>(grid, NUM_THREADS, SMEM_BYTES, stream, maps, p);
     if (transA && !transB) return launch_with_smem<gemm_bf16_wgmma_kernel<true, false>>(grid, NUM_THREADS, SMEM_BYTES, stream, maps, p);

@@ -11,6 +11,6 @@ namespace mb {
 // bf16_gemm in capi.cu stages operands that break the rule, handles K = 0 and caps fp32 accumulation chains.
 cudaError_t gemm_bf16_segments(bool transA, bool transB, int M, int N, int nseg, const int* Kseg, const void* const* A,
                                const long long* lda, const void* const* B, const long long* ldb, void* C, long long ldc,
-                               bool c_is_f32, bool accumulate, int num_sms, cudaStream_t stream, int* launches);
+                               bool c_is_f32, bool accumulate, int num_sms, cudaStream_t stream);
 
 }  // namespace mb

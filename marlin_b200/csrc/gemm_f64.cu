@@ -31,6 +31,7 @@
 // reference of the production kernels and run only when a context asks for them (mb_set_dmma_reference).
 #include "gemm_f64.h"
 #include "ptx.cuh"
+#include "launch.h"
 #include "tma.h"
 #include <cstdlib>
 
@@ -49,9 +50,6 @@ constexpr int BAND = 16;                            // tile-rows per rasterisati
 
 // The DMMA instruction shape of the mainloop: m16n8k4 in production, m8n8k4 for the reference instances.
 enum class Dmma { m8n8k4, m16n8k4 };
-
-// Set by every C-ABI entry from its context (mb_set_dmma_reference) before it launches anything.
-thread_local bool g_dmma_reference = false;
 
 struct Params {
     int M, N, K;
@@ -714,21 +712,19 @@ bool operand_map(CUtensorMap* map, const double* base, int mn, int k, long long 
 
 template <bool TA, bool TB>
 cudaError_t launch_gemm(int grid, cudaStream_t stream, const CUtensorMap& mA, const CUtensorMap& mB, const Params& p) {
-    return g_dmma_reference
+    return g_call.dmma_reference
                ? launch_with_smem<gemm_f64_dmma_kernel<TA, TB>>(grid, NUM_THREADS, SMEM_BYTES, stream, mA, mB, p)
                : launch_with_smem<gemm_f64_dmma16x8_kernel<TA, TB>>(grid, NUM_THREADS, SMEM_BYTES, stream, mA, mB, p);
 }
 
 template <bool TA, bool TB>
 cudaError_t launch_syrk(int grid, cudaStream_t stream, const CUtensorMap& mA, const Params& p, const SyrkSched& sk) {
-    return g_dmma_reference
+    return g_call.dmma_reference
                ? launch_with_smem<syrk_f64_dmma_kernel<TA, TB>>(grid, NUM_THREADS, SMEM_BYTES, stream, mA, mA, p, sk)
                : launch_with_smem<syrk_f64_dmma16x8_kernel<TA, TB>>(grid, NUM_THREADS, SMEM_BYTES, stream, mA, mA, p, sk);
 }
 
 }  // namespace
-
-void set_dmma_reference(bool on) { g_dmma_reference = on; }
 
 bool gemm_f64_tma_eligible(const double* A, long long lda, const double* B, long long ldb) {
     return ((reinterpret_cast<uintptr_t>(A) & 15) == 0) && ((reinterpret_cast<uintptr_t>(B) & 15) == 0) &&
@@ -737,13 +733,12 @@ bool gemm_f64_tma_eligible(const double* A, long long lda, const double* B, long
 
 cudaError_t gemm_f64(bool transA, bool transB, int M, int N, int K, double alpha, const double* A, long long lda,
                      const double* B, long long ldb, double beta, double* C, long long ldc, int num_sms,
-                     cudaStream_t stream, bool force_generic, int* launches) {
+                     cudaStream_t stream, bool force_generic) {
     if (M <= 0 || N <= 0) return cudaSuccess;
     if (K <= 0 || alpha == 0.0) {
         if (beta == 1.0) return cudaSuccess;
         scale_matrix_kernel<<<min(1184, (int)(((long long)M * N + 255) / 256)), 256, 0, stream>>>(M, N, beta, C, ldc);
-        if (launches) ++*launches;
-        return cudaGetLastError();
+        return launched();
     }
     if (!force_generic && gemm_f64_tma_eligible(A, lda, B, ldb)) {
         CUtensorMap mA, mB;
@@ -753,7 +748,6 @@ cudaError_t gemm_f64(bool transA, bool transB, int M, int N, int K, double alpha
             p.M = M; p.N = N; p.K = K; p.alpha = alpha; p.beta = beta; p.C = C; p.ldc = ldc;
             p.tiles_m = (M + BM - 1) / BM;
             p.tiles_n = (N + BN - 1) / BN;
-            if (launches) ++*launches;
             const int grid = min(p.tiles_m * p.tiles_n, num_sms);
             if (!transA && !transB) return launch_gemm<false, false>(grid, stream, mA, mB, p);
             if (transA && !transB) return launch_gemm<true, false>(grid, stream, mA, mB, p);
@@ -762,7 +756,6 @@ cudaError_t gemm_f64(bool transA, bool transB, int M, int N, int K, double alpha
         }
     }
     dim3 grid((M + 63) / 64, (N + 63) / 64);
-    if (launches) ++*launches;
     if (!transA && !transB)
         gemm_f64_generic_kernel<false, false><<<grid, 256, 0, stream>>>(M, N, K, alpha, A, lda, B, ldb, beta, C, ldc);
     else if (transA && !transB)
@@ -771,7 +764,7 @@ cudaError_t gemm_f64(bool transA, bool transB, int M, int N, int K, double alpha
         gemm_f64_generic_kernel<false, true><<<grid, 256, 0, stream>>>(M, N, K, alpha, A, lda, B, ldb, beta, C, ldc);
     else
         gemm_f64_generic_kernel<true, true><<<grid, 256, 0, stream>>>(M, N, K, alpha, A, lda, B, ldb, beta, C, ldc);
-    return cudaGetLastError();
+    return launched();
 }
 
 
@@ -874,7 +867,7 @@ size_t gram_workspace_doubles(int n, long long K, int num_sms) {
 }
 
 cudaError_t gram_f64(bool trans, int n, int K, const double* A, long long lda, double* G, long long ldg, double* ws,
-                     int num_sms, cudaStream_t stream, int* launches) {
+                     int num_sms, cudaStream_t stream) {
     if (n <= 0) return cudaSuccess;
     // op(A) and op(A)^T are read from the same storage in the same form, so A and B share one map
     CUtensorMap mA;
@@ -899,10 +892,9 @@ cudaError_t gram_f64(bool trans, int n, int K, const double* A, long long lda, d
         const int grid = min(sk.tri_tiles * splits, num_sms);
         e = !trans ? launch_syrk<false, true>(grid, stream, mA, p, sk) : launch_syrk<true, false>(grid, stream, mA, p, sk);
         if (e != cudaSuccess) return e;
-        if (launches) ++*launches;
     } else {
         // the whole product on the CUDA cores (views TMA cannot address), or zeros for K = 0
-        e = gemm_f64(trans, !trans, n, n, K, 1.0, A, lda, A, lda, 0.0, P, ldp, num_sms, stream, true, launches);
+        e = gemm_f64(trans, !trans, n, n, K, 1.0, A, lda, A, lda, 0.0, P, ldp, num_sms, stream, true);
         if (e != cudaSuccess) return e;
     }
     const int nb = (n + 31) / 32;
@@ -911,11 +903,10 @@ cudaError_t gram_f64(bool trans, int n, int K, const double* A, long long lda, d
         gram_reduce_mirror_kernel<true><<<grid, 256, 0, stream>>>(P, ldp, ldp * n, splits, n, G, ldg);
     else
         gram_reduce_mirror_kernel<false><<<grid, 256, 0, stream>>>(P, ldp, ldp * n, splits, n, G, ldg);
-    if (launches) ++*launches;
-    return cudaGetLastError();
+    return launched();
 }
 
-cudaError_t gemm_f64_grouped2(const G2Launch& L, int num_sms, cudaStream_t stream, int* launches) {
+cudaError_t gemm_f64_grouped2(const G2Launch& L, int num_sms, cudaStream_t stream) {
     if (L.ne <= 0) return cudaSuccess;
     if (L.ne > G2_MAX_ENTRIES || L.na > G2_MAX_OPS || L.nb > G2_MAX_OPS || !tma_encode_fn()) return cudaErrorNotSupported;
     static thread_local G2Params g;          // ~20 KB parameter block: kept off the stack, one per calling thread
@@ -963,17 +954,14 @@ cudaError_t gemm_f64_grouped2(const G2Launch& L, int num_sms, cudaStream_t strea
     g.ready = L.ready; g.ready_val = L.ready_val; g.status = L.status; g.timeout_ns = L.timeout_ns;
     g.ne = L.ne;
     g.num_tiles = tiles;
-    const cudaError_t e =
-        g_dmma_reference ? launch_with_smem<gemm_f64_dmma_grouped_kernel>(min(tiles, num_sms), NUM_THREADS, SMEM_BYTES, stream, g)
-                         : launch_with_smem<gemm_f64_dmma16x8_grouped_kernel>(min(tiles, num_sms), NUM_THREADS, SMEM_BYTES, stream, g);
-    if (launches && e == cudaSuccess) ++*launches;
-    return e;
+    return g_call.dmma_reference
+               ? launch_with_smem<gemm_f64_dmma_grouped_kernel>(min(tiles, num_sms), NUM_THREADS, SMEM_BYTES, stream, g)
+               : launch_with_smem<gemm_f64_dmma16x8_grouped_kernel>(min(tiles, num_sms), NUM_THREADS, SMEM_BYTES, stream, g);
 }
 
 cudaError_t gemm_f64_grouped(int m, int k, int n, const int* my_c, int num_c, const double* const* A, const long long* lda,
                              const double* const* B, const long long* ldb, double* const* C, const long long* ldc,
-                             const int* row_len, const int* k_len, const int* col_len, int num_sms, cudaStream_t stream,
-                             int* launches) {
+                             const int* row_len, const int* k_len, const int* col_len, int num_sms, cudaStream_t stream) {
     // my_c: the (i*n + j) ids of the C blocks to compute; A[i*k+kk], B[kk*n+j], C[i*n+j] column-major 'N' blocks.
     // One entry per C block (the whole block, every kk), operands resident: no flags, no addend.
     if (num_c <= 0) return cudaSuccess;
@@ -1010,7 +998,7 @@ cudaError_t gemm_f64_grouped(int m, int k, int n, const int* my_c, int num_c, co
         e.M = row_len[i]; e.N = col_len[j];
         e.D = C[my_c[c]]; e.ldd = ldc[my_c[c]];
     }
-    return gemm_f64_grouped2(L, num_sms, stream, launches);
+    return gemm_f64_grouped2(L, num_sms, stream);
 }
 
 }  // namespace mb

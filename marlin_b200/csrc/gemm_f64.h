@@ -9,15 +9,14 @@ namespace mb {
 // dimensions are even, otherwise (or if force_generic) the CUDA-core kernel.
 cudaError_t gemm_f64(bool transA, bool transB, int M, int N, int K, double alpha, const double* A, long long lda,
                      const double* B, long long ldb, double beta, double* C, long long ldc, int num_sms,
-                     cudaStream_t stream, bool force_generic, int* launches);
+                     cudaStream_t stream, bool force_generic);
 
 // One persistent launch for a blocked multiply: C[c] = sum_kk A[i*k+kk] * B[kk*n+j] for every c = i*n+j in my_c
 // (all 'N' column-major blocks).  Returns cudaErrorNotSupported when the group does not fit the fixed-size parameter
 // block or an operand is not TMA-addressable; the caller then falls back to one launch per block product.
 cudaError_t gemm_f64_grouped(int m, int k, int n, const int* my_c, int num_c, const double* const* A, const long long* lda,
                              const double* const* B, const long long* ldb, double* const* C, const long long* ldc,
-                             const int* row_len, const int* k_len, const int* col_len, int num_sms, cudaStream_t stream,
-                             int* launches);
+                             const int* row_len, const int* k_len, const int* col_len, int num_sms, cudaStream_t stream);
 
 // ---- the general grouped launch (see gemm_f64.cu): entries = regions of C blocks with their own K segment lists,
 //      operand readiness flags, optional staged addend (D = acc + Cin) and completion signals ----
@@ -55,7 +54,7 @@ struct G2Launch {
     unsigned long long* status = nullptr;               // device word set to 1 when an in-kernel wait times out
     long long timeout_ns = 0;                           // 0 = wait forever
 };
-cudaError_t gemm_f64_grouped2(const G2Launch& L, int num_sms, cudaStream_t stream, int* launches);
+cudaError_t gemm_f64_grouped2(const G2Launch& L, int num_sms, cudaStream_t stream);
 
 // Gramian: G (n x n, col-major, ldg) = op(A) op(A)^T with op(A) n x K (A stored n x K if !trans, K x n if trans), exactly
 // symmetric.  TMA-addressable operands run the DMMA mainloop over the lower-triangle tiles only; when the triangle has
@@ -67,12 +66,8 @@ constexpr long long GRAM_WS_CAP_DOUBLES = 32LL << 20;    // 256 MiB
 int gram_splits(int n, long long K, int num_sms);
 size_t gram_workspace_doubles(int n, long long K, int num_sms);
 cudaError_t gram_f64(bool trans, int n, int K, const double* A, long long lda, double* G, long long ldg, double* ws,
-                     int num_sms, cudaStream_t stream, int* launches);
+                     int num_sms, cudaStream_t stream);
 
 bool gemm_f64_tma_eligible(const double* A, long long lda, const double* B, long long ldb);
-
-// Run the m8n8k4 reference instances of the DMMA kernels instead of the m16n8k4 ones for the launches this thread makes
-// from now on (a test and measurement switch: mb_set_dmma_reference).  Every C-ABI entry sets it from its context.
-void set_dmma_reference(bool on);
 
 }  // namespace mb

@@ -18,6 +18,7 @@
 // bracket of a group the consumers fold the accumulator into C with an fp64 read-modify-write.
 #include "gemm_ozaki.h"
 #include "ptx.cuh"
+#include "launch.h"
 #include "tma.h"
 
 namespace mb {
@@ -353,8 +354,7 @@ bool ozaki_supported(int M, int N, int K, int s, int bits) {
 }
 
 cudaError_t gemm_f64_ozaki(int M, int N, int K, const double* A, long long lda, const double* B, long long ldb, double* C,
-                           long long ldc, bool accumulate, int s, int bits, void* workspace, int num_sms, cudaStream_t stream,
-                           int* launches) {
+                           long long ldc, bool accumulate, int s, int bits, void* workspace, int num_sms, cudaStream_t stream) {
     if (!ozaki_supported(M, N, K, s, bits)) return cudaErrorNotSupported;
     const int P = bits * s - (bits == 8 ? 2 : 1);
     const size_t ldA = round_up((size_t)K, 16), ldB = round_up((size_t)K, 16);
@@ -376,10 +376,11 @@ cudaError_t gemm_f64_ozaki(int M, int N, int K, const double* A, long long lda, 
     const int kchunk = (K + ksplit - 1) / ksplit;
     dim3 grid_a((M + 127) / 128, ksplit);
     ozaki_rowmax_kernel<<<grid_a, 128, 0, stream>>>(A, lda, M, K, kchunk, rowmax);
+    if ((e = launched()) != cudaSuccess) return e;
     ozaki_split_a_kernel<<<grid_a, 128, 0, stream>>>(A, lda, M, K, s, bits, P, rowmax, A8, (long long)ldA, (long long)planeA, eA);
+    if ((e = launched()) != cudaSuccess) return e;
     ozaki_split_b_kernel<<<N, 256, 0, stream>>>(B, ldb, K, N, s, bits, P, B8, (long long)ldB, (long long)planeB, eB);
-    if (launches) *launches += 3;
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    if ((e = launched()) != cudaSuccess) return e;
 
     CUtensorMap mA, mB;
     if (!tma_map_3d(&mA, CU_TENSOR_MAP_DATA_TYPE_UINT8, A8, K, M, s, ldA, planeA, 128, 128)) return cudaErrorNotSupported;
@@ -391,11 +392,9 @@ cudaError_t gemm_f64_ozaki(int M, int N, int K, const double* A, long long lda, 
     p.accumulate = accumulate ? 1 : 0;
     e = launch_with_smem<gemm_ozaki_i8_kernel>(min(p.tiles_m * p.tiles_n, num_sms), NUM_THREADS, SMEM_BYTES, stream, mA, mB, p);
     if (e != cudaSuccess) return e;
-    if (launches) ++*launches;
     // stream-ordered after the int8 kernel, which leaves the flagged entries of C as they were (accumulate) or +0
     ozaki_fixup_kernel<<<M + N, 128, 0, stream>>>(A, lda, B, ldb, C, ldc, M, N, K, p.accumulate, eA, eB);
-    if (launches) ++*launches;
-    return cudaGetLastError();
+    return launched();
 }
 
 }  // namespace mb

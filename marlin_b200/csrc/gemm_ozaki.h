@@ -9,7 +9,6 @@ namespace mb {
 size_t ozaki_workspace_bytes(int M, int N, int K, int s);
 bool ozaki_supported(int M, int N, int K, int s, int bits);
 cudaError_t gemm_f64_ozaki(int M, int N, int K, const double* A, long long lda, const double* B, long long ldb, double* C,
-                           long long ldc, bool accumulate, int s, int bits, void* workspace, int num_sms, cudaStream_t stream,
-                           int* launches);
+                           long long ldc, bool accumulate, int s, int bits, void* workspace, int num_sms, cudaStream_t stream);
 
 }  // namespace mb

@@ -3,6 +3,7 @@
 #pragma once
 #include "../../include/marlin_b200.h"
 #include "gemm_f64.h"
+#include "launch.h"
 #include "stream_buffer.h"
 
 #include <cuda_runtime.h>
@@ -91,8 +92,6 @@ bool stream_memops_available();
 cudaError_t stream_write64(void* flag, unsigned long long v, cudaStream_t st);
 cudaError_t stream_wait64_geq(const void* flag, unsigned long long v, cudaStream_t st);
 cudaError_t flag_wait(const void* flag, unsigned long long v, cudaStream_t st);
-cudaError_t flag_wait_bounded(const void* flag, unsigned long long v, long long timeout_ns, unsigned long long* status,
-                              cudaStream_t st, unsigned long long tag = 0);
 }  // namespace mb
 
 // thread-local message of the last failing call (defined in capi.cu)
@@ -124,7 +123,7 @@ inline int32_t check_ctx(mb_ctx* ctx) {
     if (!ctx) return fail(MB_ERR_INVALID_ARG, "null context");
     cudaError_t e = cudaSetDevice(ctx->device);
     if (e != cudaSuccess) return cuda_fail(e, "cudaSetDevice");
-    mb::set_dmma_reference(ctx->dmma_reference);    // the DMMA kernels this call launches follow its context
+    mb::begin_call(&ctx->launches, ctx->dmma_reference);    // the launches of this call are counted on, and follow, ctx
     return MB_OK;
 }
 #define MB_CTX(ctx)                        \

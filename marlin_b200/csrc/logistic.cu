@@ -17,7 +17,7 @@
 // Everything is deterministic: the same inputs give the same bits on every run.
 #include "logistic.h"
 #include "ptx.cuh"
-#include "tma.h"
+#include "launch.h"
 
 #include <cstdint>
 
@@ -181,7 +181,7 @@ cudaError_t lr_gradient_f64(const double* x, long long ld, int m, int n, double*
     cudaError_t e = launch_with_smem<lr_grad_tile_kernel>(grid, LR_THREADS, LR_SMEM, st, s, (const double*)w, part);
     if (e != cudaSuccess) return e;
     lr_fold_kernel<<<(n + 255) / 256, 256, 0, st>>>(part, grid, n, update ? nullptr : out, update ? w : nullptr, scale);
-    return cudaGetLastError();
+    return launched();
 }
 
 }  // namespace mb

@@ -14,7 +14,7 @@
 // A1, Z2, A2 and D2 exist only in shared memory and registers.  No atomics: the same inputs give the same bits.
 #include "mlp.h"
 #include "ptx.cuh"
-#include "tma.h"
+#include "launch.h"
 
 #include <cstdint>
 
@@ -261,7 +261,7 @@ cudaError_t nn_apply_f64(const double* part, long long ldp, long long stride, co
     const long long count = (long long)rows * cols;
     nn_apply_kernel<<<(unsigned)((count + 255) / 256), 256, 0, st>>>(part, ldp, stride, first, nblocks, rows, count, scale, out,
                                                                     ldo, w, ldw);
-    return cudaGetLastError();
+    return launched();
 }
 
 }  // namespace mb

@@ -18,6 +18,7 @@
 //                                      the gathers.
 #include "pagerank.h"
 #include "../../include/marlin_b200.h"
+#include "launch.h"
 
 #include <algorithm>
 
@@ -171,25 +172,22 @@ cudaError_t pagerank_plan(const CsrView& L, long long nnz, PagerankPlan* p, cuda
     if (cap > 0) {
         const unsigned grid = (unsigned)std::min<long long>((L.rows + 255) / 256, 4096);
         pagerank_bin_kernel<<<grid, 256, 0, st>>>(L, p->heavy, count);
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+        if ((e = launched()) != cudaSuccess) return e;
     }
     if ((e = cudaMemcpyAsync(&p->nheavy, count, sizeof(int), cudaMemcpyDeviceToHost, st)) != cudaSuccess) return e;
     return cudaStreamSynchronize(st);
 }
 
 cudaError_t pagerank_step(const CsrView& L, const PagerankPlan& p, const double* x, long long seg_len, double addend,
-                          double* y, cudaStream_t st, int* launches) {
-    *launches = 0;
+                          double* y, cudaStream_t st) {
     if (L.rows == 0) return cudaSuccess;
     const long long warps = (L.rows + 31) / 32;
     pagerank_step_kernel<<<(unsigned)((warps + ROW_WARPS - 1) / ROW_WARPS), 32 * ROW_WARPS, 0, st>>>(L, x, seg_len, addend, y);
-    ++*launches;
-    if (p.nheavy) {
-        pagerank_step_kernel<<<(unsigned)((p.nheavy + HEAVY_WARPS - 1) / HEAVY_WARPS), 32 * HEAVY_WARPS, 0, st>>>(
-            L, p.heavy, p.nheavy, x, seg_len, addend, y);
-        ++*launches;
-    }
-    return cudaGetLastError();
+    const cudaError_t e = launched();
+    if (e != cudaSuccess || !p.nheavy) return e;
+    pagerank_step_kernel<<<(unsigned)((p.nheavy + HEAVY_WARPS - 1) / HEAVY_WARPS), 32 * HEAVY_WARPS, 0, st>>>(
+        L, p.heavy, p.nheavy, x, seg_len, addend, y);
+    return launched();
 }
 
 }  // namespace mb

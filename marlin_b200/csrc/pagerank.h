@@ -16,6 +16,6 @@ cudaError_t pagerank_plan(const CsrView& L, long long nnz, PagerankPlan* p, cuda
 // sequential sum from 0.0 of fl(w * x_j) over the row's sources j in [s * seg_len, (s + 1) * seg_len).  x has L.cols
 // elements, y L.rows; y must not overlap x.  Two launches (light rows, heavy rows); no synchronisation.
 cudaError_t pagerank_step(const CsrView& L, const PagerankPlan& p, const double* x, long long seg_len, double addend,
-                          double* y, cudaStream_t st, int* launches);
+                          double* y, cudaStream_t st);
 
 }  // namespace mb

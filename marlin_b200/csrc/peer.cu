@@ -5,6 +5,7 @@
 // (:177) are written by the GEMM epilogue straight into the reducing rank's HBM (P2P stores), with no NCCL call
 // on the data path.
 #include "../../include/marlin_b200.h"
+#include "launch.h"
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <atomic>
@@ -21,24 +22,12 @@ __global__ void flag_signal_kernel(unsigned long long* flag, unsigned long long 
     __threadfence_system();
     asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(flag), "l"(v) : "memory");
 }
-// Bounded wait: after timeout_ns (0 = forever) the kernel sets *status = 2 and returns, so a rank whose peer died
-// mid-multiply gets an error code from the next mb_comm_check / multiply call instead of a GPU that cannot be interrupted.
-__global__ void flag_wait_kernel(const unsigned long long* flag, unsigned long long v, long long timeout_ns,
-                                 unsigned long long* status, unsigned long long tag) {
-    unsigned long long cur, t0 = 0;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
-    for (unsigned spins = 0;; ++spins) {
+__global__ void flag_wait_kernel(const unsigned long long* flag, unsigned long long v) {
+    for (;;) {
+        unsigned long long cur;
         asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(cur) : "l"(flag) : "memory");
-        if (cur >= v) break;
+        if (cur >= v) return;
         __nanosleep(256);
-        if ((spins & 1023u) == 1023u && timeout_ns > 0) {
-            unsigned long long now;
-            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
-            if ((long long)(now - t0) > timeout_ns) {
-                if (status) *status = tag ? tag : 2ull;      // which wait gave up (first one wins is not needed: any is a lead)
-                break;
-            }
-        }
     }
 }
 
@@ -178,16 +167,11 @@ cudaError_t stream_wait64_geq(const void* flag, unsigned long long v, cudaStream
 
 cudaError_t flag_signal(void* flag, unsigned long long v, cudaStream_t st) {
     flag_signal_kernel<<<1, 1, 0, st>>>(static_cast<unsigned long long*>(flag), v);
-    return cudaGetLastError();
+    return launched();
 }
 cudaError_t flag_wait(const void* flag, unsigned long long v, cudaStream_t st) {
-    flag_wait_kernel<<<1, 1, 0, st>>>(static_cast<const unsigned long long*>(flag), v, 0, nullptr, 0);
-    return cudaGetLastError();
-}
-cudaError_t flag_wait_bounded(const void* flag, unsigned long long v, long long timeout_ns, unsigned long long* status,
-                              cudaStream_t st, unsigned long long tag) {
-    flag_wait_kernel<<<1, 1, 0, st>>>(static_cast<const unsigned long long*>(flag), v, timeout_ns, status, tag);
-    return cudaGetLastError();
+    flag_wait_kernel<<<1, 1, 0, st>>>(static_cast<const unsigned long long*>(flag), v);
+    return launched();
 }
 
 }  // namespace mb

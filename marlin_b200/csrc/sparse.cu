@@ -8,6 +8,7 @@
 // of BlockMatrix.multiply (matrix/BlockMatrix.scala:177).
 #include "sparse.h"
 #include "elementwise.h"
+#include "launch.h"
 #include "stream_buffer.h"
 
 #include <algorithm>
@@ -227,41 +228,39 @@ __global__ void __launch_bounds__(128) sample_rows_kernel(int rows, int cols, in
 cudaError_t csc_to_dense(const CscView& S, DView out, cudaStream_t st) {
     if (S.rows <= 0 || S.cols <= 0) return cudaSuccess;
     csc_to_dense_kernel<<<S.cols, 256, 0, st>>>(S, out);
-    return cudaGetLastError();
+    return launched();
 }
 
 cudaError_t spmm_dense_sparse(int m, DView A, const CscView& B, DView C, bool accumulate, cudaStream_t st) {
     if (m <= 0 || B.cols <= 0) return cudaSuccess;
     const dim3 grid(B.cols, (unsigned)std::min<long long>((m + 255) / 256, 65535));
     dense_sparse_kernel<<<grid, 256, 0, st>>>(m, A, B, C, accumulate ? 1 : 0);
-    return cudaGetLastError();
+    return launched();
 }
 
-cudaError_t csc_to_csr(const CscView& S, long long nnz, int* rowptr, int* colidx, double* vals, cudaStream_t st, int* launches) {
-    *launches = 0;
+cudaError_t csc_to_csr(const CscView& S, long long nnz, int* rowptr, int* colidx, double* vals, cudaStream_t st) {
     cudaError_t e = cudaMemsetAsync(rowptr, 0, sizeof(int) * ((size_t)S.rows + 1), st);
-    if (e != cudaSuccess || S.rows <= 0) return e;
-    if (nnz > 0) {
-        const int g = (int)std::min<long long>((nnz + 255) / 256, 4096);
-        csr_count_kernel<<<g, 256, 0, st>>>(S.rowidx, nnz, rowptr + 1);
-        scan_inplace_kernel<<<1, 1024, 0, st>>>(rowptr + 1, S.rows);
-        StreamBuffer cursor;
-        if ((e = cursor.alloc(sizeof(int) * (size_t)S.rows, st)) != cudaSuccess) return e;
-        e = cudaMemcpyAsync(cursor.as<int>(), rowptr, sizeof(int) * (size_t)S.rows, cudaMemcpyDeviceToDevice, st);
-        if (e == cudaSuccess) {
-            csr_scatter_kernel<<<g, 256, 0, st>>>(S, nnz, cursor.as<int>(), colidx, vals);
-            csr_sort_kernel<<<(S.rows + 127) / 128, 128, 0, st>>>(S.rows, rowptr, colidx, vals);
-            *launches = 4;
-        }
-    }
-    return e != cudaSuccess ? e : cudaGetLastError();
+    if (e != cudaSuccess || S.rows <= 0 || nnz <= 0) return e;
+    const int g = (int)std::min<long long>((nnz + 255) / 256, 4096);
+    csr_count_kernel<<<g, 256, 0, st>>>(S.rowidx, nnz, rowptr + 1);
+    if ((e = launched()) != cudaSuccess) return e;
+    scan_inplace_kernel<<<1, 1024, 0, st>>>(rowptr + 1, S.rows);
+    if ((e = launched()) != cudaSuccess) return e;
+    StreamBuffer cursor;
+    if ((e = cursor.alloc(sizeof(int) * (size_t)S.rows, st)) != cudaSuccess) return e;
+    e = cudaMemcpyAsync(cursor.as<int>(), rowptr, sizeof(int) * (size_t)S.rows, cudaMemcpyDeviceToDevice, st);
+    if (e != cudaSuccess) return e;
+    csr_scatter_kernel<<<g, 256, 0, st>>>(S, nnz, cursor.as<int>(), colidx, vals);
+    if ((e = launched()) != cudaSuccess) return e;
+    csr_sort_kernel<<<(S.rows + 127) / 128, 128, 0, st>>>(S.rows, rowptr, colidx, vals);
+    return launched();
 }
 
 cudaError_t spmm_sparse_dense(const CsrView& A, int n, DView B, DView C, bool accumulate, cudaStream_t st) {
     if (A.rows <= 0 || n <= 0) return cudaSuccess;
     const dim3 grid((unsigned)((A.rows + 127) / 128), (unsigned)std::min(n, 65535));
     sparse_dense_kernel<<<grid, 128, 0, st>>>(A, n, B, C, accumulate ? 1 : 0);
-    return cudaGetLastError();
+    return launched();
 }
 
 cudaError_t spgemm_dense_out(const CscView& A, const CscView& B, DView C, bool accumulate, cudaStream_t st) {
@@ -271,7 +270,7 @@ cudaError_t spgemm_dense_out(const CscView& A, const CscView& B, DView C, bool a
     const long long blocks = (ntasks + SPG_WARPS - 1) / SPG_WARPS;
     if (blocks > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
     spgemm_kernel<<<(unsigned)blocks, 32 * SPG_WARPS, 0, st>>>(A, B, C, nchunks, ntasks, accumulate ? 1 : 0);
-    return cudaGetLastError();
+    return launched();
 }
 
 cudaError_t sparse_sample_rows(int rows, int cols, int s, unsigned long long state0, long long first, int* colptr,
@@ -281,7 +280,7 @@ cudaError_t sparse_sample_rows(int rows, int cols, int s, unsigned long long sta
     if (e != cudaSuccess) return e;
     sample_rows_kernel<<<(cols + 1 + 127) / 128, 128, 0, st>>>(rows, cols, s, state0, (unsigned long long)first, tab,
                                                                colptr, rowidx);
-    return cudaGetLastError();
+    return launched();
 }
 
 }  // namespace mb

@@ -28,7 +28,7 @@ cudaError_t csc_to_dense(const CscView& S, DView out, cudaStream_t st);
 // C (m x n) [+]= A (m x K, dense) * B (K x n, CSC); each C(r, j) summed over B's column j in stored order.
 cudaError_t spmm_dense_sparse(int m, DView A, const CscView& B, DView C, bool accumulate, cudaStream_t st);
 // Builds the CSR copy of S into rowptr (rows + 1), colidx (nnz), vals (nnz); deterministic.
-cudaError_t csc_to_csr(const CscView& S, long long nnz, int* rowptr, int* colidx, double* vals, cudaStream_t st, int* launches);
+cudaError_t csc_to_csr(const CscView& S, long long nnz, int* rowptr, int* colidx, double* vals, cudaStream_t st);
 // C (m x n) [+]= A (m x K, CSR copy) * B (K x n, dense); each C(r, j) summed over k ascending.
 cudaError_t spmm_sparse_dense(const CsrView& A, int n, DView B, DView C, bool accumulate, cudaStream_t st);
 // C (m x n, dense) [+]= A (m x K, CSC) * B (K x n, CSC); each C(r, j) summed over B's column j in stored order.

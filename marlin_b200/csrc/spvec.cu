@@ -18,6 +18,7 @@
 // Hash rows are sorted by column (bitonic, the empty key sorts last) before they are written.
 #include "spvec.h"
 #include "../../include/marlin_b200.h"
+#include "launch.h"
 
 #include <algorithm>
 #include <climits>
@@ -323,10 +324,10 @@ __global__ void spvec_replicate_kernel(int rows, int s, int* rowptr, int* colidx
     }
 }
 
-cudaError_t scan(int* rowptr, int rows, long long* total_d, long long* total, cudaStream_t st, int* launches) {
+cudaError_t scan(int* rowptr, int rows, long long* total_d, long long* total, cudaStream_t st) {
     spvec_scan_kernel<<<1, 1024, 0, st>>>(rowptr + 1, rows, total_d);
-    ++*launches;
-    cudaError_t e = cudaMemcpyAsync(total, total_d, sizeof(long long), cudaMemcpyDeviceToHost, st);
+    cudaError_t e = launched();
+    if (e == cudaSuccess) e = cudaMemcpyAsync(total, total_d, sizeof(long long), cudaMemcpyDeviceToHost, st);
     return e == cudaSuccess ? cudaStreamSynchronize(st) : e;
 }
 
@@ -334,9 +335,7 @@ unsigned warps_grid(long long rows) { return (unsigned)((rows * 32 + 255) / 256)
 
 }  // namespace
 
-cudaError_t spvec_count(const CsrView& A, const CsrView& B, int* rowptr, long long* total, SpvecWork* w, cudaStream_t st,
-                        int* launches) {
-    *launches = 0;
+cudaError_t spvec_count(const CsrView& A, const CsrView& B, int* rowptr, long long* total, SpvecWork* w, cudaStream_t st) {
     *total = 0;
     cudaError_t e = cudaMemsetAsync(rowptr, 0, sizeof(int) * ((size_t)A.rows + 1), st);
     if (e != cudaSuccess || A.rows == 0) return e;
@@ -346,81 +345,78 @@ cudaError_t spvec_count(const CsrView& A, const CsrView& B, int* rowptr, long lo
     int *lists = w->lists.as<int>(), *bin_size = w->bin_size.as<int>();
     if ((e = cudaMemsetAsync(bin_size, 0, 32, st)) != cudaSuccess) return e;
     spvec_bound_kernel<<<warps_grid(A.rows), 256, 0, st>>>(A, B, lists, bin_size, w->range.as<int2>());
-    ++*launches;
+    if ((e = launched()) != cudaSuccess) return e;
     if ((e = cudaMemcpyAsync(w->bins, bin_size, sizeof(w->bins), cudaMemcpyDeviceToHost, st)) != cudaSuccess) return e;
     if ((e = cudaStreamSynchronize(st)) != cudaSuccess) return e;
     const long long n = A.rows;
     if (w->bins[0]) {
         spvec_warp_kernel<false><<<(w->bins[0] + ROW_WARPS - 1) / ROW_WARPS, 32 * ROW_WARPS, 0, st>>>(A, B, lists, w->bins[0],
                                                                                                       rowptr, nullptr, nullptr);
-        ++*launches;
+        if ((e = launched()) != cudaSuccess) return e;
     }
     if (w->bins[1]) {
         spvec_cta_kernel<false><<<w->bins[1], CTA_THREADS, sizeof(int) * CTA_SLOTS, st>>>(A, B, lists + n, rowptr, nullptr,
                                                                                           nullptr);
-        ++*launches;
+        if ((e = launched()) != cudaSuccess) return e;
     }
     if (w->bins[2]) {
         const size_t smem = sizeof(unsigned) * (WINDOW / 32) + sizeof(int) * CTA_THREADS;
         spvec_window_kernel<false><<<w->bins[2], CTA_THREADS, smem, st>>>(A, B, lists + 2 * n, w->range.as<int2>(), rowptr, nullptr,
                                                                           nullptr);
-        ++*launches;
+        if ((e = launched()) != cudaSuccess) return e;
     }
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    return scan(rowptr, A.rows, reinterpret_cast<long long*>(bin_size + 4), total, st, launches);
+    return scan(rowptr, A.rows, reinterpret_cast<long long*>(bin_size + 4), total, st);
 }
 
 cudaError_t spvec_fill(const CsrView& A, const CsrView& B, const SpvecWork& w, const int* rowptr, int* colidx, double* vals,
-                       cudaStream_t st, int* launches) {
-    *launches = 0;
+                       cudaStream_t st) {
     const long long n = A.rows;
     int* rp = const_cast<int*>(rowptr);
     const int* lists = w.lists.as<int>();
+    cudaError_t e;
     if (w.bins[0]) {
         spvec_warp_kernel<true><<<(w.bins[0] + ROW_WARPS - 1) / ROW_WARPS, 32 * ROW_WARPS, 0, st>>>(A, B, lists, w.bins[0], rp,
                                                                                                     colidx, vals);
-        ++*launches;
+        if ((e = launched()) != cudaSuccess) return e;
     }
     if (w.bins[1]) {
         const size_t smem = (sizeof(int) + sizeof(float)) * CTA_SLOTS;
-        cudaError_t e = cudaFuncSetAttribute(spvec_cta_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
+        if ((e = cudaFuncSetAttribute(spvec_cta_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess)
+            return e;
         spvec_cta_kernel<true><<<w.bins[1], CTA_THREADS, smem, st>>>(A, B, lists + n, rp, colidx, vals);
-        ++*launches;
+        if ((e = launched()) != cudaSuccess) return e;
     }
     if (w.bins[2]) {
         const size_t smem = sizeof(unsigned) * (WINDOW / 32) + sizeof(int) * CTA_THREADS + sizeof(float) * WINDOW;
-        cudaError_t e = cudaFuncSetAttribute(spvec_window_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
+        if ((e = cudaFuncSetAttribute(spvec_window_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess)
+            return e;
         spvec_window_kernel<true><<<w.bins[2], CTA_THREADS, smem, st>>>(A, B, lists + 2 * n, w.range.as<int2>(), rp, colidx, vals);
-        ++*launches;
+        return launched();
     }
-    return cudaGetLastError();
+    return cudaSuccess;
 }
 
-cudaError_t dense_rows_count(DView D, int rows, int cols, int* rowptr, long long* total, cudaStream_t st, int* launches) {
-    *launches = 0;
+cudaError_t dense_rows_count(DView D, int rows, int cols, int* rowptr, long long* total, cudaStream_t st) {
     *total = 0;
     cudaError_t e = cudaMemsetAsync(rowptr, 0, sizeof(int) * ((size_t)rows + 1), st);
     if (e != cudaSuccess || rows == 0) return e;
     StreamBuffer total_d;
     if ((e = total_d.alloc(sizeof(long long), st)) != cudaSuccess) return e;
     dense_rows_kernel<false><<<warps_grid(rows), 256, 0, st>>>(D, rows, cols, rowptr, nullptr, nullptr);
-    ++*launches;
-    e = cudaGetLastError();
-    return e == cudaSuccess ? scan(rowptr, rows, total_d.as<long long>(), total, st, launches) : e;
+    e = launched();
+    return e == cudaSuccess ? scan(rowptr, rows, total_d.as<long long>(), total, st) : e;
 }
 
 cudaError_t dense_rows_compact(DView D, int rows, int cols, const int* rowptr, int* colidx, double* vals, cudaStream_t st) {
     if (rows == 0) return cudaSuccess;
     dense_rows_kernel<true><<<warps_grid(rows), 256, 0, st>>>(D, rows, cols, const_cast<int*>(rowptr), colidx, vals);
-    return cudaGetLastError();
+    return launched();
 }
 
 cudaError_t spvec_replicate_columns(int rows, int s, int* rowptr, int* colidx, cudaStream_t st) {
     const long long n = std::max<long long>((long long)rows * s, (long long)rows + 1);
     spvec_replicate_kernel<<<(unsigned)std::min<long long>((n + 255) / 256, 4096), 256, 0, st>>>(rows, s, rowptr, colidx);
-    return cudaGetLastError();
+    return launched();
 }
 
 }  // namespace mb

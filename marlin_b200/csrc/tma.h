@@ -1,7 +1,6 @@
 // Host side of the TMA GEMMs (gemm_f64.cu, gemm_bf16.cu, gemm_ozaki.cu): tensor maps from the driver's
-// cuTensorMapEncodeTiled, and the launch of a kernel whose shared-memory ring is larger than the 48 KiB default.
+// cuTensorMapEncodeTiled.
 #pragma once
-#include <atomic>
 #include <cstdint>
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -51,20 +50,6 @@ inline bool tma_map_3d(CUtensorMap* map, CUtensorMapDataType type, const void* b
     const cuuint64_t dims[3] = {d0, d1, d2}, strides[2] = {stride1, stride2};
     const cuuint32_t box[3] = {box0, box1, 1};
     return tma_encode(map, type, 3, base, dims, strides, box);
-}
-
-// Kernel<<<grid, threads, smem, stream>>>(args...), raising the kernel's dynamic shared-memory limit to smem on its first
-// launch.  Setting the attribute is idempotent, so threads that race on a first launch may both set it.
-template <auto Kernel, class... Args>
-cudaError_t launch_with_smem(int grid, int threads, int smem, cudaStream_t stream, const Args&... args) {
-    static std::atomic<bool> attr_done{false};
-    if (!attr_done.load(std::memory_order_acquire)) {
-        const cudaError_t e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-        if (e != cudaSuccess) return e;
-        attr_done.store(true, std::memory_order_release);
-    }
-    Kernel<<<grid, threads, smem, stream>>>(args...);
-    return cudaGetLastError();
 }
 
 }  // namespace mb
