@@ -153,6 +153,31 @@ int32_t mb_block_copy(mb_ctx* ctx, const mb_block* A, mb_block* out);
 /* BlockMatrix.sum per block (matrix/BlockMatrix.scala:467-472) */
 int32_t mb_block_sum(mb_ctx* ctx, const mb_block* A, double* sum_out);
 
+/* ---- DenseVecMatrix.norm(mode) (matrix/DenseVecMatrix.scala:975-999) on one row shard.  The reference's "1" never sums
+ *      (its per-row map is lazy and discarded) and its "inf" sums signed values; these are the norms its comment names:
+ *      the largest column sum of |a|, the largest row sum of |a|, and sqrt(sum a^2) (a TODO there).  "2" stays
+ *      unsupported. ---- */
+#define MB_NORM_ONE 0
+#define MB_NORM_INF 1
+#define MB_NORM_FRO 2
+/* The mode string of norm(mode): "1", "inf" or "fro" -> MB_NORM_ONE / MB_NORM_INF / MB_NORM_FRO in *kind; anything else
+ * (also "2") is MB_ERR_INVALID_ARG "Do not support mode <mode>.".  Pure logic, no GPU needed. */
+int32_t mb_norm_mode(const char* mode, int32_t* kind);
+/* One pass over any fp64 view A (m x n, element strides as the block says; a row shard's transposed view is read in
+ * place).  Blocking.  Every result is the same bits on every run.
+ *   MB_NORM_ONE: col_sums (an fp64 vector of n elements: one row or one column) := the column sums of |a|, each the sum of
+ *                fixed chunks of rows, a chunk summed in row order, the chunk partials in chunk order; *out (may be NULL)
+ *                := the largest of them.
+ *   MB_NORM_INF: *out := the largest row sum of |a|, each row a left fold s = s + |a_rc| in column order from 0.0.
+ *   MB_NORM_FRO: out[0..2] := the small, medium and big accumulators of sum a^2 as LAPACK 3.10 dnrm2 (Blue's algorithm)
+ *                keeps them; mb_norm_fro turns them into the norm.  col_sums is not used by INF and FRO.
+ * "Largest" is java.lang.Double.compare's order (RDD.max()): a NaN anywhere is the result.  A view with no rows, or the
+ * 1-norm of no columns, is MB_ERR_EMPTY "empty collection". */
+int32_t mb_block_norm(mb_ctx* ctx, const mb_block* A, int32_t kind, mb_block* col_sums, double* out);
+/* The Frobenius norm of `count` shards from their accumulator triples acc[3 * i .. 3 * i + 2] (mb_block_norm,
+ * MB_NORM_FRO), added in index order, then dnrm2's final combination: no spurious overflow or underflow.  Pure logic. */
+int32_t mb_norm_fro(const double* acc, int32_t count, double* out);
+
 /* ---- vector side of the path (SURVEY 8f-4): a vector is a block with one column (or one row) ----
  * y = A x (+ y): SubMatrix.multiply(v: Vector) (matrix/SubMatrix.scala:131-139) -> Breeze `BDM * BDV` -> netlib dgemv;
  * used per block by BlockMatrix.multiply(v: DistributedVector / BDV) (matrix/BlockMatrix.scala:240-274), whose

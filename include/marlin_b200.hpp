@@ -25,6 +25,7 @@
 #include <string>
 #include <tuple>
 #include <utility>
+#include <variant>
 #include <vector>
 
 namespace marlin {
@@ -342,6 +343,24 @@ class DenseVecMatrix;
 class DistributedVector;
 class SparseVecMatrix;
 
+// The block heights (widths) of `total` rows (columns) in `parts` blocks as every method here lays them out: block i
+// starts at i * ceil(total / parts).
+inline std::vector<int> blockExtents(long total, int parts) {
+    const int step = ceilLen(total, parts);
+    std::vector<int> e;
+    for (int i = 0; i < parts; ++i) e.push_back((int)std::min<long>(step, total - (long)i * step));
+    return e;
+}
+// Whether blocks of these heights (widths), in this order, sit where the ceil-sized grid of their sum puts them.
+inline bool isCeilGrid(const std::vector<int>& e) {
+    long total = 0;
+    for (int v : e) {
+        if (v <= 0) return false;
+        total += v;
+    }
+    return e == blockExtents(total, (int)e.size());
+}
+
 // ---------------------------------------------------------------------------------------------- BlockMatrix
 class BlockMatrix {
 public:
@@ -587,6 +606,31 @@ public:
         return BlockMatrix(res, numCols(), numRows(), numBlksByCol(), numBlksByRow());
     }
     inline DenseVecMatrix toDenseVecMatrix();                                         // :575-594
+    // cBind(other) :687-705 — with the same number of block rows, other's block columns are relabelled by
+    // + numBlksByCol() (no block copied) when the joint widths are exactly the ceil-sized grid that toBreeze, multiply and
+    // re-gridding assume; otherwise, and with a DenseVecMatrix, the DenseVecMatrix cBind of both (DESIGN §3.14)
+    inline std::variant<BlockMatrix, DenseVecMatrix> cBind(BlockMatrix& other);
+    inline DenseVecMatrix cBind(DenseVecMatrix& other);
+    // elementMultiply(other, partitioner) :673-680 — the element-wise product on matching BlockIDs (an inner join); the
+    // products are new blocks and this matrix is unchanged (the reference writes over its blocks); the partitioner is a
+    // shuffle hint and is ignored
+    BlockMatrix elementMultiply(BlockMatrix& other) {
+        if (hasSparse() || other.hasSparse())
+            throw std::invalid_argument("elementMultiply is not supported on sparse blocks: call toDenseBlocks first");
+        std::map<std::pair<int, int>, SubMatrix> theirs;
+        for (auto& kv : other.blocks) theirs[{kv.first.row, kv.first.column}] = kv.second;
+        Blocks res;
+        for (auto& kv : blocks) {
+            auto it = theirs.find({kv.first.row, kv.first.column});
+            if (it != theirs.end()) res.emplace_back(kv.first, kv.second.elementMultiply(it->second));
+        }
+        return BlockMatrix(res, numRows(), numCols(), numBlksByRow(), numBlksByCol());
+    }
+    template <class Partitioner>
+    BlockMatrix elementMultiply(BlockMatrix& other, const Partitioner&) { return elementMultiply(other); }
+    // MTUtils.repeatByRow (columns = true) / repeatByColumn (false) for times > 1: relabelled blocks when the repeated
+    // widths (heights) are the ceil-sized grid, else through the rows, re-gridded to (B_r, B_c * times) / (B_r * times, B_c)
+    inline BlockMatrix repeat(int times, bool columns);
     // toBlockMatrix(newNumByRow, newNumByCol) :610-665 — pieces cut as views and pasted into the new grid
     BlockMatrix toBlockMatrix(int newByRow, int newByCol) {
         if (blksByRow_ == newByRow && blksByCol_ == newByCol) return *this;
@@ -749,6 +793,87 @@ public:
     DenseVecMatrix dotProduct(BlockMatrix& o) { DenseVecMatrix d = o.toDenseVecMatrix(); return dotProduct(d); }
     double sum() { if (ids_.empty()) throw std::runtime_error("empty collection"); return data_.sum(); }
 
+    // norm(mode) :975-999 — "1": the largest column sum of |a|, "inf": the largest row sum of |a|, "fro": sqrt(sum a^2);
+    // any other mode ("2" too) is "Do not support mode <mode>.".  One pass over the shard (mb_block_norm); the reference's
+    // "1" never sums and its "inf" sums signed values (DESIGN §3.14)
+    double norm(const std::string& mode) {
+        int32_t kind = 0;
+        check(mb_norm_mode(mode.c_str(), &kind));
+        if (ids_.empty()) throw std::runtime_error("empty collection");
+        double out[3] = {0.0, 0.0, 0.0};
+        if (kind == MB_NORM_ONE) {
+            SubMatrix col = SubMatrix::empty(data_.cols(), 1);
+            check(mb_block_norm(Context::get(), data_.handle(), kind, col.handle(), out));
+            return out[0];
+        }
+        check(mb_block_norm(Context::get(), data_.handle(), kind, nullptr, out));
+        if (kind == MB_NORM_INF) return out[0];
+        double fro = 0.0;
+        check(mb_norm_fro(out, 1, &fro));
+        return fro;
+    }
+    // sliceByRow / sliceByColumn / getSubMatrix :928-964 — inclusive bounds, row ids shifted by -startRow, the reference's
+    // messages; end == numRows() / numCols() and start > end are rejected too (DESIGN §3.14)
+    DenseVecMatrix sliceByRow(long startRow, long endRow) {
+        if (!(startRow >= 0 && endRow < numRows() && startRow <= endRow)) throw std::invalid_argument("start row or end row mismatch the matrix num of rows");
+        return window(startRow, endRow, 0, (int)numCols() - 1);
+    }
+    DenseVecMatrix sliceByColumn(int startCol, int endCol) {
+        if (!(startCol >= 0 && endCol < numCols() && startCol <= endCol)) throw std::invalid_argument("start column or end column mismatch the matrix num of columns");
+        return window(0, numRows() - 1, startCol, endCol);
+    }
+    DenseVecMatrix getSubMatrix(long startRow, long endRow, int startCol, int endCol) {
+        if (!(startRow >= 0 && endRow < numRows() && startRow <= endRow)) throw std::invalid_argument("start row or end row dismatch the matrix num of rows");
+        if (!(startCol >= 0 && endCol < numCols() && startCol <= endCol)) throw std::invalid_argument("start column or end column dismatch the matrix num of columns");
+        return window(startRow, endRow, startCol, endCol);
+    }
+    // cBind(other) :238-252 — rows.join(that.rows): a row on one side only is dropped; each row is this ++ that
+    DenseVecMatrix cBind(DenseVecMatrix& other) {
+        if (numRows() != other.numRows()) throw std::invalid_argument("Dimension mismatch:  " + std::to_string(numRows()) + " vs " + std::to_string(other.numRows()));
+        const int n1 = (int)numCols(), n2 = (int)other.numCols();
+        std::map<long, int> theirs;
+        for (size_t p = 0; p < other.ids_.size(); ++p) theirs[other.ids_[p]] = (int)p;
+        std::vector<long> ids;
+        std::vector<int> mine, that;
+        for (size_t p = 0; p < ids_.size(); ++p) {
+            auto it = theirs.find(ids_[p]);
+            if (it == theirs.end()) continue;
+            ids.push_back(ids_[p]);
+            mine.push_back((int)p);
+            that.push_back(it->second);
+        }
+        if (ids.empty()) return DenseVecMatrix(ids, SubMatrix(), numRows(), n1 + n2);
+        SubMatrix out = SubMatrix::empty(n1 + n2, (int)ids.size()).t();
+        copyRows(data_, mine, 0, n1, out, 0);
+        copyRows(other.data_, that, 0, n2, out, n1);
+        return DenseVecMatrix(ids, out, numRows(), n1 + n2);
+    }
+    DenseVecMatrix cBind(BlockMatrix& other) {                                       // :246-248
+        if (numRows() != other.numRows()) throw std::invalid_argument("Dimension mismatch:  " + std::to_string(numRows()) + " vs " + std::to_string(other.numRows()));
+        DenseVecMatrix rows = other.toDenseVecMatrix();
+        return cBind(rows);
+    }
+    // MTUtils.repeatByRow: every row becomes `times` copies of itself side by side (numCols() * times)
+    DenseVecMatrix repeatColumns(int times) {
+        const int n = (int)numCols();
+        if (ids_.empty()) return DenseVecMatrix(ids_, SubMatrix(), numRows(), (long)n * times);
+        SubMatrix out = SubMatrix::empty(n * times, (int)ids_.size()).t();
+        for (int i = 0; i < times; ++i) out.slice(0, (int)ids_.size(), i * n, (i + 1) * n).assign(data_);
+        return DenseVecMatrix(ids_, out, numRows(), (long)n * times);
+    }
+    // MTUtils.repeatByColumn: the matrix stacked `times` times, copy i of row id holding id + i * numRows()
+    DenseVecMatrix repeatRows(int times) {
+        const long m = numRows();
+        const int n = (int)numCols(), k = (int)ids_.size();
+        std::vector<long> ids;
+        for (int i = 0; i < times; ++i)
+            for (long id : ids_) ids.push_back(id + i * m);
+        if (ids_.empty()) return DenseVecMatrix(ids, SubMatrix(), m * times, n);
+        SubMatrix out = SubMatrix::empty(n, k * times).t();
+        for (int i = 0; i < times; ++i) out.slice(i * k, (i + 1) * k, 0, n).assign(data_);
+        return DenseVecMatrix(ids, out, m * times, n);
+    }
+
     BlockMatrix transpose(int numBlocks = 2) {                                        // :1420-1436 (local[2] parallelism)
         BlockMatrix b = toBlockMatrix(std::min(numBlocks, (int)numRows() / 2), 1);
         return b.transpose();
@@ -887,6 +1012,30 @@ public:
     }
 
 private:
+    // rows src[pos[i]] (columns c0 until c1) into row i of dst from column d0; runs of consecutive positions as one copy
+    static void copyRows(const SubMatrix& src, const std::vector<int>& pos, int c0, int c1, SubMatrix& dst, int d0) {
+        for (size_t p = 0; p < pos.size();) {
+            size_t q = p;
+            while (q + 1 < pos.size() && pos[q + 1] == pos[q] + 1) ++q;
+            dst.slice((int)p, (int)q + 1, d0, d0 + c1 - c0).assign(src.slice(pos[p], pos[q] + 1, c0, c1));
+            p = q + 1;
+        }
+    }
+    // rows r0..r1 and columns c0..c1 (inclusive), row ids shifted by -r0
+    DenseVecMatrix window(long r0, long r1, int c0, int c1) {
+        std::vector<long> ids;
+        std::vector<int> keep;
+        for (size_t p = 0; p < ids_.size(); ++p)
+            if (ids_[p] >= r0 && ids_[p] <= r1) {
+                keep.push_back((int)p);
+                ids.push_back(ids_[p] - r0);
+            }
+        const int nc = c1 - c0 + 1;
+        if (keep.empty()) return DenseVecMatrix(ids, SubMatrix(), r1 - r0 + 1, nc);
+        SubMatrix out = SubMatrix::empty(nc, (int)keep.size()).t();
+        copyRows(data_, keep, c0, c1 + 1, out, 0);
+        return DenseVecMatrix(ids, out, r1 - r0 + 1, nc);
+    }
     template <class F> DenseVecMatrix unary(F f) {
         if (ids_.empty()) return *this;
         // element-wise on the underlying column-major array, re-viewed as the row shard
@@ -921,6 +1070,40 @@ inline DenseVecMatrix BlockMatrix::toDenseVecMatrix() {                         
     std::vector<long> ids(nr);
     for (int i = 0; i < nr; ++i) ids[i] = i;
     return DenseVecMatrix(ids, shard, nr, nc);
+}
+inline std::variant<BlockMatrix, DenseVecMatrix> BlockMatrix::cBind(BlockMatrix& other) {                            // :687-699
+    if (numRows() != other.numRows()) throw std::invalid_argument("Row dimension mismatches: " + std::to_string(numRows()) + " vs " + std::to_string(other.numRows()));
+    const int bc = numBlksByCol();
+    std::vector<int> widths = blockExtents(numCols(), bc), theirs = blockExtents(other.numCols(), other.numBlksByCol());
+    widths.insert(widths.end(), theirs.begin(), theirs.end());
+    if (numBlksByRow() == other.numBlksByRow() && isCeilGrid(widths)) {
+        Blocks res = blocks;
+        for (auto& kv : other.blocks) res.emplace_back(BlockID(kv.first.row, kv.first.column + bc), kv.second);
+        return BlockMatrix(res, numRows(), numCols() + other.numCols(), numBlksByRow(), (int)widths.size());
+    }
+    DenseVecMatrix a = toDenseVecMatrix(), b = other.toDenseVecMatrix();
+    return a.cBind(b);
+}
+inline DenseVecMatrix BlockMatrix::cBind(DenseVecMatrix& other) {                                                       // :700-701
+    if (numRows() != other.numRows()) throw std::invalid_argument("Row dimension mismatches: " + std::to_string(numRows()) + " vs " + std::to_string(other.numRows()));
+    DenseVecMatrix a = toDenseVecMatrix();
+    return a.cBind(other);
+}
+inline BlockMatrix BlockMatrix::repeat(int times, bool columns) {
+    const int br = numBlksByRow(), bc = numBlksByCol();
+    const long m = numRows(), n = numCols();
+    const std::vector<int> one = columns ? blockExtents(n, bc) : blockExtents(m, br);
+    std::vector<int> ext;
+    for (int i = 0; i < times; ++i) ext.insert(ext.end(), one.begin(), one.end());
+    if (isCeilGrid(ext)) {
+        Blocks res;
+        for (int i = 0; i < times; ++i)
+            for (auto& kv : blocks)
+                res.emplace_back(columns ? BlockID(kv.first.row, kv.first.column + i * bc) : BlockID(kv.first.row + i * br, kv.first.column), kv.second);
+        return columns ? BlockMatrix(res, m, n * times, br, bc * times) : BlockMatrix(res, m * times, n, br * times, bc);
+    }
+    DenseVecMatrix rows = toDenseVecMatrix();
+    return columns ? rows.repeatColumns(times).toBlockMatrix(br, bc * times) : rows.repeatRows(times).toBlockMatrix(br * times, bc);
 }
 inline BlockMatrix BlockMatrix::add(DenseVecMatrix& o) { BlockMatrix b = o.toBlockMatrix(numBlksByRow(), numBlksByCol()); return add(b); }          // :346-349 (via rows in the reference)
 inline BlockMatrix BlockMatrix::subtract(DenseVecMatrix& o) { BlockMatrix b = o.toBlockMatrix(numBlksByRow(), numBlksByCol()); return subtract(b); }
@@ -1361,8 +1544,7 @@ struct MTUtils {
     static DenseVecMatrix randomDenVecMatrix(long nRows, int nCols, int numPartitions, long seed, double lo = 0.0, double hi = 1.0) {
         std::vector<int64_t> seeds(numPartitions);
         check(mb_partition_seeds(seed, numPartitions, seeds.data()));
-        SubMatrix shardT = SubMatrix::empty(nCols, (int)nRows);
-        SubMatrix shard = shardT.t();
+        SubMatrix shard = rowShard(nRows, nCols);
         long start = 0;
         for (int p = 0; p < numPartitions; ++p) {
             const long end = ((long)(p + 1) * nRows) / numPartitions;
@@ -1372,10 +1554,39 @@ struct MTUtils {
             }
             start = end;
         }
+        return DenseVecMatrix(rowIds(nRows), shard, nRows, nCols);
+    }
+    // zerosDenVecMatrix / onesDenVecMatrix (:103-125): randomDenVecMatrix's rows, every element 0.0 / 1.0
+    static DenseVecMatrix zerosDenVecMatrix(long nRows, int nCols) { return constantRows(nRows, nCols, 0.0); }
+    static DenseVecMatrix onesDenVecMatrix(long nRows, int nCols) { return constantRows(nRows, nCols, 1.0); }
+    // repeatByRow (:446-464): despite the name the columns repeat (numCols() * times, also for a BlockMatrix, where the
+    // reference keeps numCols()); repeatByColumn (:471-491): the matrix stacked, row id + i * numRows().  times == 1
+    // returns the matrix itself
+    static DenseVecMatrix repeatByRow(DenseVecMatrix& matrix, int times) { return requireTimes(times) ? matrix : matrix.repeatColumns(times); }
+    static BlockMatrix repeatByRow(BlockMatrix& matrix, int times) { return requireTimes(times) ? matrix : matrix.repeat(times, true); }
+    static DenseVecMatrix repeatByColumn(DenseVecMatrix& matrix, int times) { return requireTimes(times) ? matrix : matrix.repeatRows(times); }
+    static BlockMatrix repeatByColumn(BlockMatrix& matrix, int times) { return requireTimes(times) ? matrix : matrix.repeat(times, false); }
+
+private:
+    // the layout of the dense row generators on one process: rows 0 .. nRows-1 in one row-major shard
+    static SubMatrix rowShard(long nRows, int nCols) { return SubMatrix::empty(nCols, (int)nRows).t(); }
+    static std::vector<long> rowIds(long nRows) {
         std::vector<long> ids(nRows);
         for (long i = 0; i < nRows; ++i) ids[i] = i;
-        return DenseVecMatrix(ids, shard, nRows, nCols);
+        return ids;
     }
+    static DenseVecMatrix constantRows(long nRows, int nCols, double value) {
+        SubMatrix shard = rowShard(nRows, nCols);
+        check(mb_block_fill(Context::get(), shard.handle(), value));
+        return DenseVecMatrix(rowIds(nRows), shard, nRows, nCols);
+    }
+    // true when times == 1 (the matrix itself is the result)
+    static bool requireTimes(int times) {
+        if (times <= 0) throw std::invalid_argument("repeat times: " + std::to_string(times) + " illegal");
+        return times == 1;
+    }
+
+public:
     // randomSpaVecMatrix (:75-85): randomDenVecMatrix's partitions and seeds; partition p's rows share one column set and
     // take successive values of its stream (mb_fill_spvec_uniform)
     static SparseVecMatrix randomSpaVecMatrix(long nRows, int nColumns, double density, int numPartitions, long seed,

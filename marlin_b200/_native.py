@@ -25,6 +25,7 @@ MB_SVD_LOCAL_LAPACK, MB_SVD_LOCAL_ARPACK, MB_SVD_DIST_ARPACK = 0, 1, 2
 MB_ALS_MAX_RANK = 128
 MB_SPVEC_WARP_BOUND, MB_SPVEC_CTA_BOUND, MB_SPVEC_WINDOW = 256, 4096, 16384
 MB_PAGERANK_LIGHT_BOUND = 256
+MB_NORM_ONE, MB_NORM_INF, MB_NORM_FRO = 0, 1, 2
 
 _LIB_PATH = Path(__file__).resolve().parent / "lib" / "libmarlin_b200.so"
 
@@ -76,6 +77,9 @@ SIGNATURES = {
     "mb_block_transpose": (c_i32, [c_ctx, c_blk, c_blk]),
     "mb_block_copy": (c_i32, [c_ctx, c_blk, c_blk]),
     "mb_block_sum": (c_i32, [c_ctx, c_blk, c_dp]),
+    "mb_norm_mode": (c_i32, [C.c_char_p, C.POINTER(c_i32)]),
+    "mb_block_norm": (c_i32, [c_ctx, c_blk, c_i32, c_blk, c_dp]),
+    "mb_norm_fro": (c_i32, [c_dp, c_i32, c_dp]),
     "mb_block_gemv": (c_i32, [c_ctx, c_blk, c_blk, c_blk, c_i32]),
     "mb_block_dot": (c_i32, [c_ctx, c_blk, c_blk, c_dp]),
     "mb_block_ger": (c_i32, [c_ctx, c_blk, c_blk, c_blk]),
@@ -183,6 +187,7 @@ class MarlinError(RuntimeError):
     def __init__(self, code: int, message: str):
         super().__init__(f"[marlin_b200 {code}] {message}")
         self.code = code
+        self.message = message
 
 
 class MarlinArgumentError(ValueError):

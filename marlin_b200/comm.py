@@ -92,16 +92,24 @@ def exchange(sends: Sequence[Tuple[int, int, object]], local: Dict[object, torch
     when it is a destination.  Returns {key: received tensor}.  All ranks must call with the same list.
     """
     import torch.distributed as dist
+    # gloo moves host memory only: device tensors travel through host copies there (ranks that share one GPU)
+    staged = dist.get_backend(group) == "gloo"
     ops = []
     received: Dict[object, torch.Tensor] = {}
+    landing: Dict[object, torch.Tensor] = {}
     for (src, dst, key) in sends:
         if src == rank:
-            ops.append(dist.P2POp(dist.isend, local[key], dst, group))
+            t = local[key]
+            ops.append(dist.P2POp(dist.isend, t.cpu() if staged and t.is_cuda else t, dst, group))
         elif dst == rank:
             buf = alloc(key)
             received[key] = buf
-            ops.append(dist.P2POp(dist.irecv, buf, src, group))
+            if staged and buf.is_cuda:
+                landing[key] = torch.empty(buf.shape, dtype=buf.dtype)
+            ops.append(dist.P2POp(dist.irecv, landing.get(key, buf), src, group))
     if ops:
         for req in dist.batch_isend_irecv(ops):
             req.wait()
+    for key, host in landing.items():
+        received[key].copy_(host)
     return received

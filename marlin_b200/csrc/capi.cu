@@ -15,6 +15,7 @@
 #include "spvec.h"
 #include "pagerank.h"
 #include "mlp.h"
+#include "norm.h"
 
 #include <cuda_runtime.h>
 #include <climits>
@@ -1004,6 +1005,42 @@ int32_t mb_block_sum(mb_ctx* ctx, const mb_block* A, double* sum_out) {
     MB_CUDA(cudaMemcpyAsync(ctx->host_scalar, ctx->scratch, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
     MB_CUDA(cudaStreamSynchronize(ctx->stream));
     *sum_out = *ctx->host_scalar;
+    return MB_OK;
+}
+
+// DenseVecMatrix.norm (matrix/DenseVecMatrix.scala:975-999) on one row shard: one pass over the view, read in place.
+int32_t mb_block_norm(mb_ctx* ctx, const mb_block* A, int32_t kind, mb_block* col_sums, double* out) {
+    MB_CTX(ctx);
+    if (!A) return fail(MB_ERR_INVALID_ARG, "mb_block_norm: null block");
+    if (kind != MB_NORM_ONE && kind != MB_NORM_INF && kind != MB_NORM_FRO)
+        return fail(MB_ERR_INVALID_ARG, "mb_block_norm: unknown norm kind %d", kind);
+    if (A->dtype != MB_F64) return fail(MB_ERR_UNSUPPORTED, "mb_block_norm: fp64 blocks only");
+    vec_view cv{nullptr, 0, 0};
+    if (kind == MB_NORM_ONE) {
+        if (!col_sums) return fail(MB_ERR_INVALID_ARG, "mb_block_norm: the 1-norm needs a col_sums block");
+        if (!as_vector(col_sums, &cv) || cv.len != A->cols)
+            return fail(MB_ERR_DIM_MISMATCH, "mb_block_norm: col_sums must be an fp64 vector of %d elements", A->cols);
+    } else if (!out) {
+        return fail(MB_ERR_INVALID_ARG, "mb_block_norm: null out");
+    }
+    // RDD.max() of no values; the 1-norm of no columns is the max of no column sums
+    if (A->rows == 0 || (kind == MB_NORM_ONE && A->cols == 0)) return fail(MB_ERR_EMPTY, "empty collection");
+    if (A->cols == 0) {                                      // rows of no entries: row sums 0.0, no squares
+        out[0] = 0.0;
+        if (kind == MB_NORM_FRO) out[1] = out[2] = 0.0;
+        return MB_OK;
+    }
+    mb::StreamBuffer ws;
+    MB_CUDA(ws.alloc(mb::norm_workspace_bytes(kind, A->rows, A->cols), ctx->stream));
+    double* res = nullptr;
+    MB_CUDA(mb::norm_f64(kind, f64_ptr(A), rs(A), cs(A), A->rows, A->cols, cv.p, cv.inc, ws.as<void>(), &res, ctx->num_sms,
+                         ctx->stream));
+    double host[3] = {0.0, 0.0, 0.0};
+    const int count = kind == MB_NORM_FRO ? 3 : 1;
+    if (out) MB_CUDA(cudaMemcpyAsync(host, res, count * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    MB_CUDA(cudaStreamSynchronize(ctx->stream));
+    if (out)
+        for (int i = 0; i < count; ++i) out[i] = host[i];
     return MB_OK;
 }
 

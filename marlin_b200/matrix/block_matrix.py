@@ -30,6 +30,18 @@ def _ceil_len(total: int, parts: int) -> int:
     return int(math.ceil(float(total) / float(parts)))
 
 
+def _extents(total: int, parts: int) -> List[int]:
+    """The block heights (widths) of `total` rows (columns) in `parts` blocks as every method here lays them out: block i
+    starts at i * ceil(total / parts)."""
+    step = _ceil_len(total, parts)
+    return [min(step, total - i * step) for i in range(parts)]
+
+
+def _is_ceil_grid(extents: List[int]) -> bool:
+    """Whether blocks of these heights (widths), in this order, sit where the ceil-sized grid of their sum puts them."""
+    return all(e > 0 for e in extents) and extents == _extents(sum(extents), len(extents))
+
+
 class BlockMatrix(DistributedMatrix):
     def __init__(self, blocks: Iterable[Tuple[BlockID, SubMatrix]], nRows: int = 0, nCols: int = 0, blksByRow: int = 0,
                  blksByCol: int = 0, placement: Optional[Callable[[int, int], int]] = None, sparse: Optional[bool] = None):
@@ -554,20 +566,9 @@ class BlockMatrix(DistributedMatrix):
                     s, d = other.owner(r, c), self.owner(r, c)
                     if s != d:
                         sends.append((s, d, (r, c)))
-            send_bufs = {}
-            for s, d, key in sends:
-                if s == rank:
-                    blk = theirs[key] if theirs[key].is_packed() else theirs[key].copy()
-                    send_bufs[key] = blk.buf[: blk.rows * blk.cols]
             mine = {(b.row, b.column): s for b, s in self.blocks}
-
-            def alloc(key):
-                p = mine[key]
-                return torch.empty(p.rows * p.cols, dtype=p.buf.dtype, device=p.buf.device)
-
-            for key, buf in comm.exchange(sends, send_bufs, alloc, rank).items():
-                p = mine[key]
-                theirs[key] = SubMatrix(buf=buf, rows=p.rows, cols=p.cols, ld=max(1, p.rows))
+            theirs.update(other._send_blocks(sends, lambda key: (mine[key].rows, mine[key].cols),
+                                             lambda key: (mine[key].buf.dtype, mine[key].buf.device)))
         fn = {"add": SubMatrix.add, "subtract": SubMatrix.subtract, "dotProduct": SubMatrix.elementMultiply}[op]
         res = [(b, fn(s, theirs[(b.row, b.column)])) for b, s in self.blocks if (b.row, b.column) in theirs]
         return BlockMatrix(res, self.numRows(), self.numCols(), self.numBlksByRow(), self.numBlksByCol(), self._placement,
@@ -584,6 +585,93 @@ class BlockMatrix(DistributedMatrix):
     def dotProduct(self, other):
         """:486-507 (element-wise product)"""
         return self._binary(other, "dotProduct")
+
+    def _send_blocks(self, sends, shape_of, dtype_device_of) -> Dict[Tuple[int, int], SubMatrix]:
+        """The blocks.join shuffle: this matrix's blocks named in `sends` ((src, dst, (row, col)), the same list on every
+        rank) travel from src to dst; returns the blocks this rank received, keyed by (row, col).  shape_of(key) and
+        dtype_device_of(key) describe a block the receiving rank does not hold."""
+        rank, _ = world()
+        held = {(b.row, b.column): s for b, s in self.blocks}
+        send_bufs = {}
+        for s, d, key in sends:
+            if s == rank:
+                blk = held[key] if held[key].is_packed() else held[key].copy()
+                send_bufs[key] = blk.buf[: blk.rows * blk.cols]
+
+        def alloc(key):
+            r, c = shape_of(key)
+            dt, dev = dtype_device_of(key)
+            return torch.empty(r * c, dtype=dt, device=dev)
+
+        got = comm.exchange(sends, send_bufs, alloc, rank)
+        return {key: SubMatrix(buf=buf, rows=shape_of(key)[0], cols=shape_of(key)[1], ld=max(1, shape_of(key)[0]))
+                for key, buf in got.items()}
+
+    def elementMultiply(self, other: "BlockMatrix", partitioner=None) -> "BlockMatrix":
+        """elementMultiply(other, partitioner) :673-680 — blocks.join(other.blocks) on the BlockID (a block present on one
+        side only is dropped), then the element-wise product of each pair.  `partitioner` is a Spark shuffle hint: it is
+        accepted and ignored, and every product stays where this matrix's block is.  The reference overwrites this
+        matrix's blocks (`:*=`); here the products are new blocks and this matrix is unchanged."""
+        self._dense_only("elementMultiply")
+        other._dense_only("elementMultiply")
+        rank, ws = world()
+        theirs = {(b.row, b.column): s for b, s in other.blocks}
+        if ws > 1:
+            # who holds which block on either side; other's blocks travel to the rank of the matching block of this one
+            mine_at = {key: r for r, key in self._all_gather_meta([(rank, (b.row, b.column)) for b, _ in self.blocks])}
+            their_at = {key: (r, shape) for r, key, shape in
+                        other._all_gather_meta([(rank, (b.row, b.column), (s.rows, s.cols)) for b, s in other.blocks])}
+            sends = [(src, mine_at[key], key) for key, (src, _) in sorted(their_at.items())
+                     if key in mine_at and src != mine_at[key]]
+            dt, dev = other._global_dtype(), Runtime.get().device
+            theirs.update(other._send_blocks(sends, lambda key: their_at[key][1], lambda key: (dt, dev)))
+        res = [(b, s.elementMultiply(theirs[(b.row, b.column)])) for b, s in self.blocks if (b.row, b.column) in theirs]
+        return BlockMatrix(res, self.numRows(), self.numCols(), self.numBlksByRow(), self.numBlksByCol(),
+                           (lambda r, c, s=self: s.owner(r, c)) if ws > 1 else None, sparse=False)
+
+    def cBind(self, other):
+        """cBind(other) :687-705.  With the same number of block rows, `other`'s block columns are relabelled by
+        + numBlksByCol() and the two block sets are united: no block moves or is copied, and the result's placement is
+        each block's present rank.  That is done only when the widths of the joint block columns are exactly those of the
+        ceil-sized grid of n1 + n2 columns, which toBreeze, toDenseVecMatrix, multiply and re-gridding assume (e.g. widths
+        3,2 and 2,2 would give 3,2,2,2 where that grid is 3,3,3,0); otherwise, with different block-row counts, or with a
+        DenseVecMatrix, the result is the DenseVecMatrix cBind of both (the values are the same either way)."""
+        from .dense_vec_matrix import DenseVecMatrix
+        if isinstance(other, DistributedMatrix) and self.numRows() != other.numRows():
+            raise nat.MarlinArgumentError(nat.MB_ERR_DIM_MISMATCH, f"Row dimension mismatches: {self.numRows()} vs {other.numRows()}")
+        if isinstance(other, BlockMatrix):
+            bc = self.numBlksByCol()
+            widths = _extents(self.numCols(), bc) + _extents(other.numCols(), other.numBlksByCol())
+            if self.numBlksByRow() == other.numBlksByRow() and _is_ceil_grid(widths):
+                blocks = self.blocks + [(BlockID(b.row, b.column + bc), s) for b, s in other.blocks]
+                placement = lambda r, c, a=self, o=other, k=bc: a.owner(r, c) if c < k else o.owner(r, c - k)
+                return BlockMatrix(blocks, self.numRows(), self.numCols() + other.numCols(), self.numBlksByRow(), len(widths),
+                                   placement, sparse=None)
+            return self.toDenseVecMatrix().cBind(other.toDenseVecMatrix())
+        if isinstance(other, DenseVecMatrix):
+            return self.toDenseVecMatrix().cBind(other)
+        raise nat.MarlinArgumentError(nat.MB_ERR_UNSUPPORTED, "have not implemented yet")
+
+    def _repeat(self, times: int, columns: bool) -> "BlockMatrix":
+        """MTUtils.repeatByRow (columns=True: copy i of block (r, c) is (r, c + i * numBlksByCol()), numCols() * times) and
+        repeatByColumn (copy i is (r + i * numBlksByRow(), c), numRows() * times): the blocks are relabelled in place when
+        the repeated heights or widths are exactly the ceil-sized grid (see cBind); otherwise the matrix is repeated
+        through its rows and re-gridded with toBlockMatrix(B_r, B_c * times) (or (B_r * times, B_c))."""
+        br, bc = self.numBlksByRow(), self.numBlksByCol()
+        m, n = self.numRows(), self.numCols()
+        ext = _extents(n, bc) if columns else _extents(m, br)
+        if _is_ceil_grid(ext * times):
+            if columns:
+                blocks = [(BlockID(b.row, b.column + i * bc), s) for i in range(times) for b, s in self.blocks]
+                placement = lambda r, c, a=self, k=bc: a.owner(r, c % k)
+                return BlockMatrix(blocks, m, n * times, br, bc * times, placement, sparse=self._sparse_flag)
+            blocks = [(BlockID(b.row + i * br, b.column), s) for i in range(times) for b, s in self.blocks]
+            placement = lambda r, c, a=self, k=br: a.owner(r % k, c)
+            return BlockMatrix(blocks, m * times, n, br * times, bc, placement, sparse=self._sparse_flag)
+        rows = self.toDenseVecMatrix()
+        if columns:
+            return rows._repeat_columns(times).toBlockMatrix(br, bc * times)
+        return rows._repeat_rows(times).toBlockMatrix(br * times, bc)
 
     def divide(self, b: float) -> "BlockMatrix":
         """:432-435"""

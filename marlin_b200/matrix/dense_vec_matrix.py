@@ -414,9 +414,11 @@ class DenseVecMatrix(DistributedMatrix):
         fn = {"add": SubMatrix.add, "subtract": SubMatrix.subtract, "dotProduct": SubMatrix.elementMultiply}[op]
         return DenseVecMatrix(ids=me.ids, data=fn(me.data, other.data), nRows=self.numRows(), nCols=self.numCols())
 
-    def _select_rows(self, positions) -> "DenseVecMatrix":
-        """The local rows at `positions` (ascending local order) as a new packed row-major shard."""
-        nc = self.numCols()
+    def _select_rows(self, positions, c0: int = 0, c1: Optional[int] = None) -> "DenseVecMatrix":
+        """The local rows at `positions` (ascending local order), columns c0 until c1 (all by default), as a new packed
+        row-major shard."""
+        c1 = self.numCols() if c1 is None else c1
+        nc = c1 - c0
         ids = self.ids[list(positions)] if len(positions) else np.zeros(0, dtype=np.int64)
         if not len(positions):
             empty = SubMatrix(buf=torch.zeros(0, dtype=self.data.buf.dtype, device=self.data.buf.device), rows=0, cols=nc,
@@ -430,7 +432,7 @@ class DenseVecMatrix(DistributedMatrix):
             q = p
             while q + 1 < len(positions) and positions[q + 1] == positions[q] + 1:
                 q += 1
-            shard.slice(p, q + 1, 0, nc).assign(self.data.slice(positions[p], positions[q] + 1, 0, nc))
+            shard.slice(p, q + 1, 0, nc).assign(self.data.slice(positions[p], positions[q] + 1, c0, c1))
             p = q + 1
         return DenseVecMatrix(ids=ids, data=shard, nRows=self._nRows, nCols=nc)
 
@@ -470,6 +472,146 @@ class DenseVecMatrix(DistributedMatrix):
         for p in parts:
             total += p
         return total
+
+    # ------------------------------------------------------------------ norm (:975-999)
+    def norm(self, mode: str) -> float:
+        """norm(mode) :975-999 with mode "1" (the largest column sum of |a|), "inf" (the largest row sum of |a|) or "fro"
+        (sqrt of the sum of a^2); any other mode, "2" included, is MarlinArgumentError "Do not support mode <mode>.".
+        Deliberate deviations (DESIGN §3.14): the reference's "1" never sums (its per-row map is lazy and discarded) and
+        its "inf" sums signed values; "fro" is a TODO there.
+
+        One pass over each rank's shard on the device (mb_block_norm).  A NaN anywhere is the result (RDD.max() order).
+        With several ranks the column sums of "1" and the accumulators of "fro" are exchanged and added in rank order on
+        every rank; the row maxima of "inf" are combined by max, so "inf" is the same bits for any number of ranks.
+        No rows on any rank is MarlinError MB_ERR_EMPTY "empty collection"."""
+        import ctypes as C
+        lib = nat.load()
+        kind = C.c_int32()
+        nat.check(lib.mb_norm_mode(str(mode).encode(), C.byref(kind)))
+        kind = kind.value
+        has_rows = self.data is not None and len(self.ids) > 0
+        local = None
+        if has_rows:
+            rt = Runtime.get()
+            rt.sync_stream()
+            try:
+                if kind == nat.MB_NORM_ONE:
+                    col = SubMatrix.empty(self.data.cols, 1, nat.MB_F64, self.data.buf.device)
+                    nat.check(rt.lib.mb_block_norm(rt.ctx, self.data.handle(), kind, col.handle(), None))
+                    local = ("ok", col.toBreeze().reshape(-1))
+                else:
+                    out = np.zeros(3)
+                    nat.check(rt.lib.mb_block_norm(rt.ctx, self.data.handle(), kind, None, out.ctypes.data_as(nat.c_dp)))
+                    local = ("ok", out)
+            except (nat.MarlinError, nat.MarlinArgumentError) as e:
+                local = ("error", (e.code, getattr(e, "message", str(e))))
+        # every rank learns of a failing shard before any rank raises; the error travels as (code, message)
+        parts = self._gather([local] if local is not None else [])
+        for status, value in parts:
+            if status == "error":
+                code, message = value
+                if code in (nat.MB_ERR_INVALID_ARG, nat.MB_ERR_DIM_MISMATCH, nat.MB_ERR_UNSUPPORTED):
+                    raise nat.MarlinArgumentError(code, message)
+                raise nat.MarlinError(code, message)
+        if not parts:
+            raise nat.MarlinError(nat.MB_ERR_EMPTY, "empty collection")
+        if kind == nat.MB_NORM_INF:
+            vals = [float(v[0]) for _, v in parts]
+            return math.nan if any(math.isnan(v) for v in vals) else max(vals)
+        total = parts[0][1].copy()
+        if kind == nat.MB_NORM_ONE:
+            for _, v in parts[1:]:
+                total = total + v
+            return float(np.max(total))                        # np.max propagates NaN
+        acc = np.ascontiguousarray(np.stack([v for _, v in parts]))
+        res = C.c_double()
+        nat.check(lib.mb_norm_fro(acc.ctypes.data_as(nat.c_dp), len(parts), C.byref(res)))
+        return float(res.value)
+
+    # ------------------------------------------------------------------ slicing (:928-964)
+    def _window(self, r0: int, r1: int, c0: int, c1: int) -> "DenseVecMatrix":
+        """Rows r0..r1 and columns c0..c1 (inclusive), row ids shifted by -r0; rows stay on their rank."""
+        keep = [p for p, i in enumerate(self.ids) if r0 <= int(i) <= r1]
+        nr, nc = r1 - r0 + 1, c1 - c0 + 1
+        if not keep:
+            return DenseVecMatrix(ids=np.zeros(0, dtype=np.int64), data=None, nRows=nr, nCols=nc)
+        part = self._select_rows(keep, c0, c1 + 1)
+        return DenseVecMatrix(ids=part.ids - r0, data=part.data, nRows=nr, nCols=nc)
+
+    def sliceByRow(self, startRow: int, endRow: int) -> "DenseVecMatrix":
+        """sliceByRow(startRow, endRow) :928-933 — rows startRow..endRow (inclusive) with ids shifted by -startRow.  The
+        reference lets endRow == numRows() through (a phantom zero row); that is rejected here with its message."""
+        if not (startRow >= 0 and endRow < self.numRows() and startRow <= endRow):
+            raise nat.MarlinArgumentError(nat.MB_ERR_INVALID_ARG, "start row or end row mismatch the matrix num of rows")
+        return self._window(int(startRow), int(endRow), 0, self.numCols() - 1)
+
+    def sliceByColumn(self, startCol: int, endCol: int) -> "DenseVecMatrix":
+        """sliceByColumn(startCol, endCol) :941-946 — columns startCol..endCol (inclusive); endCol == numCols() (short rows
+        in the reference) is rejected with its message."""
+        if not (startCol >= 0 and endCol < self.numCols() and startCol <= endCol):
+            raise nat.MarlinArgumentError(nat.MB_ERR_INVALID_ARG, "start column or end column mismatch the matrix num of columns")
+        return self._window(0, self.numRows() - 1, int(startCol), int(endCol))
+
+    def getSubMatrix(self, startRow: int, endRow: int, startCol: int, endCol: int) -> "DenseVecMatrix":
+        """getSubMatrix(startRow, endRow, startCol, endCol) :956-964 — inclusive bounds, row ids shifted by -startRow.  The
+        reference's messages ("dismatch"), and also rejecting end == numRows() / numCols() and start > end."""
+        if not (startRow >= 0 and endRow < self.numRows() and startRow <= endRow):
+            raise nat.MarlinArgumentError(nat.MB_ERR_INVALID_ARG, "start row or end row dismatch the matrix num of rows")
+        if not (startCol >= 0 and endCol < self.numCols() and startCol <= endCol):
+            raise nat.MarlinArgumentError(nat.MB_ERR_INVALID_ARG, "start column or end column dismatch the matrix num of columns")
+        return self._window(int(startRow), int(endRow), int(startCol), int(endCol))
+
+    # ------------------------------------------------------------------ cBind (:238-252)
+    def cBind(self, other):
+        """cBind(other) :238-252 — rows.join(that.rows): a row id present on one side only is dropped; each remaining row
+        is this row ++ that row, numRows() x (n1 + n2).  A BlockMatrix goes through toDenseVecMatrix() first."""
+        from .block_matrix import BlockMatrix
+        if isinstance(other, DistributedMatrix) and self.numRows() != other.numRows():
+            raise nat.MarlinArgumentError(nat.MB_ERR_DIM_MISMATCH, f"Dimension mismatch:  {self.numRows()} vs {other.numRows()}")
+        if isinstance(other, BlockMatrix):
+            return self.cBind(other.toDenseVecMatrix())
+        if not isinstance(other, DenseVecMatrix):
+            raise nat.MarlinArgumentError(nat.MB_ERR_UNSUPPORTED, f"Do not support this type {type(other)} for cBind operation")
+        n1, n2 = self.numCols(), other.numCols()
+        theirs = set(int(i) for part in self._gather([other.ids.tolist()]) for i in part)
+        keep = [p for p, i in enumerate(self.ids) if int(i) in theirs]
+        me = self if len(keep) == len(self.ids) else self._select_rows(keep)
+        that = other._aligned_to(me)                               # collective on every rank
+        if me.data is None or not len(me.ids):
+            return DenseVecMatrix(ids=me.ids, data=None, nRows=self.numRows(), nCols=n1 + n2)
+        k = len(me.ids)
+        buf = torch.empty(k * (n1 + n2), dtype=me.data.buf.dtype, device=me.data.buf.device)
+        shard = SubMatrix(buf=buf, rows=k, cols=n1 + n2, ld=n1 + n2, is_transpose=True)
+        shard.slice(0, k, 0, n1).assign(me.data)
+        shard.slice(0, k, n1, n1 + n2).assign(that.data)
+        return DenseVecMatrix(ids=me.ids, data=shard, nRows=self.numRows(), nCols=n1 + n2)
+
+    # ------------------------------------------------------------------ MTUtils.repeatByRow / repeatByColumn (:446-491)
+    def _repeat_columns(self, times: int) -> "DenseVecMatrix":
+        """Every row becomes `times` copies of itself side by side (MTUtils.repeatByRow)."""
+        n = self.numCols()
+        if self.data is None or not len(self.ids):
+            return DenseVecMatrix(ids=self.ids, data=None, nRows=self.numRows(), nCols=n * times)
+        k = len(self.ids)
+        buf = torch.empty(k * n * times, dtype=self.data.buf.dtype, device=self.data.buf.device)
+        shard = SubMatrix(buf=buf, rows=k, cols=n * times, ld=max(1, n * times), is_transpose=True)
+        for i in range(times):
+            shard.slice(0, k, i * n, (i + 1) * n).assign(self.data)
+        return DenseVecMatrix(ids=self.ids, data=shard, nRows=self.numRows(), nCols=n * times)
+
+    def _repeat_rows(self, times: int) -> "DenseVecMatrix":
+        """The matrix stacked `times` times: copy i of row id holds id + i * numRows() (MTUtils.repeatByColumn); every copy
+        stays on the rank of its row."""
+        m, n = self.numRows(), self.numCols()
+        if self.data is None or not len(self.ids):
+            return DenseVecMatrix(ids=np.zeros(0, dtype=np.int64), data=None, nRows=m * times, nCols=n)
+        k = len(self.ids)
+        buf = torch.empty(k * times * n, dtype=self.data.buf.dtype, device=self.data.buf.device)
+        shard = SubMatrix(buf=buf, rows=k * times, cols=n, ld=max(1, n), is_transpose=True)
+        for i in range(times):
+            shard.slice(i * k, (i + 1) * k, 0, n).assign(self.data)
+        ids = np.concatenate([self.ids + i * m for i in range(times)])
+        return DenseVecMatrix(ids=ids, data=shard, nRows=m * times, nCols=n)
 
     # ------------------------------------------------------------------ transpose (:1420-1436)
     def transpose(self, numBlocks: Optional[int] = None):

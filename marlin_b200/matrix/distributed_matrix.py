@@ -30,6 +30,10 @@ class DistributedMatrix:
     def transpose(self):
         raise NotImplementedError
 
+    def cBind(self, other):
+        """:63 — this matrix with the columns of `other` appended."""
+        raise NotImplementedError
+
     def toBreeze(self):
         raise NotImplementedError
 

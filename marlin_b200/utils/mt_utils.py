@@ -152,11 +152,25 @@ class MTUtils:
         same seed.  The reference's seed is System.nanoTime() and is not exposed (MTUtils.scala:63-73); the extra
         `seed` keyword makes runs reproducible."""
         dist_ = distribution or UniformGenerator(0.0, 1.0)
-        rank, ws = world()
-        P = numPartitions if numPartitions > 0 else max(ws, 2 if ws == 1 else ws)
         if seed is None:
             seed = time.time_ns()
+        P, shards, ids_arr, data = MTUtils._row_shard(nRows, nColumns, numPartitions)
         seeds = MTUtils._partition_seeds(seed, P)
+        off = 0
+        for p, s, e in shards:
+            view = data.slice(off, off + (e - s), 0, nColumns)
+            MTUtils._fill(view, seeds[p], 0, dist_, row_major=True)
+            off += e - s
+        return DenseVecMatrix(ids=ids_arr, data=data, nRows=nRows, nCols=nColumns)
+
+    @staticmethod
+    def _row_shard(nRows: int, nColumns: int, numPartitions: int = 0):
+        """The row layout of the dense generators (rdd/RandomRDD.scala:38-41, 161-182): P partitions (numPartitions, or
+        the number of ranks, at least 2 on one rank), partition p holds rows [p*N/P, (p+1)*N/P) and lives on rank p mod G.
+        Returns (P, [(p, start, end) of this rank], the row ids of this rank, an uninitialised row-major fp64 shard of
+        them or None)."""
+        rank, ws = world()
+        P = numPartitions if numPartitions > 0 else max(ws, 2 if ws == 1 else ws)
         rt = Runtime.get()
         shards, ids = [], []
         start = 0
@@ -164,18 +178,57 @@ class MTUtils:
             end = ((p + 1) * nRows) // P
             if p % ws == rank and end > start:
                 shards.append((p, start, end))
+                ids.append(np.arange(start, end, dtype=np.int64))
             start = end
         nloc = sum(e - s for _, s, e in shards)
         buf = torch.empty(nloc * nColumns, dtype=torch.float64, device=rt.device)
         data = SubMatrix(buf=buf, rows=nloc, cols=nColumns, ld=max(1, nColumns), is_transpose=True) if nloc else None
-        off = 0
-        for p, s, e in shards:
-            view = data.slice(off, off + (e - s), 0, nColumns)
-            MTUtils._fill(view, seeds[p], 0, dist_, row_major=True)
-            ids.append(np.arange(s, e, dtype=np.int64))
-            off += e - s
         ids_arr = np.concatenate(ids) if ids else np.zeros(0, dtype=np.int64)
-        return DenseVecMatrix(ids=ids_arr, data=data, nRows=nRows, nCols=nColumns)
+        return P, shards, ids_arr, data
+
+    @staticmethod
+    def _constant_rows(nRows: int, nColumns: int, value: float) -> DenseVecMatrix:
+        _, _, ids, data = MTUtils._row_shard(nRows, nColumns)
+        if data is not None:
+            rt = Runtime.get()
+            rt.sync_stream()
+            nat.check(rt.lib.mb_block_fill(rt.ctx, data.handle(), float(value)))
+        return DenseVecMatrix(ids=ids, data=data, nRows=nRows, nCols=nColumns)
+
+    @staticmethod
+    def zerosDenVecMatrix(sc, nRows: int, nColumns: int) -> DenseVecMatrix:
+        """utils/MTUtils.scala:103-109 — every element 0.0, rows laid out as randomDenVecMatrix lays them out."""
+        return MTUtils._constant_rows(nRows, nColumns, 0.0)
+
+    @staticmethod
+    def onesDenVecMatrix(sc, nRows: int, nColumns: int) -> DenseVecMatrix:
+        """utils/MTUtils.scala:119-125 — every element 1.0, rows laid out as randomDenVecMatrix lays them out."""
+        return MTUtils._constant_rows(nRows, nColumns, 1.0)
+
+    @staticmethod
+    def repeatByRow(matrix, times: int):
+        """utils/MTUtils.scala:446-464.  Despite the name, the COLUMNS repeat: every row becomes `times` copies of itself
+        side by side (numCols() * times; the reference keeps numCols() for a BlockMatrix, a deviation corrected here).
+        times == 1 returns the matrix itself; times <= 0 is rejected."""
+        return MTUtils._repeat(matrix, times, columns=True)
+
+    @staticmethod
+    def repeatByColumn(matrix, times: int):
+        """utils/MTUtils.scala:471-491 — the matrix stacked `times` times: copy i of row id is row id + i * numRows()."""
+        return MTUtils._repeat(matrix, times, columns=False)
+
+    @staticmethod
+    def _repeat(matrix, times: int, columns: bool):
+        times = int(times)
+        if times <= 0:
+            raise nat.MarlinArgumentError(nat.MB_ERR_INVALID_ARG, f"repeat times: {times} illegal")
+        if times == 1:
+            return matrix
+        if isinstance(matrix, DenseVecMatrix):
+            return matrix._repeat_columns(times) if columns else matrix._repeat_rows(times)
+        if isinstance(matrix, BlockMatrix):
+            return matrix._repeat(times, columns)
+        raise nat.MarlinArgumentError(nat.MB_ERR_UNSUPPORTED, f"Do not support this type {type(matrix)} for repeat operation")
 
     @staticmethod
     def randomSpaVecMatrix(sc, nRows: int, nColumns: int, density: float, numPartitions: int = 0,
