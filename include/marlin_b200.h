@@ -98,6 +98,16 @@ int32_t mb_block_slice(mb_ctx* ctx, const mb_block* blk, int32_t r0, int32_t r1,
  * (operands the TMA cannot address are copied to a packed buffer first), K = 0 gives C = 0, and an F32 C is built
  * from accumulation chains of at most MARLIN_B200_BF16_KCHAIN (default 8192) k per launch. */
 int32_t mb_block_gemm(mb_ctx* ctx, const mb_block* A, const mb_block* B, mb_block* C, int32_t accumulate);
+/* The trailing (Schur) update of the dist-mode block factorizations, as one call for a rank's whole step:
+ * C[e] = C[e] - A[e]*B[e] for e < count, in place, fp64.  It replaces the per-block `multiply` + `subtract` of
+ * matrix/DenseVecMatrix.scala:421-427 (LU), :531-549 (Cholesky, B[e] a transposed view) and :666-671 (inverse).
+ * Each C[e] is bit for bit mb_block_gemm(A[e], B[e]) -> tmp followed by mb_block_sub(C[e], tmp), with or without
+ * mb_set_dmma_reference.  Entries the DMMA GEMM would run are packed, in order, into grouped launches of at most
+ * 64 entries and 32 distinct A and 32 distinct B operands each (a transposed B is copied once to column-major
+ * first); the others run as exactly those two calls.  MB_ERR_DIM_MISMATCH when an entry's shapes disagree,
+ * MB_ERR_INVALID_ARG when an output overlaps another output or any operand; count == 0 launches nothing. */
+int32_t mb_block_schur_update(mb_ctx* ctx, int32_t count, mb_block* const* C, const mb_block* const* A,
+                              const mb_block* const* B);
 /* Same GEMM on raw device pointers (column-major, BLAS trans flags 'N'/'T'). */
 int32_t mb_dgemm_device(mb_ctx* ctx, char transa, char transb, int32_t m, int32_t n, int32_t k,
                         double alpha, const double* A, int32_t lda, const double* B, int32_t ldb,

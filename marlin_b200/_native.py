@@ -60,6 +60,7 @@ SIGNATURES = {
     "mb_block_view_t": (c_i32, [c_ctx, c_blk, C.POINTER(c_blk)]),
     "mb_block_slice": (c_i32, [c_ctx, c_blk, c_i32, c_i32, c_i32, c_i32, C.POINTER(c_blk)]),
     "mb_block_gemm": (c_i32, [c_ctx, c_blk, c_blk, c_blk, c_i32]),
+    "mb_block_schur_update": (c_i32, [c_ctx, c_i32, C.POINTER(c_blk), C.POINTER(c_blk), C.POINTER(c_blk)]),
     "mb_set_fp64_mode": (c_i32, [c_ctx, c_i32, c_i32]),
     "mb_set_dmma_reference": (c_i32, [c_ctx, c_i32]),
     "mb_dgemm_device": (c_i32, [c_ctx, C.c_char, C.c_char, c_i32, c_i32, c_i32, c_f64, C.c_void_p, c_i32,

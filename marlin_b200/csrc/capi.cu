@@ -603,6 +603,137 @@ int32_t mb_block_gemm(mb_ctx* ctx, const mb_block* A, const mb_block* B, mb_bloc
     return fail(MB_ERR_UNSUPPORTED, "mb_block_gemm: unsupported dtype combination (%d,%d)->%d", A->dtype, B->dtype, C->dtype);
 }
 
+// The bytes [lo, hi) a block's elements can occupy.
+static void block_span(const mb_block* b, uintptr_t* lo, uintptr_t* hi) {
+    const long long major = b->is_transpose ? b->rows : b->cols, minor = b->is_transpose ? b->cols : b->rows;
+    *lo = reinterpret_cast<uintptr_t>(elem_ptr(b));
+    *hi = *lo + (uintptr_t)(((major - 1) * (long long)b->ld + minor) * (long long)elem_size(b->dtype));
+}
+
+// C[e] -= A[e] B[e].  See the header.  Entries whose product mb_block_gemm would run on the DMMA kernel (fp64 native
+// mode, M, N, K > 1, column-major C and A, TMA-addressable A and B) become entries of grouped launches with the
+// subtracting epilogue; a transposed B is first copied once into a column-major buffer (a copy changes no value).  The
+// others run as mb_block_gemm into a temporary and mb_block_sub, which is what the grouped entries reproduce bit for bit.
+int32_t mb_block_schur_update(mb_ctx* ctx, int32_t count, mb_block* const* C, const mb_block* const* A,
+                              const mb_block* const* B) {
+    MB_CTX(ctx);
+    MB_LOCK(ctx);
+    if (count < 0 || (count > 0 && (!C || !A || !B))) return fail(MB_ERR_INVALID_ARG, "mb_block_schur_update: bad argument");
+    if (count == 0) return MB_OK;
+    std::vector<std::pair<uintptr_t, uintptr_t>> cspan(count);
+    for (int e = 0; e < count; ++e) {
+        if (!C[e] || !A[e] || !B[e]) return fail(MB_ERR_INVALID_ARG, "mb_block_schur_update: null block in entry %d", e);
+        if (C[e]->dtype != MB_F64 || A[e]->dtype != MB_F64 || B[e]->dtype != MB_F64)
+            return fail(MB_ERR_UNSUPPORTED, "mb_block_schur_update: fp64 blocks only (entry %d)", e);
+        if (A[e]->cols != B[e]->rows || C[e]->rows != A[e]->rows || C[e]->cols != B[e]->cols)
+            return fail(MB_ERR_DIM_MISMATCH, "mb_block_schur_update: entry %d is %dx%d -= %dx%d * %dx%d", e, C[e]->rows,
+                        C[e]->cols, A[e]->rows, A[e]->cols, B[e]->rows, B[e]->cols);
+        if (C[e]->rows == 0 || C[e]->cols == 0) { cspan[e] = {0, 0}; continue; }
+        block_span(C[e], &cspan[e].first, &cspan[e].second);
+    }
+    // no output may overlap another output or any operand: every entry reads what the call was given
+    std::vector<std::pair<uintptr_t, uintptr_t>> sorted;
+    for (const auto& sp : cspan) if (sp.second > sp.first) sorted.push_back(sp);
+    std::sort(sorted.begin(), sorted.end());
+    for (size_t x = 1; x < sorted.size(); ++x)
+        if (sorted[x].first < sorted[x - 1].second) return fail(MB_ERR_INVALID_ARG, "mb_block_schur_update: two entries share an output");
+    auto hits_output = [&](const mb_block* b) {
+        if (b->rows == 0 || b->cols == 0) return false;
+        uintptr_t lo, hi;
+        block_span(b, &lo, &hi);
+        auto it = std::lower_bound(sorted.begin(), sorted.end(), std::make_pair(hi, (uintptr_t)0));
+        return it != sorted.begin() && std::prev(it)->second > lo;
+    };
+    for (int e = 0; e < count; ++e)
+        if (hits_output(A[e]) || hits_output(B[e]))
+            return fail(MB_ERR_INVALID_ARG, "mb_block_schur_update: an operand of entry %d overlaps an output", e);
+
+    const int sms = ctx->num_sms;
+    auto grouped = [&](int e) {
+        const mb_block *a = A[e], *b = B[e], *c = C[e];
+        return ctx->fp64_mode == MB_FP64_NATIVE && a->rows > 1 && a->cols > 1 && b->cols > 1 && !c->is_transpose &&
+               !a->is_transpose && mb::gemm_f64_tma_eligible(f64_ptr(a), a->ld, f64_ptr(b), b->ld);
+    };
+    // column-major copies of the transposed B operands, one per distinct view
+    struct Op { const double* p; long long ld; int rows, cols, t; };
+    auto same = [](const Op& x, const Op& y) { return x.p == y.p && x.ld == y.ld && x.rows == y.rows && x.cols == y.cols && x.t == y.t; };
+    std::vector<Op> copied_of;
+    std::vector<mb::StreamBuffer> copies;
+    std::vector<Op> bop(count);
+    for (int e = 0; e < count; ++e) {
+        if (!grouped(e)) continue;
+        const mb_block* b = B[e];
+        const Op key{f64_ptr(b), b->ld, b->rows, b->cols, b->is_transpose};
+        bop[e] = key;
+        if (!b->is_transpose) continue;
+        size_t x = 0;
+        while (x < copied_of.size() && !same(copied_of[x], key)) ++x;
+        if (x == copied_of.size()) {
+            const int ld = (b->rows + 1) & ~1;
+            copies.emplace_back();
+            MB_CUDA(copies.back().alloc((size_t)ld * b->cols * sizeof(double), ctx->stream));
+            mb_block dst = block_view(copies.back().as<double>(), b->rows, b->cols, ld, false, MB_F64, ctx->device);
+            const int32_t r = copy_convert(ctx, b, &dst);
+            if (r != MB_OK) return r;
+            copied_of.push_back(key);
+        }
+        bop[e] = Op{copies[x].as<double>(), (b->rows + 1) & ~1, b->rows, b->cols, 0};
+    }
+    // grouped launches: entries in order, a launch closed when the next entry would exceed its entry or operand limits
+    static thread_local mb::G2Launch L;
+    L = mb::G2Launch();
+    std::vector<Op> la, lb;
+    auto flush = [&]() -> cudaError_t {
+        const cudaError_t e = mb::gemm_f64_grouped2(L, sms, ctx->stream);
+        L = mb::G2Launch();
+        la.clear();
+        lb.clear();
+        return e;
+    };
+    auto find = [&](const std::vector<Op>& v, const Op& o) {
+        for (size_t x = 0; x < v.size(); ++x) if (same(v[x], o)) return (int)x;
+        return -1;
+    };
+    for (int e = 0; e < count; ++e) {
+        if (!grouped(e)) continue;
+        const Op ao{f64_ptr(A[e]), A[e]->ld, A[e]->rows, A[e]->cols, 0};
+        int ia = find(la, ao), ib = find(lb, bop[e]);
+        if (L.ne == mb::G2_MAX_ENTRIES || (ia < 0 && L.na == mb::G2_MAX_OPS) || (ib < 0 && L.nb == mb::G2_MAX_OPS)) {
+            MB_CUDA(flush());
+            ia = ib = -1;
+        }
+        if (ia < 0) {
+            mb::G2Operand& o = L.A[ia = L.na++];
+            o.ptr = ao.p; o.ld = ao.ld; o.rows = ao.rows; o.cols = ao.cols;
+            la.push_back(ao);
+        }
+        if (ib < 0) {
+            mb::G2Operand& o = L.B[ib = L.nb++];
+            o.ptr = bop[e].p; o.ld = bop[e].ld; o.rows = bop[e].rows; o.cols = bop[e].cols;
+            lb.push_back(bop[e]);
+        }
+        mb::G2Entry& en = L.E[L.ne++];
+        en.nseg = 1; en.a_op[0] = ia; en.b_op[0] = ib;
+        en.M = C[e]->rows; en.N = C[e]->cols;
+        en.D = f64_ptr(C[e]); en.ldd = C[e]->ld;
+        en.Cin = f64_ptr(C[e]); en.ldcin = C[e]->ld;
+        en.sub_from_cin = true;
+    }
+    if (L.ne > 0) MB_CUDA(flush());
+    // the rest: the product into a temporary, then the subtraction in place
+    for (int e = 0; e < count; ++e) {
+        if (grouped(e) || C[e]->rows == 0 || C[e]->cols == 0) continue;
+        const int M = C[e]->rows, N = C[e]->cols;
+        mb::StreamBuffer tmp;
+        MB_CUDA(tmp.alloc((size_t)M * N * sizeof(double), ctx->stream));
+        mb_block t = block_view(tmp.as<double>(), M, N, M, false, MB_F64, ctx->device);
+        int32_t r = mb_block_gemm(ctx, A[e], B[e], &t, 0);
+        if (r == MB_OK) r = mb_block_sub(ctx, C[e], &t, C[e]);
+        if (r != MB_OK) return r;
+    }
+    return MB_OK;
+}
+
 int32_t mb_matmul_blocked_subset(mb_ctx* ctx, mb_block* const* A_tiles, mb_block* const* B_tiles, int32_t m, int32_t k,
                                  int32_t n, mb_block* const* C_tiles, const int32_t* c_ids, int32_t num_c) {
     MB_CTX(ctx);

@@ -508,7 +508,24 @@ struct AddCin {
     }
 };
 
-template <Dmma S>
+// D = Cin - acc (the Schur update C -= A B, with D == Cin allowed: every element is read and then written by the one
+// thread that owns it).  One rounding, as in a GEMM into a temporary followed by an element-wise subtraction.
+struct SubFromCin {
+    const double* Cin;
+    long long ldcin;
+    __device__ __forceinline__ double scale(double a) const { return a; }
+    __device__ __forceinline__ const double* column(int n) const { return Cin + (long long)n * ldcin; }
+    __device__ __forceinline__ void add(double& v, const double* col, int m) const { v = __ldcg(col + m) - v; }
+    __device__ __forceinline__ void add2(double& v0, double& v1, const double* col, int m) const {
+        const double2 old = __ldcg(reinterpret_cast<const double2*>(col + m));
+        v0 = old.x - v0;
+        v1 = old.y - v1;
+    }
+};
+
+// Epilogue op of a grouped launch: Op = AddCin (the blocked multiply and the multi-GPU protocol) or SubFromCin (every
+// entry subtracts its product from Cin; gemm_f64_grouped2 picks this instance when the entries ask for it).
+template <Dmma S, class Op>
 __device__ __forceinline__ void dmma_grouped(const G2Params& g) {
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -576,7 +593,7 @@ __device__ __forceinline__ void dmma_grouped(const G2Params& g) {
 
         // ---------------- epilogue: D = acc (+ Cin) ----------------
         double* D = en.D;
-        const AddCin add{en.Cin, en.ldcin};
+        const Op add{en.Cin, en.ldcin};
         const long long ldd = en.ldd;
         const int Mc = en.M, Nc = en.N;
         if (add.Cin != nullptr && en.cin_flag != nullptr && en.cin_flag != cin_seen) {
@@ -617,13 +634,23 @@ __device__ __forceinline__ void dmma_grouped(const G2Params& g) {
 
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_f64_dmma16x8_grouped_kernel(const __grid_constant__ G2Params g) {
-    dmma_grouped<Dmma::m16n8k4>(g);
+    dmma_grouped<Dmma::m16n8k4, AddCin>(g);
 }
 
 // The m8n8k4 reference instance (see the top of the file).
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_f64_dmma_grouped_kernel(const __grid_constant__ G2Params g) {
-    dmma_grouped<Dmma::m8n8k4>(g);
+    dmma_grouped<Dmma::m8n8k4, AddCin>(g);
+}
+
+// D = Cin - acc for every entry (mb_block_schur_update), and its m8n8k4 reference instance.
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+gemm_f64_dmma16x8_grouped_sub_kernel(const __grid_constant__ G2Params g) {
+    dmma_grouped<Dmma::m16n8k4, SubFromCin>(g);
+}
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+gemm_f64_dmma_grouped_sub_kernel(const __grid_constant__ G2Params g) {
+    dmma_grouped<Dmma::m8n8k4, SubFromCin>(g);
 }
 
 // -------------------------------------------------------------------------------------------
@@ -927,10 +954,12 @@ cudaError_t gemm_f64_grouped2(const G2Launch& L, int num_sms, cudaStream_t strea
         g.b_ready[i] = (short)o.ready_base;
     }
     int tiles = 0;
+    const bool sub = L.E[0].sub_from_cin;
     for (int c = 0; c < L.ne; ++c) {
         const G2Entry& s = L.E[c];
         G2Ent& d = g.e[c];
         if (s.nseg <= 0 || s.nseg > G2_MAX_SEG || s.M <= 0 || s.N <= 0) return cudaErrorNotSupported;
+        if (s.sub_from_cin != sub || (sub && (s.Cin == nullptr || s.cin_flag != nullptr))) return cudaErrorInvalidValue;
         if ((s.m_off % BM) != 0 || (s.n_off % BN) != 0) return cudaErrorInvalidValue;
         d.D = s.D; d.ldd = s.ldd; d.Cin = s.Cin; d.ldcin = s.ldcin;
         d.cin_flag = s.cin_flag; d.cin_val = s.cin_val;
@@ -954,9 +983,14 @@ cudaError_t gemm_f64_grouped2(const G2Launch& L, int num_sms, cudaStream_t strea
     g.ready = L.ready; g.ready_val = L.ready_val; g.status = L.status; g.timeout_ns = L.timeout_ns;
     g.ne = L.ne;
     g.num_tiles = tiles;
+    const int grid = min(tiles, num_sms);
+    if (sub)
+        return g_call.dmma_reference
+                   ? launch_with_smem<gemm_f64_dmma_grouped_sub_kernel>(grid, NUM_THREADS, SMEM_BYTES, stream, g)
+                   : launch_with_smem<gemm_f64_dmma16x8_grouped_sub_kernel>(grid, NUM_THREADS, SMEM_BYTES, stream, g);
     return g_call.dmma_reference
-               ? launch_with_smem<gemm_f64_dmma_grouped_kernel>(min(tiles, num_sms), NUM_THREADS, SMEM_BYTES, stream, g)
-               : launch_with_smem<gemm_f64_dmma16x8_grouped_kernel>(min(tiles, num_sms), NUM_THREADS, SMEM_BYTES, stream, g);
+               ? launch_with_smem<gemm_f64_dmma_grouped_kernel>(grid, NUM_THREADS, SMEM_BYTES, stream, g)
+               : launch_with_smem<gemm_f64_dmma16x8_grouped_kernel>(grid, NUM_THREADS, SMEM_BYTES, stream, g);
 }
 
 cudaError_t gemm_f64_grouped(int m, int k, int n, const int* my_c, int num_c, const double* const* A, const long long* lda,

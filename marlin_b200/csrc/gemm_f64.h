@@ -39,6 +39,8 @@ struct G2Entry {
     long long ldd = 0;
     const double* Cin = nullptr;                        // optional addend: D = acc + Cin
     long long ldcin = 0;
+    bool sub_from_cin = false;                          // D = Cin - acc instead (Cin required, no cin_flag; D == Cin
+                                                        // allowed); every entry of one launch must agree
     const unsigned long long* cin_flag = nullptr;       // wait until *cin_flag >= cin_val (system scope) before reading Cin
     unsigned long long cin_val = 0;
     unsigned long long* done_ctr = nullptr;             // zeroed device counter; when it reaches the entry's tile count ...

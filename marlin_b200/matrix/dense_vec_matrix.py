@@ -216,7 +216,7 @@ class DenseVecMatrix(DistributedMatrix):
 
     # ------------------------------------------------------------------ LU / Cholesky / inverse (:271-764)
     def _square_blocks(self, base: int):
-        """All blocks of the ceil(n / base)^2 grid as device blocks on THIS rank (every rank factorises a replica)."""
+        """All blocks of the ceil(n / base)^2 grid as device blocks on THIS rank ("breeze" mode: the whole matrix)."""
         from . import factorizations as fz
         n = self.numRows()
         nb, sub = fz.grid(n, base)
@@ -226,18 +226,82 @@ class DenseVecMatrix(DistributedMatrix):
                   for r in range(nb) for c in range(nb)}
         return blocks, nb, sub, n
 
+    def _grid_blocks(self, nb: int, sub: int, want=lambda r, c: True):
+        """The fp64 blocks (r, c) of the nb x nb grid (block length sub) that comm.elem_owner places on THIS rank and
+        `want` keeps, built from the rows each rank holds: the pieces of one block row that change rank travel in one
+        exchange, so no rank ever holds more than its own blocks and one block row of pieces."""
+        n = self.numRows()
+        rank, ws = world()
+        dev = self.data.buf.device if self.data is not None else Runtime.get().device
+        owner = lambda r, c: comm.elem_owner(r, c, nb, ws)
+        size = lambda k: n - sub * (nb - 1) if k == nb - 1 else sub
+        my_runs = []
+        for pos0, id0, length in (_runs(self.ids) if self.data is not None else []):
+            while length > 0:
+                br = id0 // sub
+                take = min(length, (br + 1) * sub - id0)
+                my_runs.append((rank, pos0, id0, take))
+                pos0 += take; id0 += take; length -= take
+        all_runs = self._gather(my_runs)
+        blocks = {(r, c): SubMatrix.zeros(size(r), size(c), nat.MB_F64, dev)       # BDM.zeros (:1318)
+                  for r in range(nb) for c in range(nb) if owner(r, c) == rank and want(r, c)}
+        for br in range(nb):
+            sends, send_bufs, pastes = [], {}, []
+            for (src, pos0, id0, take) in all_runs:
+                if id0 // sub != br:
+                    continue
+                for bc in range(nb):
+                    if not want(br, bc):
+                        continue
+                    dst, key = owner(br, bc), (src, id0, bc)
+                    piece = self.data.slice(pos0, pos0 + take, bc * sub, bc * sub + size(bc)) if src == rank else None
+                    if dst == rank:
+                        pastes.append((key, bc, id0 - br * sub, take, piece))
+                    elif src == rank:
+                        send_bufs[key] = piece.copy(nat.MB_F64).buf
+                    if src != dst:
+                        sends.append((src, dst, key))
+            got = comm.exchange(sends, send_bufs, lambda key: torch.empty(
+                [p[3] for p in pastes if p[0] == key][0] * size(key[2]), dtype=torch.float64, device=dev), rank) if ws > 1 else {}
+            del send_bufs
+            for key, bc, r0, take, piece in pastes:
+                if piece is None:
+                    piece = SubMatrix(buf=got.pop(key), rows=take, cols=size(bc), ld=max(1, take))
+                blocks[(br, bc)].slice(r0, r0 + take, 0, size(bc)).assign(piece)
+        return blocks
+
+    def _factor_dist(self, kind: str, base: int, keep_unfactored_diagonal: bool = False):
+        """The sharded block algorithm: this rank's result blocks (and the pivot list for LU)."""
+        from . import factorizations as fz
+        n = self.numRows()
+        nb, sub = fz.grid(n, base)
+        rank, ws = world()
+        dev = self.data.buf.device if self.data is not None else Runtime.get().device
+        want = (lambda r, c: r >= c) if kind == "cholesky" else (lambda r, c: True)
+        store = {("A", r, c): b for (r, c), b in self._grid_blocks(nb, sub, want).items()}
+        del want
+        pivots = {}
+        fz.run(kind, store, nb, sub, n, rank, ws, dev, keep_unfactored_diagonal, pivots)
+        if kind == "inverse":
+            fz.run("inverse_back", store, nb, sub, n, rank, ws, dev)
+            return {(r, c): b for (_, r, c), b in store.items()}, nb, n
+        if kind == "lu":
+            out, p_array = fz.finish_lu(store, pivots, nb, sub, n, rank, ws, dev)
+            return out, nb, n, p_array
+        return {(r, c): b for (_, r, c), b in store.items()}, nb, n
+
     def _finish(self, blocks, nb: int, n: int):
+        """Blocks already on their owner (comm.elem_owner, MatrixElemOpPartitioner order) -> the result BlockMatrix."""
         from . import factorizations as fz
         from .block_matrix import BlockMatrix
-        rank, ws = world()
-        owner = lambda r, c: comm.elem_owner(r, c, nb, ws)
-        return BlockMatrix(fz.block_pairs(blocks, owner, rank), n, n, nb, nb, sparse=False)
+        return BlockMatrix(fz.block_pairs(blocks), n, n, nb, nb, sparse=False)
 
     def luDecompose(self, mode: str = "auto", baseSize: Optional[int] = None, keepUnfactoredDiagonal: bool = False):
         """luDecompose(mode) :283-466 -> (BlockMatrix holding L (unit lower) and U packed, permutation array: row i of
         L*U is row perm[i] of this matrix).  Deviation, on purpose: the reference stores the ORIGINAL diagonal block for
         every block row but the last (`scatterRdds(i)(0) = matFirst.cache()`, :355), which makes P A = L U false;
-        `keepUnfactoredDiagonal=True` reproduces that, the default stores the factors."""
+        `keepUnfactoredDiagonal=True` reproduces that, the default stores the factors.  "dist" mode is sharded across
+        the ranks (see matrix/factorizations.py): every rank gets the full permutation array."""
         from . import factorizations as fz
         if self.numRows() != self.numCols():
             raise nat.MarlinArgumentError(nat.MB_ERR_DIM_MISMATCH, f"LU decompose only support square matrix: {self.numRows()} v.s {self.numCols()}")
@@ -245,9 +309,8 @@ class DenseVecMatrix(DistributedMatrix):
         if not fz.mode_is_dist(mode, n):
             blocks, _, _, _ = self._square_blocks(n)
             packed, perm = blocks[(0, 0)].lu()
-            return self._finish({(0, 0): packed}, 1, n), [int(p) for p in perm]
-        blocks, nb, sub, n = self._square_blocks(baseSize or conf.get("marlin.lu.basesize", 1000))
-        out, p_array = fz.lu_blocks(blocks, nb, sub, n, keepUnfactoredDiagonal)
+            return self._finish_breeze({(0, 0): packed}, n), [int(p) for p in perm]
+        out, nb, n, p_array = self._factor_dist("lu", baseSize or conf.get("marlin.lu.basesize", 1000), keepUnfactoredDiagonal)
         return self._finish(out, nb, n), p_array
 
     def choleskyDecompose(self, mode: str = "auto", baseSize: Optional[int] = None):
@@ -259,9 +322,8 @@ class DenseVecMatrix(DistributedMatrix):
         n = self.numRows()
         if not fz.mode_is_dist(mode, n):
             blocks, _, _, _ = self._square_blocks(n)
-            return self._finish({(0, 0): blocks[(0, 0)].cholesky()}, 1, n)
-        blocks, nb, _, n = self._square_blocks(baseSize or conf.get("marlin.cholesky.basesize", 1000))
-        return self._finish(fz.cholesky_blocks({k: v for k, v in blocks.items() if k[0] >= k[1]}, nb), nb, n)
+            return self._finish_breeze({(0, 0): blocks[(0, 0)].cholesky()}, n)
+        return self._finish(*self._factor_dist("cholesky", baseSize or conf.get("marlin.cholesky.basesize", 1000)))
 
     def inverse(self, mode: str = "auto", baseSize: Optional[int] = None):
         """inverse() :271-273, inverse(mode) :568-764"""
@@ -271,9 +333,13 @@ class DenseVecMatrix(DistributedMatrix):
         n = self.numRows()
         if not fz.mode_is_dist(mode, n):
             blocks, _, _, _ = self._square_blocks(n)
-            return self._finish({(0, 0): blocks[(0, 0)].inverse()}, 1, n)
-        blocks, nb, _, n = self._square_blocks(baseSize or conf.get("marlin.inverse.basesize", 1000))
-        return self._finish(fz.inverse_blocks(blocks, nb), nb, n)
+            return self._finish_breeze({(0, 0): blocks[(0, 0)].inverse()}, n)
+        return self._finish(*self._factor_dist("inverse", baseSize or conf.get("marlin.inverse.basesize", 1000)))
+
+    def _finish_breeze(self, blocks, n: int):
+        """"breeze" mode: every rank computed the one block; rank 0 (its elem_owner) keeps it."""
+        rank, _ = world()
+        return self._finish(blocks if rank == 0 else {}, 1, n)
 
     # ------------------------------------------------------------------ SVD (:1464-1652)
     def computeSVD(self, k: int, computeU: bool = False, rCond: float = 1e-9, mode: str = "auto"):
