@@ -247,6 +247,44 @@ int32_t mb_svd_mode(int64_t n, int32_t k, const char* mode, int32_t* compute_mod
  * Returns sk (>= 0) or a negative error code. */
 int32_t mb_svd_rank(const double* sigmas, int32_t count, int32_t k, double rcond);
 
+/* ---- f5, the overload computeSVD(k, computeU, rCond, maxIter, tol, mode) (:1557-1652): the eigs modes run a Lanczos
+ *      solver on the device instead of a full decomposition of G.  "dist-eigs" never forms G. ---- */
+/* The chooser of that overload: mb_svd_mode's rules and messages, except that the 65535-column cap of
+ * computeGramianMatrix applies only to the modes that form G ("local-svd", "local-eigs"); "dist-eigs" takes any n up to
+ * INT32_MAX.  max_iter <= 0 is rejected in the eigs modes (ARPACK's info = -4).  Pure logic, no GPU needed. */
+int32_t mb_svd_plan(int64_t n, int32_t k, const char* mode, int32_t max_iter, double tol, int32_t* compute_mode);
+/* multiplyGramianMatrixBy (:1444-1459) over one shard: y = A^T (A x), or y += it when accumulate != 0.  A is an fp64
+ * m x n view; x and y are fp64 vectors of n elements.  A row-major view (a row shard's transposed view, any ld, 8-byte
+ * alignment) or a single column is read in place; any other view is first packed into a row-major copy (one more
+ * launch and 16 m n more bytes).  Rows n <= 5118 wide cross HBM once (8 m n bytes); wider rows are streamed twice
+ * (16 m n).  Fixed summation order, no atomics, every multiply and add rounded separately: the same inputs give the
+ * same bits on every run.  m = 0 gives zeros (y unchanged when accumulating).  Two kernel launches when m > 0. */
+int32_t mb_block_gram_matvec(mb_ctx* ctx, const mb_block* A, const mb_block* x, mb_block* y, int32_t accumulate);
+/* EigenValueDecomposition.symmetricEigs (:1725-1834) by reverse communication, as ARPACK's dsaupd / dseupd loop:
+ * thick-restart Lanczos (Wu-Simon; for a symmetric operator equivalent to ARPACK's implicit restart with exact shifts)
+ * for the nev eigenvalues of largest magnitude of an n x n symmetric operator, with an ncv-vector basis (the reference
+ * uses ncv = min(2 nev, n)).  Each restart keeps nev + min(nconv, (ncv - nev) / 2) Ritz vectors (dsaup2), at most
+ * ncv - 1.  A pair is converged when |beta y_last| <= tol max(eps^(2/3), |theta|) (dsconv), or when that residual is
+ * already at the operator's rounding level (<= 2^-46 max |theta|); tol <= 0 means eps = 2^-53.  Every new basis
+ * vector is orthogonalised against the whole basis by classical Gram-Schmidt run twice.  The start vector is
+ * mb_fill_uniform's stream `seed` on [-1, 1), so every rank that uses the same seed starts from the same bits; if the
+ * Krylov space becomes invariant a fresh vector from the same stream continues it (dgetv0).  Device memory:
+ * 8 n (2 ncv + 3) bytes.  max_iter bounds the restarts; running out is MB_ERR_NO_CONVERGENCE with the reference's
+ * info = 1 message. */
+typedef struct mb_eigs mb_eigs;
+int32_t mb_eigs_create(mb_ctx* ctx, int32_t n, int32_t nev, int32_t ncv, double tol, int32_t max_iter, int64_t seed,
+                       mb_eigs** out);
+/* One turn of the loop.  *ido == 1: write y = Op x (both device n x 1 views the solver owns) and call again;
+ * *ido == 99: done (mb_eigs_result).  At most one host synchronisation per call. */
+int32_t mb_eigs_step(mb_ctx* ctx, mb_eigs* eigs, int32_t* ido, mb_block** x, mb_block** y);
+/* The nev eigenvalues, descending, into the HOST array w (may be NULL) and their orthonormal eigenvectors into Z (an fp64
+ * n x nev block, may be NULL); *nconv and *iters (may be NULL): the converged pairs and the restarts taken.  Blocking. */
+int32_t mb_eigs_result(mb_ctx* ctx, mb_eigs* eigs, double* w, mb_block* Z, int32_t* nconv, int32_t* iters);
+int32_t mb_eigs_destroy(mb_eigs* eigs);
+/* The solver's projected problem on the host: all eigenpairs of a symmetric n x n matrix T (column-major, lower triangle
+ * read) by cyclic Jacobi; w receives the eigenvalues descending, Z (column-major n x n) the eigenvectors.  Pure logic. */
+int32_t mb_eigs_projected(int32_t n, const double* T, double* w, double* Z);
+
 /* ---- DenseVecMatrix.lr (matrix/DenseVecMatrix.scala:1005-1035): logistic regression by gradient steps over the rows.
  *      `rows` is an fp64 view with one training row per matrix row (a row shard's transposed view is read in place, any
  *      other view is first copied into a row-major buffer).  Column 0 is the label; the features are the row with

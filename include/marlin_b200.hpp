@@ -975,25 +975,34 @@ public:
         check(mb_svd_mode(n, k, mode.c_str(), &cm));
         SubMatrix g = data_.gramian();
         auto eig = g.symmetricEigen();
-        std::vector<double> sigmas(eig.first.size());
-        for (size_t i = 0; i < sigmas.size(); ++i) sigmas[i] = std::sqrt(std::fabs(eig.first[i]));
-        const int32_t sk = mb_svd_rank(sigmas.data(), (int32_t)sigmas.size(), k, rCond);
-        if (sk < 0) check(sk);
-        SVD out;
-        out.s.assign(sigmas.begin(), sigmas.begin() + sk);
-        out.V = DenseMatrix((int)n, sk);
-        if (sk == 0) return out;
-        out.V = eig.second.slice(0, (int)n, 0, sk).copy().denseBlock();
-        if (computeU) {
-            // N = V_k S_k^-1 (:1635-1646) column by column on the device, then U = this.multiply(N) (:1647)
-            SubMatrix nm = SubMatrix::empty((int)n, sk);
-            for (int j = 0; j < sk; ++j) {
-                SubMatrix dst = nm.slice(0, (int)n, j, j + 1);
-                check(mb_block_div(Context::get(), eig.second.slice(0, (int)n, j, j + 1).handle(), sigmas[(size_t)j], 0, dst.handle()));
-            }
-            out.U = std::make_shared<DenseVecMatrix>(multiply(nm.denseBlock()));
+        return finishSVD(eig.first, eig.second, k, computeU, rCond);
+    }
+    // The reference's full overload (:1557-1652): its eigs modes run the restarted Lanczos solver of the C ABI
+    // (mb_eigs_*) for the k largest eigenvalues of G; "dist-eigs" never forms G (mb_block_gram_matvec), "local-eigs"
+    // applies G with mb_block_gemv, "local-svd" is the Gramian and Jacobi path above.  Modes are chosen by mb_svd_plan.
+    SVD computeSVD(int k, bool computeU, double rCond, int maxIter, double tol, const std::string& mode) {
+        const long n = numCols();
+        int32_t cm = 0;
+        check(mb_svd_plan(n, k, mode.c_str(), maxIter, tol, &cm));
+        if (cm == MB_SVD_LOCAL_LAPACK) return computeSVD(k, computeU, rCond, mode);
+        mb_ctx* ctx = Context::get();
+        SubMatrix g;
+        if (cm == MB_SVD_LOCAL_ARPACK) g = data_.gramian();
+        mb_eigs* raw = nullptr;
+        check(mb_eigs_create(ctx, (int32_t)n, k, (int32_t)std::min<long>(2L * k, n), tol, maxIter, 1557, &raw));
+        std::unique_ptr<mb_eigs, int32_t (*)(mb_eigs*)> eigs(raw, mb_eigs_destroy);
+        for (;;) {
+            int32_t ido = 0;
+            mb_block *x = nullptr, *y = nullptr;
+            check(mb_eigs_step(ctx, eigs.get(), &ido, &x, &y));
+            if (ido == 99) break;
+            check(cm == MB_SVD_LOCAL_ARPACK ? mb_block_gemv(ctx, g.handle(), x, y, 0)
+                                            : mb_block_gram_matvec(ctx, data_.handle(), x, y, 0));
         }
-        return out;
+        std::vector<double> w((size_t)k);
+        SubMatrix z = SubMatrix::empty((int)n, k);
+        check(mb_eigs_result(ctx, eigs.get(), w.data(), z.handle(), nullptr, nullptr));
+        return finishSVD(w, z, k, computeU, rCond);
     }
 
     // ---- lr(stepSize, iters) :1005-1035 (one process: every row is local, the whole loop runs on the device).  Column 0
@@ -1012,6 +1021,29 @@ public:
     }
 
 private:
+    // :1607-1652 from the eigenvalues w of G (in the solver's order) and their vectors, the columns of vecs
+    SVD finishSVD(const std::vector<double>& w, SubMatrix& vecs, int k, bool computeU, double rCond) {
+        const long n = numCols();
+        std::vector<double> sigmas(w.size());
+        for (size_t i = 0; i < sigmas.size(); ++i) sigmas[i] = std::sqrt(std::fabs(w[i]));
+        const int32_t sk = mb_svd_rank(sigmas.data(), (int32_t)sigmas.size(), k, rCond);
+        if (sk < 0) check(sk);
+        SVD out;
+        out.s.assign(sigmas.begin(), sigmas.begin() + sk);
+        out.V = DenseMatrix((int)n, sk);
+        if (sk == 0) return out;
+        out.V = vecs.slice(0, (int)n, 0, sk).copy().denseBlock();
+        if (computeU) {
+            // N = V_k S_k^-1 (:1635-1646) column by column on the device, then U = this.multiply(N) (:1647)
+            SubMatrix nm = SubMatrix::empty((int)n, sk);
+            for (int j = 0; j < sk; ++j) {
+                SubMatrix dst = nm.slice(0, (int)n, j, j + 1);
+                check(mb_block_div(Context::get(), vecs.slice(0, (int)n, j, j + 1).handle(), sigmas[(size_t)j], 0, dst.handle()));
+            }
+            out.U = std::make_shared<DenseVecMatrix>(multiply(nm.denseBlock()));
+        }
+        return out;
+    }
     // rows src[pos[i]] (columns c0 until c1) into row i of dst from column d0; runs of consecutive positions as one copy
     static void copyRows(const SubMatrix& src, const std::vector<int>& pos, int c0, int c1, SubMatrix& dst, int d0) {
         for (size_t p = 0; p < pos.size();) {

@@ -93,6 +93,13 @@ SIGNATURES = {
     "mb_block_syev": (c_i32, [c_ctx, c_blk, c_blk, c_dp, C.POINTER(c_i32)]),
     "mb_svd_mode": (c_i32, [c_i64, c_i32, C.c_char_p, C.POINTER(c_i32)]),
     "mb_svd_rank": (c_i32, [c_dp, c_i32, c_i32, c_f64]),
+    "mb_svd_plan": (c_i32, [c_i64, c_i32, C.c_char_p, c_i32, c_f64, C.POINTER(c_i32)]),
+    "mb_block_gram_matvec": (c_i32, [c_ctx, c_blk, c_blk, c_blk, c_i32]),
+    "mb_eigs_create": (c_i32, [c_ctx, c_i32, c_i32, c_i32, c_f64, c_i32, c_i64, C.POINTER(C.c_void_p)]),
+    "mb_eigs_step": (c_i32, [c_ctx, C.c_void_p, C.POINTER(c_i32), C.POINTER(c_blk), C.POINTER(c_blk)]),
+    "mb_eigs_result": (c_i32, [c_ctx, C.c_void_p, c_dp, c_blk, C.POINTER(c_i32), C.POINTER(c_i32)]),
+    "mb_eigs_destroy": (c_i32, [C.c_void_p]),
+    "mb_eigs_projected": (c_i32, [c_i32, c_dp, c_dp, c_dp]),
     "mb_lr_gradient": (c_i32, [c_ctx, c_blk, c_dp, c_dp]),
     "mb_lr_train": (c_i32, [c_ctx, c_blk, c_i64, c_f64, c_i32, c_dp]),
     "mb_als_links": (c_i32, [c_i64, C.c_void_p, C.c_void_p, C.c_void_p, c_i32, c_i32, C.c_void_p, C.c_void_p, C.c_void_p,

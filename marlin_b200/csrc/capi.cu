@@ -16,6 +16,7 @@
 #include "pagerank.h"
 #include "mlp.h"
 #include "norm.h"
+#include "eigs.h"
 
 #include <cuda_runtime.h>
 #include <climits>
@@ -1442,6 +1443,308 @@ int32_t mb_lr_train(mb_ctx* ctx, const mb_block* rows, int64_t data_size, double
     }
     MB_CUDA(cudaMemcpyAsync(w_out, wd, sizeof(double) * n, cudaMemcpyDeviceToHost, ctx->stream));
     MB_CUDA(cudaStreamSynchronize(ctx->stream));
+    return MB_OK;
+}
+
+// ------------------------------------------------------------------------ computeSVD dist-eigs: A^T (A x) and Lanczos
+// multiplyGramianMatrixBy (matrix/DenseVecMatrix.scala:1444-1459) over one shard.  A row-major view (a row shard's
+// transposed view) or a single column is read in place; any other view is first packed into a row-major copy.
+int32_t mb_block_gram_matvec(mb_ctx* ctx, const mb_block* A, const mb_block* x, mb_block* y, int32_t accumulate) {
+    MB_CTX(ctx);
+    MB_LOCK(ctx);
+    if (!A || !x || !y) return fail(MB_ERR_INVALID_ARG, "mb_block_gram_matvec: null block");
+    vec_view xv, yv;
+    if (A->dtype != MB_F64 || !as_vector(x, &xv) || !as_vector(y, &yv))
+        return fail(MB_ERR_UNSUPPORTED, "mb_block_gram_matvec: fp64 matrix and fp64 single-column (or single-row) vectors only");
+    if (A->cols != xv.len)
+        return fail(MB_ERR_DIM_MISMATCH, "Dimension mismatch during matrix-vector multiplication: %d vs %d", A->cols, xv.len);
+    if (A->cols != yv.len)
+        return fail(MB_ERR_DIM_MISMATCH, "mb_block_gram_matvec: result vector has %d elements, expected %d", yv.len, A->cols);
+    const int m = A->rows, n = A->cols;
+    if (n == 0) return MB_OK;
+    mb::StreamBuffer staged, part;
+    mb_block v = *A;
+    if (!A->is_transpose && n > 1 && m > 0) {
+        MB_CUDA(staged.alloc((size_t)m * n * sizeof(double), ctx->stream));
+        v = block_view(staged.as<void>(), m, n, n, true, MB_F64, ctx->device);
+        const int32_t r = copy_convert(ctx, A, &v);
+        if (r) return r;
+    }
+    const int parts = mb::gram_matvec_parts(m, n, ctx->num_sms);
+    if (parts) MB_CUDA(part.alloc((size_t)parts * n * sizeof(double), ctx->stream));
+    MB_CUDA(mb::gram_matvec_f64(f64_ptr(&v), rs(&v), m, n, xv.p, xv.inc, yv.p, yv.inc, accumulate != 0, part.as<double>(),
+                                ctx->num_sms, ctx->stream));
+    return MB_OK;
+}
+
+// EigenValueDecomposition.symmetricEigs (:1725-1834) as thick-restart Lanczos (Wu-Simon) with full reorthogonalisation.
+// V holds the basis (n x (ncv + 1), column-major) and W the next one while restarting.  The operator writes y = Op x into
+// V's next column, which is then orthogonalised in place (classical Gram-Schmidt twice) and normalised.
+struct mb_eigs {
+    int device = 0;
+    int n = 0, nev = 0, ncv = 0;
+    double tol = 0.0;
+    int32_t max_iter = 0;
+    int64_t seed = 0;
+    double *V = nullptr, *W = nullptr;   // n x (ncv + 1) each
+    double* gemv_ws = nullptr;           // the partial vectors of the basis products
+    double* small = nullptr;             // h1, h2, -h (ncv + 1 each), two dot scratches, the ncv x ncv rotation
+    double* host = nullptr;              // pinned: h1, h2, |y1|^2, |y2|^2
+    mb_block xb, yb;
+    std::vector<double> T;               // the projected matrix V^T Op V (ncv x ncv, column-major)
+    std::vector<double> w;               // the final eigenvalues (nev, descending) and their vectors in the basis
+    std::vector<double> Y;
+    int j = -1;                          // Op was asked for V[:, j]; -1 before the start vector
+    int iters = 0, draws = 0, nconv = 0;
+    int phase = 0;                       // 0 running, 1 converged, 2 out of restarts
+    int dot_len = 0;
+    double* h1() const { return small; }
+    double* h2() const { return small + (ncv + 1); }
+    double* hn() const { return small + 2 * (ncv + 1); }
+    double* dot1() const { return small + 3 * (ncv + 1); }
+    double* dot2() const { return dot1() + dot_len; }
+    double* rot() const { return dot2() + dot_len; }
+    double* col(double* B, int c) const { return B + (size_t)c * n; }
+};
+
+namespace {
+
+constexpr double EIGS_EPS = 0x1p-53;                     // dlamch('EpsMach')
+const char* const EIGS_MAX_ITER_MSG =
+    "ARPACK returns non-zero info = 1 Maximum number of iterations taken. (Refer ARPACK user guide for details)";
+
+// y := y - V[:, 0:k] (V[:, 0:k]^T y), twice; |y|^2 after each pass into dot1 / dot2 and h of each pass into h1 / h2.
+cudaError_t eigs_orthogonalise(mb_ctx* ctx, mb_eigs* E, double* y, int k) {
+    const int n = E->n;
+    cudaError_t e = cudaSuccess;
+    for (int pass = 0; pass < 2 && e == cudaSuccess; ++pass) {
+        double* h = pass ? E->h2() : E->h1();
+        e = mb::gemv_f64(true, n, k, E->V, n, y, 1, h, 1, false, E->gemv_ws, ctx->stream);
+        if (e == cudaSuccess) e = mb::ew_unary(mb::EW_AXPB, k, 1, h, 1, k, E->hn(), 1, k, -1.0, 0.0, ctx->stream);
+        if (e == cudaSuccess) e = mb::gemv_f64(false, n, k, E->V, n, E->hn(), 1, y, 1, true, E->gemv_ws, ctx->stream);
+        if (e == cudaSuccess) e = mb::dot_f64(n, y, 1, y, 1, pass ? E->dot2() : E->dot1(), ctx->stream);
+    }
+    return e;
+}
+
+// h1, h2 (k each) and the two squared norms to the host: the step's one synchronisation.
+cudaError_t eigs_fetch(mb_ctx* ctx, mb_eigs* E, int k) {
+    const int c = E->ncv + 1;
+    cudaError_t e = cudaMemcpyAsync(E->host, E->h1(), sizeof(double) * k, cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(E->host + c, E->h2(), sizeof(double) * k, cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(E->host + 2 * c, E->dot1(), sizeof(double), cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(E->host + 2 * c + 1, E->dot2(), sizeof(double), cudaMemcpyDeviceToHost, ctx->stream);
+    return e == cudaSuccess ? cudaStreamSynchronize(ctx->stream) : e;
+}
+
+// A fresh seeded vector in V[:, k], orthogonal to V[:, 0:k] and normalised (dgetv0).  ARPACK's dgetv0 also gives up
+// after a few tries; a vector that survives none of three draws is a failure of the basis, not of the input.
+int32_t eigs_fresh(mb_ctx* ctx, mb_eigs* E, int k) {
+    const int n = E->n;
+    double* v = E->col(E->V, k);
+    for (int attempt = 0; attempt < 3; ++attempt) {
+        MB_CUDA(mb::fill_uniform_f64(v, 1, n, n, 1, 0, (unsigned long long)mb_hash_seed(E->seed),
+                                     (long long)E->draws++ * n, -1.0, 1.0, ctx->stream));
+        if (k > 0) {
+            MB_CUDA(eigs_orthogonalise(ctx, E, v, k));
+        } else {
+            MB_CUDA(mb::dot_f64(n, v, 1, v, 1, E->dot2(), ctx->stream));
+            MB_CUDA(mb::dot_f64(n, v, 1, v, 1, E->dot1(), ctx->stream));
+        }
+        MB_CUDA(eigs_fetch(ctx, E, k));
+        const double r1 = std::sqrt(E->host[2 * (E->ncv + 1)]), r2 = std::sqrt(E->host[2 * (E->ncv + 1) + 1]);
+        if (r2 > 0.717 * r1 && r2 > 0.0) {
+            MB_CUDA(mb::ew_unary(mb::EW_DIV, n, 1, v, 1, n, v, 1, n, r2, 0.0, ctx->stream));
+            return MB_OK;
+        }
+    }
+    return fail(MB_ERR_NO_CONVERGENCE, "eigs: no start vector independent of the %d-vector basis after three draws", k);
+}
+
+// Ask the caller for Op V[:, j], written into V[:, j + 1].
+void eigs_request(mb_eigs* E, int32_t* ido, mb_block** x, mb_block** y) {
+    E->xb = block_view(E->col(E->V, E->j), E->n, 1, E->n, false, MB_F64, E->device);
+    E->yb = block_view(E->col(E->V, E->j + 1), E->n, 1, E->n, false, MB_F64, E->device);
+    *x = &E->xb;
+    *y = &E->yb;
+    *ido = 1;
+}
+
+// The basis is full: Ritz pairs of T, the convergence test, and either the end or a thick restart.
+int32_t eigs_restart(mb_ctx* ctx, mb_eigs* E, double beta) {
+    const int ncv = E->ncv, nev = E->nev, n = E->n;
+    std::vector<double> theta(ncv), S((size_t)ncv * ncv);
+    int32_t r = mb_eigs_projected(ncv, E->T.data(), theta.data(), S.data());
+    if (r) return r;
+    // "LM": the wanted pairs are the nev largest in magnitude (ties: larger value first, as sorted)
+    std::vector<int> order(ncv);
+    for (int i = 0; i < ncv; ++i) order[i] = i;
+    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return std::fabs(theta[a]) > std::fabs(theta[b]); });
+    const double eps23 = std::pow(EIGS_EPS, 2.0 / 3.0);
+    const double floor_res = 0x1p-46 * std::fabs(theta[order[0]]);
+    int nconv = 0;
+    for (int i = 0; i < nev; ++i) {
+        const int c = order[i];
+        const double res = std::fabs(beta * S[(size_t)c * ncv + ncv - 1]);
+        if (res <= E->tol * std::max(eps23, std::fabs(theta[c])) || res <= floor_res) ++nconv;
+    }
+    ++E->iters;
+    E->nconv = nconv;
+    if (nconv >= nev) {
+        std::vector<int> want(order.begin(), order.begin() + nev);
+        std::stable_sort(want.begin(), want.end(), [&](int a, int b) { return theta[a] > theta[b]; });
+        E->w.resize(nev);
+        E->Y.resize((size_t)ncv * nev);
+        for (int i = 0; i < nev; ++i) {
+            E->w[i] = theta[want[i]];
+            std::memcpy(E->Y.data() + (size_t)i * ncv, S.data() + (size_t)want[i] * ncv, sizeof(double) * ncv);
+        }
+        E->phase = 1;
+        return MB_OK;
+    }
+    if (E->iters >= E->max_iter) {
+        E->phase = 2;
+        return fail(MB_ERR_NO_CONVERGENCE, "%s", EIGS_MAX_ITER_MSG);
+    }
+    // keep nev + min(nconv, (ncv - nev) / 2) Ritz vectors (dsaup2), at most ncv - 1
+    const int kk = std::min(ncv - 1, nev + std::min(nconv, (ncv - nev) / 2));
+    std::vector<double> Yk((size_t)ncv * kk);
+    for (int i = 0; i < kk; ++i) std::memcpy(Yk.data() + (size_t)i * ncv, S.data() + (size_t)order[i] * ncv, sizeof(double) * ncv);
+    MB_CUDA(cudaMemcpyAsync(E->rot(), Yk.data(), sizeof(double) * Yk.size(), cudaMemcpyHostToDevice, ctx->stream));
+    mb_block Vb = block_view(E->V, n, ncv, n, false, MB_F64, E->device);
+    mb_block Yb = block_view(E->rot(), ncv, kk, ncv, false, MB_F64, E->device);
+    mb_block Wb = block_view(E->W, n, kk, n, false, MB_F64, E->device);
+    r = mb_block_gemm(ctx, &Vb, &Yb, &Wb, 0);
+    if (r) return r;
+    MB_CUDA(cudaMemcpyAsync(E->col(E->W, kk), E->col(E->V, ncv), sizeof(double) * n, cudaMemcpyDeviceToDevice, ctx->stream));
+    MB_CUDA(cudaStreamSynchronize(ctx->stream));      // Yk leaves scope
+    std::swap(E->V, E->W);
+    std::fill(E->T.begin(), E->T.end(), 0.0);
+    for (int i = 0; i < kk; ++i) {
+        E->T[(size_t)i * ncv + i] = theta[order[i]];
+        E->T[(size_t)kk * ncv + i] = E->T[(size_t)i * ncv + kk] = beta * S[(size_t)order[i] * ncv + ncv - 1];
+    }
+    E->j = kk;
+    return MB_OK;
+}
+
+}  // namespace
+
+int32_t mb_eigs_create(mb_ctx* ctx, int32_t n, int32_t nev, int32_t ncv, double tol, int32_t max_iter, int64_t seed,
+                       mb_eigs** out) {
+    if (out) *out = nullptr;
+    MB_CTX(ctx);
+    if (!out) return fail(MB_ERR_INVALID_ARG, "mb_eigs_create: null output");
+    if (!(n > nev)) return fail(MB_ERR_INVALID_ARG, "Number of required eigenvalues %d must be smaller than matrix dimension %d", nev, n);
+    if (nev <= 0)
+        return fail(MB_ERR_INVALID_ARG, "ARPACK returns non-zero info = -2 NEV must be positive. (Refer ARPACK user guide for details)");
+    if (!(ncv > nev && ncv <= n))
+        return fail(MB_ERR_INVALID_ARG, "ARPACK returns non-zero info = -3 NCV must be greater than NEV and less than or "
+                    "equal to N. (Refer ARPACK user guide for details)");
+    if (max_iter <= 0)
+        return fail(MB_ERR_INVALID_ARG, "ARPACK returns non-zero info = -4 The maximum number of Arnoldi update iterations "
+                    "allowed must be greater than zero. (Refer ARPACK user guide for details)");
+    std::unique_ptr<mb_eigs, void (*)(mb_eigs*)> E(new (std::nothrow) mb_eigs(), [](mb_eigs* p) { mb_eigs_destroy(p); });
+    if (!E) return fail(MB_ERR_OOM, "host allocation failed");
+    E->device = ctx->device;
+    E->n = n; E->nev = nev; E->ncv = ncv; E->max_iter = max_iter; E->seed = seed;
+    E->tol = tol > 0.0 ? tol : EIGS_EPS;
+    E->dot_len = mb::dot_scratch_doubles();
+    const size_t basis = (size_t)n * (ncv + 1) * sizeof(double);
+    const size_t ws = std::max(mb::gemv_workspace_doubles(true, n, ncv + 1), mb::gemv_workspace_doubles(false, n, ncv + 1));
+    MB_CUDA(cudaMalloc(&E->V, basis));
+    MB_CUDA(cudaMalloc(&E->W, basis));
+    MB_CUDA(cudaMalloc(&E->gemv_ws, ws * sizeof(double)));
+    MB_CUDA(cudaMalloc(&E->small, (3 * (size_t)(ncv + 1) + 2 * E->dot_len + (size_t)ncv * ncv) * sizeof(double)));
+    MB_CUDA(cudaMallocHost(&E->host, (2 * (size_t)(ncv + 1) + 2) * sizeof(double)));
+    E->T.assign((size_t)ncv * ncv, 0.0);
+    *out = E.release();
+    return MB_OK;
+}
+
+int32_t mb_eigs_step(mb_ctx* ctx, mb_eigs* E, int32_t* ido, mb_block** x, mb_block** y) {
+    MB_CTX(ctx);
+    MB_LOCK(ctx);
+    if (!E || !ido || !x || !y) return fail(MB_ERR_INVALID_ARG, "mb_eigs_step: null argument");
+    *x = *y = nullptr;
+    if (E->phase == 2) { *ido = 99; return fail(MB_ERR_NO_CONVERGENCE, "%s", EIGS_MAX_ITER_MSG); }
+    if (E->phase == 1) { *ido = 99; return MB_OK; }
+    const int n = E->n, ncv = E->ncv, c = ncv + 1;
+    int32_t r;
+    if (E->j < 0) {                                      // the seeded start vector
+        r = eigs_fresh(ctx, E, 0);
+        if (r) return r;
+        E->j = 0;
+        eigs_request(E, ido, x, y);
+        return MB_OK;
+    }
+    // the caller wrote Op V[:, j] into V[:, j + 1]
+    const int j = E->j, k = j + 1;
+    double* v = E->col(E->V, k);
+    MB_CUDA(eigs_orthogonalise(ctx, E, v, k));
+    MB_CUDA(eigs_fetch(ctx, E, k));
+    for (int i = 0; i < k; ++i) {
+        const double h = E->host[i] + E->host[c + i];
+        E->T[(size_t)j * ncv + i] = E->T[(size_t)i * ncv + j] = h;
+    }
+    const double r1 = std::sqrt(E->host[2 * c]), r2 = std::sqrt(E->host[2 * c + 1]);
+    // the second pass removed much of what the first left: v lies in the basis' span (dsaitr's refinement test)
+    const bool invariant = !(r2 > 0.717 * r1) || !(r2 > 0.0);
+    double beta = invariant ? 0.0 : r2;
+    if (!invariant) {
+        MB_CUDA(mb::ew_unary(mb::EW_DIV, n, 1, v, 1, n, v, 1, n, beta, 0.0, ctx->stream));
+    } else if (k < ncv) {
+        r = eigs_fresh(ctx, E, k);                       // dgetv0: continue from a new direction
+        if (r) return r;
+    } else {
+        MB_CUDA(cudaMemsetAsync(v, 0, sizeof(double) * n, ctx->stream));
+    }
+    if (k < ncv) {
+        E->j = k;
+        eigs_request(E, ido, x, y);
+        return MB_OK;
+    }
+    r = eigs_restart(ctx, E, beta);
+    if (r) { *ido = 99; return r; }
+    if (E->phase == 1) { *ido = 99; return MB_OK; }
+    eigs_request(E, ido, x, y);
+    return MB_OK;
+}
+
+int32_t mb_eigs_result(mb_ctx* ctx, mb_eigs* E, double* w, mb_block* Z, int32_t* nconv, int32_t* iters) {
+    MB_CTX(ctx);
+    MB_LOCK(ctx);
+    if (!E) return fail(MB_ERR_INVALID_ARG, "mb_eigs_result: null solver");
+    if (nconv) *nconv = E->nconv;
+    if (iters) *iters = E->iters;
+    if (E->phase == 2) return fail(MB_ERR_NO_CONVERGENCE, "%s", EIGS_MAX_ITER_MSG);
+    if (E->phase != 1) return fail(MB_ERR_INVALID_ARG, "mb_eigs_result: the solver has not finished (step until ido = 99)");
+    if (w) std::memcpy(w, E->w.data(), sizeof(double) * E->nev);
+    if (!Z) return MB_OK;
+    if (Z->dtype != MB_F64 || Z->rows != E->n || Z->cols != E->nev)
+        return fail(MB_ERR_DIM_MISMATCH, "mb_eigs_result: Z must be an fp64 %d x %d block, got %d x %d", E->n, E->nev, Z->rows, Z->cols);
+    MB_CUDA(cudaMemcpyAsync(E->rot(), E->Y.data(), sizeof(double) * E->Y.size(), cudaMemcpyHostToDevice, ctx->stream));
+    mb_block Vb = block_view(E->V, E->n, E->ncv, E->n, false, MB_F64, E->device);
+    mb_block Yb = block_view(E->rot(), E->ncv, E->nev, E->ncv, false, MB_F64, E->device);
+    const int32_t r = mb_block_gemm(ctx, &Vb, &Yb, Z, 0);
+    if (r) return r;
+    MB_CUDA(cudaStreamSynchronize(ctx->stream));
+    return MB_OK;
+}
+
+int32_t mb_eigs_destroy(mb_eigs* E) {
+    if (!E) return MB_OK;
+    int prev = 0;
+    cudaGetDevice(&prev);
+    cudaSetDevice(E->device);
+    cudaDeviceSynchronize();
+    cudaFree(E->V);
+    cudaFree(E->W);
+    cudaFree(E->gemv_ws);
+    cudaFree(E->small);
+    if (E->host) cudaFreeHost(E->host);
+    cudaSetDevice(prev);
+    delete E;
     return MB_OK;
 }
 

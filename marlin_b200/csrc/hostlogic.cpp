@@ -256,6 +256,100 @@ int32_t mb_svd_mode(int64_t n, int32_t k, const char* mode, int32_t* compute_mod
     return MB_OK;
 }
 
+// The same chooser for the overload computeSVD(k, computeU, rCond, maxIter, tol, mode) (:1557-1652), whose eigs modes
+// run the Lanczos solver: the column cap belongs to computeGramianMatrix, so only the modes that form G check it.
+int32_t mb_svd_plan(int64_t n, int32_t k, const char* mode, int32_t max_iter, double tol, int32_t* compute_mode) {
+    (void)tol;                                         // any tol is valid: tol <= 0 asks for machine precision, as in ARPACK
+    if (!mode || !compute_mode) return mb_fail(MB_ERR_INVALID_ARG, "mb_svd_plan: null argument");
+    if (!(k > 0 && k <= n))
+        return mb_fail(MB_ERR_INVALID_ARG, "Request up to n singular values but got k=%d and n=%lld.", k, (long long)n);
+    int cm;
+    if (std::strcmp(mode, "auto") == 0) {
+        if (n < 100 || k > n / 2) cm = k < n / 3 ? MB_SVD_LOCAL_ARPACK : MB_SVD_LOCAL_LAPACK;
+        else cm = MB_SVD_DIST_ARPACK;
+    } else if (std::strcmp(mode, "local-svd") == 0) {
+        cm = MB_SVD_LOCAL_LAPACK;
+    } else if (std::strcmp(mode, "local-eigs") == 0) {
+        cm = MB_SVD_LOCAL_ARPACK;
+    } else if (std::strcmp(mode, "dist-eigs") == 0) {
+        cm = MB_SVD_DIST_ARPACK;
+    } else {
+        return mb_fail(MB_ERR_INVALID_ARG, "Do not support mode %s.", mode);
+    }
+    if (cm != MB_SVD_LOCAL_LAPACK && !(k < n))
+        return mb_fail(MB_ERR_INVALID_ARG, "k must be smaller than n in %s mode but got k=%d and n=%lld.",
+                       cm == MB_SVD_LOCAL_ARPACK ? "local-eigs" : "dist-eigs", k, (long long)n);
+    if (cm != MB_SVD_DIST_ARPACK && n > 65535)
+        return mb_fail(MB_ERR_INVALID_ARG, "Argument with more than 65535 cols: %lld", (long long)n);
+    if (n > INT32_MAX) return mb_fail(MB_ERR_INVALID_ARG, "Argument with more than %d cols: %lld", INT32_MAX, (long long)n);
+    if (cm != MB_SVD_LOCAL_LAPACK && max_iter <= 0)
+        return mb_fail(MB_ERR_INVALID_ARG, "ARPACK returns non-zero info = -4 The maximum number of Arnoldi update "
+                       "iterations allowed must be greater than zero. (Refer ARPACK user guide for details)");
+    *compute_mode = cm;
+    return MB_OK;
+}
+
+// The projected problem of the Lanczos solver: all eigenpairs of a symmetric n x n matrix (column-major, lower triangle
+// read) by cyclic Jacobi with Rutishauser's rotations, sweeping until no off-diagonal entry changes a diagonal one.
+// w: eigenvalues descending (ties: lower index first); Z: the eigenvectors as columns (column-major n x n).
+int32_t mb_eigs_projected(int32_t n, const double* T, double* w, double* Z) {
+    if (n < 0 || (n > 0 && (!T || !w || !Z))) return mb_fail(MB_ERR_INVALID_ARG, "mb_eigs_projected: bad argument");
+    std::vector<double> a((size_t)n * n), v((size_t)n * n, 0.0);
+    for (int32_t j = 0; j < n; ++j)
+        for (int32_t i = 0; i < n; ++i) a[(size_t)j * n + i] = i >= j ? T[(size_t)j * n + i] : T[(size_t)i * n + j];
+    for (int32_t i = 0; i < n; ++i) v[(size_t)i * n + i] = 1.0;
+    for (size_t i = 0; i < a.size(); ++i)
+        if (!std::isfinite(a[i])) return mb_fail(MB_ERR_INVALID_ARG, "mb_eigs_projected: the matrix holds NaN or Inf");
+    auto A = [&](int32_t i, int32_t j) -> double& { return a[(size_t)j * n + i]; };
+    double frob = 0.0;
+    for (double x : a) frob += x * x;
+    // below this an entry moves no eigenvalue by more than eps^2 ||T||
+    const double floor_abs = 0x1p-106 * std::sqrt(frob);
+    bool rotated = true;
+    for (int sweep = 0; sweep < 100 && rotated; ++sweep) {
+        rotated = false;
+        for (int32_t p = 0; p < n - 1; ++p)
+            for (int32_t q = p + 1; q < n; ++q) {
+                const double apq = A(p, q);
+                if (apq == 0.0) continue;
+                const double app = A(p, p), aqq = A(q, q);
+                // negligible relative to both diagonal entries, or to the whole matrix
+                if (std::fabs(apq) <= 0x1p-54 * std::sqrt(std::fabs(app)) * std::sqrt(std::fabs(aqq)) ||
+                    std::fabs(apq) <= floor_abs) {
+                    A(p, q) = A(q, p) = 0.0;
+                    continue;
+                }
+                rotated = true;
+                const double theta = (aqq - app) / (2.0 * apq);
+                const double t = (theta >= 0 ? 1.0 : -1.0) / (std::fabs(theta) + std::sqrt(theta * theta + 1.0));
+                const double c = 1.0 / std::sqrt(t * t + 1.0), s = t * c, tau = s / (1.0 + c);
+                for (int32_t r = 0; r < n; ++r) {
+                    if (r == p || r == q) continue;
+                    const double arp = A(r, p), arq = A(r, q);
+                    A(r, p) = A(p, r) = arp - s * (arq + tau * arp);
+                    A(r, q) = A(q, r) = arq + s * (arp - tau * arq);
+                }
+                A(p, p) = app - t * apq;
+                A(q, q) = aqq + t * apq;
+                A(p, q) = A(q, p) = 0.0;
+                for (int32_t r = 0; r < n; ++r) {
+                    const double vrp = v[(size_t)p * n + r], vrq = v[(size_t)q * n + r];
+                    v[(size_t)p * n + r] = vrp - s * (vrq + tau * vrp);
+                    v[(size_t)q * n + r] = vrq + s * (vrp - tau * vrq);
+                }
+            }
+    }
+    if (rotated) return mb_fail(MB_ERR_NO_CONVERGENCE, "mb_eigs_projected: no convergence after 100 sweeps (n = %d)", n);
+    std::vector<int32_t> order(n);
+    for (int32_t i = 0; i < n; ++i) order[i] = i;
+    std::stable_sort(order.begin(), order.end(), [&](int32_t x, int32_t y) { return A(x, x) > A(y, y); });
+    for (int32_t i = 0; i < n; ++i) {
+        w[i] = A(order[i], order[i]);
+        std::memcpy(Z + (size_t)i * n, v.data() + (size_t)order[i] * n, sizeof(double) * n);
+    }
+    return MB_OK;
+}
+
 // matrix/DenseVecMatrix.scala:975-999: the reference matches "1" and "inf" (a MatchError otherwise); "fro" is its TODO,
 // provided here, and "2" stays out as it does there.
 int32_t mb_norm_mode(const char* mode, int32_t* kind) {

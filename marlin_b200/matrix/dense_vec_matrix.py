@@ -30,6 +30,38 @@ def _ceil_len(total: int, parts: int) -> int:
     return int(math.ceil(float(total) / float(parts)))
 
 
+# the stream of the Lanczos start vector: every rank starts from the same bits
+EIGS_SEED = 1557
+
+
+def symmetric_eigs(op, n: int, k: int, tol: float, max_iter: int):
+    """EigenValueDecomposition.symmetricEigs (:1725-1834) on the device: the k largest-magnitude eigenpairs of the
+    symmetric operator `op(x, y)` (writes y = Op x; both are mb_block handles of n x 1 device vectors), ncv =
+    min(2k, n).  -> (eigenvalues descending, their eigenvectors as the columns of an n x k SubMatrix,
+    {"applications": operator calls, "restarts": restarts taken})."""
+    import ctypes as C
+    rt = Runtime.get()
+    rt.sync_stream()
+    h = C.c_void_p()
+    nat.check(rt.lib.mb_eigs_create(rt.ctx, n, k, min(2 * k, n), float(tol), int(max_iter), EIGS_SEED, C.byref(h)))
+    try:
+        ido, x, y = C.c_int32(0), nat.c_blk(), nat.c_blk()
+        applications = 0
+        while True:
+            nat.check(rt.lib.mb_eigs_step(rt.ctx, h, C.byref(ido), C.byref(x), C.byref(y)))
+            if ido.value == 99:
+                break
+            op(x, y)
+            applications += 1
+        w = np.zeros(k)
+        Z = SubMatrix.empty(n, k, nat.MB_F64, rt.device)
+        nconv, iters = C.c_int32(), C.c_int32()
+        nat.check(rt.lib.mb_eigs_result(rt.ctx, h, w.ctypes.data_as(nat.c_dp), Z.handle(), C.byref(nconv), C.byref(iters)))
+    finally:
+        rt.lib.mb_eigs_destroy(h)
+    return w, Z, {"applications": applications, "restarts": int(iters.value)}
+
+
 def _runs(ids: np.ndarray) -> List[Tuple[int, int, int]]:
     """Maximal runs (pos0, id0, length) of rows whose ids are consecutive in storage order."""
     out = []
@@ -342,12 +374,13 @@ class DenseVecMatrix(DistributedMatrix):
         return self._finish(blocks if rank == 0 else {}, 1, n)
 
     # ------------------------------------------------------------------ SVD (:1464-1652)
-    def computeSVD(self, k: int, computeU: bool = False, rCond: float = 1e-9, mode: str = "auto"):
+    def computeSVD(self, k: int, computeU: bool = False, rCond: float = 1e-9, mode: str = "auto", *,
+                   maxIter: Optional[int] = None, tol: Optional[float] = None):
         """computeSVD(k, computeU, rCond) :1531-1541 and the private mode overload :1557-1652 ->
         (U: DenseVecMatrix or None, s: ndarray of the sk leading singular values, V: ndarray n x sk).
 
-        mode is chosen and validated exactly as in the reference (mb_svd_mode: "auto", "local-svd", "local-eigs",
-        "dist-eigs", with its `require` messages).  Deliberate deviations, on every mode:
+        Without maxIter and tol, mode is chosen and validated exactly as in the reference (mb_svd_mode: "auto",
+        "local-svd", "local-eigs", "dist-eigs", with its `require` messages).  Deliberate deviations, on every mode:
           * one Gramian G = A^T A on the device (split-K DMMA, summed in a fixed order) and one full eigendecomposition
             of G by parallel Jacobi; "dist-eigs" exists in the reference to keep n^2 doubles off the driver.  Device
             memory, not the 65535-column cap, bounds n: G, V and the eigensolver's four working copies take about
@@ -356,14 +389,41 @@ class DenseVecMatrix(DistributedMatrix):
           * the Gramian's summation order differs from the reference's row-by-row dspr, so the results agree with it
             within rounding, not bitwise;
           * s = sqrt(|w|), the singular values of G as local-svd (dgesdd) returns them.
-        With several ranks every rank forms the Gramian of its rows (zeros if it holds none); the partials are exchanged
-        and summed in rank order on every rank, so all ranks hold the same G bit for bit and compute the same s and V.
-        The rows of U stay on the rank that holds the matching rows of this matrix."""
+        Passing maxIter or tol selects the reference's full overload computeSVD(k, computeU, rCond, maxIter, tol, mode)
+        (an omitted one takes the reference's default, max(300, 3k) or 1e-10), whose eigs modes run the restarted
+        Lanczos solver (mb_eigs_*) for the k largest eigenvalues of G, chosen by mb_svd_plan: "local-eigs" forms G and
+        applies it with mb_block_gemv; "dist-eigs" never forms G, its operator is mb_block_gram_matvec over the rows
+        (any n up to 2^31 - 1, 8 n (2 ncv + 3) bytes of device memory besides A, ncv = min(2k, n)); "local-svd" is the
+        Gramian and Jacobi path above.
+        With several ranks every rank forms the Gramian of its rows (or, in dist-eigs, the product with its rows), zeros
+        if it holds none; the partials are exchanged and summed in rank order on every rank, so all ranks hold the same
+        bits and compute the same s and V.  The rows of U stay on the rank that holds the matching rows of this matrix."""
         import ctypes as C
         lib = nat.load()
         n = self.numCols()
         cm = C.c_int32()
-        nat.check(lib.mb_svd_mode(n, int(k), str(mode).encode(), C.byref(cm)))
+        if maxIter is None and tol is None:
+            nat.check(lib.mb_svd_mode(n, int(k), str(mode).encode(), C.byref(cm)))
+            w, vblk = self._gramian().symmetricEigen()
+            return self._svd_finish(w, vblk, int(k), computeU, rCond)
+        maxIter = max(300, 3 * int(k)) if maxIter is None else int(maxIter)
+        tol = 1e-10 if tol is None else float(tol)
+        nat.check(lib.mb_svd_plan(n, int(k), str(mode).encode(), maxIter, tol, C.byref(cm)))
+        if cm.value == nat.MB_SVD_LOCAL_LAPACK:
+            w, vblk = self._gramian().symmetricEigen()
+            return self._svd_finish(w, vblk, int(k), computeU, rCond)
+        rt = Runtime.get()
+        if cm.value == nat.MB_SVD_LOCAL_ARPACK:
+            g = self._gramian()
+            op = lambda x, y: nat.check(rt.lib.mb_block_gemv(rt.ctx, g.handle(), x, y, 0))
+        else:
+            op = self._gram_matvec_op(n)
+        w, vblk, self.last_eigs_stats = symmetric_eigs(op, n, int(k), tol, maxIter)
+        return self._svd_finish(w, vblk, int(k), computeU, rCond)
+
+    def _gramian(self) -> SubMatrix:
+        """G = A^T A over all ranks' rows, identical bits on every rank."""
+        n = self.numCols()
         rank, ws = world()
         dev = self.data.buf.device if self.data is not None else Runtime.get().device
         if self.data is not None and len(self.ids):
@@ -378,9 +438,46 @@ class DenseVecMatrix(DistributedMatrix):
             g = parts[0]
             for p in parts[1:]:
                 g = g.add(p)
-        w, vblk = g.symmetricEigen()
+        return g
+
+    def _gram_matvec_op(self, n: int):
+        """The dist-eigs operator y = sum over the ranks, in rank order, of A_r^T (A_r x)."""
+        rt = Runtime.get()
+        rank, ws = world()
+        has_rows = self.data is not None and len(self.ids) > 0
+        # every rank learns of a bad shard before any rank enters the exchanges
+        problems = [(nat.MB_ERR_UNSUPPORTED, "computeSVD: fp64 rows only")] if has_rows and self.data.dtype != nat.MB_F64 else []
+        problems = self._gather(problems)
+        if problems:
+            raise nat.MarlinArgumentError(*problems[0])
+        if ws == 1:
+            if not has_rows:
+                raise nat.MarlinError(nat.MB_ERR_EMPTY, "empty collection")
+            return lambda x, y: nat.check(rt.lib.mb_block_gram_matvec(rt.ctx, self.data.handle(), x, y, 0))
+        dev = self.data.buf.device if self.data is not None else rt.device
+        mine = SubMatrix.zeros(n, 1, nat.MB_F64, dev)
+        sends = [(src, dst, ("gmv", src)) for src in range(ws) for dst in range(ws) if src != dst]
+
+        def op(x, y):
+            rt.sync_stream()
+            if has_rows:
+                nat.check(rt.lib.mb_block_gram_matvec(rt.ctx, self.data.handle(), x, mine.handle(), 0))
+            got = comm.exchange(sends, {("gmv", rank): mine.buf}, lambda key: torch.empty(n, dtype=torch.float64, device=dev),
+                                rank)
+            parts = [mine if r == rank else SubMatrix(buf=got[("gmv", r)], rows=n, cols=1, ld=n) for r in range(ws)]
+            total = parts[0]
+            for p in parts[1:]:
+                total = total.add(p)
+            nat.check(rt.lib.mb_block_copy(rt.ctx, total.handle(), y))
+        return op
+
+    def _svd_finish(self, w: np.ndarray, vblk: SubMatrix, k: int, computeU: bool, rCond: float):
+        """:1607-1652 from the eigenvalues w of G (in the solver's order) and their vectors, the columns of vblk."""
+        lib = nat.load()
+        n = vblk.rows
+        dev = vblk.buf.device
         sigmas = np.sqrt(np.abs(w))
-        sk = lib.mb_svd_rank(sigmas.ctypes.data_as(nat.c_dp), n, int(k), float(rCond))
+        sk = lib.mb_svd_rank(sigmas.ctypes.data_as(nat.c_dp), len(sigmas), k, float(rCond))
         if sk < 0:
             nat.check(sk)
         s = sigmas[:sk].copy()
