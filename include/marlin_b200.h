@@ -376,6 +376,29 @@ int32_t mb_coo_to_dense_rows(mb_ctx* ctx, int64_t nnz, const int32_t* row_pos, c
  * (row_major=1: DenseVecMatrix rows, Array.fill(cols); row_major=0: BDM.create column-major). */
 int32_t mb_fill_uniform(mb_ctx* ctx, mb_block* blk, int64_t partition_seed, int64_t first,
                         double lo, double hi, int32_t row_major);
+/* StandardNormalGenerator(mean, variance) (utils/RandomDataGenerator.scala:70-82, rdd/RandomRDD.scala:70-112): fills blk
+ * with the first rows * cols values of partition stream `partition_seed`, bit-exact with nextValue() =
+ * mean + sqrt(variance) * nextGaussian(), in the order of mb_fill_uniform's `row_major` (rows one after another, so one
+ * stream runs across rows and a pair of Gaussians may straddle two rows; or BDM.create column-major).  nextGaussian is
+ * java.util.Random's polar method over XORShiftRandom.next (:113-131): attempt a takes nextDouble positions 2a and 2a + 1,
+ * v = 2u - 1, s = v1*v1 + v2*v2, rejected when s >= 1 or s == 0, else m = StrictMath.sqrt(-2 * StrictMath.log(s) / s)
+ * (fdlibm's log) and the attempt gives v1*m, then v2*m.  Each multiply and add is rounded separately; sqrt(variance) is
+ * one correctly rounded value, so variance < 0 or NaN gives NaN everywhere and variance == 0 gives mean + (+-0.0).  The
+ * generator starts fresh: no cached value comes in, and an odd count drops the last one.  fp64 blocks only (a view may
+ * be strided; nothing outside it is written).  positions_out (may be NULL) receives 2A, the nextDouble positions the
+ * values consumed, A being the index of the last attempt used plus one.  Blocking (see MB_NORMAL_TILE_ATTEMPTS).
+ * More than 2^39 stream positions counted is MB_ERR_UNSUPPORTED. */
+int32_t mb_fill_normal(mb_ctx* ctx, mb_block* blk, int64_t partition_seed, double mean, double variance, int32_t row_major,
+                       int64_t* positions_out);
+/* mb_fill_normal's three passes.  The attempts are cut into tiles of MB_NORMAL_TILE_ATTEMPTS; a count pass counts the
+ * accepted attempts of a range of tiles, a scan turns the counts into prefixes, and a write pass regenerates the tiles that
+ * hold needed pairs.  With pairs = ceil(n / 2), the first round counts
+ *   ceil(ceil(pairs * 4.0 / 3.141592653589793) / MB_NORMAL_TILE_ATTEMPTS) tiles
+ * (the product and the quotient in double arithmetic).  While the accepted attempts of the tiles counted fall short of
+ * pairs by d > 0, a further round counts the next ceil(ceil(d * 4.0 / 3.141592653589793) / MB_NORMAL_TILE_ATTEMPTS)
+ * tiles.  Each round is two kernel launches and one stream synchronisation, the write pass one launch (and one more
+ * synchronisation for positions_out).  The budget never changes a result. */
+#define MB_NORMAL_TILE_ATTEMPTS 32768
 /* Host-side pieces of the same generator (pure integer logic, exported for the host mirror):
  * MTUtils.hashSeed (MurmurHash3.bytesHash over a 64-byte buffer) and the per-partition seeds
  * = successive java.util.Random(seed).nextLong() (rdd/RandomRDD.scala:28-45). */
@@ -479,6 +502,12 @@ int32_t mb_dense_rows_to_sparse(mb_ctx* ctx, const mb_block* rows, mb_sparse** o
  *           (mb_fill_sparse_uniform's sampler) over positions [s*P, s*P + nColumns) of the same stream.
  * The reference draws the set from an unseeded java.util.Random; here it is a function of (seed, partition). */
 int32_t mb_fill_spvec_uniform(mb_ctx* ctx, mb_sparse* S, int64_t partition_seed, double lo, double hi);
+/* randomSpaVecMatrix with StandardNormalGenerator(mean, variance): S as for mb_fill_spvec_uniform, its values the first
+ * s * P values of mb_fill_normal's stream for the partition (row r takes [r*s, (r+1)*s)).  For both entries the one column
+ * set is drawn from the stream positions right after those the values consumed: [2A, 2A + nColumns) here, 2A as
+ * mb_fill_normal's positions_out; [s*P, s*P + nColumns) for the uniform values, which consume exactly s*P positions.
+ * Blocking. */
+int32_t mb_fill_spvec_normal(mb_ctx* ctx, mb_sparse* S, int64_t partition_seed, double mean, double variance);
 
 /* ---- PageRank (examples/PageRank.scala).  The link matrix is held as the in-link CSR of the target pages: the CSC handle
  *      of its transpose, an mb_sparse with rows = n (source pages) and cols = the number of target rows, whose colptr is the

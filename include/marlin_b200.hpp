@@ -1539,6 +1539,12 @@ inline SparseVecMatrix DenseVecMatrix::toSparseVecMatrix() {
     return SparseVecMatrix::fromHandle(s, ids_, m, n);
 }
 
+// StandardNormalGenerator (utils/RandomDataGenerator.scala:70-82): mean + sqrt(variance) * nextGaussian() over the
+// partition's XORShift stream, bit-exact (mb_fill_normal)
+struct StandardNormalGenerator {
+    double mean = 0.0, variance = 1.0;
+};
+
 struct MTUtils {
     // utils/MTUtils.scala:228-243 — `row col value [timestamp]`, fields split on `,\s?|\s+`; the value is rounded once to
     // float32 (std::from_chars, locale-independent, as Float.parseFloat); blank lines are skipped
@@ -1574,19 +1580,15 @@ struct MTUtils {
     static long hashSeed(long seed) { return mb_hash_seed(seed); }                       // :18-21
     // randomDenVecMatrix (:63-73): partition p holds rows [p*N/P, (p+1)*N/P), its own XORShift stream
     static DenseVecMatrix randomDenVecMatrix(long nRows, int nCols, int numPartitions, long seed, double lo = 0.0, double hi = 1.0) {
-        std::vector<int64_t> seeds(numPartitions);
-        check(mb_partition_seeds(seed, numPartitions, seeds.data()));
-        SubMatrix shard = rowShard(nRows, nCols);
-        long start = 0;
-        for (int p = 0; p < numPartitions; ++p) {
-            const long end = ((long)(p + 1) * nRows) / numPartitions;
-            if (end > start) {
-                SubMatrix view = shard.slice((int)start, (int)end, 0, nCols);
-                check(mb_fill_uniform(Context::get(), view.handle(), seeds[p], 0, lo, hi, 1));
-            }
-            start = end;
-        }
-        return DenseVecMatrix(rowIds(nRows), shard, nRows, nCols);
+        return randomRows(nRows, nCols, numPartitions, seed, [&](mb_block* v, int64_t s) {
+            return mb_fill_uniform(Context::get(), v, s, 0, lo, hi, 1);
+        });
+    }
+    // ... with StandardNormalGenerator(mean, variance) values
+    static DenseVecMatrix randomDenVecMatrix(long nRows, int nCols, int numPartitions, long seed, StandardNormalGenerator g) {
+        return randomRows(nRows, nCols, numPartitions, seed, [&](mb_block* v, int64_t s) {
+            return mb_fill_normal(Context::get(), v, s, g.mean, g.variance, 1, nullptr);
+        });
     }
     // zerosDenVecMatrix / onesDenVecMatrix (:103-125): randomDenVecMatrix's rows, every element 0.0 / 1.0
     static DenseVecMatrix zerosDenVecMatrix(long nRows, int nCols) { return constantRows(nRows, nCols, 0.0); }
@@ -1600,6 +1602,67 @@ struct MTUtils {
     static BlockMatrix repeatByColumn(BlockMatrix& matrix, int times) { return requireTimes(times) ? matrix : matrix.repeat(times, false); }
 
 private:
+    // randomDenVecMatrix's partitions: fill(view, seed) writes partition p's rows from its seed
+    template <class Fill>
+    static DenseVecMatrix randomRows(long nRows, int nCols, int numPartitions, long seed, Fill fill) {
+        std::vector<int64_t> seeds(numPartitions);
+        check(mb_partition_seeds(seed, numPartitions, seeds.data()));
+        SubMatrix shard = rowShard(nRows, nCols);
+        long start = 0;
+        for (int p = 0; p < numPartitions; ++p) {
+            const long end = ((long)(p + 1) * nRows) / numPartitions;
+            if (end > start) {
+                SubMatrix view = shard.slice((int)start, (int)end, 0, nCols);
+                check(fill(view.handle(), seeds[p]));
+            }
+            start = end;
+        }
+        return DenseVecMatrix(rowIds(nRows), shard, nRows, nCols);
+    }
+    // randomSpaVecMatrix's partitions: fill(handle, seed) writes a partition's values and its one column set
+    template <class Fill>
+    static SparseVecMatrix randomSparseRows(long nRows, int nColumns, double density, int numPartitions, long seed, Fill fill) {
+        if (nRows <= 0 || nColumns <= 0 || numPartitions <= 0) throw std::invalid_argument("randomSpaVecMatrix: bad dimensions");
+        int32_t s = 0;
+        check(mb_sparse_column_count(nColumns, nColumns, density, &s));
+        std::vector<int64_t> seeds(numPartitions);
+        check(mb_partition_seeds(seed, numPartitions, seeds.data()));
+        std::vector<SparseVecMatrix::Row> rows;
+        long start = 0;
+        for (int p = 0; p < numPartitions; ++p) {
+            const long end = ((long)(p + 1) * nRows) / numPartitions;
+            if (end > start) {
+                mb_sparse* blk = nullptr;
+                check(mb_sparse_alloc(Context::get(), nColumns, (int)(end - start), (long)s * (end - start), &blk));
+                const int32_t rc = fill(blk, seeds[p]);
+                if (rc != MB_OK) { mb_sparse_free(Context::get(), blk); check(rc); }
+                std::vector<long> ids;
+                for (long i = start; i < end; ++i) ids.push_back(i);
+                SparseVecMatrix part = SparseVecMatrix::fromHandle(blk, ids, nRows, nColumns);
+                for (auto& r : part.rows_) rows.push_back(std::move(r));
+            }
+            start = end;
+        }
+        return SparseVecMatrix(std::move(rows), nRows, nColumns);
+    }
+    // randomBlockMatrix's blocks: fill(block, seed) writes block idx column-major from its seed
+    template <class Fill>
+    static BlockMatrix randomBlocks(long nRows, long nCols, int numByRow, int numByCol, long seed, Fill fill) {
+        const int brs = ceilLen(nRows, numByRow), bcs = ceilLen(nCols, numByCol);
+        const int byRow = (int)std::ceil((double)nRows / brs), byCol = (int)std::ceil((double)nCols / bcs);
+        std::vector<int64_t> seeds((size_t)byRow * byCol);
+        check(mb_partition_seeds(seed, byRow * byCol, seeds.data()));
+        BlockMatrix::Blocks blocks;
+        for (int idx = 0; idx < byRow * byCol; ++idx) {
+            int rows = brs, cols = bcs;
+            if (idx >= (byRow - 1) * byCol && (long)brs * byRow > nRows) rows = (int)(nRows - (long)brs * (byRow - 1));
+            if ((idx + 1) % byCol == 0 && (long)bcs * byCol > nCols) cols = (int)(nCols - (long)bcs * (byCol - 1));
+            SubMatrix blk = SubMatrix::empty(rows, cols);
+            check(fill(blk.handle(), seeds[idx]));
+            blocks.emplace_back(BlockID(idx / byCol, idx % byCol), blk);
+        }
+        return BlockMatrix(blocks, nRows, nCols, byRow, byCol);
+    }
     // the layout of the dense row generators on one process: rows 0 .. nRows-1 in one row-major shard
     static SubMatrix rowShard(long nRows, int nCols) { return SubMatrix::empty(nCols, (int)nRows).t(); }
     static std::vector<long> rowIds(long nRows) {
@@ -1623,45 +1686,29 @@ public:
     // take successive values of its stream (mb_fill_spvec_uniform)
     static SparseVecMatrix randomSpaVecMatrix(long nRows, int nColumns, double density, int numPartitions, long seed,
                                               double lo = 0.0, double hi = 1.0) {
-        if (nRows <= 0 || nColumns <= 0 || numPartitions <= 0) throw std::invalid_argument("randomSpaVecMatrix: bad dimensions");
-        int32_t s = 0;
-        check(mb_sparse_column_count(nColumns, nColumns, density, &s));
-        std::vector<int64_t> seeds(numPartitions);
-        check(mb_partition_seeds(seed, numPartitions, seeds.data()));
-        std::vector<SparseVecMatrix::Row> rows;
-        long start = 0;
-        for (int p = 0; p < numPartitions; ++p) {
-            const long end = ((long)(p + 1) * nRows) / numPartitions;
-            if (end > start) {
-                mb_sparse* blk = nullptr;
-                check(mb_sparse_alloc(Context::get(), nColumns, (int)(end - start), (long)s * (end - start), &blk));
-                const int32_t rc = mb_fill_spvec_uniform(Context::get(), blk, seeds[p], lo, hi);
-                if (rc != MB_OK) { mb_sparse_free(Context::get(), blk); check(rc); }
-                std::vector<long> ids;
-                for (long i = start; i < end; ++i) ids.push_back(i);
-                SparseVecMatrix part = SparseVecMatrix::fromHandle(blk, ids, nRows, nColumns);
-                for (auto& r : part.rows_) rows.push_back(std::move(r));
-            }
-            start = end;
-        }
-        return SparseVecMatrix(std::move(rows), nRows, nColumns);
+        return randomSparseRows(nRows, nColumns, density, numPartitions, seed, [&](mb_sparse* blk, int64_t s) {
+            return mb_fill_spvec_uniform(Context::get(), blk, s, lo, hi);
+        });
     }
-    // randomBlockMatrix (:34-50): one partition per block    // randomBlockMatrix (:34-50): one partition per block in row-major BlockID order, column-major fill
+    // ... with StandardNormalGenerator(mean, variance) values; the column set is drawn after the positions the values
+    // consumed (mb_fill_spvec_normal)
+    static SparseVecMatrix randomSpaVecMatrix(long nRows, int nColumns, double density, int numPartitions, long seed,
+                                              StandardNormalGenerator g) {
+        return randomSparseRows(nRows, nColumns, density, numPartitions, seed, [&](mb_sparse* blk, int64_t s) {
+            return mb_fill_spvec_normal(Context::get(), blk, s, g.mean, g.variance);
+        });
+    }
+    // randomBlockMatrix (:34-50): one partition per block in row-major BlockID order, column-major fill
     static BlockMatrix randomBlockMatrix(long nRows, long nCols, int numByRow, int numByCol, long seed, double lo = 0.0, double hi = 1.0) {
-        const int brs = ceilLen(nRows, numByRow), bcs = ceilLen(nCols, numByCol);
-        const int byRow = (int)std::ceil((double)nRows / brs), byCol = (int)std::ceil((double)nCols / bcs);
-        std::vector<int64_t> seeds((size_t)byRow * byCol);
-        check(mb_partition_seeds(seed, byRow * byCol, seeds.data()));
-        BlockMatrix::Blocks blocks;
-        for (int idx = 0; idx < byRow * byCol; ++idx) {
-            int rows = brs, cols = bcs;
-            if (idx >= (byRow - 1) * byCol && (long)brs * byRow > nRows) rows = (int)(nRows - (long)brs * (byRow - 1));
-            if ((idx + 1) % byCol == 0 && (long)bcs * byCol > nCols) cols = (int)(nCols - (long)bcs * (byCol - 1));
-            SubMatrix blk = SubMatrix::empty(rows, cols);
-            check(mb_fill_uniform(Context::get(), blk.handle(), seeds[idx], 0, lo, hi, 0));
-            blocks.emplace_back(BlockID(idx / byCol, idx % byCol), blk);
-        }
-        return BlockMatrix(blocks, nRows, nCols, byRow, byCol);
+        return randomBlocks(nRows, nCols, numByRow, numByCol, seed, [&](mb_block* b, int64_t s) {
+            return mb_fill_uniform(Context::get(), b, s, 0, lo, hi, 0);
+        });
+    }
+    // ... with StandardNormalGenerator(mean, variance) values
+    static BlockMatrix randomBlockMatrix(long nRows, long nCols, int numByRow, int numByCol, long seed, StandardNormalGenerator g) {
+        return randomBlocks(nRows, nCols, numByRow, numByCol, seed, [&](mb_block* b, int64_t s) {
+            return mb_fill_normal(Context::get(), b, s, g.mean, g.variance, 0, nullptr);
+        });
     }
     // randomBlockMatrix(..., sparseInfo = (true, density)) (:34-50, RandomRDD.scala:83-101, Matrices.scala:157-173): seeded
     // sparse blocks, s = (int)(block cols * density) per column (mb_fill_sparse_uniform); every block shape is checked first

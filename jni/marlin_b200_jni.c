@@ -135,6 +135,10 @@ NATIVE(void, fillUniform)(JNIEnv* e, jobject o, jlong ctx, jlong blk, jlong part
                           jboolean rowMajor) {
     raise(e, mb_fill_uniform(CTX(ctx), BLK(blk), partitionSeed, first, lo, hi, rowMajor ? 1 : 0));
 }
+NATIVE(void, fillNormal)(JNIEnv* e, jobject o, jlong ctx, jlong blk, jlong partitionSeed, jdouble mean, jdouble variance,
+                         jboolean rowMajor) {
+    raise(e, mb_fill_normal(CTX(ctx), BLK(blk), partitionSeed, mean, variance, rowMajor ? 1 : 0, NULL));
+}
 /* ---- f4: the Breeze/LAPACK leaves of luDecompose / choleskyDecompose / inverse (matrix/DenseVecMatrix.scala:283-764) ---- */
 NATIVE(void, lu)(JNIEnv* e, jobject o, jlong ctx, jlong a, jintArray permOut) {
     /* in place, dgetrf packing; permOut (rows entries) = the reference's permutation array: row i of L*U is row perm[i] of A */

@@ -112,6 +112,7 @@ SIGNATURES = {
                                    c_f64, c_f64, c_i32, C.c_void_p, C.c_void_p]),
     "mb_coo_to_dense_rows": (c_i32, [c_ctx, c_i64, C.c_void_p, C.c_void_p, C.c_void_p, c_blk]),
     "mb_fill_uniform": (c_i32, [c_ctx, c_blk, c_i64, c_i64, c_f64, c_f64, c_i32]),
+    "mb_fill_normal": (c_i32, [c_ctx, c_blk, c_i64, c_f64, c_f64, c_i32, C.POINTER(c_i64)]),
     "mb_sparse_check": (c_i32, [c_i32, c_i32, C.c_void_p, C.c_void_p]),
     "mb_sparse_wrap": (c_i32, [c_ctx, c_i32, c_i32, c_i64, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(c_sp)]),
     "mb_sparse_upload": (c_i32, [c_ctx, c_i32, c_i32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(c_sp)]),
@@ -132,6 +133,7 @@ SIGNATURES = {
     "mb_spvec_coo": (c_i32, [c_ctx, c_sp, C.c_void_p, C.c_void_p, C.c_void_p]),
     "mb_dense_rows_to_sparse": (c_i32, [c_ctx, c_blk, C.POINTER(c_sp)]),
     "mb_fill_spvec_uniform": (c_i32, [c_ctx, c_sp, c_i64, c_f64, c_f64]),
+    "mb_fill_spvec_normal": (c_i32, [c_ctx, c_sp, c_i64, c_f64, c_f64]),
     "mb_pagerank_links": (c_i32, [c_i32, c_i64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, c_i32, c_i32, c_f64, C.c_void_p,
                                   C.c_void_p, C.c_void_p, C.POINTER(c_i64)]),
     "mb_pagerank_step": (c_i32, [c_ctx, c_sp, c_blk, c_i64, c_f64, c_blk]),

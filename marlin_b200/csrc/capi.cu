@@ -17,6 +17,7 @@
 #include "mlp.h"
 #include "norm.h"
 #include "eigs.h"
+#include "normal.h"
 
 #include <cuda_runtime.h>
 #include <climits>
@@ -1978,6 +1979,34 @@ int32_t mb_fill_uniform(mb_ctx* ctx, mb_block* blk, int64_t partition_seed, int6
     return MB_OK;
 }
 
+static_assert(MB_NORMAL_TILE_ATTEMPTS == mb::NORMAL_TILE_ATTEMPTS, "the documented tile size is the kernels' tile size");
+
+// generator.setSeed(partition.seed) and Array.fill(n)(nextValue()) of StandardNormalGenerator into an fp64 view; the counted
+// attempts may reach `extra` positions short of the jump tables' 2^39 (room for what the caller draws after the values)
+static int32_t fill_normal(mb_ctx* ctx, double* out, long long rs, long long cs, int rows, int cols, int row_major,
+                           int64_t partition_seed, double mean, double variance, long long extra, int64_t* positions,
+                           const char* what) {
+    const unsigned long long state0 = (unsigned long long)mb_hash_seed(partition_seed);
+    long long attempts = 0;
+    const cudaError_t e = mb::fill_normal_f64(out, rs, cs, rows, cols, row_major, state0, mean, std::sqrt(variance),
+                                              (1LL << 39) - 1 - extra, positions ? &attempts : nullptr, ctx->stream);
+    if (e == cudaErrorInvalidValue)
+        return fail(MB_ERR_UNSUPPORTED, "%s: %dx%d values exceed the generator's 2^39 stream positions", what, rows, cols);
+    if (e != cudaSuccess) return cuda_fail(e, what);
+    if (positions) *positions = 2 * attempts;
+    return MB_OK;
+}
+
+int32_t mb_fill_normal(mb_ctx* ctx, mb_block* blk, int64_t partition_seed, double mean, double variance, int32_t row_major,
+                       int64_t* positions_out) {
+    MB_CTX(ctx);
+    if (positions_out) *positions_out = 0;
+    if (!blk) return fail(MB_ERR_INVALID_ARG, "mb_fill_normal: bad argument");
+    if (blk->dtype != MB_F64) return fail(MB_ERR_UNSUPPORTED, "mb_fill_normal: fp64 blocks only (convert afterwards)");
+    return fill_normal(ctx, f64_ptr(blk), rs(blk), cs(blk), blk->rows, blk->cols, row_major ? 1 : 0, partition_seed, mean,
+                       variance, 0, positions_out, "mb_fill_normal");
+}
+
 // ------------------------------------------------------------------------------------------- sparse blocks (SURVEY 8 f6)
 static mb::CscView csc(const mb_sparse* S) { return mb::CscView{S->rows, S->cols, S->colptr, S->rowidx, S->values}; }
 static mb::DView dview(const mb_block* b) { return mb::DView{f64_ptr(b), rs(b), cs(b)}; }
@@ -2290,6 +2319,29 @@ int32_t mb_fill_spvec_uniform(mb_ctx* ctx, mb_sparse* S, int64_t partition_seed,
     MB_CUDA(mb::fill_uniform_f64(S->values, 1, S->nnz, (int)S->nnz, 1, 0, state0, 0, lo, hi, ctx->stream));
     // row 0's columns: one "column" of the sampler over nColumns positions, from position s*P
     MB_CUDA(mb::sparse_sample_rows(S->rows, 1, s, state0, S->nnz, S->colptr, S->rowidx, ctx->stream));
+    MB_CUDA(mb::spvec_replicate_columns(S->cols, s, S->colptr, S->rowidx, ctx->stream));
+    return MB_OK;
+}
+
+int32_t mb_fill_spvec_normal(mb_ctx* ctx, mb_sparse* S, int64_t partition_seed, double mean, double variance) {
+    MB_CTX(ctx);
+    if (!S) return fail(MB_ERR_INVALID_ARG, "mb_fill_spvec_normal: null block");
+    if (S->cols == 0 || S->nnz == 0) {
+        if (S->nnz != 0) return fail(MB_ERR_INVALID_ARG, "mb_fill_spvec_normal: %lld non-zeros in 0 rows", (long long)S->nnz);
+        MB_CUDA(cudaMemsetAsync(S->colptr, 0, sizeof(int) * ((size_t)S->cols + 1), ctx->stream));     // s = 0: empty rows
+        return MB_OK;
+    }
+    if (S->nnz % S->cols != 0)
+        return fail(MB_ERR_INVALID_ARG, "mb_fill_spvec_normal: nnz %lld is not a multiple of %d rows", (long long)S->nnz, S->cols);
+    const int s = (int)(S->nnz / S->cols);
+    if (s > S->rows) return fail(MB_ERR_INVALID_ARG, "mb_fill_spvec_normal: %d columns per row of %d", s, S->rows);
+    int64_t positions = 0;
+    const int32_t r = fill_normal(ctx, S->values, 1, S->nnz, (int)S->nnz, 1, 0, partition_seed, mean, variance, S->rows,
+                                  &positions, "mb_fill_spvec_normal");
+    if (r) return r;
+    // row 0's columns: one "column" of the sampler over nColumns positions, from the first position the values left
+    const unsigned long long state0 = (unsigned long long)mb_hash_seed(partition_seed);
+    MB_CUDA(mb::sparse_sample_rows(S->rows, 1, s, state0, positions, S->colptr, S->rowidx, ctx->stream));
     MB_CUDA(mb::spvec_replicate_columns(S->cols, s, S->colptr, S->rowidx, ctx->stream));
     return MB_OK;
 }

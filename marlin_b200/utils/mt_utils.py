@@ -103,6 +103,46 @@ class UniformGenerator:
         self.start, self.end = float(start), float(end)
 
 
+class StandardNormalGenerator:
+    """utils/RandomDataGenerator.scala:70-82 — mean + sqrt(variance) * nextGaussian() over XORShiftRandom, bit-exact
+    (mb_fill_normal).  A negative or NaN variance gives NaN values, as math.sqrt does on the JVM."""
+
+    def __init__(self, mean: float = 0.0, variance: float = 1.0):
+        self.mean, self.variance = float(mean), float(variance)
+
+
+class ZerosGenerator:
+    """utils/RandomDataGenerator.scala:29-38 — every value 0.0."""
+
+
+class OnesGenerator:
+    """utils/RandomDataGenerator.scala:40-49 — every value 1.0."""
+
+
+class PoissonGenerator:
+    """utils/RandomDataGenerator.scala:89-101 — Colt's Poisson over DRand.  Not generated here: it calls Math.exp and
+    Math.log, which the JVM does not specify bit for bit, so there is no value to match; every generator rejects it."""
+
+    def __init__(self, mean: float):
+        self.mean = float(mean)
+
+
+def _check_distribution(dist, what: str, sparse: bool = False) -> None:
+    """MB_ERR_UNSUPPORTED naming the generator, before anything is generated (every rank raises together)."""
+    if isinstance(dist, (UniformGenerator, StandardNormalGenerator)):
+        return
+    name = type(dist).__name__
+    if isinstance(dist, (ZerosGenerator, OnesGenerator)):
+        if not sparse:
+            return
+        raise nat.MarlinArgumentError(nat.MB_ERR_UNSUPPORTED, f"{what}: {name} is not supported for sparse rows (every "
+                                      "stored value would be the same constant)")
+    if isinstance(dist, PoissonGenerator):
+        raise nat.MarlinArgumentError(nat.MB_ERR_UNSUPPORTED, f"{what}: PoissonGenerator is not supported (Colt's Poisson "
+                                      "calls Math.exp / Math.log, which have no bit-exact definition)")
+    raise nat.MarlinArgumentError(nat.MB_ERR_UNSUPPORTED, f"{what}: unsupported distribution {name}")
+
+
 def _svm_vector(items, vectorLen: int) -> np.ndarray:
     """The `i:v` entries of one SVM-format line as a dense vector: entry i sets element i - 1 (a later entry for the same
     index wins); an index outside 1..vectorLen is rejected (ArrayIndexOutOfBoundsException on the JVM)."""
@@ -130,9 +170,17 @@ class MTUtils:
         return [int(v) for v in out]
 
     @staticmethod
-    def _fill(blk: SubMatrix, partition_seed: int, first: int, dist: UniformGenerator, row_major: bool) -> None:
+    def _fill(blk: SubMatrix, partition_seed: int, first: int, dist, row_major: bool) -> None:
+        """generator.setSeed(partition_seed) and blk's values in fill order (rdd/RandomRDD.scala:70-112), the uniform
+        stream from value `first` on; the normal stream always starts at its first value, and Zeros and Ones draw
+        nothing."""
         rt = Runtime.get(); rt.sync_stream()
-        nat.check(rt.lib.mb_fill_uniform(rt.ctx, blk.handle(), partition_seed, first, dist.start, dist.end, int(row_major)))
+        if isinstance(dist, UniformGenerator):
+            nat.check(rt.lib.mb_fill_uniform(rt.ctx, blk.handle(), partition_seed, first, dist.start, dist.end, int(row_major)))
+        elif isinstance(dist, StandardNormalGenerator):
+            nat.check(rt.lib.mb_fill_normal(rt.ctx, blk.handle(), partition_seed, dist.mean, dist.variance, int(row_major), None))
+        else:
+            nat.check(rt.lib.mb_block_fill(rt.ctx, blk.handle(), 1.0 if isinstance(dist, OnesGenerator) else 0.0))
 
     @staticmethod
     def _sparse_block(rows: int, cols: int, density: float, partition_seed: int) -> SubMatrix:
@@ -145,13 +193,15 @@ class MTUtils:
     # ------------------------------------------------------------------ generators
     @staticmethod
     def randomDenVecMatrix(sc, nRows: int, nColumns: int, numPartitions: int = 0,
-                           distribution: Optional[UniformGenerator] = None, seed: Optional[int] = None) -> DenseVecMatrix:
+                           distribution=None, seed: Optional[int] = None) -> DenseVecMatrix:
         """utils/MTUtils.scala:63-73 -> RandomDenVecRDD (rdd/RandomRDD.scala:161-182).  Partition p holds rows
         [p*N/P, (p+1)*N/P) (:38-41) and is generated on the GPU that owns it (rank p mod G) from the p-th
         nextLong of java.util.Random(seed); values are bit-identical to the reference's XORShift stream for the
         same seed.  The reference's seed is System.nanoTime() and is not exposed (MTUtils.scala:63-73); the extra
-        `seed` keyword makes runs reproducible."""
+        `seed` keyword makes runs reproducible.  `distribution`: UniformGenerator (the default U[0, 1)),
+        StandardNormalGenerator, ZerosGenerator or OnesGenerator."""
         dist_ = distribution or UniformGenerator(0.0, 1.0)
+        _check_distribution(dist_, "randomDenVecMatrix")
         if seed is None:
             seed = time.time_ns()
         P, shards, ids_arr, data = MTUtils._row_shard(nRows, nColumns, numPartitions)
@@ -232,14 +282,18 @@ class MTUtils:
 
     @staticmethod
     def randomSpaVecMatrix(sc, nRows: int, nColumns: int, density: float, numPartitions: int = 0,
-                           distribution: Optional[UniformGenerator] = None, seed: Optional[int] = None) -> SparseVecMatrix:
+                           distribution=None, seed: Optional[int] = None) -> SparseVecMatrix:
         """utils/MTUtils.scala:75-85 -> RandomSpaVecRDD (rdd/RandomRDD.scala:47-65, 136-159): the partitions, seeds and rank
         placement of randomDenVecMatrix.  Every row of partition p has the same s = (int)(nColumns * density) sorted columns
         and takes the next s values of the partition's stream, bit-identical to randomDenVecMatrix's values at the same
         stream positions.  The reference draws the column set from an unseeded java.util.Random; here it is drawn by
         selection sampling from the same stream, after the values (mb_fill_spvec_uniform), so it is a function of
-        (seed, partition).  density <= 0 and s > nColumns (where the reference never ends) are rejected."""
+        (seed, partition).  density <= 0 and s > nColumns (where the reference never ends) are rejected.
+        `distribution`: UniformGenerator or StandardNormalGenerator (mb_fill_spvec_normal: the values are the first s
+        values of each row from the partition's normal stream, the column set is drawn right after the positions they
+        consumed)."""
         dist_ = distribution or UniformGenerator(0.0, 1.0)
+        _check_distribution(dist_, "randomSpaVecMatrix", sparse=True)
         if nRows <= 0 or nColumns <= 0:
             raise nat.MarlinArgumentError(nat.MB_ERR_INVALID_ARG, f"randomSpaVecMatrix: {nRows} x {nColumns}")
         s = column_count(nColumns, nColumns, density)
@@ -261,7 +315,10 @@ class MTUtils:
             end = ((p + 1) * nRows) // P
             if p % ws == rank and end > start:
                 blk = SparseBlock.empty(nColumns, end - start, s * (end - start))
-                nat.check(rt.lib.mb_fill_spvec_uniform(rt.ctx, blk.handle(), seeds[p], dist_.start, dist_.end))
+                if isinstance(dist_, UniformGenerator):
+                    nat.check(rt.lib.mb_fill_spvec_uniform(rt.ctx, blk.handle(), seeds[p], dist_.start, dist_.end))
+                else:
+                    nat.check(rt.lib.mb_fill_spvec_normal(rt.ctx, blk.handle(), seeds[p], dist_.mean, dist_.variance))
                 ids.append(np.arange(start, end, dtype=np.int64))
                 rps.append(blk.colptr[(1 if rps else 0):] + base)
                 cis.append(blk.rowidx)
@@ -278,8 +335,7 @@ class MTUtils:
 
     @staticmethod
     def randomBlockMatrix(sc, nRows: int, nColumns: int, numByRow: int, numByCol: int, sparseInfo=(False, 1.0),
-                          distribution: Optional[UniformGenerator] = None, seed: Optional[int] = None,
-                          dtype: int = nat.MB_F64) -> BlockMatrix:
+                          distribution=None, seed: Optional[int] = None, dtype: int = nat.MB_F64) -> BlockMatrix:
         """utils/MTUtils.scala:34-50 -> RandomBlockRDD (rdd/RandomRDD.scala:184-223): one partition per block in
         row-major BlockID order, `BDM.create(rows, cols, Array.fill(rows*cols)(nextValue()))` (column-major).
 
@@ -288,7 +344,8 @@ class MTUtils:
         so its blocks change on every run; here block b is a function of (seed, b) alone: its values are positions
         [0, s*cols) of the same XORShift stream the dense generator gives that block, and its rows come from selection
         sampling over the next rows*cols positions (mb_fill_sparse_uniform).  density <= 0 and s > block rows are
-        rejected; so is a `distribution`, which the reference ignores for sparse blocks."""
+        rejected; so is a `distribution`, which the reference ignores for sparse blocks.  Dense blocks take
+        randomDenVecMatrix's distributions, filled in fp64 and converted to `dtype` afterwards."""
         sparse, density = bool(sparseInfo[0]), float(sparseInfo[1])
         if sparse and distribution is not None:
             raise nat.MarlinArgumentError(nat.MB_ERR_INVALID_ARG, "sparse blocks always draw U[0,1) values: the "
@@ -296,6 +353,7 @@ class MTUtils:
         if sparse and dtype != nat.MB_F64:
             raise nat.MarlinArgumentError(nat.MB_ERR_UNSUPPORTED, "sparse blocks are fp64 only")
         dist_ = distribution or UniformGenerator(0.0, 1.0)
+        _check_distribution(dist_, "randomBlockMatrix")
         brs = int(math.ceil(float(nRows) / float(numByRow)))
         bcs = int(math.ceil(float(nColumns) / float(numByCol)))
         by_row, by_col = int(math.ceil(nRows / brs)), int(math.ceil(nColumns / bcs))
@@ -334,13 +392,13 @@ class MTUtils:
         return BlockMatrix(blocks, nRows, nColumns, by_row, by_col, sparse=sparse)
 
     @staticmethod
-    def randomDistVector(sc, length: int, numSplits: int, distribution: Optional[UniformGenerator] = None,
-                         seed: Optional[int] = None):
+    def randomDistVector(sc, length: int, numSplits: int, distribution=None, seed: Optional[int] = None):
         """utils/MTUtils.scala:86-93 -> RandomDistVectorRDD (rdd/RandomRDD.scala:116-134,103-112): one partition per
         piece, piece i = the first splitLength values of the stream seeded with the i-th nextLong of Random(seed);
-        the last piece takes the remainder."""
+        the last piece takes the remainder.  `distribution` as in randomDenVecMatrix."""
         from ..matrix.distributed_vector import DistributedVector
         dist_ = distribution or UniformGenerator(0.0, 1.0)
+        _check_distribution(dist_, "randomDistVector")
         if seed is None:
             seed = time.time_ns()
         seeds = MTUtils._partition_seeds(seed, numSplits)

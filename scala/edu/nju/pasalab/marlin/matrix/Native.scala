@@ -44,6 +44,8 @@ object Native {
   @native def ger(ctx: Long, x: Long, y: Long, out: Long): Unit
   @native def fillUniform(ctx: Long, blk: Long, partitionSeed: Long, first: Long, lo: Double, hi: Double,
                           rowMajor: Boolean): Unit
+  // StandardNormalGenerator(mean, variance) values of a partition stream (mb_fill_normal)
+  @native def fillNormal(ctx: Long, blk: Long, partitionSeed: Long, mean: Double, variance: Double, rowMajor: Boolean): Unit
   @native def setFp64Mode(ctx: Long, mode: Int, slices: Int): Unit
 
   // the Breeze/LAPACK leaves of luDecompose / choleskyDecompose / inverse (brzLU, brzCholesky, brzInv, `\`)

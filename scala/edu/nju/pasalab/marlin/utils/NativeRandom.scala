@@ -29,6 +29,22 @@ private[marlin] object NativeRandom {
     new SubMatrix(blk, vectorSize, size).t                             // seen as size x vectorSize, no copy
   }
 
+  /** `uniformBlock` with `StandardNormalGenerator(mean, variance)` (utils/RandomDataGenerator.scala:70-82): the block's
+   *  values are mean + sqrt(variance) * nextGaussian() of its partition stream, bit for bit (`mb_fill_normal`). */
+  def normalBlock(partitionSeed: Long, blockRows: Int, blockCols: Int, mean: Double = 0.0, variance: Double = 1.0): SubMatrix = {
+    val blk = Native.alloc(Ctx.get, blockRows, blockCols, Native.F64)
+    Native.fillNormal(Ctx.get, blk, partitionSeed, mean, variance, false)
+    new SubMatrix(blk, blockRows, blockCols)
+  }
+
+  /** `uniformRows` with `StandardNormalGenerator(mean, variance)`: one stream across the partition's rows, so a pair of
+   *  Gaussians may straddle two rows, as `Array.fill` in `RandomDenVecRDD.compute` draws them. */
+  def normalRows(partitionSeed: Long, size: Int, vectorSize: Int, mean: Double = 0.0, variance: Double = 1.0): SubMatrix = {
+    val blk = Native.alloc(Ctx.get, vectorSize, size, Native.F64)          // column j of the block = row j of the shard
+    Native.fillNormal(Ctx.get, blk, partitionSeed, mean, variance, false)
+    new SubMatrix(blk, vectorSize, size).t                             // seen as size x vectorSize, no copy
+  }
+
   /** A sparse block of `MTUtils.randomBlockMatrix(..., sparseInfo = (true, density))` (RandomRDD.scala:97-99,
    *  SparseMatrix.rand, Matrices.scala:157-173), seeded: s = (blockCols * density).toInt rows per column (density <= 0
    *  and s > blockRows are IllegalArgumentException), values from the block's partition stream, rows by selection
