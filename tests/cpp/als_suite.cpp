@@ -3,6 +3,7 @@
 // toDenseVecMatrix with its duplicate check, the coordinate-file loader, and the argument errors.  Exits 3 without a GPU
 // (there is no CPU fallback), 1 on a failed check.
 #include "marlin_b200.hpp"
+#include "suite.h"
 
 #include <cmath>
 #include <cstdio>
@@ -11,21 +12,8 @@
 
 using namespace marlin;
 
-static int failed = 0;
-#define CHECK(c) do { if (!(c)) { std::printf("FAILED %s:%d: %s\n", __FILE__, __LINE__, #c); ++failed; } } while (0)
-
-template <class F> static bool throws(F f) {
-    try { f(); } catch (const std::exception&) { return true; }
-    return false;
-}
-
 int main() {
-    try {
-        Context::get();
-    } catch (const std::exception& e) {
-        std::printf("cannot initialise marlin_b200: %s\n", e.what());
-        return 3;
-    }
+    if (!require_gpu()) return 3;
     const long r[] = {0, 0, 1, 1, 2, 2, 3, 3, 4, 4, 0, 2, 5, 5, 1, 3};
     const long c[] = {0, 1, 1, 2, 0, 3, 2, 3, 1, 4, 4, 2, 0, 3, 4, 0};
     const float v[] = {5, 3, 4, 1, 2, 5, 3.5f, 4, 1, 2, 2.5f, 3, 4, 1.5f, 5, 2};
@@ -87,6 +75,5 @@ int main() {
     CHECK(throws([&] { m.ALS(129, 1, 0.1, 2, 3, false, 1.0, 7); }));
     CHECK(throws([&] { m.ALS(3, 1, -1.0, 2, 3, false, 1.0, 7); }));
     CHECK(throws([] { CoordinateMatrix({}).ALS(3, 1, 0.1, 2, 3, false, 1.0, 7); }));
-    std::printf("als suite: %d failed checks\n", failed);
-    return failed ? 1 : 0;
+    return finish("als suite");
 }

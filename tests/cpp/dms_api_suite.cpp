@@ -3,6 +3,7 @@
 // include/marlin_b200.hpp.  Every expected value is a small integer, so assertions are exact.  Needs an H100; without one
 // the first call throws the library's "no CPU fallback" error and the program exits with status 3.
 #include "marlin_b200.hpp"
+#include "suite.h"
 
 #include <cmath>
 #include <cstdio>
@@ -12,22 +13,17 @@
 using namespace marlin;
 using BDM = DenseMatrix;
 
-static int failures = 0, passed = 0;
-#define CHECK(cond)                                                              \
-    do {                                                                         \
-        if (!(cond)) { std::printf("  FAILED %s:%d  %s\n", __FILE__, __LINE__, #cond); ++failures; } \
-    } while (0)
-
 template <class F>
 static std::string invalidArgument(F f) {
     try { f(); } catch (const std::invalid_argument& e) { return e.what(); } catch (...) { return "<other exception>"; }
     return "<no exception>";
 }
+static int passed = 0;
 static void test(const char* name, const std::function<void()>& body) {
-    const int before = failures;
-    try { body(); } catch (const std::exception& e) { std::printf("  EXCEPTION in '%s': %s\n", name, e.what()); ++failures; }
-    if (failures == before) ++passed;
-    std::printf("[%s] %s\n", failures == before ? " ok " : "FAIL", name);
+    const int before = failed;
+    try { body(); } catch (const std::exception& e) { std::printf("  EXCEPTION in '%s': %s\n", name, e.what()); ++failed; }
+    if (failed == before) ++passed;
+    std::printf("[%s] %s\n", failed == before ? " ok " : "FAIL", name);
 }
 
 // DMS.scala:15-19 — rows deliberately out of order
@@ -66,12 +62,7 @@ static BDM tile(const BDM& a, int down, int across) {
 }
 
 int main() {
-    try {
-        Context::get();
-    } catch (const std::exception& e) {
-        std::printf("cannot initialise marlin_b200: %s\n", e.what());
-        return 3;
-    }
+    if (!require_gpu()) return 3;
     const BDM dense{{0.0, 1.0, 2.0, 3.0}, {2.0, 3.0, 4.0, 5.0}, {3.0, 2.0, 1.0, 0.0}, {1.0, 1.0, 1.0, 1.0}};
 
     test("slice the matrix", [&] {                                                // :207-223
@@ -173,6 +164,6 @@ int main() {
         CHECK(invalidArgument([&] { mat.norm("2"); }) == "Do not support mode 2.");
     });
 
-    std::printf("%d passed, %d failed\n", passed, failures);
-    return failures == 0 ? 0 : 1;
+    std::printf("%d tests passed\n", passed);
+    return finish("dms_api suite");
 }

@@ -4,6 +4,7 @@
 // integers, so assertions are exact).  Needs an H100; without one the first call throws the library's
 // "no CPU fallback" error and the program exits with status 3.
 #include "marlin_b200.hpp"
+#include "suite.h"
 
 #include <cstdio>
 #include <functional>
@@ -12,22 +13,12 @@
 using namespace marlin;
 using BDM = DenseMatrix;
 
-static int failures = 0, passed = 0;
-#define CHECK(cond)                                                              \
-    do {                                                                         \
-        if (!(cond)) { std::printf("  FAILED %s:%d  %s\n", __FILE__, __LINE__, #cond); ++failures; } \
-    } while (0)
-
-template <class Ex, class F>
-static bool throws(F f) {
-    try { f(); } catch (const Ex&) { return true; } catch (...) { return false; }
-    return false;
-}
+static int passed = 0;
 static void test(const char* name, const std::function<void()>& body) {
-    const int before = failures;
-    try { body(); } catch (const std::exception& e) { std::printf("  EXCEPTION in '%s': %s\n", name, e.what()); ++failures; }
-    if (failures == before) ++passed;
-    std::printf("[%s] %s\n", failures == before ? " ok " : "FAIL", name);
+    const int before = failed;
+    try { body(); } catch (const std::exception& e) { std::printf("  EXCEPTION in '%s': %s\n", name, e.what()); ++failed; }
+    if (failed == before) ++passed;
+    std::printf("[%s] %s\n", failed == before ? " ok " : "FAIL", name);
 }
 
 // DMS.scala:15-24 — the shared fixture: rows deliberately out of order; the same matrix as a 2x2 grid of 2x2 blocks
@@ -45,12 +36,7 @@ static bool contains(BlockMatrix& m, BlockID id, const BDM& expected) {
 }
 
 int main() {
-    try {
-        Context::get();
-    } catch (const std::exception& e) {
-        std::printf("cannot initialise marlin_b200: %s\n", e.what());
-        return 3;
-    }
+    if (!require_gpu()) return 3;
     const BDM expectedDense{{0.0, 1.0, 2.0, 3.0}, {2.0, 3.0, 4.0, 5.0}, {3.0, 2.0, 1.0, 0.0}, {1.0, 1.0, 1.0, 1.0}};
     const BDM expectedProduct{{11.0, 10.0, 9.0, 8.0}, {23.0, 24.0, 25.0, 26.0}, {7.0, 11.0, 15.0, 19.0}, {6.0, 7.0, 8.0, 9.0}};
 
@@ -259,6 +245,6 @@ int main() {
         CHECK(p.transpose().toBreeze() == rb.toBreeze());
     });
 
-    std::printf("%d passed, %d failed checks\n", passed, failures);
-    return failures ? 1 : 0;
+    std::printf("%d tests passed\n", passed);
+    return finish("dms suite");
 }

@@ -2,6 +2,7 @@
 // small tall matrix against the four-argument overload's Gramian and Jacobi path.  Exits 3 without a GPU (there is no
 // CPU fallback), 1 on a failed check.
 #include "marlin_b200.hpp"
+#include "suite.h"
 
 #include <cmath>
 #include <cstdio>
@@ -9,16 +10,8 @@
 
 using namespace marlin;
 
-static int failed = 0;
-#define CHECK(c) do { if (!(c)) { std::printf("FAILED %s:%d: %s\n", __FILE__, __LINE__, #c); ++failed; } } while (0)
-
 int main() {
-    try {
-        Context::get();
-    } catch (const std::exception& e) {
-        std::printf("cannot initialise marlin_b200: %s\n", e.what());
-        return 3;
-    }
+    if (!require_gpu()) return 3;
     std::mt19937_64 gen(17);
     std::normal_distribution<double> nd;
     std::vector<DenseVecMatrix::Row> tall;
@@ -45,6 +38,5 @@ int main() {
     std::string msg;
     try { big.computeSVD(8, false, 1e-9, 0, 1e-10, "dist-eigs"); } catch (const std::invalid_argument& e) { msg = e.what(); }
     CHECK(msg.rfind("ARPACK returns non-zero info = -4", 0) == 0);
-    std::printf("eigs suite: %d failed checks\n", failed);
-    return failed ? 1 : 0;
+    return finish("eigs suite");
 }

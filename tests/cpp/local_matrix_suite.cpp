@@ -3,13 +3,11 @@
 // toDenseBlocks, a sparse BlockMatrix multiply and the sparse generator's checks.  Exits 3 without a GPU (there is no CPU
 // fallback), 1 on a failed check.
 #include "marlin_b200.hpp"
+#include "suite.h"
 
 #include <cstdio>
 
 using namespace marlin;
-
-static int failed = 0;
-#define CHECK(c) do { if (!(c)) { std::printf("FAILED %s:%d: %s\n", __FILE__, __LINE__, #c); ++failed; } } while (0)
 
 template <class F> static bool throwsInvalid(F f, const char* needle) {
     try { f(); } catch (const std::invalid_argument& e) { return std::string(e.what()).find(needle) != std::string::npos; }
@@ -17,12 +15,7 @@ template <class F> static bool throwsInvalid(F f, const char* needle) {
 }
 
 int main() {
-    try {
-        Context::get();
-    } catch (const std::exception& e) {
-        std::printf("cannot initialise marlin_b200: %s\n", e.what());
-        return 3;
-    }
+    if (!require_gpu()) return 3;
     const SparseMatrix spMat(4, 4, {SparseVector(4, {1}, {1.0}), SparseVector(4, {0, 3}, {2.0, 1.0}), SparseVector(4, {0}, {3.0}),
                                     SparseVector(4, {2}, {4.0})});
     const DenseMatrix deMat{{0.0, 1.0, 2.0, 3.0}, {2.0, 3.0, 4.0, 5.0}, {3.0, 2.0, 1.0, 0.0}, {1.0, 1.0, 1.0, 1.0}};
@@ -73,6 +66,5 @@ int main() {
     }
     CHECK(throwsInvalid([] { MTUtils::randomBlockMatrix(10, 200, 1, 1, {true, 0.1}, 1); }, "non-zeros per column asked"));
     CHECK(throwsInvalid([] { MTUtils::randomBlockMatrix(10, 10, 1, 1, {true, 0.0}, 1); }, "must be positive"));
-    std::printf("local_matrix_suite: %d failed checks\n", failed);
-    return failed ? 1 : 0;
+    return finish("local_matrix_suite");
 }

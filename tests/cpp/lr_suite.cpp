@@ -2,15 +2,13 @@
 // 50-step run against a host restatement of :1005-1035, and the empty matrix.  Exits 3 without a GPU (there is no CPU
 // fallback), 1 on a failed check.
 #include "marlin_b200.hpp"
+#include "suite.h"
 
 #include <cmath>
 #include <cstdio>
 #include <random>
 
 using namespace marlin;
-
-static int failed = 0;
-#define CHECK(c) do { if (!(c)) { std::printf("FAILED %s:%d: %s\n", __FILE__, __LINE__, #c); ++failed; } } while (0)
 
 // :1005-1035 on the host, rows in order, no FMA contraction in the expressions that matter (volatile temporaries)
 static std::vector<double> host_lr(const std::vector<DenseVecMatrix::Row>& rows, long dataSize, double step, int iters) {
@@ -31,12 +29,7 @@ static std::vector<double> host_lr(const std::vector<DenseVecMatrix::Row>& rows,
 }
 
 int main() {
-    try {
-        Context::get();
-    } catch (const std::exception& e) {
-        std::printf("cannot initialise marlin_b200: %s\n", e.what());
-        return 3;
-    }
+    if (!require_gpu()) return 3;
     // dyadic features, labels 0 / 1, 64 rows: the first step is exact in any summation order
     std::mt19937_64 gen(3);
     std::vector<DenseVecMatrix::Row> rows;
@@ -62,13 +55,8 @@ int main() {
     const std::vector<double> gw = g.lr(1.0, 1), gwant = host_lr(gap, 10, 1.0, 1);
     CHECK(gw[0] == gwant[0] && gw[1] == gwant[1]);
     // rows of another width than numCols(): an error, not a w of the wrong size
-    bool wide = false;
-    try { DenseVecMatrix(rows, 0, 5).lr(1.0, 1); } catch (const std::invalid_argument&) { wide = true; }
-    CHECK(wide);
+    CHECK(throws<std::invalid_argument>([&] { DenseVecMatrix(rows, 0, 5).lr(1.0, 1); }));
     // the empty matrix
-    bool threw = false;
-    try { DenseVecMatrix(std::vector<DenseVecMatrix::Row>{}, 0, 0).lr(1.0, 1); } catch (const std::runtime_error&) { threw = true; }
-    CHECK(threw);
-    std::printf("lr suite: %d failed checks\n", failed);
-    return failed ? 1 : 0;
+    CHECK(throws<std::runtime_error>([] { DenseVecMatrix(std::vector<DenseVecMatrix::Row>{}, 0, 0).lr(1.0, 1); }));
+    return finish("lr suite");
 }

@@ -5,26 +5,14 @@
 // D2(r, j) = 0.125 (-0.125 at the label), E1(r, h) = s_h t_r with s = (1, -1) and t_r = 0.125 (sum(v) - 2 v[y_r]),
 // D1 = 0.25 E1.  Every product and sum below is exact in binary floating point.
 #include "marlin_b200.hpp"
+#include "suite.h"
 
 #include <cstdio>
 
 using namespace marlin;
 
-static int failed = 0;
-#define CHECK(c) do { if (!(c)) { std::printf("FAILED %s:%d: %s\n", __FILE__, __LINE__, #c); ++failed; } } while (0)
-
-template <class F> static bool throws(F f) {
-    try { f(); } catch (const std::exception&) { return true; }
-    return false;
-}
-
 int main() {
-    try {
-        Context::get();
-    } catch (const std::exception& e) {
-        std::printf("cannot initialise marlin_b200: %s\n", e.what());
-        return 3;
-    }
+    if (!require_gpu()) return 3;
     DenseMatrix W1{{1.0, 2.0}, {-1.0, -2.0}}, W2(2, 10);
     double vsum = 0.0;
     for (int j = 0; j < 10; ++j) { W2(0, j) = j + 1.0; W2(1, j) = -(j + 1.0); vsum += j + 1.0; }
@@ -60,6 +48,5 @@ int main() {
     examples::NeuralNetwork narrow(DenseMatrix(3, 2), W2);
     narrow.addBlock(DenseMatrix(2, 2), {1, 2});
     CHECK(throws([&] { narrow.step({0}, 1.0, 4); }));                           // 2 features against 3 weight rows
-    std::printf("%d failed checks\n", failed);
-    return failed ? 1 : 0;
+    return finish("nn suite");
 }

@@ -3,27 +3,15 @@
 // tests/test_cpp_pagerank.py ("piece float-bits" per line) for the test to compare with the Python API bit for bit.
 // Exits 3 without a GPU (there is no CPU fallback), 1 on a failed check.
 #include "marlin_b200.hpp"
+#include "suite.h"
 
 #include <cstdio>
 #include <cstring>
 
 using namespace marlin;
 
-static int failed = 0;
-#define CHECK(c) do { if (!(c)) { std::printf("FAILED %s:%d: %s\n", __FILE__, __LINE__, #c); ++failed; } } while (0)
-
-template <class F> static bool throws(F f) {
-    try { f(); } catch (const std::exception&) { return true; }
-    return false;
-}
-
 int main(int argc, char** argv) {
-    try {
-        Context::get();
-    } catch (const std::exception& e) {
-        std::printf("cannot initialise marlin_b200: %s\n", e.what());
-        return 3;
-    }
+    if (!require_gpu()) return 3;
     // pages 1 -> 2, 2 -> 3, 3 -> 4, 4 -> 1 (0-based rows): every rank stays 0.85 * 1 + 0.15 = 1
     SparseVecMatrix ring({{0, {1}, {1.0}}, {1, {2}, {1.0}}, {2, {3}, {1.0}}, {3, {0}, {1.0}}}, 4, 4);
     auto r = pageRank(ring, 3);
@@ -64,6 +52,5 @@ int main(int argc, char** argv) {
             }
         std::fclose(out);
     }
-    std::printf("%d failed checks\n", failed);
-    return failed ? 1 : 0;
+    return finish("pagerank suite");
 }

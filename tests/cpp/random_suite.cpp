@@ -3,15 +3,13 @@
 // (java.util.Random.nextGaussian over XORShiftRandom.next, fdlibm's log), value for value.  Build with -ffp-contract=off:
 // the JVM never fuses a multiply and an add.  Exits 3 without a GPU (there is no CPU fallback), 1 on a failed check.
 #include "marlin_b200.hpp"
+#include "suite.h"
 
 #include <cmath>
 #include <cstdio>
 #include <cstring>
 
 using namespace marlin;
-
-static int failed = 0;
-#define CHECK(c) do { if (!(c)) { std::printf("FAILED %s:%d: %s\n", __FILE__, __LINE__, #c); ++failed; } } while (0)
 
 // fdlibm e_log.c for positive normal x < 1
 static double fdlibm_log(double x) {
@@ -81,12 +79,7 @@ struct Normal {
 static bool sameBits(double a, double b) { return std::memcmp(&a, &b, 8) == 0; }
 
 int main() {
-    try {
-        Context::get();
-    } catch (const std::exception& e) {
-        std::printf("cannot initialise marlin_b200: %s\n", e.what());
-        return 3;
-    }
+    if (!require_gpu()) return 3;
     const StandardNormalGenerator g{3.5, 0.25};
 
     {   // rows of 3 partitions, one stream per partition across its rows
@@ -142,6 +135,5 @@ int main() {
         }
         CHECK(bad == 0);
     }
-    std::printf("random suite: %d failed checks\n", failed);
-    return failed ? 1 : 0;
+    return finish("random suite");
 }

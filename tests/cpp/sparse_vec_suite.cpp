@@ -4,6 +4,7 @@
 // 150, 0.05, 2, seed 6) there ("row col float-bits" per line) for tests/test_cpp_spvec.py to compare with the Python API.
 // Exits 3 without a GPU (there is no CPU fallback), 1 on a failed check.
 #include "marlin_b200.hpp"
+#include "suite.h"
 
 #include <cmath>
 #include <cstdio>
@@ -11,21 +12,8 @@
 
 using namespace marlin;
 
-static int failed = 0;
-#define CHECK(c) do { if (!(c)) { std::printf("FAILED %s:%d: %s\n", __FILE__, __LINE__, #c); ++failed; } } while (0)
-
-template <class F> static bool throws(F f) {
-    try { f(); } catch (const std::exception&) { return true; }
-    return false;
-}
-
 int main(int argc, char** argv) {
-    try {
-        Context::get();
-    } catch (const std::exception& e) {
-        std::printf("cannot initialise marlin_b200: %s\n", e.what());
-        return 3;
-    }
+    if (!require_gpu()) return 3;
     // DistributedMatrixSuite.scala:27-32, 152-162
     std::vector<SparseVecMatrix::Row> data = {{0, {1, 3}, {2.0, 3.0}}, {1, {0, 1}, {5.0, 1.0}}, {2, {3}, {2.0}}, {3, {1, 2}, {1.0, 1.0}}};
     SparseVecMatrix sm(data, 4, 4), sm2(data, 4, 4);
@@ -69,6 +57,5 @@ int main(int argc, char** argv) {
         }
         std::fclose(f);
     }
-    std::printf("%d failed checks\n", failed);
-    return failed ? 1 : 0;
+    return finish("sparse_vec suite");
 }

@@ -2,6 +2,7 @@
 // (DistributedMatrixSuite.scala:375-388, commented out there), a tall random matrix against its own Gramian, and the
 // reference's argument errors.  Exits 3 without a GPU (there is no CPU fallback), 1 on a failed check.
 #include "marlin_b200.hpp"
+#include "suite.h"
 
 #include <cmath>
 #include <cstdio>
@@ -9,16 +10,8 @@
 
 using namespace marlin;
 
-static int failed = 0;
-#define CHECK(c) do { if (!(c)) { std::printf("FAILED %s:%d: %s\n", __FILE__, __LINE__, #c); ++failed; } } while (0)
-
 int main() {
-    try {
-        Context::get();
-    } catch (const std::exception& e) {
-        std::printf("cannot initialise marlin_b200: %s\n", e.what());
-        return 3;
-    }
+    if (!require_gpu()) return 3;
     const std::vector<DenseVecMatrix::Row> rows = {{0, {2.0, 0.0, 8.0, 6.0, 0.0}}, {1, {1.0, 6.0, 0.0, 1.0, 7.0}},
                                                    {2, {5.0, 0.0, 7.0, 4.0, 0.0}}, {3, {7.0, 0.0, 8.0, 5.0, 0.0}},
                                                    {4, {0.0, 10.0, 0.0, 0.0, 7.0}}};
@@ -67,6 +60,5 @@ int main() {
     CHECK(message(0, "auto") == "Request up to n singular values but got k=0 and n=5.");
     CHECK(message(2, "lanczos") == "Do not support mode lanczos.");
     CHECK(message(5, "local-eigs") == "k must be smaller than n in local-eigs mode but got k=5 and n=5.");
-    std::printf("svd suite: %d failed checks\n", failed);
-    return failed ? 1 : 0;
+    return finish("svd suite");
 }

@@ -1,52 +1,21 @@
 """The compiled host mirror (include/marlin_b200.hpp): the C++ port of the reference's DistributedMatrixSuite builds
 against the C ABI with plain g++, refuses to run without a GPU, and passes on an H100."""
-import shutil
-import subprocess
-from pathlib import Path
-
 import pytest
 
-ROOT = Path(__file__).resolve().parents[1]
-BIN = ROOT / "scripts" / "bin" / "dms_suite"
-
-
-def build_suite() -> Path:
-    from marlin_b200 import _native as nat
-    nat.load()                                   # make sure libmarlin_b200.so exists
-    BIN.parent.mkdir(parents=True, exist_ok=True)
-    cmd = [shutil.which("g++") or "g++", "-std=c++17", "-O1", "-Wall", "-Werror", f"-I{ROOT / 'include'}",
-           str(ROOT / "tests" / "cpp" / "dms_suite.cpp"), f"-L{ROOT / 'marlin_b200' / 'lib'}", "-lmarlin_b200",
-           "-Wl,-rpath,$ORIGIN/../../marlin_b200/lib", "-o", str(BIN)]
-    subprocess.run(cmd, check=True, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    return BIN
+from tests.harness import build_cpp, no_gpu_check, run_cpp
 
 
 def test_cpp_suite_builds_and_fails_loudly_without_gpu():
-    import torch
-    exe = build_suite()
-    if torch.cuda.is_available():
-        pytest.skip("GPU present: covered by test_cpp_suite_on_gpu")
-    out = subprocess.run([str(exe)], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=120)
-    assert out.returncode == 3
-    assert "no CPU fallback" in out.stdout
+    no_gpu_check(build_cpp("dms_suite"))
 
 
 @pytest.mark.gpu
 def test_cpp_suite_on_gpu():
-    exe = build_suite()
-    out = subprocess.run([str(exe)], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=300)
-    assert out.returncode == 0, out.stdout[-3000:]
-    assert "0 failed checks" in out.stdout
+    assert "0 failed checks" in run_cpp(build_cpp("dms_suite"))
 
 
 def test_cpp_rank_program_builds_and_fails_loudly_without_gpu():
     """tests/cpp/dist_multiply.cpp (the compiled caller of the multi-GPU multiply) builds with -Werror against the host mirror
     and, like everything else, refuses to run without a GPU."""
-    import torch
     from tests.test_gpu_dist_cabi import build_cpp_rank_program
-    exe = build_cpp_rank_program()
-    if torch.cuda.is_available():
-        pytest.skip("GPU present: covered by test_compiled_host_mirror_multiplies_across_two_ranks")
-    out = subprocess.run([str(exe), "0", "1", "nogpu", "1"], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=120)
-    assert out.returncode == 3
-    assert "no CPU fallback" in out.stdout
+    no_gpu_check(build_cpp_rank_program(), 0, 1, "nogpu", 1)

@@ -21,20 +21,12 @@ import numpy as np
 import pytest
 
 from marlin_b200 import _native as nat
+from tests.harness import gpu  # noqa: F401  (a fixture)
 from tests.test_gpu_fp64_edges import bf16_rne
 
 pytestmark = pytest.mark.gpu
 ROOT = Path(__file__).resolve().parents[1]
 KCHAIN_DEFAULT = 8192
-
-
-@pytest.fixture(scope="module")
-def gpu():
-    lib = nat.load()
-    ctx = nat.c_ctx()
-    nat.check(lib.mb_init(0, C.byref(ctx)))
-    yield lib, ctx
-    lib.mb_shutdown(ctx)
 
 
 # ------------------------------------------------------------------------------------------------------------ helpers

@@ -10,18 +10,10 @@ import numpy as np
 import pytest
 
 from marlin_b200 import _native as nat
+from tests.harness import gpu  # noqa: F401  (a fixture)
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-10
-
-
-@pytest.fixture(scope="module")
-def gpu():
-    lib = nat.load()
-    ctx = nat.c_ctx()
-    nat.check(lib.mb_init(0, C.byref(ctx)))
-    yield lib, ctx
-    lib.mb_shutdown(ctx)
 
 
 def _vp(a):

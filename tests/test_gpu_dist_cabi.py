@@ -9,6 +9,8 @@ from pathlib import Path
 
 import pytest
 
+from tests.harness import build_cpp
+
 pytestmark = pytest.mark.gpu
 ROOT = Path(__file__).resolve().parents[1]
 
@@ -76,19 +78,8 @@ def test_fused_reduce_scatter_full_size_back_to_back():
     assert "big fused" in "".join(o for _, o in outs)
 
 
-CPP_BIN = ROOT / "scripts" / "bin" / "dist_multiply"
-
-
 def build_cpp_rank_program() -> Path:
-    import shutil
-    from marlin_b200 import _native as nat
-    nat.load()
-    CPP_BIN.parent.mkdir(parents=True, exist_ok=True)
-    subprocess.run([shutil.which("g++") or "g++", "-std=c++17", "-O2", "-Wall", "-Wextra", "-Werror", f"-I{ROOT / 'include'}",
-                    str(ROOT / "tests" / "cpp" / "dist_multiply.cpp"), f"-L{ROOT / 'marlin_b200' / 'lib'}", "-lmarlin_b200",
-                    "-Wl,-rpath,$ORIGIN/../../marlin_b200/lib", "-o", str(CPP_BIN)], check=True, stdout=subprocess.PIPE,
-                   stderr=subprocess.STDOUT, text=True)
-    return CPP_BIN
+    return build_cpp("dist_multiply", opt="-O2", extra=("-Wextra",))
 
 
 @pytest.mark.parametrize("dims", [(700, 528, 900, 2, 3, 2), (512, 1024, 512, 1, 2, 1), (701, 530, 899, 2, 3, 2)],

@@ -10,18 +10,10 @@ import pytest
 import scipy.linalg as sla
 
 from marlin_b200 import _native as nat
+from tests.harness import gpu  # noqa: F401  (a fixture)
 from tests.test_gpu_cabi import alloc, download, upload_mat
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def gpu():
-    lib = nat.load()
-    ctx = nat.c_ctx()
-    nat.check(lib.mb_init(0, C.byref(ctx)))
-    yield lib, ctx
-    lib.mb_shutdown(ctx)
 
 
 def lu_gpu(gpu, A):

@@ -17,20 +17,11 @@ import pytest
 
 from marlin_b200 import _native as nat
 from tests import exact_oracle as eo
+from tests.harness import gpu  # noqa: F401  (a fixture)
 from tests.test_gpu_cabi import alloc, download, upload_mat
 
 pytestmark = pytest.mark.gpu
 EPS = np.finfo(np.float64).eps
-
-
-@pytest.fixture(scope="module")
-def gpu():
-    lib = nat.load()
-    ctx = nat.c_ctx()
-    nat.check(lib.mb_init(0, C.byref(ctx)))
-    yield lib, ctx
-    lib.mb_set_fp64_mode(ctx, 0, 7)
-    lib.mb_shutdown(ctx)
 
 
 # ------------------------------------------------------------------------------------------------------------ helpers

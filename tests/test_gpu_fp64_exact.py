@@ -20,6 +20,7 @@ import pytest
 
 from marlin_b200 import _native as nat
 from tests import exact_gemm as xg
+from tests.harness import gpu  # noqa: F401  (a fixture)
 from tests.test_gpu_bf16_exact import Stored
 
 pytestmark = pytest.mark.gpu
@@ -29,15 +30,6 @@ GROUPED = "gemm_f64_dmma16x8_grouped_kernel"
 GENERIC = "gemm_f64_generic_kernel"
 FORMS = [(0, 0), (1, 0), (0, 1), (1, 1)]
 FORM_IDS = ["NN", "TN", "NT", "TT"]
-
-
-@pytest.fixture(scope="module")
-def gpu():
-    lib = nat.load()
-    ctx = nat.c_ctx()
-    nat.check(lib.mb_init(0, C.byref(ctx)))
-    yield lib, ctx
-    lib.mb_shutdown(ctx)
 
 
 # ------------------------------------------------------------------------------------------------------------ helpers

@@ -9,18 +9,9 @@ import numpy as np
 import pytest
 
 from marlin_b200 import _native as nat
+from tests.harness import gpu  # noqa: F401  (a fixture)
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def gpu():
-    lib = nat.load()
-    ctx = nat.c_ctx()
-    nat.check(lib.mb_init(0, C.byref(ctx)))
-    yield lib, ctx
-    lib.mb_set_fp64_mode(ctx, 0, 7)
-    lib.mb_shutdown(ctx)
 
 
 def run(gpu, A, B, slices, C0=None, mode=1):

@@ -14,7 +14,8 @@ import pytest
 
 from marlin_b200 import _native as nat
 from tests import marlin_cases as mc
-from tests.test_gpu_cabi import alloc, download, gpu, upload, upload_mat  # noqa: F401  (gpu is a fixture)
+from tests.harness import gpu  # noqa: F401  (a fixture)
+from tests.test_gpu_cabi import alloc, download, upload, upload_mat
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-10
