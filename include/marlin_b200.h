@@ -40,6 +40,7 @@ extern "C" {
 #define MB_ERR_CUDA          -4   /* -> RuntimeException                                     */
 #define MB_ERR_OOM           -5
 #define MB_ERR_EMPTY         -6   /* -> RuntimeException (empty RDD: DistributedMatrixSuite "empty rows") */
+#define MB_ERR_IO            -9   /* a file that cannot be opened or written -> java.io.IOException */
 
 typedef enum { MB_F64 = 0, MB_BF16 = 1, MB_F32 = 2 } mb_dtype;
 
@@ -695,6 +696,23 @@ int32_t mb_matmul_blocked_dist_host(mb_comm* comm, const double* const* A_host, 
 /* Pinned host memory shared by the processes of one box (POSIX shm `name` + cudaHostRegister). */
 int32_t mb_host_alloc_shared(const char* name, int64_t bytes, void** out);
 int32_t mb_host_free_shared(const char* name, void* ptr, int64_t bytes, int32_t unlink_name);
+
+/* ---- f3: matrix text files, written on the device (matrix/DenseVecMatrix.scala:1042-1046, matrix/BlockMatrix.scala:550-555).
+ * Every value is printed as java.lang.Double.toString prints it: the shortest decimal that reads back as the same double
+ * (the closest one when several are as short), plain for 1e-3 <= |v| < 1e7, d.dddE[-]n otherwise, NaN, Infinity,
+ * -Infinity, -0.0.  Where the JVM picks a closer two-digit form of a one-digit decimal, this keeps the shortest one:
+ * Double.MIN_VALUE is 5.0E-324 (4.9E-324 on the JVM).  fp32 and bf16 blocks are widened to double first.  The text is
+ * formatted in chunks of at most MB_TEXT_CHUNK_VALUES values, two kernel launches each, and streamed to the file through
+ * pinned host memory; a view that holds no values is formatted on the host.  Each entry writes one part file, truncating
+ * it; a file that cannot be opened or written is MB_ERR_IO naming it.  Blocking. */
+#define MB_TEXT_CHUNK_VALUES 2097152
+/* DenseVecMatrix.saveToFileSystem's part file: `row_ids[r]:DenseVector(v, v, ...)` and a newline for each row r of the
+ * shard `rows` (a rows x cols view, read row by row; a row with no columns is `id:DenseVector()`).  rows may be NULL: an
+ * empty shard, an empty file.  row_ids: host int64[rows->rows]. */
+int32_t mb_save_rows(mb_ctx* ctx, const mb_block* rows, const int64_t* row_ids, const char* path);
+/* BlockMatrix.saveToFileSystem(path, "blockmatrix")'s part file: for block i, `r-c-rows-cols:v,v,...` and a newline, with
+ * (r, c) = (block_rc[2i], block_rc[2i + 1]) and the values column by column. */
+int32_t mb_save_blocks(mb_ctx* ctx, const mb_block* const* blocks, const int32_t* block_rc, int32_t count, const char* path);
 
 /* ---- rows <-> blocks on device (matrix/DenseVecMatrix.scala:1084-1223, 1259-1328;
  *      matrix/BlockMatrix.scala:575-594): a DenseVecMatrix shard is a row-major (rows x cols)

@@ -16,7 +16,9 @@
 #include <cctype>
 #include <cmath>
 #include <cstdint>
+#include <filesystem>
 #include <fstream>
+#include <ios>
 #include <map>
 #include <memory>
 #include <regex>
@@ -35,6 +37,7 @@ inline void check(int32_t rc) {
     if (rc == MB_OK) return;
     const std::string msg = mb_last_error();
     if (rc == MB_ERR_INVALID_ARG || rc == MB_ERR_DIM_MISMATCH || rc == MB_ERR_UNSUPPORTED) throw std::invalid_argument(msg);
+    if (rc == MB_ERR_IO) throw std::ios_base::failure(msg);                   // java.io.IOException
     throw std::runtime_error(msg);
 }
 
@@ -606,6 +609,9 @@ public:
         return BlockMatrix(res, numCols(), numRows(), numBlksByCol(), numBlksByRow());
     }
     inline DenseVecMatrix toDenseVecMatrix();                                         // :575-594
+    // saveToFileSystem(path, format) :550-559 — "blockmatrix" (any case): path/part-00000 with a line
+    // `row-col-rows-cols:v,v,...` per block, the values column by column; any other format: the DenseVecMatrix file
+    inline void saveToFileSystem(const std::string& path, const std::string& format = " ");
     // cBind(other) :687-705 — with the same number of block rows, other's block columns are relabelled by
     // + numBlksByCol() (no block copied) when the joint widths are exactly the ceil-sized grid that toBreeze, multiply and
     // re-gridding assume; otherwise, and with a DenseVecMatrix, the DenseVecMatrix cBind of both (DESIGN §3.14)
@@ -792,6 +798,24 @@ public:
     DenseVecMatrix subtract(BlockMatrix& o) { DenseVecMatrix d = o.toDenseVecMatrix(); return subtract(d); }
     DenseVecMatrix dotProduct(BlockMatrix& o) { DenseVecMatrix d = o.toDenseVecMatrix(); return dotProduct(d); }
     double sum() { if (ids_.empty()) throw std::runtime_error("empty collection"); return data_.sum(); }
+    // saveToFileSystem(path) :1042-1046 — path/part-00000 with a line `id:DenseVector(v, v, ...)` per row, formatted on
+    // the device (mb_save_rows)
+    void saveToFileSystem(const std::string& path) {
+        static_assert(sizeof(long) == sizeof(int64_t), "row ids are int64");
+        std::filesystem::create_directories(path);
+        const std::string part = path + "/part-00000";
+        check(mb_save_rows(Context::get(), ids_.empty() ? nullptr : data_.handle(), reinterpret_cast<const int64_t*>(ids_.data()),
+                           part.c_str()));
+    }
+    // saveWithDescription(path) :1055-1064 — the rows as above and path/_description: `MatrixName\tN/A` and
+    // `MatrixSize\t<rows> <cols>`
+    void saveWithDescription(const std::string& path) {
+        saveToFileSystem(path);
+        const std::string desc = "MatrixName\tN/A\nMatrixSize\t" + std::to_string(numRows()) + " " + std::to_string(numCols());
+        std::ofstream f(path + "/_description", std::ios::binary);
+        f << desc;
+        if (!f.flush()) throw std::ios_base::failure("cannot write " + path + "/_description");
+    }
 
     // norm(mode) :975-999 — "1": the largest column sum of |a|, "inf": the largest row sum of |a|, "fro": sqrt(sum a^2);
     // any other mode ("2" too) is "Do not support mode <mode>.".  One pass over the shard (mb_block_norm); the reference's
@@ -1102,6 +1126,25 @@ inline DenseVecMatrix BlockMatrix::toDenseVecMatrix() {                         
     std::vector<long> ids(nr);
     for (int i = 0; i < nr; ++i) ids[i] = i;
     return DenseVecMatrix(ids, shard, nr, nc);
+}
+inline void BlockMatrix::saveToFileSystem(const std::string& path, const std::string& format) {        // :550-559
+    std::string f = format;
+    for (char& ch : f) ch = (char)std::tolower((unsigned char)ch);
+    if (f != "blockmatrix") {
+        toDenseVecMatrix().saveToFileSystem(path);
+        return;
+    }
+    if (hasSparse()) throw std::invalid_argument("saveToFileSystem is not supported on sparse blocks: call toDenseBlocks first");
+    std::filesystem::create_directories(path);
+    std::vector<const mb_block*> hs;
+    std::vector<int32_t> rc;
+    for (auto& kv : blocks) {
+        hs.push_back(kv.second.handle());
+        rc.push_back(kv.first.row);
+        rc.push_back(kv.first.column);
+    }
+    const std::string part = path + "/part-00000";
+    check(mb_save_blocks(Context::get(), hs.data(), rc.data(), (int32_t)hs.size(), part.c_str()));
 }
 inline std::variant<BlockMatrix, DenseVecMatrix> BlockMatrix::cBind(BlockMatrix& other) {                            // :687-699
     if (numRows() != other.numRows()) throw std::invalid_argument("Row dimension mismatches: " + std::to_string(numRows()) + " vs " + std::to_string(other.numRows()));

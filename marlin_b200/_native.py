@@ -19,6 +19,7 @@ MB_ERR_OOM = -5
 MB_ERR_EMPTY = -6
 MB_ERR_TIMEOUT = -7
 MB_ERR_NO_CONVERGENCE = -8
+MB_ERR_IO = -9
 
 MB_F64, MB_BF16, MB_F32 = 0, 1, 2
 MB_SVD_LOCAL_LAPACK, MB_SVD_LOCAL_ARPACK, MB_SVD_DIST_ARPACK = 0, 1, 2
@@ -26,6 +27,7 @@ MB_ALS_MAX_RANK = 128
 MB_SPVEC_WARP_BOUND, MB_SPVEC_CTA_BOUND, MB_SPVEC_WINDOW = 256, 4096, 16384
 MB_PAGERANK_LIGHT_BOUND = 256
 MB_NORM_ONE, MB_NORM_INF, MB_NORM_FRO = 0, 1, 2
+MB_TEXT_CHUNK_VALUES = 2097152
 
 _LIB_PATH = Path(__file__).resolve().parent / "lib" / "libmarlin_b200.so"
 
@@ -113,6 +115,8 @@ SIGNATURES = {
     "mb_coo_to_dense_rows": (c_i32, [c_ctx, c_i64, C.c_void_p, C.c_void_p, C.c_void_p, c_blk]),
     "mb_fill_uniform": (c_i32, [c_ctx, c_blk, c_i64, c_i64, c_f64, c_f64, c_i32]),
     "mb_fill_normal": (c_i32, [c_ctx, c_blk, c_i64, c_f64, c_f64, c_i32, C.POINTER(c_i64)]),
+    "mb_save_rows": (c_i32, [c_ctx, c_blk, C.c_void_p, C.c_char_p]),
+    "mb_save_blocks": (c_i32, [c_ctx, C.POINTER(c_blk), C.c_void_p, c_i32, C.c_char_p]),
     "mb_sparse_check": (c_i32, [c_i32, c_i32, C.c_void_p, C.c_void_p]),
     "mb_sparse_wrap": (c_i32, [c_ctx, c_i32, c_i32, c_i64, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(c_sp)]),
     "mb_sparse_upload": (c_i32, [c_ctx, c_i32, c_i32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(c_sp)]),

@@ -16,7 +16,7 @@ CSRC = PKG / "csrc"
 LIBDIR = PKG / "lib"
 LIB = LIBDIR / "libmarlin_b200.so"
 
-SOURCES = ["capi.cu", "gemm_f64.cu", "gemm_bf16.cu", "gemm_ozaki.cu", "elementwise.cu", "blas12.cu", "peer.cu", "dist.cu", "factor.cu", "eigen.cu", "sparse.cu", "logistic.cu", "als.cu", "spvec.cu", "pagerank.cu", "mlp.cu", "norm.cu", "eigs.cu", "normal.cu", "hostlogic.cpp"]
+SOURCES = ["capi.cu", "gemm_f64.cu", "gemm_bf16.cu", "gemm_ozaki.cu", "elementwise.cu", "blas12.cu", "peer.cu", "dist.cu", "factor.cu", "eigen.cu", "sparse.cu", "logistic.cu", "als.cu", "spvec.cu", "pagerank.cu", "mlp.cu", "norm.cu", "eigs.cu", "normal.cu", "text.cu", "hostlogic.cpp"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",

@@ -18,8 +18,10 @@
 #include "norm.h"
 #include "eigs.h"
 #include "normal.h"
+#include "text.h"
 
 #include <cuda_runtime.h>
+#include <cerrno>
 #include <climits>
 #include <algorithm>
 #include <cmath>
@@ -2617,6 +2619,68 @@ int32_t mb_nn_step(mb_ctx* ctx, const mb_block* const* X, const mb_block* const*
     MB_CTX(ctx);
     MB_LOCK(ctx);
     return nn_run(ctx, X, XT, labels, nsel, W1, W2, scale, nullptr, nullptr, nullptr, true);
+}
+
+// ------------------------------------------------------------------------------------------- matrix text files (SURVEY 8 f3)
+// One part file: the segments' text through mb::save_text.  The file is opened (truncated) before anything else, so an
+// unwritable path fails without touching the device.
+static int32_t save_segments(mb_ctx* ctx, const mb::TextSegment* segs, const long long* const* host_ids, int count,
+                             const char* path, const char* what) {
+    FILE* f = std::fopen(path, "wb");
+    if (!f) return fail(MB_ERR_IO, "%s: cannot open %s: %s", what, path, std::strerror(errno));
+    mb::TextIo io{ctx->stream, nullptr, {}, f};
+    cudaError_t e = ensure_copy_streams(ctx);
+    for (int i = 0; i < 4 && e == cudaSuccess; ++i) e = next_event(ctx, &io.events[i]);
+    int io_errno = 0;
+    if (e == cudaSuccess) {
+        io.copy_stream = ctx->d2h_stream;
+        e = mb::save_text(segs, host_ids, count, io, &io_errno);
+    }
+    const bool closed = std::fclose(f) == 0;
+    if (e != cudaSuccess) return cuda_fail(e, what);
+    if (io_errno || !closed) return fail(MB_ERR_IO, "%s: cannot write %s: %s", what, path, std::strerror(io_errno ? io_errno : errno));
+    return MB_OK;
+}
+
+static mb::TextSegment text_segment(const mb_block* b) {
+    return mb::TextSegment{elem_ptr(b), rs(b), cs(b), b->rows, b->cols, b->dtype, nullptr, 0, 0};
+}
+
+// DenseVecMatrix.scala:1042-1046: rdd.map(t => t._1 + ":" + t._2.toString).saveAsTextFile(path), one partition
+int32_t mb_save_rows(mb_ctx* ctx, const mb_block* rows, const int64_t* row_ids, const char* path) {
+    MB_CTX(ctx);
+    MB_LOCK(ctx);
+    if (!path || (rows && rows->rows > 0 && !row_ids) || (rows && (rows->rows < 0 || rows->cols < 0)))
+        return fail(MB_ERR_INVALID_ARG, "mb_save_rows: bad argument");
+    ctx->events_used = 0;
+    mb::TextSegment seg{};
+    const long long* host_ids = reinterpret_cast<const long long*>(row_ids);
+    mb::StreamBuffer ids;
+    const int count = rows && rows->rows > 0 ? 1 : 0;
+    if (count) {
+        seg = text_segment(rows);
+        MB_CUDA(ids.upload(row_ids, sizeof(long long) * (size_t)rows->rows, ctx->stream));
+        seg.ids = ids.as<long long>();
+    }
+    return save_segments(ctx, &seg, &host_ids, count, path, "mb_save_rows");
+}
+
+// BlockMatrix.scala:550-555: blocks.map(t => t._1.row + "-" + t._1.column + "-" + t._2.rows + "-" + t._2.cols + ":" +
+// t._2.data.mkString(",")).saveAsTextFile(path), one partition (data: the column-major array)
+int32_t mb_save_blocks(mb_ctx* ctx, const mb_block* const* blocks, const int32_t* block_rc, int32_t count, const char* path) {
+    MB_CTX(ctx);
+    MB_LOCK(ctx);
+    if (!path || count < 0 || (count > 0 && (!blocks || !block_rc))) return fail(MB_ERR_INVALID_ARG, "mb_save_blocks: bad argument");
+    std::vector<mb::TextSegment> segs;
+    for (int i = 0; i < count; ++i) {
+        if (!blocks[i]) return fail(MB_ERR_INVALID_ARG, "mb_save_blocks: block %d is null", i);
+        segs.push_back(text_segment(blocks[i]));
+        segs.back().block_row = block_rc[2 * i];
+        segs.back().block_col = block_rc[2 * i + 1];
+    }
+    ctx->events_used = 0;
+    std::vector<const long long*> host_ids((size_t)count, nullptr);
+    return save_segments(ctx, segs.data(), host_ids.data(), count, path, "mb_save_blocks");
 }
 
 }  // extern "C"

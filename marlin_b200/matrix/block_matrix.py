@@ -770,17 +770,29 @@ class BlockMatrix(DistributedMatrix):
     # ------------------------------------------------------------------ I/O (next-row (f)-3)
     def saveToFileSystem(self, path: str, format: str = " ") -> None:
         """:550-559 — "blockmatrix": `row-col-rows-cols:v,v,...` column-major; else DenseVecMatrix format."""
-        from ..utils.mt_utils import _jdouble
         self._dense_only("saveToFileSystem")
         if format.lower() == "blockmatrix":
+            import ctypes as C
+            import os
+            rank, ws = world()
+            os.makedirs(path, exist_ok=True)
+            part = os.path.join(path, f"part-{rank:05d}")
+            on_device = any(s.buf.is_cuda for _, s in self.blocks) if self.blocks else Runtime.available()
+            if on_device:
+                # the device writer (mb_save_blocks): only text crosses PCIe
+                rt = Runtime.get()
+                rt.sync_stream()
+                handles = (nat.c_blk * max(1, len(self.blocks)))(*[s.handle() for _, s in self.blocks])
+                rc = np.array([[b.row, b.column] for b, _ in self.blocks], dtype=np.int32).reshape(-1)
+                nat.check(rt.lib.mb_save_blocks(rt.ctx, handles, rc.ctypes.data_as(C.c_void_p), len(self.blocks),
+                                                os.fsencode(part)))
+                return
+            from ..utils.mt_utils import _jdouble
             lines = []
-            for b, s in self.blocks:
+            for b, s in self.blocks:                   # host-resident blocks, which exist without a GPU only
                 data = s.toBreeze().reshape(-1, order="F")
                 lines.append(f"{b.row}-{b.column}-{s.rows}-{s.cols}:" + ",".join(_jdouble(v) for v in data))
-            rank, ws = world()
-            import os
-            os.makedirs(path, exist_ok=True)
-            with open(os.path.join(path, f"part-{rank:05d}"), "w") as fh:
+            with open(part, "w") as fh:
                 fh.write("\n".join(lines) + ("\n" if lines else ""))
         else:
             self.toDenseVecMatrix().saveToFileSystem(path)

@@ -908,12 +908,25 @@ class DenseVecMatrix(DistributedMatrix):
 
     # ------------------------------------------------------------------ I/O (next-row (f)-3)
     def _save_rows(self, path: str) -> None:
+        """This rank's part file.  Device-resident rows are formatted by the device writer (mb_save_rows), which sends
+        only text across PCIe; the host loop serves host-resident rows, which exist without a GPU only."""
         import os
-        from ..utils.mt_utils import _jdouble
         rank, ws = world()
         os.makedirs(path, exist_ok=True)
-        arr = self.data.toBreeze() if self.data is not None and len(self.ids) else np.zeros((0, 0))
-        with open(os.path.join(path, f"part-{rank:05d}"), "w") as fh:
+        part = os.path.join(path, f"part-{rank:05d}")
+        has_rows = self.data is not None and len(self.ids) > 0
+        on_device = self.data.buf.is_cuda if has_rows else Runtime.available()
+        if on_device:
+            import ctypes as C
+            rt = Runtime.get()
+            rt.sync_stream()
+            ids = np.ascontiguousarray(self.ids, dtype=np.int64)
+            nat.check(rt.lib.mb_save_rows(rt.ctx, self.data.handle() if has_rows else None,
+                                          ids.ctypes.data_as(C.c_void_p) if has_rows else None, os.fsencode(part)))
+            return
+        from ..utils.mt_utils import _jdouble
+        arr = self.data.toBreeze() if has_rows else np.zeros((0, 0))
+        with open(part, "w") as fh:
             for pos, idx in enumerate(self.ids):
                 fh.write(f"{int(idx)}:DenseVector(" + ", ".join(_jdouble(v) for v in arr[pos, :]) + ")\n")
 
