@@ -301,8 +301,9 @@ inline void bands_of(int extent, int most, int& band, int& nbands) {
     nbands = (extent + band - 1) / band;
 }
 
-// Fused reduce-scatter: of a C tile N columns wide the owner reduces [0, half_cols(N)), the partner the rest.
-inline int half_cols(int N) { return std::min(N, ((N / 2 + 127) / 128) * 128); }
+// Fused reduce-scatter: of a C tile N columns wide the owner reduces [0, half_cols(N)), the partner the rest.  The
+// owner's half is never empty (at N = 1, N / 2 rounds to nothing): a grouped entry zero columns wide is refused.
+inline int half_cols(int N) { return std::min(N, std::max(128, ((N / 2 + 127) / 128) * 128)); }
 
 // ---------------------------------------------------------------------------------------- staging
 // Per-source slots: src only ever writes [src * slot_bytes, +slot_bytes) of dst's buffer, so two sources can never
